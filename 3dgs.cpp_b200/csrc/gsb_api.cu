@@ -135,7 +135,7 @@ cudaError_t launch_frame_init(Control* ctl, uint32_t* project_status, uint32_t p
                               uint32_t num_extra_words) {
     const uint32_t work = std::max<uint32_t>(std::max(std::max(std::max(project_chunks, emit_chunks), num_tiles), num_extra_words),
                                              (uint32_t)(sizeof(Control) / 4));
-    const uint32_t blocks = std::min<uint32_t>((work + 255) / 256, 148u * 4u);
+    const uint32_t blocks = std::min<uint32_t>((work + 255) / 256, 132u * 4u);  // 4 CTAs per H100 SM; grid-stride
     k_frame_init<<<blocks, 256, 0, s>>>(ctl, project_status, project_chunks, emit_status, emit_chunks, ranges, num_tiles, extra_words,
                                         num_extra_words);
     return cudaGetLastError();
@@ -391,7 +391,6 @@ int enqueue_blend(gsb_ctx* ctx, const FramePlan& fp, uint32_t b0, uint32_t b1, v
     bp.mode = ctx->mode;
     bp.variant = ctx->blend_variant;
     bp.stats = ctx->debug ? 2 : (ctx->timers ? 1 : 0);  // 2 also counts blend_pixel_hits (a few % of the kernel)
-    bp.one = 1.0f;
     bp.ctl = ctx->ctl;
     CK(launch_blend(bp, stream));
     return GSB_OK;
@@ -483,12 +482,12 @@ int gsb_create(int device, gsb_ctx** out) {
     if ((e = cudaSetDevice(device)) != cudaSuccess) return bail("cudaSetDevice", e);
     cudaDeviceProp prop;
     if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return bail("cudaGetDeviceProperties", e);
-    // The library carries sm_100a SASS only (arch-specific, no forward-compatible PTX): any other device would pass
+    // The library carries sm_90a SASS only (arch-specific, no forward-compatible PTX): any other device would pass
     // here and fail at its first launch with "no kernel image".  Probe a kernel image instead of trusting major/minor.
     cudaFuncAttributes fa;
-    if (prop.major != 10 || prop.minor != 0 || cudaFuncGetAttributes(&fa, k_frame_init) != cudaSuccess) {
+    if (prop.major != 9 || prop.minor != 0 || cudaFuncGetAttributes(&fa, k_frame_init) != cudaSuccess) {
         cudaGetLastError();
-        g_create_error = "libgsb200 is built for sm_100a (B200, compute capability 10.0) only; device is sm_" +
+        g_create_error = "libgsb200 is built for sm_90a (H100, compute capability 9.0) only; device is sm_" +
                          std::to_string(prop.major) + std::to_string(prop.minor);
         gsb_destroy(ctx);
         return GSB_ERR_NO_DEVICE;

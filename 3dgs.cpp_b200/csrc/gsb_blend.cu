@@ -26,10 +26,10 @@ namespace {
 constexpr int BLEND_THREADS = 256;
 constexpr unsigned FULL = 0xffffffffu;
 
-// Bit-defined exp for x in [-87, 0]; mirrors gso_exp_shared() in oracle/gs_oracle.c op for op: Cody-Waite
-// reduction, degree-5 Horner with the constant term 1, 2^n applied through the exponent bits (13 instructions).
-__device__ __forceinline__ float exp_shared(float x) {
-    x = fmaxf(x, -87.0f);
+// Bit-defined exp for x in [-87, 0] without the clamp; mirrors gso_exp_shared() in oracle/gs_oracle.c op for op: Cody-Waite
+// reduction, degree-5 Horner with the constant term 1, 2^n applied through the exponent bits (12 instructions).  Callers
+// that only use results with power in [cut, 0] (cut >= -87) call it directly: the clamp is the identity there.
+__device__ __forceinline__ float exp_shared_inrange(float x) {
     const float t = __fmul_rn(x, 1.44269504088896341f);
     const float tm = __fadd_rn(t, 12582912.0f);  // low mantissa bits = rint(t) in two's complement
     const float n = __fsub_rn(tm, 12582912.0f);
@@ -42,23 +42,7 @@ __device__ __forceinline__ float exp_shared(float x) {
     p = __fmaf_rn(p, r, 1.0f);
     return __uint_as_float(__float_as_uint(p) + (__float_as_uint(tm) << 23));
 }
-
-#if GSB_BLEND_TDONE
-// same sequence without the clamp: only evaluated results with power in [cut, 0] are used (identity there)
-__device__ __forceinline__ float exp_shared_inrange(float x) {
-    const float t = __fmul_rn(x, 1.44269504088896341f);
-    const float tm = __fadd_rn(t, 12582912.0f);
-    const float n = __fsub_rn(tm, 12582912.0f);
-    float r = __fmaf_rn(n, -0.693359375f, x);
-    r = __fmaf_rn(n, 2.12194440e-4f, r);
-    float p = __fmaf_rn(8.290082216262817e-3f, r, 4.1899293661117554e-2f);
-    p = __fmaf_rn(p, r, 1.6667647659778595e-1f);
-    p = __fmaf_rn(p, r, 4.9999138712882996e-1f);
-    p = __fmaf_rn(p, r, 9.999997019767761e-1f);
-    p = __fmaf_rn(p, r, 1.0f);
-    return __uint_as_float(__float_as_uint(p) + (__float_as_uint(tm) << 23));
-}
-#endif
+__device__ __forceinline__ float exp_shared(float x) { return exp_shared_inrange(fmaxf(x, -87.0f)); }
 
 // shared-memory loads by 32-bit shared-window address (one LDS each, immediate offsets, no generic-pointer arithmetic)
 __device__ __forceinline__ float4 lds_f4(uint32_t addr) {
@@ -103,7 +87,7 @@ struct __align__(16) StagedRec {
 };
 
 #ifndef GSB_BLEND_CHECK
-#define GSB_BLEND_CHECK 8  // records walked between two "is the whole warp done" votes (measured: 8 -> 0.673 ms, 16 -> 0.685, 32 -> 0.733)
+#define GSB_BLEND_CHECK 8  // records walked between two "is the whole warp done" votes
 #endif
 #ifndef GSB_BLEND_TDONE
 #define GSB_BLEND_TDONE 0  // 1: a finished pixel is T == 0 (no separate flag in the walk); needs GSB_BLEND_PREDICATED
@@ -112,7 +96,7 @@ struct __align__(16) StagedRec {
 #define GSB_BLEND_PREDICATED 1
 #endif
 #ifndef GSB_BLEND_MIN_BLOCKS
-#define GSB_BLEND_MIN_BLOCKS 5  // <= 51 registers, 5 CTAs per SM (measured: 0.873 ms; 4 CTAs 0.886, 6 CTAs 0.891, 80 registers 0.972)
+#define GSB_BLEND_MIN_BLOCKS 5  // <= 51 registers, 5 CTAs per SM
 #endif
 template <int MODE>
 __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(const __grid_constant__ BlendParams P) {
@@ -282,74 +266,16 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
 
 
 // ------------------------------------------------------------------------------------------------------------------
-// k_blend2 -- two pixels per thread, packed fp32 (Blackwell FMUL2 / FADD2 / FFMA2 = PTX *.f32x2).
+// k_blend2 -- two pixels per thread.
 //
 // One CTA of 128 threads owns one 16x16 tile; warp w owns the 8x8 pixel block at (8 (w & 1), 8 (w >> 1)) and lane
-// (lx = lane & 7, ly = lane >> 3) owns the two pixels (lx, ly) and (lx, ly + 4) of it.  Every arithmetic step of
-// render.comp:64-88 is issued once for both pixels as one packed instruction; each half of a packed instruction is the
-// same single correctly rounded IEEE operation as its scalar form, so EXACT mode stays bit-identical to the oracle.
-// Measured on B200 (tools/ubench/f32x2.cu): FMUL2 / FADD2 issue at the scalar rate (2x the lanes per issue slot), FFMA2
-// at half of it (same lanes per cycle as FFMA) -- the kernel is issue-bound, so what counts is that the per-record loop
-// drops from 51.5 instructions per 32 pixels to ~66 per 64 pixels.  The comparisons and selects of the shader's
-// `continue` / `break` logic have no packed form and stay per pixel.
-// Staged records are stored pre-broadcast ((ux, ux), (A', A'), ...) so that every packed operand is an aligned register
-// pair straight out of an LDS.128: no MOVs in the loop.  Per-warp survivor lists, per-block conservative culling
-// (8x8 blocks) and the batch pipeline are those of k_blend.
+// (lx = lane & 7, ly = lane >> 3) owns the two pixels (lx, ly) and (lx, ly + 4) of it.  The two pixels share a column,
+// so one staged record (three LDS.128) serves both, and the terms of render.comp:64-66 that depend on dx only are
+// computed once per record instead of once per pixel; everything else is two independent scalar chains (ILP for the
+// issue-bound walk).  Every step is the same single correctly rounded IEEE operation as in k_blend (-fmad=false: no
+// contraction), so EXACT mode stays bit-identical to the oracle.  Per-warp survivor lists, per-block conservative
+// culling (8x8 blocks) and the batch pipeline are those of k_blend.
 // ------------------------------------------------------------------------------------------------------------------
-typedef unsigned long long u64;
-__device__ __forceinline__ u64 pk2(float lo, float hi) {
-    u64 r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void upk2(u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ u64 mul2(u64 a, u64 b) {
-    u64 d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
-__device__ __forceinline__ u64 add2(u64 a, u64 b) {
-    u64 d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
-__device__ __forceinline__ u64 sub2(u64 a, u64 b) {
-    u64 d;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
-__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
-    u64 d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
-}
-// EXACT-mode add whose first operand is a packed PRODUCT.  ptxas 12.9 contracts mul.rn.f32x2 + add.rn.f32x2 into FFMA2 even
-// though both carry .rn (it honours .rn for scalar f32; -fmad=false, volatile asm and a constant 1.0 multiplier do not
-// stop it -- checked in SASS), which would change the rounding of render.comp:66/:87.  Two ways to keep the two roundings:
-//   GSB_BLEND2_ADD == 1: a + b = fma(a, 1.0, b) with the 1.0 coming from a kernel argument (opaque to ptxas), one FFMA2
-//                        with a uniform-register operand;
-//   GSB_BLEND2_ADD == 0: two scalar add.rn.f32 on the halves.
-#ifndef GSB_BLEND2_ADD
-#define GSB_BLEND2_ADD 0  // measured on the bench scene: k_blend2 0.597 ms with the scalar adds, 0.665 ms with FFMA2 (half-rate on B200)
-#endif
-#ifndef GSB_BLEND2_PRED
-#define GSB_BLEND2_PRED 1  // colour / transmittance updates: 1 = predicated scalar adds, 0 = packed adds + selects
-#endif
-__device__ __forceinline__ u64 add2_of_product(u64 prod, u64 b, u64 one2) {
-#if GSB_BLEND2_ADD
-    return fma2(prod, one2, b);
-#else
-    float p0, p1, b0, b1;
-    upk2(prod, p0, p1);
-    upk2(b, b0, b1);
-    return pk2(__fadd_rn(p0, b0), __fadd_rn(p1, b1));
-#endif
-}
-// two 64-bit register pairs out of one LDS.128
-__device__ __forceinline__ void lds_2x64(uint32_t addr, u64& a, u64& b) {
-    asm volatile("ld.shared.v2.u64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "r"(addr));
-}
-
 #ifndef GSB_BLEND2_BATCH
 #define GSB_BLEND2_BATCH 256  // records staged per batch (2 per thread)
 #endif
@@ -367,12 +293,10 @@ constexpr int B2_SEG = 4 * B2_THREADS;  // list entries scanned per batch at mos
 constexpr int B2_BATCH = GSB_BLEND2_BATCH;
 constexpr int B2_WARPS = B2_THREADS / 32;
 
-struct __align__(16) StagedRec2 {  // 80 B: five 16-B slots = five LDS.128 per visited record
-    float4 q0;  // ux ux uy uy
-    float4 q1;  // -A/2 -A/2 -B -B       (exact power-of-two / sign scalings of the conic, as in k_blend)
-    float4 q2;  // -C/2 -C/2 opacity opacity
-    float4 q3;  // r r g g
-    float4 q4;  // b b power_cut bits(index in batch)
+struct __align__(16) StagedRec2 {  // 48 B: three 16-B slots = three LDS.128 per visited record
+    float4 q0;  // ux uy -A/2 -B       (exact power-of-two / sign scalings of the conic, as in k_blend)
+    float4 q1;  // -C/2 opacity r g
+    float4 q2;  // b power_cut bits(index in batch) -
 };
 
 __device__ __forceinline__ uint32_t block_mask2(float ux, float uy, float A, float B, float C, float cut, float tile_x0, float tile_y0) {
@@ -385,27 +309,6 @@ __device__ __forceinline__ uint32_t block_mask2(float ux, float uy, float A, flo
         if (rect_may_contribute(ux, uy, A, B, C, inv_a, inv_c, x0, y0, 8.0f, 8.0f, cut)) mask |= 1u << w;
     }
     return mask;
-}
-
-// exp for both pixels; same operation sequence as exp_shared without the clamp at -87 (identity on [cut, 0] with
-// cut >= -87, and results for powers outside that range are never selected)
-__device__ __forceinline__ void exp_shared2(u64 x, u64 one2, float& e0, float& e1) {
-    const u64 L2E = pk2(1.44269504088896341f, 1.44269504088896341f), MAGIC = pk2(12582912.0f, 12582912.0f);
-    const u64 t = mul2(x, L2E);
-    const u64 tm = add2_of_product(t, MAGIC, one2);
-    const u64 n = sub2(tm, MAGIC);
-    u64 r = fma2(n, pk2(-0.693359375f, -0.693359375f), x);
-    r = fma2(n, pk2(2.12194440e-4f, 2.12194440e-4f), r);
-    u64 p = fma2(pk2(8.290082216262817e-3f, 8.290082216262817e-3f), r, pk2(4.1899293661117554e-2f, 4.1899293661117554e-2f));
-    p = fma2(p, r, pk2(1.6667647659778595e-1f, 1.6667647659778595e-1f));
-    p = fma2(p, r, pk2(4.9999138712882996e-1f, 4.9999138712882996e-1f));
-    p = fma2(p, r, pk2(9.999997019767761e-1f, 9.999997019767761e-1f));
-    p = fma2(p, r, pk2(1.0f, 1.0f));
-    float p0, p1, m0, m1;
-    upk2(p, p0, p1);
-    upk2(tm, m0, m1);
-    e0 = __uint_as_float(__float_as_uint(p0) + (__float_as_uint(m0) << 23));
-    e1 = __uint_as_float(__float_as_uint(p1) + (__float_as_uint(m1) << 23));
 }
 
 // COARSE (gsb_set_tile_cull level 2): the list is that of a block of 2^cs x 2^cs tiles and every entry's key carries the mask
@@ -446,8 +349,7 @@ __global__ void __launch_bounds__(B2_THREADS, GSB_BLEND2_MIN_BLOCKS) k_blend2(co
     const uint32_t px = tx * GSB_TILE + (warp & 1) * 8 + (lane & 7);
     const uint32_t py0 = ty * GSB_TILE + (warp >> 1) * 8 + (lane >> 3), py1 = py0 + 4;
     const bool in0 = px < P.width && py0 < P.height, in1 = px < P.width && py1 < P.height;  // :37-39
-    const u64 fx2 = pk2((float)px, (float)px), fy2 = pk2((float)py0, (float)py1);
-    const u64 one2 = pk2(P.one, P.one);  // 1.0f the compiler cannot see (add2_of_product)
+    const float fx = (float)px, fy0 = (float)py0, fy1 = (float)py1;
     const float tile_x0 = (float)(tx * GSB_TILE), tile_y0 = (float)(ty * GSB_TILE);
     if (tid == 0) {
         s_used = 0;
@@ -572,13 +474,10 @@ __global__ void __launch_bounds__(B2_THREADS, GSB_BLEND2_MIN_BLOCKS) k_blend2(co
                 const float cut = power_cut(b.y);
                 const uint32_t m = block_mask2(a.x, a.y, a.z, a.w, b.x, cut, tile_x0, tile_y0);
                 if (m) {
-                    const float na = -0.5f * a.z, nb = -a.w, nc = -0.5f * b.x;
-                    s_rec[li].q0 = make_float4(a.x, a.x, a.y, a.y);
-                    s_rec[li].q1 = make_float4(na, na, nb, nb);
-                    s_rec[li].q2 = make_float4(nc, nc, b.y, b.y);
-                    s_rec[li].q3 = make_float4(col.x, col.x, col.y, col.y);
-                    // q4.w: position in the list relative to the batch's base offset (the consumed-entries statistic)
-                    s_rec[li].q4 = make_float4(col.z, col.z, cut, __uint_as_float(COARSE ? s_eidx[li] : li));
+                    s_rec[li].q0 = make_float4(a.x, a.y, -0.5f * a.z, -a.w);
+                    s_rec[li].q1 = make_float4(-0.5f * b.x, b.y, col.x, col.y);
+                    // q2.z: position in the list relative to the batch's base offset (the consumed-entries statistic)
+                    s_rec[li].q2 = make_float4(col.z, cut, __uint_as_float(COARSE ? s_eidx[li] : li), 0.f);
                 }
                 s_mask[li] = (uint8_t)m;
             }
@@ -600,64 +499,53 @@ __global__ void __launch_bounds__(B2_THREADS, GSB_BLEND2_MIN_BLOCKS) k_blend2(co
                 const uint32_t k1 = min(n, k0 + (uint32_t)GSB_BLEND2_CHECK);
                 for (uint32_t k = k0; k < k1; k++) {
                     const uint32_t addr = lds_u16(list_sh + 2u * k);
-                    u64 ux2, uy2, A2, B2, C2, op2, r2, g2, b2, misc;
-                    lds_2x64(addr, ux2, uy2);
-                    lds_2x64(addr + 16u, A2, B2);
-                    lds_2x64(addr + 32u, C2, op2);
-                    lds_2x64(addr + 48u, r2, g2);
-                    lds_2x64(addr + 64u, b2, misc);
-                    float cut, idxf;
-                    upk2(misc, cut, idxf);
-                    const u64 dx2 = sub2(ux2, fx2), dy2 = sub2(uy2, fy2);  // :64
+                    const float4 q0 = lds_f4(addr), q1 = lds_f4(addr + 16u), q2 = lds_f4(addr + 32u);
+                    const float cut = q2.y;
+                    const float dx = q0.x - fx, dy0 = q0.y - fy0, dy1 = q0.y - fy1;  // :64 (one column: dx is shared)
                     float pw0, pw1, al0, al1;
-                    u64 alpha2;
                     if (MODE == GSB_MODE_EXACT) {
                         // :66 with the pre-scaled conic: ((A' dx) dx + (C' dy) dy) + (B' dx) dy
-                        const u64 s2 = add2_of_product(mul2(mul2(A2, dx2), dx2), mul2(mul2(C2, dy2), dy2), one2);
-                        const u64 pw2 = add2_of_product(mul2(mul2(B2, dx2), dy2), s2, one2);  // s + t3 == t3 + s (commutative, one rounding)
-                        upk2(pw2, pw0, pw1);
-                        float e0, e1;
-                        exp_shared2(pw2, one2, e0, e1);
-                        float o0, o1;
-                        upk2(mul2(op2, pk2(e0, e1)), o0, o1);  // :77
-                        al0 = fminf(0.99f, o0);
-                        al1 = fminf(0.99f, o1);
+                        const float adx = (q0.z * dx) * dx, bdx = q0.w * dx;
+                        pw0 = (adx + (q1.x * dy0) * dy0) + bdx * dy0;
+                        pw1 = (adx + (q1.x * dy1) * dy1) + bdx * dy1;
+                        al0 = fminf(0.99f, q1.y * exp_shared_inrange(pw0));  // :77
+                        al1 = fminf(0.99f, q1.y * exp_shared_inrange(pw1));
                     } else {
-                        const u64 pw2 = fma2(mul2(A2, dx2), dx2, fma2(mul2(C2, dy2), dy2, mul2(mul2(B2, dx2), dy2)));
-                        upk2(pw2, pw0, pw1);
-                        float o0, o1;
-                        upk2(op2, o0, o1);
-                        al0 = fminf(0.99f, o0 * __expf(pw0));
-                        al1 = fminf(0.99f, o1 * __expf(pw1));
+                        const float ad = q0.z * dx, bdx = q0.w * dx;
+                        pw0 = fmaf(ad, dx, fmaf(q1.x * dy0, dy0, bdx * dy0));
+                        pw1 = fmaf(ad, dx, fmaf(q1.x * dy1, dy1, bdx * dy1));
+                        al0 = fminf(0.99f, q1.y * __expf(pw0));
+                        al1 = fminf(0.99f, q1.y * __expf(pw1));
                     }
-                    alpha2 = pk2(al0, al1);
                     // A finished (or out-of-image) pixel carries T == 0 (a live one has T >= 1e-4): its test_T is 0, so it
                     // "finishes" again at every record it would touch, never accumulates, and needs no separate flag.
                     // in0 / in1: :68-70 and, below the Gaussian's cut, alpha < 1/255 (:78); a NaN power passes like in the shader
                     const bool in0k = !(pw0 > 0.0f || pw0 < cut) && !(al0 < 1.0f / 255.0f);  // :78-80
                     const bool in1k = !(pw1 > 0.0f || pw1 < cut) && !(al1 < 1.0f / 255.0f);
-                    float tt0, tt1;
-                    const u64 T2 = pk2(T0, T1);
-                    upk2(mul2(T2, sub2(pk2(1.0f, 1.0f), alpha2)), tt0, tt1);  // :82
+                    const float tt0 = T0 * (1.0f - al0), tt1 = T1 * (1.0f - al1);  // :82
                     const bool ok0 = in0k && !(tt0 < 0.0001f), ok1 = in1k && !(tt1 < 0.0001f);  // :83-85 (the break)
                     if (STATS) {
-                        const uint32_t u = base_off + __float_as_uint(idxf) + 1u;
+                        const uint32_t u = base_off + __float_as_uint(q2.z) + 1u;
                         used = ((in0k && !ok0 && T0 != 0.0f) || (in1k && !ok1 && T1 != 0.0f)) ? max(used, u) : used;
                         if (P.stats > 1) hits += (in0k && T0 != 0.0f ? 1u : 0u) + (in1k && T1 != 0.0f ? 1u : 0u);  // debug frames only
                     }
-#if GSB_BLEND2_PRED
-                    // predicated scalar accumulates (FMA pipe) instead of packed adds + selects (the half-rate ALU pipe is
-                    // this kernel's bottleneck: profiles/)
+                    // the products are computed unconditionally, only the accumulates and the transmittance are predicated
                     float w0a, w1a, w0b, w1b, w0c, w1c;
                     if (MODE == GSB_MODE_EXACT) {
-                        upk2(mul2(mul2(r2, alpha2), T2), w0a, w1a);  // :87
-                        upk2(mul2(mul2(g2, alpha2), T2), w0b, w1b);
-                        upk2(mul2(mul2(b2, alpha2), T2), w0c, w1c);
+                        w0a = (q1.z * al0) * T0;  // :87
+                        w1a = (q1.z * al1) * T1;
+                        w0b = (q1.w * al0) * T0;
+                        w1b = (q1.w * al1) * T1;
+                        w0c = (q2.x * al0) * T0;
+                        w1c = (q2.x * al1) * T1;
                     } else {
-                        const u64 w2 = mul2(alpha2, T2);
-                        upk2(mul2(r2, w2), w0a, w1a);
-                        upk2(mul2(g2, w2), w0b, w1b);
-                        upk2(mul2(b2, w2), w0c, w1c);
+                        const float w0 = al0 * T0, w1 = al1 * T1;
+                        w0a = q1.z * w0;
+                        w1a = q1.z * w1;
+                        w0b = q1.w * w0;
+                        w1b = q1.w * w1;
+                        w0c = q2.x * w0;
+                        w1c = q2.x * w1;
                     }
                     if (ok0) {
                         ca0 = __fadd_rn(ca0, w0a);
@@ -671,27 +559,6 @@ __global__ void __launch_bounds__(B2_THREADS, GSB_BLEND2_MIN_BLOCKS) k_blend2(co
                     }
                     if (in0k) T0 = ok0 ? tt0 : 0.0f;  // :88, or the break
                     if (in1k) T1 = ok1 ? tt1 : 0.0f;
-#else
-                    float na0, na1, nb0, nb1, nc0, nc1;
-                    if (MODE == GSB_MODE_EXACT) {
-                        upk2(add2_of_product(mul2(mul2(r2, alpha2), T2), pk2(ca0, ca1), one2), na0, na1);  // :87
-                        upk2(add2_of_product(mul2(mul2(g2, alpha2), T2), pk2(cb0, cb1), one2), nb0, nb1);
-                        upk2(add2_of_product(mul2(mul2(b2, alpha2), T2), pk2(cc0, cc1), one2), nc0, nc1);
-                    } else {
-                        const u64 w2 = mul2(alpha2, T2);
-                        upk2(fma2(r2, w2, pk2(ca0, ca1)), na0, na1);
-                        upk2(fma2(g2, w2, pk2(cb0, cb1)), nb0, nb1);
-                        upk2(fma2(b2, w2, pk2(cc0, cc1)), nc0, nc1);
-                    }
-                    ca0 = ok0 ? na0 : ca0;
-                    cb0 = ok0 ? nb0 : cb0;
-                    cc0 = ok0 ? nc0 : cc0;
-                    T0 = in0k ? (ok0 ? tt0 : 0.0f) : T0;  // :88, or the break
-                    ca1 = ok1 ? na1 : ca1;
-                    cb1 = ok1 ? nb1 : cb1;
-                    cc1 = ok1 ? nc1 : cc1;
-                    T1 = in1k ? (ok1 ? tt1 : 0.0f) : T1;
-#endif
                 }
             }
             if (STATS) {

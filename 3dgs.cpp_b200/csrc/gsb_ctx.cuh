@@ -30,7 +30,7 @@ struct MiddleGraph {
 
 struct gsb_ctx {
     int device = 0;
-    int num_sms = 148;
+    int num_sms = 132;  // H100 SXM; gsb_create reads the device's own count
     cudaStream_t stream = nullptr;
     std::string err;
 

@@ -153,7 +153,6 @@ struct BlendParams {
     int mode;               // gsb_mode
     int variant;            // 2 = k_blend2 (two pixels per thread, packed fp32; default), 1 = k_blend
     int stats;              // 1: count blend_consumed / blend_walked (~4 instructions per record); 2: blend_hits as well
-    float one;              // 1.0f, passed as data so that ptxas cannot fold it (gsb_blend.cu, add2_of_product)
     Control* ctl;
 };
 cudaError_t launch_blend(const BlendParams& p, cudaStream_t s);

@@ -138,7 +138,7 @@ __device__ __forceinline__ void compute_sh(const float4* __restrict__ sh4, float
 // k_project
 // ------------------------------------------------------------------------------------------
 #ifndef GSB_PROJECT_MIN_BLOCKS
-#define GSB_PROJECT_MIN_BLOCKS 6  // <= 42 registers: 6 CTAs (48 warps) per SM hide the SH gather latency (measured 0.264 ms vs 0.30 at 5 CTAs, 0.42 at 80 registers)
+#define GSB_PROJECT_MIN_BLOCKS 6  // <= 42 registers: 6 CTAs (48 warps) per SM hide the SH gather latency
 #endif
 // ROUTED (frame sharding, gsb_shard.cu): the single stream compaction becomes one compaction per destination band -- G
 // simultaneous decoupled look-back scans over G-wide status vectors, warp d walking column d -- and the record goes straight

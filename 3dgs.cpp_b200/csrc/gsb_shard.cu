@@ -12,7 +12,7 @@
 //             deterministic: rank d's buffer is divided into G regions of S slots, region s receives rank s's survivors in
 //             Gaussian-index order (G simultaneous decoupled look-back scans on the source), so the band's survivor list is
 //             in global index order exactly like k_project's compaction on one GPU, and the band's pixels are bit-identical
-//             to the single-GPU frame.  (A separate k_route pass over the compacted records cost 0.1-0.2 ms more.)
+//             to the single-GPU frame, without a separate routing pass over the compacted records.
 //   k_blend2  stores its band straight into the whole-frame buffer of EVERY rank (the all-gather of the framebuffer,
 //             done by the producer's stores; GSB_SHARD_GATHER=nccl replaces it by one in-place ncclAllGather).
 // Cross-GPU ordering uses mailbox words in peer memory: `routed` (+ counts: a rank's records for my band have landed) and
@@ -327,9 +327,9 @@ constexpr long long WAIT_TIMEOUT_CYCLES = 6000000000ll;  // ~3 s at 1.9 GHz: a d
 // A process that drives ONE rank enqueues 1-3 back to back.  A group that drives every rank from one host thread enqueues
 // phase k of EVERY rank before phase k + 1 of any: each wait is then enqueued after all the signals it depends on, so a
 // host-side call that blocks until another device drains (first-use module loading, cudaMalloc / cudaFree with peer
-// mappings) can never sit between a spinning wait and the signal that would release it.  (Measured on 2 x B200:
-// enqueuing rank 0's whole frame first left it spinning in k_shard_wait until the 3 s timeout while rank 1's first
-// launches were stuck behind it.)
+// mappings) can never sit between a spinning wait and the signal that would release it.  (Enqueuing rank 0's
+// whole frame first can leave it spinning in k_shard_wait until the 3 s timeout while rank 1's first launches are stuck
+// behind it.)
 struct ShardFrame {
     gsb_uniforms ubo;
     int fmt = 0;

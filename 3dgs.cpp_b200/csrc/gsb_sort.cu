@@ -22,7 +22,7 @@ namespace {
 #endif
 constexpr int SORT_IPT = 16;  // pairs per thread
 #ifndef GSB_SORT_THREADS
-#define GSB_SORT_THREADS 256  // 256 threads x 16 = 4096-pair tiles, TWO persistent CTAs per SM.  With ballot ranking one 512-thread CTA per SM was faster (shorter look-back chain: 0.240 vs 0.257 ms per pass); with atomicOr matching the two layouts tie on the 17 M-pair tile sort (0.132 ms) and 2 x 256 wins on the 2.6 M-pair depth sort (0.132 vs 0.142 ms for hist + 4 passes: finer tiles balance 148 SMs better)
+#define GSB_SORT_THREADS 256  // 256 threads x 16 = 4096-pair tiles, TWO persistent CTAs per SM: finer tiles balance the SMs better on the small depth sort
 #endif
 constexpr int SORT_THREADS = GSB_SORT_THREADS;
 constexpr int SORT_TILE = SORT_THREADS * SORT_IPT;
@@ -31,7 +31,7 @@ constexpr int RADIX = 256;
 constexpr unsigned FULL = 0xffffffffu;
 
 #ifndef GSB_HIST_CTAS
-#define GSB_HIST_CTAS 3  // k_sort_hist CTAs per SM (measured on 17 M keys: 2 -> 0.049 ms, 3 or 4 -> 0.044)
+#define GSB_HIST_CTAS 3  // k_sort_hist CTAs per SM
 #endif
 constexpr int HIST_THREADS = 512;
 constexpr int HIST_IPT = 8;

@@ -74,7 +74,7 @@ public:
     const void* render(uint32_t width, uint32_t height) { return render(width, height, GSB_FORMAT_RGBA32F); }
     // The last frame.  The buffer is page-locked (gsb_host_alloc): gsb_render's blend stores the pixels straight into it over
     // PCIe while it runs -- the analogue of the reference's host-visible swapchain image (render.comp:98) -- instead of a
-    // device frame + a pageable cudaMemcpy (measured 16 ms per 3200x1400 BGRA8 frame through a std::vector).
+    // device frame + a pageable cudaMemcpy (slow: pageable copies are staged by the driver).
     struct HostFrame {
         unsigned char* ptr = nullptr;
         size_t bytes = 0, capacity = 0;

@@ -18,7 +18,7 @@ LIB_PATH = Path(os.environ.get("GSB200_LIB", PKG_ROOT / "libgsb200.so"))  # over
 HOST_LIB_PATH = PKG_ROOT / "libgsb200_host.so"
 
 if not LIB_PATH.exists():
-    raise ImportError(f"{LIB_PATH} not built: run `python __graft_entry__.py build` (nvcc, sm_100a)")
+    raise ImportError(f"{LIB_PATH} not built: run `python __graft_entry__.py build` (nvcc, sm_90a)")
 if not HOST_LIB_PATH.exists():
     raise ImportError(f"{HOST_LIB_PATH} not built: run `python __graft_entry__.py build`")
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- frames/s of the 3DGS forward hot path (project+SH -> bin -> sort -> blend) on B200.
+"""bench.py -- frames/s of the 3DGS forward hot path (project+SH -> bin -> sort -> blend) on one or more H100s.
 
 Contract: `python bench.py --gpus N --steps K --warmup W [--impl reference]` prints ONE JSON line
 (rank 0).  A "step" is one frame of the hot path.  Workload at N=1: BASELINE.json's headline config
@@ -92,7 +92,7 @@ def bench_config(wl_name, wl):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -133,7 +133,7 @@ def measured_peak_gbs():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 def use_all_cores(o):
@@ -198,7 +198,13 @@ def main():
     ap.add_argument("--sh16", action="store_true", help="gsb_set_sh_storage(1): fp16 SH coefficients -- NOT a parity mode, never the default")
     ap.add_argument("--no-extra", action="store_true", help="skip the C4 / C5 extra workload measured at --gpus 4 / 8")
     ap.add_argument("--tile-cull", type=int, default=2, help="gsb_set_tile_cull level: 0 reference lists, 1 exact per-tile instance culling, 2 coarse bins (image bit-identical in all three)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed frame (float32 .npy, at most 64 MB; a seeded pixel sample for large frames) under DIR")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the CUDA path's frame; the reference arm has none")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -253,7 +259,7 @@ def main():
 
     import gs_b200 as g  # raises if the CUDA library is not built: no fallback
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ CUDA arm
     import torch
     import torch.distributed as dist
 
@@ -299,6 +305,25 @@ class _DevFrame:
 
     def __init__(self, ptr, shape):
         self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": "|u1", "data": (int(ptr), False), "version": 2}
+
+
+DUMP_BYTES = 64 << 20
+DUMP_SAMPLE_PIXELS = 1 << 21
+
+
+def dump_outputs(out_dir, frame):
+    """Writes the framebuffer of the last timed step (H x W x 4 BGRA8) as float32 .npy files under out_dir, so that two
+    builds can be compared output for output.  A frame whose float32 copy exceeds DUMP_BYTES is written as a fixed, seeded
+    sample of whole pixels (frame_sample.npy, k x 4) plus their row-major pixel indices (frame_sample_index.npy, float64)."""
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    px = frame.reshape(-1, frame.shape[-1])
+    if px.size * 4 <= DUMP_BYTES:
+        np.save(out / "frame.npy", frame.astype(np.float32))
+        return
+    idx = np.sort(np.random.default_rng(0).choice(px.shape[0], size=min(px.shape[0], DUMP_SAMPLE_PIXELS), replace=False))
+    np.save(out / "frame_sample.npy", px[idx].astype(np.float32))
+    np.save(out / "frame_sample_index.npy", idx.astype(np.float64))
 
 
 def measure(env, wl_name, wl, steps, warmup, headline):
@@ -403,6 +428,9 @@ def measure(env, wl_name, wl, steps, warmup, headline):
     barrier()
     ms_step = reduce_max(e0.elapsed_time(e1)) / steps
     ctx.stats()  # raises GSB_ERR_OVERFLOW if any async frame overflowed the arena (sticky flag)
+    if headline and rank == 0 and args.dump_outputs:  # the last timed frame, before the loops below overwrite it
+        last = torch.as_tensor(_DevFrame(ctx.frame_ptr(), (H, W, bpp)), device=dev) if sharded else dev_fb[0]
+        dump_outputs(args.dump_outputs, last.cpu().numpy())
 
     # ---- per-frame distribution (SURVEY 8d: median / p95): the same frames again with an event after every frame ----
     nd = min(steps, 200)
@@ -499,17 +527,11 @@ def measure(env, wl_name, wl, steps, warmup, headline):
                 "alg_bytes_per_launch": alg[k], "achieved_gbs": alg[k] / (dur[k] * 1e-3) / 1e9 if dur[k] > 0 else None,
                 "share_of_step": share[k] / stage["frame_ms"] if stage["frame_ms"] > 0 else None} for k in alg}
     dom = max(share, key=share.get)
-    traffic = None
-    try:  # DRAM bytes per launch of the dominant kernel from the committed ncu --set full capture (headline workload, N = 1)
-        tj = json.loads((ROOT / "profiles" / "ncu_traffic.json").read_text())
-        traffic = (tj["dram_bytes_per_launch"].get(dom) or tj["dram_bytes_per_launch"].get(dom + "2")) if (headline and not sharded) else None
-    except Exception:
-        pass
     roof = {"kernel": dom, "bound": "hbm", "achieved": kern[dom]["achieved_gbs"], "peak": peak, "unit": "GB/s",
-            "frac": kern[dom]["achieved_gbs"] / peak if kern[dom]["achieved_gbs"] else None, "traffic": traffic,
+            "frac": kern[dom]["achieved_gbs"] / peak if kern[dom]["achieved_gbs"] else None,
             "peak_source": peak_src,
             "note": "k_blend is FP32-issue bound, not HBM bound (SURVEY 8d): its HBM fraction is reported as required; "
-                    "blend_warp_visits_per_s x the SASS instructions per visit (profiles/) is its issue-slot utilisation"}
+                    "blend_warp_visits_per_s x the SASS instructions per visit is its issue-slot utilisation"}
     out = {
         "metric": "frames/sec", "value": 1000.0 / ms_step, "unit": "frames/s", "n_gpus": world, "steps": steps,
         "warmup": warmup, "ms_per_step": ms_step, "higher_is_better": True, "scaling": "strong",
@@ -517,7 +539,7 @@ def measure(env, wl_name, wl, steps, warmup, headline):
         "config": {**bench_config(wl_name, wl),
                    "instances_M": M, "instances_aabb": float(np.mean(aabb_acc)), "tile_cull": int(args.tile_cull), "visible": NV,
                    "sort_passes": passes, "blend_mode": args.mode, "sh_storage": "fp16 (NON-PARITY)" if args.sh16 else "fp32", "output": "BGRA8", "scene_load_s": t_load,
-                   "l2": "inputs (scene + sort keys, > 1 GB) larger than the 126 MB L2; 8 camera poses alternate; no flush",
+                   "l2": "inputs (scene + sort keys, > 1 GB) larger than the 50 MB L2; 8 camera poses alternate; no flush",
                    "parallelism": (f"scene sharded by Gaussian index x{world}, frame by tile-row bands x{world}; survivors and framebuffer "
                                    f"exchanged by stores into peer memory (NVLink), no collective in the frame" if sharded else "single GPU")},
         "e2e": {"value": e2e_fps, "unit": "frames/s", "h2d_bytes_per_step": 160, "d2h_bytes_per_step": int(H * W * bpp) + 64,

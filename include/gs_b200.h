@@ -1,5 +1,5 @@
 /*
- * gs_b200.h -- C ABI of libgsb200.so: the B200 (sm_100a) CUDA replacement for the per-frame
+ * gs_b200.h -- C ABI of libgsb200.so: the H100 (sm_90a) CUDA replacement for the per-frame
  * compute path of shg8/3DGS.cpp (project+SH -> bin -> sort -> blend).
  *
  * The reference has no plugin/FFI seam for this path; the seam is compile-time inside

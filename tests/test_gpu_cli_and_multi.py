@@ -1,7 +1,7 @@
 """(1) The C++ headless viewer (apps/viewer/main.cpp's flags without a window) end to end on a small PLY.
-(2) Frame sharding over real GPUs (skipped on a one-GPU box; tests/test_gpu_shard.py covers the protocol on one GPU): one
-process per GPU through gsb_create_sharded / gsb_render_sharded, and one process driving all GPUs through gsb_group_*; the
-frame every rank ends up with must be bit-identical to the single-GPU frame."""
+(2) Frame sharding over real GPUs: one process per GPU through gsb_create_sharded / gsb_render_sharded (skipped on a
+one-GPU box; tests/test_gpu_shard.py covers the protocol on one GPU), and one process driving all GPUs through gsb_group_*
+(two ranks on cuda:0 on a one-GPU box); the frame every rank ends up with must be bit-identical to the single-GPU frame."""
 import json
 import os
 import subprocess
@@ -117,11 +117,11 @@ def test_two_gpu_sharded_frame_equals_single_gpu(gs, tmp_path, gather):
 
 def test_in_process_group_over_all_gpus(gs, ctx):
     n = _gpus()
-    if n < 2:
-        pytest.skip("needs 2 GPUs")
+    # a group needs two ranks; on a one-GPU machine both ranks share cuda:0 (a group may list a device more than once)
+    devices = list(range(min(n, 8))) if n >= 2 else [0, 0]
     _, vtx, _ = scenes.c1()
     ctx.upload(vtx)
-    grp = gs.Group(list(range(min(n, 8))))
+    grp = gs.Group(devices)
     try:
         grp.upload(vtx)
         for cam in ("c1", "odd_size", "wide"):

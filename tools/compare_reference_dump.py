@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Second half of the reference-harness patch kit (patches/reference_offscreen.patch, SURVEY 8f row 3).
 
-On a Vulkan-capable B200, the patched reference prints one JSON line and writes a float32 RGBA dump:
+On a Vulkan-capable GPU, the patched reference prints one JSON line and writes a float32 RGBA dump:
 
     GS_BENCH_FRAMES=200 GS_BENCH_WARMUP=20 GS_BENCH_CAMERA="0,0,5,1,0,0,0,45" GS_BENCH_DUMP=ref.f32 \
         ./vulkan_splatting_viewer -w 3200 -h 1400 --no-gui -i scene.ply > ref.json

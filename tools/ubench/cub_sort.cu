@@ -2,7 +2,7 @@
 // cub::DeviceRadixSort::SortPairs (Onesweep in CUDA 12.9) vs libgsb200's gsb_sort_pairs32 on the frame's shapes:
 //   (a) M = 17.2 M pairs, 15 key bits (tile ids of 3200x1400), keys skewed like a tile histogram,
 //   (b) N_v = 2.56 M pairs, 32 key bits (depth bits).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -I../../include -o cub_sort cub_sort.cu -L../../3dgs.cpp_b200 -lgsb200 -Xlinker -rpath,'$ORIGIN/../../3dgs.cpp_b200'
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -I../../include -o cub_sort cub_sort.cu -L../../3dgs.cpp_b200 -lgsb200 -Xlinker -rpath,'$ORIGIN/../../3dgs.cpp_b200'
 #include <cstdio>
 #include <cstdlib>
 #include <vector>

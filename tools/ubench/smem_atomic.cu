@@ -1,7 +1,7 @@
-// Microbenchmark: throughput of the building blocks a radix-rank can be made of, per SM, on sm_100a:
+// Microbenchmark: throughput of the building blocks a radix-rank can be made of, per SM, on sm_90a:
 //   ATOMS.OR / ATOMS.ADD to spread shared-memory addresses (one per lane), plain LDS / STS, __match_any_sync,
 //   and the 8-ballot digit match.  Prints cycles per warp-instruction per SM with 8 and 16 resident warps.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o smem_atomic smem_atomic.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o smem_atomic smem_atomic.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 constexpr int ITERS = 2048;
@@ -53,12 +53,12 @@ __global__ void k(unsigned* out, long long* cyc, unsigned seed) {
 template <int MODE>
 void run(const char* name) {
     unsigned* out; long long* cyc;
-    cudaMalloc(&out, 148 * 2 * 512 * 4); cudaMalloc(&cyc, 148 * 2 * 8);
+    cudaMalloc(&out, 132 * 2 * 512 * 4); cudaMalloc(&cyc, 132 * 2 * 8);
     for (int threads : {256, 512}) for (int ctas : {1, 2}) {
-        k<MODE><<<148 * ctas, threads>>>(out, cyc, 1); cudaDeviceSynchronize();
-        k<MODE><<<148 * ctas, threads>>>(out, cyc, 2); cudaDeviceSynchronize();
-        long long h[296]; cudaMemcpy(h, cyc, 148 * ctas * 8, cudaMemcpyDeviceToHost);
-        double avg = 0; for (int i = 0; i < 148 * ctas; i++) avg += h[i]; avg /= 148 * ctas;
+        k<MODE><<<132 * ctas, threads>>>(out, cyc, 1); cudaDeviceSynchronize();
+        k<MODE><<<132 * ctas, threads>>>(out, cyc, 2); cudaDeviceSynchronize();
+        long long h[264]; cudaMemcpy(h, cyc, 132 * ctas * 8, cudaMemcpyDeviceToHost);
+        double avg = 0; for (int i = 0; i < 132 * ctas; i++) avg += h[i]; avg /= 132 * ctas;
         const double warp_instr_per_sm = (double)ITERS * (threads / 32) * ctas;
         printf("%-34s threads %3d x %d CTA/SM: %7.2f cycles per warp-op per SM (%.2f per lane)\n", name, threads, ctas, avg / warp_instr_per_sm, avg / warp_instr_per_sm / 32);
     }
