@@ -115,7 +115,7 @@ int wait_frame(gsb_ctx* ctx) {
 
 static __global__ void k_frame_init(Control* ctl, uint32_t* __restrict__ project_status, uint32_t project_chunks,
                                     unsigned long long* __restrict__ emit_status, uint32_t emit_chunks, uint2* __restrict__ ranges,
-                                    uint32_t num_tiles, uint32_t* __restrict__ extra_words, uint32_t num_extra_words) {
+                                    uint32_t num_tiles, uint32_t* __restrict__ route_status, uint32_t route_words) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
     uint32_t* w = reinterpret_cast<uint32_t*>(ctl);
     for (uint32_t k = i; k < sizeof(Control) / 4; k += stride) {
@@ -127,17 +127,17 @@ static __global__ void k_frame_init(Control* ctl, uint32_t* __restrict__ project
     for (uint32_t k = i; k < project_chunks; k += stride) project_status[k] = 0u;
     for (uint32_t k = i; k < emit_chunks; k += stride) emit_status[k] = 0ull;
     for (uint32_t k = i; k < num_tiles; k += stride) ranges[k] = make_uint2(0xffffffffu, 0xffffffffu);  // tile_boundary's fillBuffer (Renderer.cpp:633)
-    for (uint32_t k = i; k < num_extra_words; k += stride) extra_words[k] = 0u;  // frame sharding: k_route's look-back words
+    for (uint32_t k = i; k < route_words; k += stride) route_status[k] = 0u;  // frame sharding: the routed k_project's look-back words
 }
 
 cudaError_t launch_frame_init(Control* ctl, uint32_t* project_status, uint32_t project_chunks, unsigned long long* emit_status,
-                              uint32_t emit_chunks, uint2* ranges, uint32_t num_tiles, cudaStream_t s, uint32_t* extra_words,
-                              uint32_t num_extra_words) {
-    const uint32_t work = std::max<uint32_t>(std::max(std::max(std::max(project_chunks, emit_chunks), num_tiles), num_extra_words),
+                              uint32_t emit_chunks, uint2* ranges, uint32_t num_tiles, cudaStream_t s, uint32_t* route_status,
+                              uint32_t route_words) {
+    const uint32_t work = std::max<uint32_t>(std::max(std::max(std::max(project_chunks, emit_chunks), num_tiles), route_words),
                                              (uint32_t)(sizeof(Control) / 4));
     const uint32_t blocks = std::min<uint32_t>((work + 255) / 256, 132u * 4u);  // 4 CTAs per H100 SM; grid-stride
-    k_frame_init<<<blocks, 256, 0, s>>>(ctl, project_status, project_chunks, emit_status, emit_chunks, ranges, num_tiles, extra_words,
-                                        num_extra_words);
+    k_frame_init<<<blocks, 256, 0, s>>>(ctl, project_status, project_chunks, emit_status, emit_chunks, ranges, num_tiles, route_status,
+                                        route_words);
     return cudaGetLastError();
 }
 
@@ -304,8 +304,8 @@ int plan_frame(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, 
     fp.nv_q = std::min<uint32_t>(quantise_hint(ctx->nv_hint ? ctx->nv_hint : n), quantise_hint(n));
     fp.m_q = quantise_hint(ctx->m_hint ? ctx->m_hint : std::min<uint64_t>(ctx->capacity, 4u * 1024 * 1024));
     // gsb_set_tile_cull level 2: the instance sort bins by blocks of 2^cs x 2^cs tiles; every tile of a block walks the block's
-    // list and keeps the records whose AABB holds the tile (k_blend2).  Debug downloads expose per-tile lists: level 2 is off then.
-    fp.cs = (ctx->tile_cull == 2 && !ctx->debug && ctx->blend_variant == 2) ? ctx->coarse_shift : 0u;
+    // list and keeps the records whose AABB holds the tile (k_blend).  Debug downloads expose per-tile lists: level 2 is off then.
+    fp.cs = (ctx->tile_cull == 2 && !ctx->debug) ? ctx->coarse_shift : 0u;
     fp.bins_x = (fp.tiles_x + (1u << fp.cs) - 1) >> fp.cs;
     fp.bins = fp.bins_x * ((fp.tiles_y + (1u << fp.cs) - 1) >> fp.cs);
     if (fp.cs && fp.bins > 65536u) {  // the block id must fit the 16 key bits below the tile mask (8K x 4K frames still do)
@@ -389,7 +389,6 @@ int enqueue_blend(gsb_ctx* ctx, const FramePlan& fp, uint32_t b0, uint32_t b1, v
     bp.row_pitch_bytes = pitch;
     bp.format = fmt;
     bp.mode = ctx->mode;
-    bp.variant = ctx->blend_variant;
     bp.stats = ctx->debug ? 2 : (ctx->timers ? 1 : 0);  // 2 also counts blend_pixel_hits (a few % of the kernel)
     bp.ctl = ctx->ctl;
     CK(launch_blend(bp, stream));
@@ -493,7 +492,6 @@ int gsb_create(int device, gsb_ctx** out) {
         return GSB_ERR_NO_DEVICE;
     }
     ctx->num_sms = prop.multiProcessorCount;
-    if (const char* v = getenv("GSB_BLEND_VARIANT")) ctx->blend_variant = atoi(v) == 1 ? 1 : 2;
     if (const char* v = getenv("GSB_HOST_DIRECT")) ctx->host_direct = atoi(v) != 0;
     if (const char* v = getenv("GSB_COARSE_SHIFT")) ctx->coarse_shift = (uint32_t)std::min(2, std::max(1, atoi(v)));  // 2x2 or 4x4 tiles: the mask has 16 bits
     if ((e = sort_prepare()) != cudaSuccess) return bail("sort_prepare", e);
@@ -761,7 +759,7 @@ int gsb_render(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, 
     const size_t tight = (size_t)ubo->width * bytes_per_pixel(fmt);
 
     // Host output.  If `out` is page-locked (gsb_host_alloc / cudaHostAlloc / cudaHostRegister) the blend stores the frame
-    // straight into it over PCIe: k_blend2 writes whole 64-B tile rows, the stores are posted and the kernel is issue-bound,
+    // straight into it over PCIe: k_blend writes whole 64-B tile rows, the stores are posted and the kernel is issue-bound,
     // so the 17.9 MB of a 3200x1400 BGRA8 frame leave the GPU while the blend is still running and no copy is left at the
     // end (the reference likewise stores into a host-visible swapchain image, render.comp:98).  Pageable memory goes
     // through a device staging frame and one cudaMemcpy2D.

@@ -1,17 +1,20 @@
 // gsb_blend.cu -- per-16x16-tile front-to-back alpha blending.
 // Replaces render.comp:30-99 (dispatch src/Renderer.cpp:654-677).  The reference makes every
 // pixel thread gather idx + uv + conic + colour from global memory for every Gaussian of the
-// tile's run (render.comp:62-65,87; README.md:87 lists staging as a TODO).  Here one CTA owns one
-// tile and
+// tile's run (render.comp:62-65,87; README.md:87 lists staging as a TODO).  Here one CTA of 128
+// threads owns one tile; warp w owns the 8x8 pixel block at (8 (w & 1), 8 (w >> 1)) and each lane
+// two pixels of one column of it.  The CTA
 //   * stages the run in batches of 256 compact 48-B records into shared memory once;
-//   * while staging, each thread classifies its Gaussian against the eight 8x4-pixel blocks of
-//     the tile (one block per warp): a block whose best-case exponent is below the shader's own
-//     alpha < 1/255 cut (with an fp32 error margin) can never contribute, so that warp never
-//     touches the record (bit-identical result: those pairs hit `continue` in render.comp:78);
+//   * while staging, each thread classifies its Gaussians against the four 8x8 blocks of the tile:
+//     a block whose best-case exponent is below the shader's own alpha < 1/255 cut (with an fp32
+//     error margin) can never contribute, so that warp never touches the record (bit-identical
+//     result: those pairs hit `continue` in render.comp:78);
 //   * each warp compacts the batch with one ballot per 32 records and walks only its survivors,
 //     reading each record as a shared-memory broadcast; the walk is branch-free per lane (the
-//     shader's `continue`s and `break` are predicates on the four state updates).
-// The per-pixel `break` (render.comp:83-85) becomes a per-lane done flag + warp / block votes.
+//     shader's `continue`s and `break` are predicates on the state updates).
+// With coarse bins (gsb_set_tile_cull level 2) the tile's run is filtered out of its block's list,
+// which is fetched in segments by TMA bulk copies.  The per-pixel `break` (render.comp:83-85)
+// becomes T == 0 + warp / block votes.
 //
 // EXACT mode: -fmad=false, ops in render.comp's order, exp = the fixed IEEE sequence below
 // (bit-identical to oracle exp-mode 1).  FAST mode: explicit FMA + ex2.approx.
@@ -23,12 +26,11 @@ namespace gsb {
 
 namespace {
 
-constexpr int BLEND_THREADS = 256;
 constexpr unsigned FULL = 0xffffffffu;
 
 // Bit-defined exp for x in [-87, 0] without the clamp; mirrors gso_exp_shared() in oracle/gs_oracle.c op for op: Cody-Waite
-// reduction, degree-5 Horner with the constant term 1, 2^n applied through the exponent bits (12 instructions).  Callers
-// that only use results with power in [cut, 0] (cut >= -87) call it directly: the clamp is the identity there.
+// reduction, degree-5 Horner with the constant term 1, 2^n applied through the exponent bits (12 instructions).  The blend
+// only uses results with power in [cut, 0] (cut >= -87), where the oracle's clamp is the identity.
 __device__ __forceinline__ float exp_shared_inrange(float x) {
     const float t = __fmul_rn(x, 1.44269504088896341f);
     const float tm = __fadd_rn(t, 12582912.0f);  // low mantissa bits = rint(t) in two's complement
@@ -42,17 +44,10 @@ __device__ __forceinline__ float exp_shared_inrange(float x) {
     p = __fmaf_rn(p, r, 1.0f);
     return __uint_as_float(__float_as_uint(p) + (__float_as_uint(tm) << 23));
 }
-__device__ __forceinline__ float exp_shared(float x) { return exp_shared_inrange(fmaxf(x, -87.0f)); }
-
 // shared-memory loads by 32-bit shared-window address (one LDS each, immediate offsets, no generic-pointer arithmetic)
 __device__ __forceinline__ float4 lds_f4(uint32_t addr) {
     float4 v;
     asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-    return v;
-}
-__device__ __forceinline__ float2 lds_f2(uint32_t addr) {
-    float2 v;
-    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
     return v;
 }
 __device__ __forceinline__ uint32_t lds_u16(uint32_t addr) {
@@ -66,245 +61,42 @@ __device__ __forceinline__ uint32_t unorm8(float v) {
     return __float2uint_rn(v * 255.0f);
 }
 
-// Bit w set <=> warp w's 8x4 pixel block may receive a contribution from this Gaussian (gsb_cull.cuh).
-__device__ __forceinline__ uint32_t block_mask(float ux, float uy, float A, float B, float C, float cut, float tile_x0, float tile_y0) {
-    if (!(A > 0.0f) || !(C > 0.0f)) return 0xffu;  // not positive definite / NaN: never cull
-    const float inv_a = __frcp_rn(A), inv_c = __frcp_rn(C);
-    uint32_t mask = 0;
-#pragma unroll
-    for (int w = 0; w < 8; w++) {
-        const float x0 = tile_x0 + (float)((w & 1) * 8), y0 = tile_y0 + (float)((w >> 1) * 4);
-        if (rect_may_contribute(ux, uy, A, B, C, inv_a, inv_c, x0, y0, 8.0f, 4.0f, cut)) mask |= 1u << w;
-    }
-    return mask;
-}
-
-// one staged record (48 B): three 16-B slots so the inner loop addresses it with one byte offset
-struct __align__(16) StagedRec {
-    float4 r0;  // uv.x uv.y -conic.x/2 -conic.y      (exact sign / power-of-two scalings: render.comp:66 becomes
-    float4 r1;  // -conic.z/2 power_cut opacity r       ((-A/2 dx) dx + (-C/2 dy) dy) + ((-B) dx) dy, bit for bit)
-    float4 r2;  // g b - -
-};
-
+// ------------------------------------------------------------------------------------------------------------------
+// k_blend -- two pixels per thread.
+//
+// Lane (lx = lane & 7, ly = lane >> 3) of warp w owns the two pixels (lx, ly) and (lx, ly + 4) of the warp's 8x8 block.
+// The two pixels share a column, so one staged record (three LDS.128) serves both, and the terms of render.comp:64-66
+// that depend on dx only are computed once per record instead of once per pixel; everything else is two independent
+// scalar chains (ILP for the issue-bound walk).  Every step is a single correctly rounded IEEE operation (-fmad=false:
+// no contraction), so EXACT mode stays bit-identical to the oracle.
+// ------------------------------------------------------------------------------------------------------------------
+#ifndef GSB_BLEND_BATCH
+#define GSB_BLEND_BATCH 256  // records staged per batch (2 per thread)
+#endif
+#ifndef GSB_BLEND_MIN_BLOCKS
+#define GSB_BLEND_MIN_BLOCKS 8
+#endif
 #ifndef GSB_BLEND_CHECK
 #define GSB_BLEND_CHECK 8  // records walked between two "is the whole warp done" votes
 #endif
-#ifndef GSB_BLEND_TDONE
-#define GSB_BLEND_TDONE 0  // 1: a finished pixel is T == 0 (no separate flag in the walk); needs GSB_BLEND_PREDICATED
-#endif
-#ifndef GSB_BLEND_PREDICATED
-#define GSB_BLEND_PREDICATED 1
-#endif
-#ifndef GSB_BLEND_MIN_BLOCKS
-#define GSB_BLEND_MIN_BLOCKS 5  // <= 51 registers, 5 CTAs per SM
-#endif
-template <int MODE>
-__global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(const __grid_constant__ BlendParams P) {
-    __shared__ StagedRec s_rec[BLEND_THREADS];
-    __shared__ uint32_t s_mask[BLEND_THREADS];
-    __shared__ uint16_t s_list[BLEND_THREADS / 32][BLEND_THREADS];  // per warp: byte offsets of the records it must visit
-    __shared__ uint32_t s_used;
+constexpr int BLEND_THREADS = 128;
+constexpr int BLEND_SEG = 4 * BLEND_THREADS;  // list entries scanned per batch at most
+constexpr int BLEND_BATCH = GSB_BLEND_BATCH;
+constexpr int BLEND_WARPS = BLEND_THREADS / 32;
 
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t tx = blockIdx.x % P.tiles_x;
-    const uint32_t ty = P.tile_row_begin + blockIdx.x / P.tiles_x;
-    uint2 range = P.ranges[ty * P.tiles_x + tx];  // render.comp:43-44; stored as (start, ~end), empty = all ones
-    range.y = ~range.y;
-    // warp w owns the 8x4 pixel block at (8 * (w & 1), 4 * (w >> 1)) of the tile
-    const uint32_t px = tx * GSB_TILE + (warp & 1) * 8 + (lane & 7);
-    const uint32_t py = ty * GSB_TILE + (warp >> 1) * 4 + (lane >> 3);
-    const bool inside = px < P.width && py < P.height;  // :37-39
-    const float fx = (float)px, fy = (float)py;
-    const float tile_x0 = (float)(tx * GSB_TILE), tile_y0 = (float)(ty * GSB_TILE);
-    if (tid == 0) s_used = 0;
-    __syncthreads();
-
-    float T = 1.0f, c0 = 0.0f, c1 = 0.0f, c2 = 0.0f;
-#if GSB_BLEND_TDONE
-    if (!inside) T = 0.0f;
-#define BLEND_DONE (T == 0.0f)
-#else
-    bool done = !inside;
-#define BLEND_DONE done
-#endif
-    uint32_t used = 0;
-    const uint32_t rec_sh = (uint32_t)__cvta_generic_to_shared(&s_rec[0]);  // < 64 KiB: fits the u16 list entries
-
-    for (uint32_t base = range.x; base < range.y; base += BLEND_THREADS) {
-        const uint32_t cnt = min((uint32_t)BLEND_THREADS, range.y - base);
-        if ((uint32_t)tid < cnt) {
-            const uint32_t cid = __ldg(P.vals + base + tid);
-            const float4* rec = P.recs + (size_t)cid * GSB_REC_F4;
-            const float4 a = __ldg(rec), col = __ldg(rec + 2);
-            const float2 b = __ldg(reinterpret_cast<const float2*>(rec + 1));  // conic.z, opacity
-            const float cut = power_cut(b.y);
-            s_rec[tid].r0 = make_float4(a.x, a.y, -0.5f * a.z, -a.w);
-            s_rec[tid].r1 = make_float4(-0.5f * b.x, cut, b.y, col.x);
-            s_rec[tid].r2 = make_float4(col.y, col.z, 0.f, 0.f);
-            s_mask[tid] = block_mask(a.x, a.y, a.z, a.w, b.x, cut, tile_x0, tile_y0);
-        }
-        __syncthreads();
-        if (!__all_sync(FULL, BLEND_DONE)) {
-#if GSB_BLEND_TDONE
-            const bool was_done = BLEND_DONE;
-#endif
-            // compact this warp's survivors of the batch into a list of shared-memory addresses (one ballot per 32 records)
-            uint32_t n = 0;
-            for (uint32_t c = 0; c < cnt; c += 32) {
-                const bool mine = (c + lane < cnt) && ((s_mask[c + lane] >> warp) & 1u);
-                const unsigned bits = __ballot_sync(FULL, mine);
-                if (mine) s_list[warp][n + __popc(bits & ((1u << lane) - 1u))] = (uint16_t)(rec_sh + (c + lane) * sizeof(StagedRec));
-                n += __popc(bits);
-            }
-            __syncwarp();
-            // The walk is branch-free per lane: the shader's `continue`s (render.comp:68-70, :78-80) and `break` (:83-85)
-            // become the predicate `ok`; only the every-16 "whole warp done" test is a (warp-uniform) branch.
-            const uint32_t list_sh = (uint32_t)__cvta_generic_to_shared(&s_list[warp][0]);
-            uint32_t fin_k = 0xffffffffu;
-            for (uint32_t k0 = 0; k0 < n; k0 += GSB_BLEND_CHECK) {
-                if (__all_sync(FULL, BLEND_DONE)) break;
-                const uint32_t k1 = min(n, k0 + (uint32_t)GSB_BLEND_CHECK);
-                for (uint32_t k = k0; k < k1; k++) {
-                    const uint32_t addr = lds_u16(list_sh + 2u * k);
-                    const float4 a = lds_f4(addr);
-                    const float4 b = lds_f4(addr + 16u);
-                    const float2 gb = lds_f2(addr + 32u);
-                    const float dx = a.x - fx, dy = a.y - fy;  // :64
-                    float power, alpha;
-                    if (MODE == GSB_MODE_EXACT) {
-                        power = ((a.z * dx) * dx + (b.x * dy) * dy) + (a.w * dx) * dy;  // :66 (pre-scaled conic)
-#if GSB_BLEND_TDONE
-                        alpha = fminf(0.99f, b.z * exp_shared_inrange(power));             // :77
-#else
-                        alpha = fminf(0.99f, b.z * exp_shared(power));                     // :77
-#endif
-                    } else {
-                        power = fmaf(a.z * dx, dx, fmaf(b.x * dy, dy, (a.w * dx) * dy));
-                        alpha = fminf(0.99f, b.z * __expf(power));
-                    }
-#if GSB_BLEND_TDONE
-                    // A finished pixel carries T == 0 (a live one has T >= 1e-4): its test_T is 0, so it "finishes" again at
-                    // every record it would touch and never accumulates; fin_k keeps the FIRST such record.  A NaN power
-                    // fails both comparisons and is skipped, as in the oracle (its exp clamps NaN to exp(-87)).
-                    bool ok = (power <= 0.0f && power >= b.y) && !(alpha < 1.0f / 255.0f);  // :68-70, :78-80
-                    const float test_T = T * (1.0f - alpha);                               // :82
-                    const bool fin = ok && test_T < 0.0001f;                               // :83-85
-                    fin_k = fin ? min(fin_k, k) : fin_k;
-                    ok = ok && !fin;
-#else
-                    // :68-70 and, below the Gaussian's cut, alpha < 1/255 (:78); a NaN power passes like in the shader
-                    bool ok = !done && !(power > 0.0f || power < b.y) && !(alpha < 1.0f / 255.0f);  // :78-80
-                    const float test_T = T * (1.0f - alpha);  // :82
-                    if (ok && test_T < 0.0001f) {             // :83-85
-                        done = true;
-                        fin_k = k;
-                        ok = false;
-                    }
-#endif
-#if GSB_BLEND_PREDICATED
-                    // select form: the products are computed unconditionally, only the four state updates are predicated
-                    if (MODE == GSB_MODE_EXACT) {
-                        const float n0 = c0 + (b.w * alpha) * T, n1 = c1 + (gb.x * alpha) * T, n2 = c2 + (gb.y * alpha) * T;  // :87
-                        c0 = ok ? n0 : c0;
-                        c1 = ok ? n1 : c1;
-                        c2 = ok ? n2 : c2;
-                    } else {
-                        const float w = alpha * T;
-                        c0 = ok ? fmaf(b.w, w, c0) : c0;
-                        c1 = ok ? fmaf(gb.x, w, c1) : c1;
-                        c2 = ok ? fmaf(gb.y, w, c2) : c2;
-                    }
-#if GSB_BLEND_TDONE
-                    T = fin ? 0.0f : (ok ? test_T : T);  // :88, and the break
-#else
-                    T = ok ? test_T : T;  // :88
-#endif
-#else
-                    if (ok) {
-                        if (MODE == GSB_MODE_EXACT) {
-                            c0 = c0 + (b.w * alpha) * T;  // :87
-                            c1 = c1 + (gb.x * alpha) * T;
-                            c2 = c2 + (gb.y * alpha) * T;
-                        } else {
-                            const float w = alpha * T;
-                            c0 = fmaf(b.w, w, c0);
-                            c1 = fmaf(gb.x, w, c1);
-                            c2 = fmaf(gb.y, w, c2);
-                        }
-                        T = test_T;  // :88
-                    }
-#endif
-                }
-            }
-#if GSB_BLEND_TDONE
-            if (!was_done && fin_k != 0xffffffffu) used = base - range.x + (s_list[warp][fin_k] - rec_sh) / (uint32_t)sizeof(StagedRec) + 1;
-            else if (!BLEND_DONE) used = base - range.x + cnt;
-#else
-            if (fin_k != 0xffffffffu) used = base - range.x + (s_list[warp][fin_k] - rec_sh) / (uint32_t)sizeof(StagedRec) + 1;
-            else if (!done) used = base - range.x + cnt;
-#endif
-        }
-        if (__syncthreads_and(BLEND_DONE)) break;
-    }
-
-    if (inside) {
-        atomicMax(&s_used, used);
-        const uint32_t row = py - P.out_first_row;
-        unsigned char* dst = static_cast<unsigned char*>(P.out) + (size_t)row * P.row_pitch_bytes;
-        if (P.format == GSB_FORMAT_RGBA32F) {
-            reinterpret_cast<float4*>(dst)[px] = make_float4(c0, c1, c2, 1.0f);  // :98 vec4(c, 1)
-        } else {
-            const uint32_t r = unorm8(c0), g = unorm8(c1), b = unorm8(c2);
-            const uint32_t v = (P.format == GSB_FORMAT_BGRA8) ? (b | (g << 8) | (r << 16) | 0xff000000u)
-                                                              : (r | (g << 8) | (b << 16) | 0xff000000u);
-            reinterpret_cast<uint32_t*>(dst)[px] = v;
-        }
-    }
-    __syncthreads();
-    if (tid == 0 && s_used) atomicAdd(&P.ctl->blend_consumed, (unsigned long long)s_used);
-}
-
-
-// ------------------------------------------------------------------------------------------------------------------
-// k_blend2 -- two pixels per thread.
-//
-// One CTA of 128 threads owns one 16x16 tile; warp w owns the 8x8 pixel block at (8 (w & 1), 8 (w >> 1)) and lane
-// (lx = lane & 7, ly = lane >> 3) owns the two pixels (lx, ly) and (lx, ly + 4) of it.  The two pixels share a column,
-// so one staged record (three LDS.128) serves both, and the terms of render.comp:64-66 that depend on dx only are
-// computed once per record instead of once per pixel; everything else is two independent scalar chains (ILP for the
-// issue-bound walk).  Every step is the same single correctly rounded IEEE operation as in k_blend (-fmad=false: no
-// contraction), so EXACT mode stays bit-identical to the oracle.  Per-warp survivor lists, per-block conservative
-// culling (8x8 blocks) and the batch pipeline are those of k_blend.
-// ------------------------------------------------------------------------------------------------------------------
-#ifndef GSB_BLEND2_BATCH
-#define GSB_BLEND2_BATCH 256  // records staged per batch (2 per thread)
-#endif
-#ifndef GSB_BLEND2_MIN_BLOCKS
-#define GSB_BLEND2_MIN_BLOCKS 8
-#endif
-#ifndef GSB_BLEND2_CHECK
-#define GSB_BLEND2_CHECK 8
-#endif
-#ifndef GSB_BLEND_TMA
-#define GSB_BLEND_TMA 1  // coarse bins: list segments staged by TMA bulk copies (0: per-thread __ldg)
-#endif
-constexpr int B2_THREADS = 128;
-constexpr int B2_SEG = 4 * B2_THREADS;  // list entries scanned per batch at most
-constexpr int B2_BATCH = GSB_BLEND2_BATCH;
-constexpr int B2_WARPS = B2_THREADS / 32;
-
-struct __align__(16) StagedRec2 {  // 48 B: three 16-B slots = three LDS.128 per visited record
-    float4 q0;  // ux uy -A/2 -B       (exact power-of-two / sign scalings of the conic, as in k_blend)
-    float4 q1;  // -C/2 opacity r g
+struct __align__(16) StagedRec {  // 48 B: three 16-B slots = three LDS.128 per visited record
+    float4 q0;  // ux uy -A/2 -B       (exact power-of-two / sign scalings of the conic: render.comp:66 becomes
+    float4 q1;  // -C/2 opacity r g     ((-A/2 dx) dx + (-C/2 dy) dy) + ((-B) dx) dy, bit for bit)
     float4 q2;  // b power_cut bits(index in batch) -
 };
 
-__device__ __forceinline__ uint32_t block_mask2(float ux, float uy, float A, float B, float C, float cut, float tile_x0, float tile_y0) {
+// Bit w set <=> warp w's 8x8 pixel block may receive a contribution from this Gaussian (gsb_cull.cuh).
+__device__ __forceinline__ uint32_t block_mask(float ux, float uy, float A, float B, float C, float cut, float tile_x0, float tile_y0) {
     if (!(A > 0.0f) || !(C > 0.0f)) return 0xfu;  // not positive definite / NaN: never cull
     const float inv_a = __frcp_rn(A), inv_c = __frcp_rn(C);
     uint32_t mask = 0;
 #pragma unroll
-    for (int w = 0; w < B2_WARPS; w++) {
+    for (int w = 0; w < BLEND_WARPS; w++) {
         const float x0 = tile_x0 + (float)((w & 1) * 8), y0 = tile_y0 + (float)((w >> 1) * 8);
         if (rect_may_contribute(ux, uy, A, B, C, inv_a, inv_c, x0, y0, 8.0f, 8.0f, cut)) mask |= 1u << w;
     }
@@ -315,27 +107,25 @@ __device__ __forceinline__ uint32_t block_mask2(float ux, float uy, float A, flo
 // of the block's tiles inside the Gaussian's tile AABB.  Staging becomes a stream compaction: the CTA scans the list 128
 // entries at a time (keys + payloads only, coalesced), keeps the entries whose mask has this tile's bit -- in list order, so
 // the tile's own (depth, index) order is preserved -- and gathers records only for those, until the batch holds up to
-// B2_BATCH of them.  The walk is unchanged.
+// BLEND_BATCH of them.  The walk is unchanged.
 template <int MODE, bool STATS, bool COARSE>
-__global__ void __launch_bounds__(B2_THREADS, GSB_BLEND2_MIN_BLOCKS) k_blend2(const __grid_constant__ BlendParams P) {
-    __shared__ StagedRec2 s_rec[B2_BATCH];
-    __shared__ uint8_t s_mask[B2_BATCH];
-    __shared__ uint32_t s_wc[B2_WARPS];
-#if GSB_BLEND_TMA
+__global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(const __grid_constant__ BlendParams P) {
+    __shared__ StagedRec s_rec[BLEND_BATCH];
+    __shared__ uint8_t s_mask[BLEND_BATCH];
+    __shared__ uint32_t s_wc[BLEND_WARPS];
     // COARSE: the next segment of the block's (key, payload) run, fetched by TMA (cp.async.bulk) while the current batch is
     // gathered and walked: BASELINE north_star's "TMA bulk staging of per-tile Gaussian runs into shared memory"
-    __shared__ alignas(16) uint32_t s_seg[COARSE ? 2 : 1][COARSE ? B2_SEG + 4 : 4];
+    __shared__ alignas(16) uint32_t s_seg[COARSE ? 2 : 1][COARSE ? BLEND_SEG + 4 : 4];
     __shared__ unsigned long long s_bar;
-#endif
-    __shared__ alignas(16) uint16_t s_list[B2_WARPS][B2_BATCH];  // per warp: shared-window addresses of the records it must visit
+    __shared__ alignas(16) uint16_t s_list[BLEND_WARPS][BLEND_BATCH];  // per warp: shared-window addresses of the records it must visit
     // COARSE: compact id and list position of the batch's entries.  They live in the same 2 KB as the per-warp lists: written
     // by the fill, read by the record gather, and only then (a barrier later) do the warps build their lists; the barrier at
     // the end of the batch separates the walk from the next fill.  (27 KB instead of 29 KB per CTA = 8 instead of 7 per SM.)
-    static_assert(sizeof(uint16_t) * B2_WARPS * B2_BATCH >= 2 * sizeof(uint32_t) * B2_BATCH, "s_cid + s_eidx alias s_list");
+    static_assert(sizeof(uint16_t) * BLEND_WARPS * BLEND_BATCH >= 2 * sizeof(uint32_t) * BLEND_BATCH, "s_cid + s_eidx alias s_list");
     uint32_t* const s_cid = reinterpret_cast<uint32_t*>(&s_list[0][0]);
-    uint32_t* const s_eidx = s_cid + B2_BATCH;
+    uint32_t* const s_eidx = s_cid + BLEND_BATCH;
     __shared__ uint32_t s_used, s_walked, s_hits;
-    static_assert(sizeof(StagedRec2) * B2_BATCH < 65536, "u16 list entries hold shared-window addresses");
+    static_assert(sizeof(StagedRec) * BLEND_BATCH < 65536, "u16 list entries hold shared-window addresses");
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t tx = blockIdx.x % P.tiles_x;
@@ -360,14 +150,13 @@ __global__ void __launch_bounds__(B2_THREADS, GSB_BLEND2_MIN_BLOCKS) k_blend2(co
 
     // transmittance (0 = finished or outside the image) and colour a/b/c of pixel 0/1
     float T0 = in0 ? 1.0f : 0.0f, T1 = in1 ? 1.0f : 0.0f, ca0 = 0.f, ca1 = 0.f, cb0 = 0.f, cb1 = 0.f, cc0 = 0.f, cc1 = 0.f;
-#define B2_DONE (T0 == 0.0f && T1 == 0.0f)
+#define BLEND_DONE (T0 == 0.0f && T1 == 0.0f)
     uint32_t used = 0, walked = 0, hits = 0, staged = 0;
     const uint32_t rec_sh = (uint32_t)__cvta_generic_to_shared(&s_rec[0]);
     const uint32_t list_sh = (uint32_t)__cvta_generic_to_shared(&s_list[warp][0]);
 
     const uint32_t tbit = 16u + (((ty & ((1u << cs) - 1u)) << cs) | (tx & ((1u << cs) - 1u)));  // this tile's bit in a coarse key
     uint32_t cursor = range.x;  // COARSE: next list entry to scan
-#if GSB_BLEND_TMA
     uint32_t seg_a = range.x & ~3u, seg_parity = 0u;
     bool seg_pending = COARSE && range.x < range.y;  // a bulk copy into s_seg is in flight
     if (COARSE) {
@@ -375,7 +164,7 @@ __global__ void __launch_bounds__(B2_THREADS, GSB_BLEND2_MIN_BLOCKS) k_blend2(co
             mbar_init(&s_bar, 1);
             mbar_fence_init();
             if (range.x < range.y) {
-                const uint32_t bytes = (((min(range.y, range.x + (uint32_t)B2_SEG) - seg_a) + 3u) & ~3u) * 4u;
+                const uint32_t bytes = (((min(range.y, range.x + (uint32_t)BLEND_SEG) - seg_a) + 3u) & ~3u) * 4u;
                 mbar_expect_tx(&s_bar, 2u * bytes);
                 tma_load(s_seg[0], P.keys + seg_a, bytes, &s_bar);
                 tma_load(s_seg[1], P.vals + seg_a, bytes, &s_bar);
@@ -383,14 +172,12 @@ __global__ void __launch_bounds__(B2_THREADS, GSB_BLEND2_MIN_BLOCKS) k_blend2(co
         }
         __syncthreads();  // the barrier object is initialised before anyone waits on it
     }
-#endif
-    for (uint32_t base = range.x; COARSE ? (cursor < range.y) : (base < range.y); base += B2_BATCH) {
+    for (uint32_t base = range.x; COARSE ? (cursor < range.y) : (base < range.y); base += BLEND_BATCH) {
         uint32_t cnt;
         if constexpr (COARSE) {
             // ---- fill: scan up to 4 x 128 entries (loads issued together), compact this tile's entries in list order ----
             constexpr int STEPS = 4;
             uint32_t kk[STEPS], vv[STEPS];
-#if GSB_BLEND_TMA
             // the segment that starts at `cursor` (16-B aligned start seg_a <= cursor).  One warp polls the mbarrier, the others
             // sleep on the hardware barrier: 128 threads spinning on try_wait cost issue slots the other CTAs' walks need
             if (warp == 0) mbar_wait(&s_bar, seg_parity);
@@ -399,7 +186,7 @@ __global__ void __launch_bounds__(B2_THREADS, GSB_BLEND2_MIN_BLOCKS) k_blend2(co
             seg_pending = false;
 #pragma unroll
             for (int j = 0; j < STEPS; j++) {
-                const uint32_t e = cursor + (uint32_t)(j * B2_THREADS + tid);
+                const uint32_t e = cursor + (uint32_t)(j * BLEND_THREADS + tid);
                 kk[j] = 0u;
                 vv[j] = 0u;
                 if (e < range.y) {
@@ -407,72 +194,58 @@ __global__ void __launch_bounds__(B2_THREADS, GSB_BLEND2_MIN_BLOCKS) k_blend2(co
                     vv[j] = s_seg[1][e - seg_a];
                 }
             }
-#else
-#pragma unroll
-            for (int j = 0; j < STEPS; j++) {
-                const uint32_t e = cursor + (uint32_t)(j * B2_THREADS + tid);
-                kk[j] = 0u;
-                vv[j] = 0u;
-                if (e < range.y) {
-                    kk[j] = __ldg(P.keys + e);
-                    vv[j] = __ldg(P.vals + e);
-                }
-            }
-#endif
             uint32_t nfill = 0, steps = 0;
 #pragma unroll
             for (int j = 0; j < STEPS; j++) {
-                if (cursor + (uint32_t)(j * B2_THREADS) >= range.y || nfill > (uint32_t)(B2_BATCH - B2_THREADS)) break;  // uniform
+                if (cursor + (uint32_t)(j * BLEND_THREADS) >= range.y || nfill > (uint32_t)(BLEND_BATCH - BLEND_THREADS)) break;  // uniform
                 const bool match = (kk[j] >> tbit) & 1u;
                 const unsigned bits = __ballot_sync(FULL, match);
                 if (lane == 0) s_wc[warp] = __popc(bits);
                 __syncthreads();
                 uint32_t off = nfill + __popc(bits & ((1u << lane) - 1u)), tot = 0;
 #pragma unroll
-                for (int w = 0; w < B2_WARPS; w++) {
+                for (int w = 0; w < BLEND_WARPS; w++) {
                     const uint32_t c = s_wc[w];
                     if (w < warp) off += c;
                     tot += c;
                 }
                 if (match) {
                     s_cid[off] = vv[j];
-                    s_eidx[off] = cursor - range.x + (uint32_t)(j * B2_THREADS + tid);
+                    s_eidx[off] = cursor - range.x + (uint32_t)(j * BLEND_THREADS + tid);
                 }
                 nfill += tot;
                 steps++;
                 __syncthreads();  // s_wc is reused by the next step; s_cid / s_eidx are read below
             }
-            cursor = min(range.y, cursor + steps * (uint32_t)B2_THREADS);
+            cursor = min(range.y, cursor + steps * (uint32_t)BLEND_THREADS);
             cnt = nfill;
-#if GSB_BLEND_TMA
             // every thread has read its entries (the barriers of the steps above): fetch the next segment now, it lands while
             // this batch's records are gathered and walked
             if (cursor < range.y) {
                 seg_a = cursor & ~3u;
                 seg_pending = true;
                 if (tid == 0) {
-                    const uint32_t bytes = (((min(range.y, cursor + (uint32_t)B2_SEG) - seg_a) + 3u) & ~3u) * 4u;
+                    const uint32_t bytes = (((min(range.y, cursor + (uint32_t)BLEND_SEG) - seg_a) + 3u) & ~3u) * 4u;
                     fence_proxy_async();
                     mbar_expect_tx(&s_bar, 2u * bytes);
                     tma_load(s_seg[0], P.keys + seg_a, bytes, &s_bar);
                     tma_load(s_seg[1], P.vals + seg_a, bytes, &s_bar);
                 }
             }
-#endif
         } else {
-            cnt = min((uint32_t)B2_BATCH, range.y - base);
+            cnt = min((uint32_t)BLEND_BATCH, range.y - base);
         }
         if (STATS) staged += cnt;
 #pragma unroll
-        for (int j = 0; j < B2_BATCH / B2_THREADS; j++) {
-            const uint32_t li = (uint32_t)(j * B2_THREADS + tid);
+        for (int j = 0; j < BLEND_BATCH / BLEND_THREADS; j++) {
+            const uint32_t li = (uint32_t)(j * BLEND_THREADS + tid);
             if (li < cnt) {
                 const uint32_t cid = COARSE ? s_cid[li] : __ldg(P.vals + base + li);
                 const float4* rec = P.recs + (size_t)cid * GSB_REC_F4;
                 const float4 a = __ldg(rec), col = __ldg(rec + 2);
                 const float2 b = __ldg(reinterpret_cast<const float2*>(rec + 1));  // conic.z, opacity
                 const float cut = power_cut(b.y);
-                const uint32_t m = block_mask2(a.x, a.y, a.z, a.w, b.x, cut, tile_x0, tile_y0);
+                const uint32_t m = block_mask(a.x, a.y, a.z, a.w, b.x, cut, tile_x0, tile_y0);
                 if (m) {
                     s_rec[li].q0 = make_float4(a.x, a.y, -0.5f * a.z, -a.w);
                     s_rec[li].q1 = make_float4(-0.5f * b.x, b.y, col.x, col.y);
@@ -483,20 +256,20 @@ __global__ void __launch_bounds__(B2_THREADS, GSB_BLEND2_MIN_BLOCKS) k_blend2(co
             }
         }
         __syncthreads();
-        if (!__all_sync(FULL, B2_DONE)) {
+        if (!__all_sync(FULL, BLEND_DONE)) {
             uint32_t n = 0;
             for (uint32_t c = 0; c < cnt; c += 32) {  // one ballot per 32 records
                 const bool mine = (c + lane < cnt) && ((s_mask[c + lane] >> warp) & 1u);
                 const unsigned bits = __ballot_sync(FULL, mine);
-                if (mine) s_list[warp][n + __popc(bits & ((1u << lane) - 1u))] = (uint16_t)(rec_sh + (c + lane) * sizeof(StagedRec2));
+                if (mine) s_list[warp][n + __popc(bits & ((1u << lane) - 1u))] = (uint16_t)(rec_sh + (c + lane) * sizeof(StagedRec));
                 n += __popc(bits);
             }
             __syncwarp();
             const uint32_t base_off = COARSE ? 0u : base - range.x;
             uint32_t k0 = 0;
-            for (; k0 < n; k0 += GSB_BLEND2_CHECK) {
-                if (__all_sync(FULL, B2_DONE)) break;
-                const uint32_t k1 = min(n, k0 + (uint32_t)GSB_BLEND2_CHECK);
+            for (; k0 < n; k0 += GSB_BLEND_CHECK) {
+                if (__all_sync(FULL, BLEND_DONE)) break;
+                const uint32_t k1 = min(n, k0 + (uint32_t)GSB_BLEND_CHECK);
                 for (uint32_t k = k0; k < k1; k++) {
                     const uint32_t addr = lds_u16(list_sh + 2u * k);
                     const float4 q0 = lds_f4(addr), q1 = lds_f4(addr + 16u), q2 = lds_f4(addr + 32u);
@@ -563,15 +336,13 @@ __global__ void __launch_bounds__(B2_THREADS, GSB_BLEND2_MIN_BLOCKS) k_blend2(co
             }
             if (STATS) {
                 walked += min(k0, n);
-                if (!B2_DONE) used = COARSE ? cursor - range.x : base_off + cnt;  // a live pixel read the whole batch
+                if (!BLEND_DONE) used = COARSE ? cursor - range.x : base_off + cnt;  // a live pixel read the whole batch
             }
         }
-        if (__syncthreads_and(B2_DONE)) break;
+        if (__syncthreads_and(BLEND_DONE)) break;
     }
-#undef B2_DONE
-#if GSB_BLEND_TMA
+#undef BLEND_DONE
     if (COARSE && seg_pending) mbar_wait(&s_bar, seg_parity);  // never leave with a bulk copy still writing this CTA's shared memory
-#endif
 
     if (STATS) {
         if (in0 || in1) atomicMax(&s_used, used);
@@ -638,23 +409,20 @@ cudaError_t launch_blend(const BlendParams& p, cudaStream_t s) {
     const uint32_t rows = p.tile_row_end - p.tile_row_begin;
     const uint32_t blocks = rows * p.tiles_x;
     if (blocks == 0) return cudaSuccess;
-    if (p.variant == 1 && p.num_peers == 0 && p.coarse_shift == 0) {  // round-1 kernel (one pixel per thread), kept for A/B: GSB_BLEND_VARIANT=1
-        if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT><<<blocks, BLEND_THREADS, 0, s>>>(p);
-        else k_blend<GSB_MODE_FAST><<<blocks, BLEND_THREADS, 0, s>>>(p);
-    } else if (p.coarse_shift) {
+    if (p.coarse_shift) {
         if (p.stats) {
-            if (p.mode == GSB_MODE_EXACT) k_blend2<GSB_MODE_EXACT, true, true><<<blocks, B2_THREADS, 0, s>>>(p);
-            else k_blend2<GSB_MODE_FAST, true, true><<<blocks, B2_THREADS, 0, s>>>(p);
+            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            else k_blend<GSB_MODE_FAST, true, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
         } else {
-            if (p.mode == GSB_MODE_EXACT) k_blend2<GSB_MODE_EXACT, false, true><<<blocks, B2_THREADS, 0, s>>>(p);
-            else k_blend2<GSB_MODE_FAST, false, true><<<blocks, B2_THREADS, 0, s>>>(p);
+            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            else k_blend<GSB_MODE_FAST, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
         }
     } else if (p.stats) {
-        if (p.mode == GSB_MODE_EXACT) k_blend2<GSB_MODE_EXACT, true, false><<<blocks, B2_THREADS, 0, s>>>(p);
-        else k_blend2<GSB_MODE_FAST, true, false><<<blocks, B2_THREADS, 0, s>>>(p);
+        if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, false><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        else k_blend<GSB_MODE_FAST, true, false><<<blocks, BLEND_THREADS, 0, s>>>(p);
     } else {
-        if (p.mode == GSB_MODE_EXACT) k_blend2<GSB_MODE_EXACT, false, false><<<blocks, B2_THREADS, 0, s>>>(p);
-        else k_blend2<GSB_MODE_FAST, false, false><<<blocks, B2_THREADS, 0, s>>>(p);
+        if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, false><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        else k_blend<GSB_MODE_FAST, false, false><<<blocks, BLEND_THREADS, 0, s>>>(p);
     }
     return cudaGetLastError();
 }

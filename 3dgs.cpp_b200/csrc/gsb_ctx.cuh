@@ -75,7 +75,6 @@ struct gsb_ctx {
     bool frame_debug = false;   // the last frame ran with gsb_set_debug on (its debug buffers and sorted keys exist)
     bool frame_timers = false;  // the last frame recorded the stage events (gsb_get_stats may read them)
     bool host_direct = true;    // gsb_render to page-locked host memory: blend straight into it (GSB_HOST_DIRECT=0: always stage)
-    int blend_variant = 2;      // GSB_BLEND_VARIANT=1 selects the round-1 one-pixel-per-thread kernel (A/B only)
     bool use_graph = true;      // replay the sorts + key emission from a captured CUDA graph when timers and debug are off
     uint64_t alloc_gen = 0;     // bumped by every (re)allocation a captured graph could point into
     uint64_t graph_clock = 0;

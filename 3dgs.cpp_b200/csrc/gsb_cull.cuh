@@ -1,5 +1,6 @@
-// gsb_cull.cuh -- conservative "can this Gaussian contribute anywhere in this pixel rectangle?" test,
-// shared by k_blend (8x4 pixel blocks, per warp) and k_emit (16x16 tiles, optional instance culling).
+// gsb_cull.cuh -- conservative "can this Gaussian contribute anywhere in this pixel rectangle?" test of
+// k_blend (8x8 pixel blocks, one per warp); its per-Gaussian cut power_cut() is also the threshold of
+// k_emit's instance culling (16x16 tiles, gsb_set_tile_cull level 1).
 //
 // render.comp:66-80 skips a (pixel, Gaussian) pair when alpha = opacity * exp(power) < 1/255; with
 // opacity <= 1 (sigmoid, GSScene.cpp:44) that is implied by power < POWER_CUT = -5.55.  The exponent

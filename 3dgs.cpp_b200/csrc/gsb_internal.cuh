@@ -46,13 +46,12 @@ struct Control {
     unsigned long long instances_total;  // unclamped M
     unsigned long long blend_consumed;
     unsigned long long candidates_total;  // AABB instances before tile culling (the reference's M)
-    unsigned long long blend_walked;      // (warp, record) visits of the blend's inner loop (k_blend2 with stats on)
+    unsigned long long blend_walked;      // (warp, record) visits of the blend's inner loop (k_blend with stats on)
     unsigned long long blend_hits;        // (pixel, Gaussian) pairs of those visits that passed the shader's tests
     unsigned long long blend_staged;      // records gathered into shared memory by the blend
     SortCtl sort_depth;        // Gaussian-level sort (32-bit depth keys)
     SortCtl sort_tile;         // instance-level sort (tile-id keys); also used by gsb_sort_pairs
-    // frame sharding (gsb_shard.cu): k_route's chunk tickets and per-destination-band survivor totals
-    uint32_t route_ticket;
+    // frame sharding (gsb_shard.cu): per-destination-band survivor totals of the routed k_project
     uint32_t route_total[GSB_MAX_SHARDS];
 };
 
@@ -96,7 +95,7 @@ struct EmitParams {
     Control* ctl;
     int num_sms;
     const float4* recs;          // survivor records: tile AABB (+ centre, conic, opacity for the optional instance culling)
-    int cull;                    // gsb_set_tile_cull level 1: exact per-tile instance culling (k_emit_cull)
+    int cull;                    // gsb_set_tile_cull level 1: exact per-tile instance culling (k_emit<true>)
     uint32_t coarse_shift;       // gsb_set_tile_cull level 2: bin by 2^shift x 2^shift tile blocks (tiles_x = bins per row); 0 = by tile
     unsigned long long* dbg_offsets;  // debug (may be null): exclusive instance offset of each depth-sorted survivor
 };
@@ -129,10 +128,11 @@ cudaError_t launch_sort(const SortParams& p, uint32_t* passes, cudaStream_t s);
 uint32_t sort_tile_items();
 
 // One kernel instead of four memsets: zeroes the control block (keeping overflow_sticky) and the look-back words of
-// k_project / k_emit, and fills the tile ranges with (0xFFFFFFFF, 0xFFFFFFFF) = empty.
+// k_project / k_emit (and, on a sharded context, the route_words look-back words of the routed k_project), and fills the
+// tile ranges with (0xFFFFFFFF, 0xFFFFFFFF) = empty.
 cudaError_t launch_frame_init(Control* ctl, uint32_t* project_status, uint32_t project_chunks, unsigned long long* emit_status,
-                              uint32_t emit_chunks, uint2* ranges, uint32_t num_tiles, cudaStream_t s, uint32_t* extra_words = nullptr,
-                              uint32_t num_extra_words = 0);
+                              uint32_t emit_chunks, uint2* ranges, uint32_t num_tiles, cudaStream_t s, uint32_t* route_status = nullptr,
+                              uint32_t route_words = 0);
 cudaError_t sort_prepare();  // one-time function attributes (dynamic shared memory opt-in) of the Onesweep kernels
 cudaError_t launch_ranges_single_tile(const uint32_t* d_m, uint2* ranges, cudaStream_t s);
 
@@ -151,7 +151,6 @@ struct BlendParams {
     size_t row_pitch_bytes;
     int format;             // gsb_format
     int mode;               // gsb_mode
-    int variant;            // 2 = k_blend2 (two pixels per thread, packed fp32; default), 1 = k_blend
     int stats;              // 1: count blend_consumed / blend_walked (~4 instructions per record); 2: blend_hits as well
     Control* ctl;
 };

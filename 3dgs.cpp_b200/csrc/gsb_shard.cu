@@ -13,7 +13,7 @@
 //             Gaussian-index order (G simultaneous decoupled look-back scans on the source), so the band's survivor list is
 //             in global index order exactly like k_project's compaction on one GPU, and the band's pixels are bit-identical
 //             to the single-GPU frame, without a separate routing pass over the compacted records.
-//   k_blend2  stores its band straight into the whole-frame buffer of EVERY rank (the all-gather of the framebuffer,
+//   k_blend   stores its band straight into the whole-frame buffer of EVERY rank (the all-gather of the framebuffer,
 //             done by the producer's stores; GSB_SHARD_GATHER=nccl replaces it by one in-place ncclAllGather).
 // Cross-GPU ordering uses mailbox words in peer memory: `routed` (+ counts: a rank's records for my band have landed) and
 // `framed` (+ overflow flag: its band of the framebuffer has landed).  A signal is a one-warp kernel after the producing kernel, a wait a one-warp kernel that

@@ -13,4 +13,4 @@ for f in csrc/*.cu; do
 done
 wait
 nvcc -gencode arch=compute_90a,code=sm_90a -shared -o libgsb200v_$name.so $objs -cudart static
-grep -h -A2 "k_blend\|k_onesweep\|k_project\|k_emit_cull\|k_sort_hist" /tmp/gsb_var_$name/*.log | grep -E "Used" | sort | uniq -c | head -20
+grep -h -A2 "k_blend\|k_onesweep\|k_project\|k_emit\|k_sort_hist" /tmp/gsb_var_$name/*.log | grep -E "Used" | sort | uniq -c | head -20
