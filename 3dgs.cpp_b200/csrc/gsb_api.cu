@@ -75,6 +75,7 @@ int ensure_arena(gsb_ctx* ctx, uint64_t capacity) {
     dev_free(ctx->vals[1]);
     ctx->capacity = 0;
     ctx->alloc_gen++;
+    ctx->frame_recorded = false;  // the last frame's sorted lists are gone: nothing left to differentiate
     // + 16 entries: the blend's TMA segments are 16-B granular and may read up to 3 entries past the end of the last run
     CK(dev_alloc(&ctx->keys[0], capacity + 16));
     CK(dev_alloc(&ctx->keys[1], capacity + 16));
@@ -304,8 +305,9 @@ int plan_frame(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, 
     fp.nv_q = std::min<uint32_t>(quantise_hint(ctx->nv_hint ? ctx->nv_hint : n), quantise_hint(n));
     fp.m_q = quantise_hint(ctx->m_hint ? ctx->m_hint : std::min<uint64_t>(ctx->capacity, 4u * 1024 * 1024));
     // gsb_set_tile_cull level 2: the instance sort bins by blocks of 2^cs x 2^cs tiles; every tile of a block walks the block's
-    // list and keeps the records whose AABB holds the tile (k_blend).  Debug downloads expose per-tile lists: level 2 is off then.
-    fp.cs = (ctx->tile_cull == 2 && !ctx->debug) ? ctx->coarse_shift : 0u;
+    // list and keeps the records whose AABB holds the tile (k_blend).  Debug downloads expose per-tile lists: level 2 is off then,
+    // and so it is under gsb_set_backward, whose recording and reverse walk are over per-tile lists.
+    fp.cs = (ctx->tile_cull == 2 && !ctx->debug && !ctx->backward) ? ctx->coarse_shift : 0u;
     fp.bins_x = (fp.tiles_x + (1u << fp.cs) - 1) >> fp.cs;
     fp.bins = fp.bins_x * ((fp.tiles_y + (1u << fp.cs) - 1) >> fp.cs);
     if (fp.cs && fp.bins > 65536u) {  // the block id must fit the 16 key bits below the tile mask (8K x 4K frames still do)
@@ -391,6 +393,8 @@ int enqueue_blend(gsb_ctx* ctx, const FramePlan& fp, uint32_t b0, uint32_t b1, v
     bp.mode = ctx->mode;
     bp.stats = ctx->debug ? 2 : (ctx->timers ? 1 : 0);  // 2 also counts blend_pixel_hits (a few % of the kernel)
     bp.ctl = ctx->ctl;
+    // gsb_set_backward: the per-pixel state of gsb_render_backward (plain contexts, per-tile lists)
+    bp.record = (ctx->backward && fp.cs == 0 && num_peer_frames == 0) ? ctx->bw_record : nullptr;
     CK(launch_blend(bp, stream));
     return GSB_OK;
 }
@@ -417,12 +421,31 @@ int enqueue_tail(gsb_ctx* ctx, const FramePlan& fp, cudaStream_t stream) {
 // Enqueue one whole frame on `stream`; out_dev is device memory.
 static int enqueue_frame(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, void* out_dev, size_t pitch, int fmt,
                   cudaStream_t stream) {
+    ctx->frame_recorded = false;
+    if (ctx->backward) {  // W x H per-pixel state of the reverse pass, grown on demand while gsb_set_backward is on
+        const size_t pixels = (size_t)ubo->width * ubo->height;
+        if (pixels > ctx->bw_record_pixels) {
+            dev_free(ctx->bw_record);
+            ctx->bw_record_pixels = 0;
+            CK(dev_alloc(&ctx->bw_record, pixels));
+            ctx->bw_record_pixels = pixels;
+        }
+    }
     FramePlan fp{};
     int rc = enqueue_front(ctx, ubo, rb, re, stream, &fp);
     if (rc != GSB_OK) return rc;
     rc = enqueue_blend(ctx, fp, rb, re, out_dev, pitch, fmt, stream);
     if (rc != GSB_OK) return rc;
-    return enqueue_tail(ctx, fp, stream);
+    rc = enqueue_tail(ctx, fp, stream);
+    if (rc != GSB_OK) return rc;
+    // what gsb_render_backward checks and reads about this frame
+    ctx->any_frame = true;
+    ctx->frame_recorded = ctx->backward && fp.cs == 0;
+    ctx->frame_band = !(rb == 0 && re == fp.tiles_y);
+    ctx->frame_scene_gen = ctx->scene_gen;
+    ctx->frame_mode = ctx->mode;
+    ctx->last_ubo = *ubo;
+    return GSB_OK;
 }
 
 int check_render_args(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t& rb, uint32_t& re, const void* out, size_t& pitch,
@@ -538,6 +561,8 @@ void gsb_destroy(gsb_ctx* ctx) {
     dev_free(ctx->dbg_aabb);
     dev_free(ctx->dbg_keys_unsorted);
     dev_free(ctx->dbg_vals_unsorted);
+    dev_free(ctx->bw_record);
+    dev_free(ctx->bw_scratch);
     for (auto& ev : ctx->ev)
         if (ev) cudaEventDestroy(ev);
     for (auto& ev : ctx->ev_sort)
@@ -571,6 +596,7 @@ int gsb_scene_upload(gsb_ctx* ctx, const float* vertices, uint64_t n, gsb_memory
     dev_free(ctx->dbg_offsets);
     ctx->n = 0;
     ctx->alloc_gen++;
+    ctx->scene_gen++;  // the last frame no longer describes this scene (gsb_render_backward)
     drop_graphs(ctx);
     CK(dev_alloc(&ctx->pos_op, n));
     CK(dev_alloc(&ctx->cov_a, n));
@@ -872,6 +898,73 @@ int gsb_get_stats(gsb_ctx* ctx, gsb_stats* out) {
         return fail(ctx, GSB_ERR_OVERFLOW, c->overflow ? "last frame overflowed the instance arena (gsb_render regrows; gsb_render_async does not)"
                                                        : "an earlier gsb_render_async frame overflowed the instance arena (its image is incomplete)");
     }
+    return GSB_OK;
+}
+
+int gsb_set_backward(gsb_ctx* ctx, int enabled) {
+    if (!ctx) return GSB_ERR_INVALID;
+    if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, "gsb_set_backward: sharded contexts have no backward pass");
+    CK(cudaSetDevice(ctx->device));
+    ctx->backward = enabled != 0;
+    if (!ctx->backward) {  // the per-pixel state exists only while the switch is on
+        CK(cudaStreamSynchronize(ctx->stream));
+        dev_free(ctx->bw_record);
+        ctx->bw_record_pixels = 0;
+        ctx->frame_recorded = false;
+    }
+    return GSB_OK;
+}
+
+int gsb_render_backward(gsb_ctx* ctx, const float* vertices, const float* grad_image, size_t pitch, float* grad_vertices, void* stream) {
+    if (!ctx) return GSB_ERR_INVALID;
+    if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: sharded contexts have no backward pass");
+    if (!ctx->pos_op || !ctx->any_frame) return fail(ctx, GSB_ERR_NO_SCENE, "gsb_render_backward: no scene uploaded or no frame rendered");
+    if (ctx->frame_scene_gen != ctx->scene_gen) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: the scene was uploaded again after the last frame");
+    if (ctx->scene_sh_half) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: fp16 SH storage has no backward pass");
+    if (!ctx->frame_recorded) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: the last frame was rendered with gsb_set_backward off");
+    if (ctx->frame_band) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: the last frame was a band of tile rows, not the whole frame");
+    if (!vertices || !grad_image || !grad_vertices) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: null argument");
+    const gsb_uniforms& U = ctx->last_ubo;
+    const size_t tight = (size_t)U.width * sizeof(float4);
+    if (pitch == 0) pitch = tight;
+    if (pitch < tight || pitch % sizeof(float4) != 0) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: bad row pitch");
+    CK(cudaSetDevice(ctx->device));
+    int rc = wait_frame(ctx);
+    if (rc != GSB_OK) return rc;
+    if (ctx->ctl_host->overflow) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: the last frame overflowed the instance arena (its lists are incomplete)");
+    const uint64_t n = ctx->n;
+    if (n > ctx->bw_scratch_n) {  // zeroed once here; k_preprocess_backward returns every entry it reads to zero
+        dev_free(ctx->bw_scratch);
+        ctx->bw_scratch_n = 0;
+        CK(dev_alloc(&ctx->bw_scratch, (size_t)n * 9));
+        CK(cudaMemsetAsync(ctx->bw_scratch, 0, (size_t)n * 9 * sizeof(double), ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        ctx->bw_scratch_n = n;
+    }
+    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    CK(cudaMemsetAsync(grad_vertices, 0, (size_t)n * 60 * sizeof(float), s));
+    if (n == 0) return GSB_OK;
+    BackwardParams bp{};
+    bp.recs = ctx->recs;
+    bp.vals = ctx->vals[ctx->last_final];
+    bp.ranges = ctx->ranges;
+    bp.record = ctx->bw_record;
+    bp.ctl = ctx->ctl;
+    bp.width = U.width;
+    bp.height = U.height;
+    bp.tiles_x = ctx->last_tiles_x;
+    bp.num_tiles = ctx->last_tiles_x * ctx->last_tiles_y;
+    bp.mode = ctx->frame_mode;
+    bp.ubo = U;
+    bp.vertices = vertices;
+    bp.cov_a = ctx->cov_a;
+    bp.cov_b = ctx->cov_b;
+    bp.grad_image = grad_image;
+    bp.row_pitch_bytes = pitch;
+    bp.scratch = ctx->bw_scratch;
+    bp.grad_vertices = grad_vertices;
+    bp.num_sms = ctx->num_sms;
+    CK(launch_backward(bp, s));
     return GSB_OK;
 }
 

@@ -16,9 +16,10 @@
 // which is fetched in segments by TMA bulk copies.  The per-pixel `break` (render.comp:83-85)
 // becomes T == 0 + warp / block votes.
 //
-// EXACT mode: -fmad=false, ops in render.comp's order, exp = the fixed IEEE sequence below
+// EXACT mode: -fmad=false, ops in render.comp's order, exp = the fixed IEEE sequence of gsb_exp.cuh
 // (bit-identical to oracle exp-mode 1).  FAST mode: explicit FMA + ex2.approx.
 #include "gsb_cull.cuh"
+#include "gsb_exp.cuh"
 #include "gsb_internal.cuh"
 #include "gsb_tma.cuh"
 
@@ -28,22 +29,6 @@ namespace {
 
 constexpr unsigned FULL = 0xffffffffu;
 
-// Bit-defined exp for x in [-87, 0] without the clamp; mirrors gso_exp_shared() in oracle/gs_oracle.c op for op: Cody-Waite
-// reduction, degree-5 Horner with the constant term 1, 2^n applied through the exponent bits (12 instructions).  The blend
-// only uses results with power in [cut, 0] (cut >= -87), where the oracle's clamp is the identity.
-__device__ __forceinline__ float exp_shared_inrange(float x) {
-    const float t = __fmul_rn(x, 1.44269504088896341f);
-    const float tm = __fadd_rn(t, 12582912.0f);  // low mantissa bits = rint(t) in two's complement
-    const float n = __fsub_rn(tm, 12582912.0f);
-    float r = __fmaf_rn(n, -0.693359375f, x);
-    r = __fmaf_rn(n, 2.12194440e-4f, r);
-    float p = __fmaf_rn(8.290082216262817e-3f, r, 4.1899293661117554e-2f);
-    p = __fmaf_rn(p, r, 1.6667647659778595e-1f);
-    p = __fmaf_rn(p, r, 4.9999138712882996e-1f);
-    p = __fmaf_rn(p, r, 9.999997019767761e-1f);
-    p = __fmaf_rn(p, r, 1.0f);
-    return __uint_as_float(__float_as_uint(p) + (__float_as_uint(tm) << 23));
-}
 // shared-memory loads by 32-bit shared-window address (one LDS each, immediate offsets, no generic-pointer arithmetic)
 __device__ __forceinline__ float4 lds_f4(uint32_t addr) {
     float4 v;
@@ -103,13 +88,45 @@ __device__ __forceinline__ uint32_t block_mask(float ux, float uy, float A, floa
     return mask;
 }
 
+// Per-pixel state of gsb_set_backward frames (k_blend<..., RECORD = true>): for each of the thread's two pixels, the
+// transmittance after its last contributor and that contributor's list position + 1 (0 = none).  Empty otherwise, so the
+// plain instantiations carry no trace of it.
+template <bool ON>
+struct BlendRecord {
+    float t0 = 1.0f, t1 = 1.0f;
+    uint32_t last0 = 0, last1 = 0;
+    __device__ __forceinline__ void note(bool ok0, bool ok1, float tt0, float tt1, uint32_t pos1) {
+        if (ok0) {
+            t0 = tt0;
+            last0 = pos1;
+        }
+        if (ok1) {
+            t1 = tt1;
+            last1 = pos1;
+        }
+    }
+    __device__ __forceinline__ void store(const BlendParams& P, bool in0, bool in1, uint32_t px, uint32_t py0, uint32_t py1) const {
+        if (in0) P.record[(size_t)py0 * P.width + px] = make_uint2(__float_as_uint(t0), last0);
+        if (in1) P.record[(size_t)py1 * P.width + px] = make_uint2(__float_as_uint(t1), last1);
+    }
+};
+template <>
+struct BlendRecord<false> {
+    __device__ __forceinline__ void note(bool, bool, float, float, uint32_t) {}
+    __device__ __forceinline__ void store(const BlendParams&, bool, bool, uint32_t, uint32_t, uint32_t) const {}
+};
+
 // COARSE (gsb_set_tile_cull level 2): the list is that of a block of 2^cs x 2^cs tiles and every entry's key carries the mask
 // of the block's tiles inside the Gaussian's tile AABB.  Staging becomes a stream compaction: the CTA scans the list 128
 // entries at a time (keys + payloads only, coalesced), keeps the entries whose mask has this tile's bit -- in list order, so
 // the tile's own (depth, index) order is preserved -- and gathers records only for those, until the batch holds up to
 // BLEND_BATCH of them.  The walk is unchanged.
-template <int MODE, bool STATS, bool COARSE>
+// RECORD (gsb_set_backward, per-tile lists only): each pixel also stores its final transmittance (the product of 1 - alpha
+// over its contributors: the T the shader holds at its break or at the end of the list) and the list position + 1 of its
+// last contributor into P.record -- what gsb_backward.cu needs to walk the list back to front.  The image is unchanged.
+template <int MODE, bool STATS, bool COARSE, bool RECORD = false>
 __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(const __grid_constant__ BlendParams P) {
+    static_assert(!(RECORD && COARSE), "the backward state is recorded on per-tile lists only");
     __shared__ StagedRec s_rec[BLEND_BATCH];
     __shared__ uint8_t s_mask[BLEND_BATCH];
     __shared__ uint32_t s_wc[BLEND_WARPS];
@@ -152,6 +169,7 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
     float T0 = in0 ? 1.0f : 0.0f, T1 = in1 ? 1.0f : 0.0f, ca0 = 0.f, ca1 = 0.f, cb0 = 0.f, cb1 = 0.f, cc0 = 0.f, cc1 = 0.f;
 #define BLEND_DONE (T0 == 0.0f && T1 == 0.0f)
     uint32_t used = 0, walked = 0, hits = 0, staged = 0;
+    BlendRecord<RECORD> brec;
     const uint32_t rec_sh = (uint32_t)__cvta_generic_to_shared(&s_rec[0]);
     const uint32_t list_sh = (uint32_t)__cvta_generic_to_shared(&s_list[warp][0]);
 
@@ -330,6 +348,7 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
                         cb1 = __fadd_rn(cb1, w1b);
                         cc1 = __fadd_rn(cc1, w1c);
                     }
+                    if constexpr (RECORD) brec.note(ok0, ok1, tt0, tt1, base_off + __float_as_uint(q2.z) + 1u);
                     if (in0k) T0 = ok0 ? tt0 : 0.0f;  // :88, or the break
                     if (in1k) T1 = ok1 ? tt1 : 0.0f;
                 }
@@ -343,6 +362,7 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
     }
 #undef BLEND_DONE
     if (COARSE && seg_pending) mbar_wait(&s_bar, seg_parity);  // never leave with a bulk copy still writing this CTA's shared memory
+    if constexpr (RECORD) brec.store(P, in0, in1, px, py0, py1);
 
     if (STATS) {
         if (in0 || in1) atomicMax(&s_used, used);
@@ -416,6 +436,14 @@ cudaError_t launch_blend(const BlendParams& p, cudaStream_t s) {
         } else {
             if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
             else k_blend<GSB_MODE_FAST, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        }
+    } else if (p.record) {  // gsb_set_backward
+        if (p.stats) {
+            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            else k_blend<GSB_MODE_FAST, true, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        } else {
+            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            else k_blend<GSB_MODE_FAST, false, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
         }
     } else if (p.stats) {
         if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, false><<<blocks, BLEND_THREADS, 0, s>>>(p);

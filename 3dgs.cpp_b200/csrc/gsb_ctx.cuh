@@ -95,6 +95,20 @@ struct gsb_ctx {
     uint64_t dbg_m = 0;
     unsigned long long* dbg_offsets = nullptr;  // N: k_emit's exclusive scan value per depth-sorted survivor
 
+    // reverse mode (gsb_set_backward / gsb_render_backward)
+    bool backward = false;          // frames record the per-pixel state the backward needs
+    uint2* bw_record = nullptr;     // W x H (bits(final T), last contributor position + 1) of the last recorded frame
+    size_t bw_record_pixels = 0;
+    double* bw_scratch = nullptr;   // n x 9 per-survivor fp64 accumulators of the blend backward (kept zero between calls)
+    uint64_t bw_scratch_n = 0;
+    uint64_t scene_gen = 0;         // bumped by every gsb_scene_upload
+    bool any_frame = false;         // a frame has been rendered on this context since its creation
+    bool frame_recorded = false;    // the last frame stored the backward state (whole frame, per-tile lists)
+    bool frame_band = false;        // the last frame was a band of tile rows
+    uint64_t frame_scene_gen = 0;   // scene_gen of the last frame
+    int frame_mode = GSB_MODE_EXACT;
+    gsb_uniforms last_ubo{};        // the last frame's camera
+
     // frame sharding over several GPUs (gsb_shard.cu); null for a plain context
     gsb::ShardState* shard = nullptr;
     uint32_t middle_tag = 0;  // distinguishes captured graphs that read different record buffers (the shard exchange parity)

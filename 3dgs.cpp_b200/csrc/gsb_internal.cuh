@@ -153,7 +153,34 @@ struct BlendParams {
     int mode;               // gsb_mode
     int stats;              // 1: count blend_consumed / blend_walked (~4 instructions per record); 2: blend_hits as well
     Control* ctl;
+    // gsb_set_backward (per-tile lists only): per pixel of the W x H frame, (bits(final transmittance), list position + 1 of the
+    // last contributing entry, 0 = none).  Null: a plain frame.  Appended last so the other fields keep their offsets.
+    uint2* record;
 };
 cudaError_t launch_blend(const BlendParams& p, cudaStream_t s);
+
+// gsb_backward.cu: the reverse pass of one whole frame recorded by k_blend<..., RECORD = true>
+struct BackwardParams {
+    // forward state of the frame
+    const float4* recs;       // survivor records (compact id order)
+    const uint32_t* vals;     // sorted per-tile lists (compact ids)
+    const uint2* ranges;      // (start, ~end) per tile
+    const uint2* record;      // per pixel: (bits(final T), last contributor position + 1)
+    const Control* ctl;       // num_visible
+    uint32_t width, height, tiles_x, num_tiles;
+    int mode;                 // gsb_mode of the frame
+    gsb_uniforms ubo;         // the frame's camera
+    // scene
+    const float* vertices;    // n x 60: the records last uploaded (scale, rotation, SH, position)
+    const float4* cov_a;      // the uploaded Sigma (what k_project read)
+    const float2* cov_b;
+    // upstream gradient and outputs
+    const float* grad_image;  // H x W float4, row_pitch_bytes apart
+    size_t row_pitch_bytes;
+    double* scratch;          // n x 9 per survivor: d uv (2), d conic (3), d opacity, d colour (3); zero on entry, zero again on exit
+    float* grad_vertices;     // n x 60, zeroed by the caller
+    int num_sms;
+};
+cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s);
 
 }  // namespace gsb

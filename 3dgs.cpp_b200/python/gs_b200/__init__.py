@@ -40,6 +40,8 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_scene_upload", "gsb_scene_size", "gsb_set_mode", "gsb_set_debug", "gsb_set_timers", "gsb_set_tile_cull", "gsb_set_sh_storage",
     "gsb_reserve_instances", "gsb_render", "gsb_render_async", "gsb_get_stats", "gsb_debug_size",
     "gsb_debug_download", "gsb_sort_pairs", "gsb_sort_pairs32", "gsb_set_graph", "gsb_host_alloc", "gsb_host_free",
+    # reverse mode
+    "gsb_set_backward", "gsb_render_backward",
     # frame sharding over several GPUs
     "gsb_group_create", "gsb_group_destroy", "gsb_group_size", "gsb_group_context", "gsb_group_last_error",
     "gsb_group_scene_upload", "gsb_group_render", "gsb_group_render_async",
@@ -118,6 +120,8 @@ lib.gsb_debug_size.restype = C.c_size_t
 lib.gsb_debug_download.argtypes = [_vp, C.c_int, _vp, C.c_size_t]
 lib.gsb_sort_pairs.argtypes = [_vp, _vp, _vp, _vp, _vp, C.c_uint64, C.c_uint32, _vp]
 lib.gsb_sort_pairs32.argtypes = [_vp, _vp, _vp, _vp, _vp, C.c_uint64, C.c_uint32, _vp]
+lib.gsb_set_backward.argtypes = [_vp, C.c_int]
+lib.gsb_render_backward.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp]
 
 lib.gsb_group_create.argtypes = [C.c_int, C.POINTER(C.c_int), C.POINTER(_vp)]
 lib.gsb_group_destroy.argtypes = [_vp]
@@ -280,6 +284,7 @@ class Context:
             handle = h
         self.h = handle
         self.device = device
+        self.frames = 0  # frames rendered through this wrapper (render_torch checks it between forward and backward)
 
     def close(self):
         if self.h and self._own:
@@ -304,6 +309,7 @@ class Context:
         else:  # torch tensor on this device
             assert vertices.is_cuda and vertices.is_contiguous() and vertices.dtype.itemsize == 4
             self._ck(lib.gsb_scene_upload(self.h, vertices.data_ptr(), vertices.numel() // 60, MEM_DEVICE))
+        self.frames += 1  # a new scene invalidates the last frame as well
 
     @property
     def num_gaussians(self):
@@ -343,12 +349,14 @@ class Context:
         """Render to a HOST numpy array through gsb_render (band = tile rows [rb, re))."""
         rb, re, nrows = self.band_rows(u, rows)
         out = np.empty((nrows, u.width, 4), np.float32 if fmt == FORMAT_RGBA32F else np.uint8)
+        self.frames += 1
         self._ck(lib.gsb_render(self.h, C.byref(u), rb, re, out.ctypes.data, 0, MEM_HOST, fmt, None))
         return out
 
     def render_into(self, u: Uniforms, out_ptr: int, fmt=FORMAT_RGBA32F, rows=None, stream=None, sync=True):
         """Render into DEVICE memory at out_ptr (e.g. tensor.data_ptr())."""
         rb, re, _ = self.band_rows(u, rows)
+        self.frames += 1
         if sync:
             self._ck(lib.gsb_render(self.h, C.byref(u), rb, re, out_ptr, 0, MEM_DEVICE, fmt, stream_ptr(stream)))
         else:
@@ -358,6 +366,15 @@ class Context:
         s = Stats()
         self._ck(lib.gsb_get_stats(self.h, C.byref(s)))
         return s
+
+    def set_backward(self, on=True):
+        """gsb_set_backward: the next frames keep what gsb_render_backward needs (tile-cull level 2 falls back to 1)."""
+        self._ck(lib.gsb_set_backward(self.h, int(on)))
+
+    def render_backward(self, vertices_ptr, grad_image_ptr, grad_vertices_ptr, stream=None, row_pitch_bytes=0):
+        """gsb_render_backward on device pointers: dL/d(image) (H x W float4) -> dL/d(vertices) (n x 60, overwritten)."""
+        self._ck(lib.gsb_render_backward(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
+                                         stream_ptr(stream)))
 
     def download(self, which) -> np.ndarray:
         nbytes = lib.gsb_debug_size(self.h, which)
@@ -381,6 +398,63 @@ class Context:
     def sort_pairs32(self, keys_ptr, vals_ptr, keys_tmp_ptr, vals_tmp_ptr, m, key_bits=32, stream=None):
         self._ck(lib.gsb_sort_pairs32(self.h, keys_ptr, vals_ptr, keys_tmp_ptr, vals_tmp_ptr, m, key_bits,
                                       stream_ptr(stream)))
+
+
+# ---------------------------------------------------------------- differentiable rendering (torch imported lazily)
+_RenderFn = None
+CUDA_STREAM_LEGACY = 1  # cudaStreamLegacy: the C ABI reads a NULL stream as "the context's own stream"
+
+
+def _torch_stream_arg(torch_stream):
+    """cudaStream_t for the C ABI that IS the given torch stream.  torch's default stream is the legacy NULL stream, which
+    stream_ptr() would hand over as NULL -- the context's own stream, unordered with torch's work."""
+    return C.c_void_p(torch_stream.cuda_stream or CUDA_STREAM_LEGACY)
+
+
+def _render_fn():
+    global _RenderFn
+    if _RenderFn is None:
+        import torch
+
+        class RenderFn(torch.autograd.Function):
+            @staticmethod
+            def forward(fctx, ctx, vertices, u):
+                v = vertices.detach().contiguous()
+                ctx.set_backward(True)
+                stream = torch.cuda.current_stream(v.device)
+                stream.synchronize()  # the upload runs on the context's own stream: v must be complete
+                ctx.upload(v)
+                img = torch.empty((u.height, u.width, 4), dtype=torch.float32, device=v.device)
+                ctx.frames += 1
+                ctx._ck(lib.gsb_render(ctx.h, C.byref(u), 0, ALL_ROWS, img.data_ptr(), 0, MEM_DEVICE, FORMAT_RGBA32F,
+                                       _torch_stream_arg(stream)))
+                fctx.gs_ctx, fctx.frame, fctx.vertices = ctx, ctx.frames, v
+                return img
+
+            @staticmethod
+            def backward(fctx, grad_img):
+                ctx = fctx.gs_ctx
+                if ctx.frames != fctx.frame:
+                    raise RuntimeError("render_torch: another frame was rendered on this context between forward and backward")
+                v = fctx.vertices
+                g = grad_img.detach().to(torch.float32).contiguous()
+                grad_v = torch.empty_like(v)
+                # enqueued on torch's current stream (the engine runs backward on the forward's stream), so grad_v is
+                # complete for whatever torch enqueues after it
+                ctx._ck(lib.gsb_render_backward(ctx.h, v.data_ptr(), g.data_ptr(), 0, grad_v.data_ptr(),
+                                                _torch_stream_arg(torch.cuda.current_stream(v.device))))
+                return None, grad_v, None
+
+        _RenderFn = RenderFn
+    return _RenderFn
+
+
+def render_torch(ctx: "Context", vertices, u: Uniforms):
+    """Differentiable frame: vertices is a CUDA float32 tensor (n, 60) of GSScene::Vertex records (activated parameters, as
+    gsb_scene_upload takes them).  Uploads it from device memory, renders the whole frame as an (H, W, 4) RGBA32F tensor and,
+    on backward, returns dL/dvertices through gsb_render_backward.  Turns gsb_set_backward on for `ctx`.  The frame on the
+    context must still be this one when backward runs."""
+    return _render_fn().apply(ctx, vertices, u)
 
 
 # ---------------------------------------------------------------- one frame over several GPUs

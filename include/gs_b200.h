@@ -206,6 +206,25 @@ int gsb_render_async(gsb_ctx *ctx, const gsb_uniforms *ubo, uint32_t tile_row_be
 /* Waits for the last frame and fills stats (the retrieveTimestamps analogue, Renderer.cpp:85-100). */
 int gsb_get_stats(gsb_ctx *ctx, gsb_stats *out);
 
+/* ---- reverse mode: gradient of one rendered frame with respect to the scene (no reference counterpart) ----
+ * Keep what the next frames need for gsb_render_backward (default 0).  The image is unchanged.  Set before gsb_render.
+ * While on, tile-cull level 2 falls back to 1, as under gsb_set_debug; every frame also stores 8 B per pixel (its final
+ * transmittance and the list position of its last contributing Gaussian).  Sharded contexts: GSB_ERR_INVALID. */
+int gsb_set_backward(gsb_ctx *ctx, int enabled);
+
+/* Gradient of the last frame.  All pointers are device memory, enqueued on `stream` (NULL = the context's stream).
+ *   vertices      n x 60 floats: the records last passed to gsb_scene_upload (scale and rotation are read from here)
+ *   grad_image    H x W float4 (RGBA32F layout, row_pitch_bytes apart, 0 = tight); the A channel is ignored (the output is 1)
+ *   grad_vertices n x 60 floats, OVERWRITTEN: d/d position xyz, scale xyz, opacity, rotation wxyz (as stored, no
+ *                 normalisation), sh[48]; zero for position.w, for culled Gaussians and for Gaussians outside every list used
+ * The parameters are the activated ones gsb_scene_upload receives (exp(s), sigmoid(o), the normalised quaternion); a caller
+ * chains through its own activations.  Gradients are accumulated with (fp64) atomics, so they are not guaranteed to be bitwise
+ * reproducible from run to run.  GSB_ERR_NO_SCENE before any upload or frame; GSB_ERR_INVALID if the last frame was rendered with
+ * gsb_set_backward off, was a band rather than the whole frame, or overflowed the instance arena (gsb_render_async), if
+ * the scene was uploaded again after it, if the scene stores fp16 SH, or on a sharded context. */
+int gsb_render_backward(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,
+                        float *grad_vertices, void *stream);
+
 /* Size in bytes of a debug buffer for the last frame (0 if unavailable), and its download. */
 size_t gsb_debug_size(gsb_ctx *ctx, gsb_buffer which);
 int gsb_debug_download(gsb_ctx *ctx, gsb_buffer which, void *dst, size_t bytes);
