@@ -563,6 +563,7 @@ void gsb_destroy(gsb_ctx* ctx) {
     dev_free(ctx->dbg_vals_unsorted);
     dev_free(ctx->bw_record);
     dev_free(ctx->bw_scratch);
+    dev_free(ctx->bw_cam_partials);
     for (auto& ev : ctx->ev)
         if (ev) cudaEventDestroy(ev);
     for (auto& ev : ctx->ev_sort)
@@ -915,23 +916,27 @@ int gsb_set_backward(gsb_ctx* ctx, int enabled) {
     return GSB_OK;
 }
 
-int gsb_render_backward(gsb_ctx* ctx, const float* vertices, const float* grad_image, size_t pitch, float* grad_vertices, void* stream) {
+// The checks and the launch shared by gsb_render_backward and gsb_render_backward_camera (fn names the entry in messages).
+// grad_ubo == nullptr: the scene gradient only (grad_vertices required); otherwise also dL/d(UBO), grad_vertices optional.
+static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const float* vertices, const float* grad_image, size_t pitch,
+                           float* grad_vertices, gsb_uniforms* grad_ubo, void* stream) {
     if (!ctx) return GSB_ERR_INVALID;
-    if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: sharded contexts have no backward pass");
-    if (!ctx->pos_op || !ctx->any_frame) return fail(ctx, GSB_ERR_NO_SCENE, "gsb_render_backward: no scene uploaded or no frame rendered");
-    if (ctx->frame_scene_gen != ctx->scene_gen) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: the scene was uploaded again after the last frame");
-    if (ctx->scene_sh_half) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: fp16 SH storage has no backward pass");
-    if (!ctx->frame_recorded) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: the last frame was rendered with gsb_set_backward off");
-    if (ctx->frame_band) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: the last frame was a band of tile rows, not the whole frame");
-    if (!vertices || !grad_image || !grad_vertices) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: null argument");
+    auto msg = [&](const char* what) { return std::string(fn) + ": " + what; };
+    if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, msg("sharded contexts have no backward pass").c_str());
+    if (!ctx->pos_op || !ctx->any_frame) return fail(ctx, GSB_ERR_NO_SCENE, msg("no scene uploaded or no frame rendered").c_str());
+    if (ctx->frame_scene_gen != ctx->scene_gen) return fail(ctx, GSB_ERR_INVALID, msg("the scene was uploaded again after the last frame").c_str());
+    if (ctx->scene_sh_half) return fail(ctx, GSB_ERR_INVALID, msg("fp16 SH storage has no backward pass").c_str());
+    if (!ctx->frame_recorded) return fail(ctx, GSB_ERR_INVALID, msg("the last frame was rendered with gsb_set_backward off").c_str());
+    if (ctx->frame_band) return fail(ctx, GSB_ERR_INVALID, msg("the last frame was a band of tile rows, not the whole frame").c_str());
+    if (!args_ok) return fail(ctx, GSB_ERR_INVALID, msg("null argument").c_str());
     const gsb_uniforms& U = ctx->last_ubo;
     const size_t tight = (size_t)U.width * sizeof(float4);
     if (pitch == 0) pitch = tight;
-    if (pitch < tight || pitch % sizeof(float4) != 0) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: bad row pitch");
+    if (pitch < tight || pitch % sizeof(float4) != 0) return fail(ctx, GSB_ERR_INVALID, msg("bad row pitch").c_str());
     CK(cudaSetDevice(ctx->device));
     int rc = wait_frame(ctx);
     if (rc != GSB_OK) return rc;
-    if (ctx->ctl_host->overflow) return fail(ctx, GSB_ERR_INVALID, "gsb_render_backward: the last frame overflowed the instance arena (its lists are incomplete)");
+    if (ctx->ctl_host->overflow) return fail(ctx, GSB_ERR_INVALID, msg("the last frame overflowed the instance arena (its lists are incomplete)").c_str());
     const uint64_t n = ctx->n;
     if (n > ctx->bw_scratch_n) {  // zeroed once here; k_preprocess_backward returns every entry it reads to zero
         dev_free(ctx->bw_scratch);
@@ -941,9 +946,14 @@ int gsb_render_backward(gsb_ctx* ctx, const float* vertices, const float* grad_i
         CK(cudaStreamSynchronize(ctx->stream));
         ctx->bw_scratch_n = n;
     }
+    if (grad_ubo && !ctx->bw_cam_partials)  // one row per CTA of k_preprocess_backward (4 per SM), fully overwritten by each call
+        CK(dev_alloc(&ctx->bw_cam_partials, (size_t)ctx->num_sms * 4 * GSB_UBO_WORDS));
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-    CK(cudaMemsetAsync(grad_vertices, 0, (size_t)n * 60 * sizeof(float), s));
-    if (n == 0) return GSB_OK;
+    if (grad_vertices) CK(cudaMemsetAsync(grad_vertices, 0, (size_t)n * 60 * sizeof(float), s));
+    if (n == 0) {
+        if (grad_ubo) CK(cudaMemsetAsync(grad_ubo, 0, sizeof(gsb_uniforms), s));
+        return GSB_OK;
+    }
     BackwardParams bp{};
     bp.recs = ctx->recs;
     bp.vals = ctx->vals[ctx->last_final];
@@ -964,8 +974,21 @@ int gsb_render_backward(gsb_ctx* ctx, const float* vertices, const float* grad_i
     bp.scratch = ctx->bw_scratch;
     bp.grad_vertices = grad_vertices;
     bp.num_sms = ctx->num_sms;
+    bp.cam_partials = grad_ubo ? ctx->bw_cam_partials : nullptr;
+    bp.grad_ubo = grad_ubo;
     CK(launch_backward(bp, s));
     return GSB_OK;
+}
+
+int gsb_render_backward(gsb_ctx* ctx, const float* vertices, const float* grad_image, size_t pitch, float* grad_vertices, void* stream) {
+    return render_backward(ctx, "gsb_render_backward", vertices && grad_image && grad_vertices, vertices, grad_image, pitch, grad_vertices,
+                           nullptr, stream);
+}
+
+int gsb_render_backward_camera(gsb_ctx* ctx, const float* vertices, const float* grad_image, size_t pitch, float* grad_vertices,
+                               gsb_uniforms* grad_uniforms, void* stream) {
+    return render_backward(ctx, "gsb_render_backward_camera", vertices && grad_image && grad_uniforms, vertices, grad_image, pitch,
+                           grad_vertices, grad_uniforms, stream);
 }
 
 size_t gsb_debug_size(gsb_ctx* ctx, gsb_buffer which) {

@@ -15,7 +15,10 @@
 //                         survivor's Gaussian from the scene and the frame's camera and chains colour -> SH + view direction,
 //                         conic -> cov2d -> (Sigma, J) -> position, uv -> ndc -> clip position -> position,
 //                         Sigma -> scale and (stored, unnormalised) rotation.  It writes the Gaussian's 60-float gradient
-//                         record and returns its scratch accumulators to zero for the next call.
+//                         record and returns its scratch accumulators to zero for the next call.  The CAMERA instantiation
+//                         (gsb_render_backward_camera) also keeps the camera's share of that chain rule -- view matrix,
+//                         projection matrix, camera position, tan_fov -- summed per thread, then per CTA into one fp64 row.
+//   k_camera_reduce       one CTA: sums those rows in a fixed order into the fp32 gsb_uniforms of gradients.
 //
 // The atomics make the sums depend on the order in which warps and CTAs add their partial sums: gradients are NOT guaranteed
 // to be bitwise reproducible from run to run (fp64 accumulation makes a difference in the final fp32 value rare).
@@ -165,11 +168,30 @@ __device__ constexpr float SH_C3_0 = -0.5900435899266435f, SH_C3_1 = 2.890611442
                            SH_C3_3 = 0.3731763325901154f, SH_C3_4 = -0.4570457994644658f, SH_C3_5 = 1.445305721320277f,
                            SH_C3_6 = -0.5900435899266435f;
 
+// gsb_uniforms word offsets of the fields the camera gradient has
+constexpr int U_CAMPOS = 0, U_PROJ = 4, U_VIEW = 20, U_TANX = 38, U_TANY = 39;
+// Words of dL/d(UBO) that can be non-zero: camera_position.xyz, proj_mat rows 0, 1, 3, view_mat rows 0-2, tan_fovx / tan_fovy.
+// The rest (camera_position.w, proj row 2 = depth, view row 3, width, height) feed only step functions or nothing.
+__host__ __device__ constexpr bool cam_word_live(int j) {
+    return j < 3 || (j >= U_PROJ && j < U_VIEW && (j & 3) != 2) || (j >= U_VIEW && j < 36 && (j & 3) != 3) || j >= U_TANX;
+}
+
+// CAMERA (gsb_render_backward_camera): each thread also accumulates, over its survivors, their share of dL/d(UBO) in the
+// UBO's word layout (fp32), and each CTA writes one fp64 row of partial sums (warp shuffles, then a fixed-order sum over the
+// warps) into P.cam_partials for k_camera_reduce.  The vertex gradient is written only when P.grad_vertices is set.
+// CAMERA = false is the plain reverse pass: its code is the same as before the camera gradient existed.
+template <bool CAMERA>
 __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ BackwardParams P) {
     const uint32_t nv = P.ctl->num_visible;
     const gsb_uniforms& U = P.ubo;
     const float* pm = U.proj_mat;
     const float* vm = U.view_mat;
+    const bool store_v = !CAMERA || P.grad_vertices != nullptr;  // frozen scene: camera only
+    float cam[GSB_UBO_WORDS];
+    if constexpr (CAMERA) {
+#pragma unroll
+        for (int j = 0; j < GSB_UBO_WORDS; j++) cam[j] = 0.f;
+    }
     for (uint32_t cid = blockIdx.x * blockDim.x + threadIdx.x; cid < nv; cid += gridDim.x * blockDim.x) {
         double* sc = P.scratch + (size_t)cid * BW_NACC;
         float d[BW_NACC];
@@ -296,9 +318,11 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         float vk[16];
 #pragma unroll
         for (int k = 0; k < 16; k++) {
-            gv[12 + 3 * k + 0] = basis[k] * dcr;
-            gv[12 + 3 * k + 1] = basis[k] * dcg;
-            gv[12 + 3 * k + 2] = basis[k] * dcb;
+            if (store_v) {
+                gv[12 + 3 * k + 0] = basis[k] * dcr;
+                gv[12 + 3 * k + 1] = basis[k] * dcg;
+                gv[12 + 3 * k + 2] = basis[k] * dcb;
+            }
             vk[k] = (sh[3 * k] * dcr + sh[3 * k + 1] * dcg) + sh[3 * k + 2] * dcb;
         }
         const float ddx = -SH_C1 * vk[3] + SH_C2_0 * y * vk[4] - 2.0f * SH_C2_2 * x * vk[6] + SH_C2_3 * z * vk[7] + 2.0f * SH_C2_4 * x * vk[8] +
@@ -316,6 +340,40 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         dp[0] += (ddx - x * dot) / len;
         dp[1] += (ddy - y * dot) / len;
         dp[2] += (ddz - z * dot) / len;
+
+        if constexpr (CAMERA) {  // ---- this survivor's share of dL/d(UBO), the UBO's fields taken as independent inputs ----
+            const float p3[3] = {px, py, pz}, dv[3] = {dvx, dvy, dvz}, dh[4] = {dhx, dhy, 0.f, dhw};
+#pragma unroll
+            for (int r = 0; r < 3; r++) {
+                // v = V p (rows 0-2), through J's dependence on v
+#pragma unroll
+                for (int c = 0; c < 3; c++) cam[U_VIEW + c * 4 + r] += dv[r] * p3[c];
+                cam[U_VIEW + 12 + r] += dv[r];
+                // the view rotation inside J W
+                cam[U_VIEW + r * 4 + 0] += dT0[r] * ja;
+                cam[U_VIEW + r * 4 + 1] += dT1[r] * jb;
+                cam[U_VIEW + r * 4 + 2] += dT0[r] * g0 + dT1[r] * g1;
+            }
+#pragma unroll
+            for (int k = 0; k < 4; k++) {  // h = P p (rows 0, 1, 3)
+                if (k == 2) continue;
+#pragma unroll
+                for (int c = 0; c < 3; c++) cam[U_PROJ + c * 4 + k] += dh[k] * p3[c];
+                cam[U_PROJ + 12 + k] += dh[k];
+            }
+            // the view direction p - camera_position
+            cam[U_CAMPOS + 0] -= (ddx - x * dot) / len;
+            cam[U_CAMPOS + 1] -= (ddy - y * dot) / len;
+            cam[U_CAMPOS + 2] -= (ddz - z * dot) / len;
+            // focal = size / (2 tan_fov) feeds ja / jb and g0 / g1; the clamp limit is 1.3 tan_fov
+            const float dfx = dja / vz - (tx / (vz * vz)) * dg0, dfy = djb / vz - (ty / (vz * vz)) * dg1;
+            float dtfx = -(focal_x / U.tan_fovx) * dfx, dtfy = -(focal_y / U.tan_fovy) * dfy;
+            if (txtz < -limx || txtz > limx) dtfx += (txtz > 0.0f ? 1.3f : -1.3f) * vz * dtx;
+            if (tytz < -limy || tytz > limy) dtfy += (tytz > 0.0f ? 1.3f : -1.3f) * vz * dty;
+            cam[U_TANX] += dtfx;
+            cam[U_TANY] += dtfy;
+        }
+        if (!store_v) continue;
 
         // ---- Sigma = M^T M, M = diag(s) R(q) (precomp_cov3d.comp:25-48, the quaternion as stored) ----
         const float s[3] = {v[4], v[5], v[6]};
@@ -360,6 +418,41 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         gv[10] = dqy;
         gv[11] = dqz;
     }
+    if constexpr (CAMERA) {  // one row of fp64 partial sums per CTA
+        __shared__ double s_cam[PB_THREADS / 32][GSB_UBO_WORDS];
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+        for (int j = 0; j < GSB_UBO_WORDS; j++) {
+            double a = 0.0;
+            if (cam_word_live(j)) {
+                a = (double)cam[j];
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(FULL, a, o);
+            }
+            if (lane == 0) s_cam[warp][j] = a;
+        }
+        __syncthreads();
+        if (threadIdx.x < GSB_UBO_WORDS) {
+            double a = 0.0;
+#pragma unroll
+            for (int w = 0; w < PB_THREADS / 32; w++) a += s_cam[w][threadIdx.x];
+            P.cam_partials[(size_t)blockIdx.x * GSB_UBO_WORDS + threadIdx.x] = a;
+        }
+    }
+}
+
+// Sums the `rows` partial rows of k_preprocess_backward<true> in a fixed order (warp w owns words w and w + 32; each lane a
+// strided set of rows, then a shuffle tree) and writes the whole fp32 gsb_uniforms of gradients, zero words included.
+constexpr int CR_THREADS = 1024;
+__global__ void __launch_bounds__(CR_THREADS) k_camera_reduce(const double* __restrict__ partials, uint32_t rows, gsb_uniforms* out) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int j = warp; j < GSB_UBO_WORDS; j += CR_THREADS / 32) {
+        double a = 0.0;
+        for (uint32_t r = lane; r < rows; r += 32) a += partials[(size_t)r * GSB_UBO_WORDS + j];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(FULL, a, o);
+        if (lane == 0) reinterpret_cast<float*>(out)[j] = (float)a;  // 0.0f is also the bit pattern of width = height = 0
+    }
 }
 
 }  // namespace
@@ -372,7 +465,15 @@ cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s) {
         if (e != cudaSuccess) return e;
     }
     // grid-stride over N_v, which stays on the device: the grid comes from the SM count
-    k_preprocess_backward<<<(unsigned)p.num_sms * 4u, PB_THREADS, 0, s>>>(p);
+    const unsigned grid = (unsigned)p.num_sms * 4u;
+    if (!p.grad_ubo) {
+        k_preprocess_backward<false><<<grid, PB_THREADS, 0, s>>>(p);
+        return cudaGetLastError();
+    }
+    k_preprocess_backward<true><<<grid, PB_THREADS, 0, s>>>(p);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    k_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo);
     return cudaGetLastError();
 }
 

@@ -101,6 +101,7 @@ struct gsb_ctx {
     size_t bw_record_pixels = 0;
     double* bw_scratch = nullptr;   // n x 9 per-survivor fp64 accumulators of the blend backward (kept zero between calls)
     uint64_t bw_scratch_n = 0;
+    double* bw_cam_partials = nullptr;  // [4 * num_sms][GSB_UBO_WORDS] per-CTA fp64 partial sums of gsb_render_backward_camera
     uint64_t scene_gen = 0;         // bumped by every gsb_scene_upload
     bool any_frame = false;         // a frame has been rendered on this context since its creation
     bool frame_recorded = false;    // the last frame stored the backward state (whole frame, per-tile lists)

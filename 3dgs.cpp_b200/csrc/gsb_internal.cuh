@@ -178,9 +178,13 @@ struct BackwardParams {
     const float* grad_image;  // H x W float4, row_pitch_bytes apart
     size_t row_pitch_bytes;
     double* scratch;          // n x 9 per survivor: d uv (2), d conic (3), d opacity, d colour (3); zero on entry, zero again on exit
-    float* grad_vertices;     // n x 60, zeroed by the caller
+    float* grad_vertices;     // n x 60, zeroed by the caller; may be null when grad_ubo is set (frozen scene)
     int num_sms;
+    // gsb_render_backward_camera (null otherwise).  Appended last so the other fields keep their offsets.
+    double* cam_partials;     // [num_sms * 4][GSB_UBO_WORDS] per-CTA partial sums of dL/d(UBO), fully overwritten
+    gsb_uniforms* grad_ubo;   // fp32 dL/d(UBO), fully overwritten
 };
+#define GSB_UBO_WORDS 40  // 4-byte words of gsb_uniforms; the camera gradient is reduced in this layout
 cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s);
 
 }  // namespace gsb

@@ -41,7 +41,7 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_reserve_instances", "gsb_render", "gsb_render_async", "gsb_get_stats", "gsb_debug_size",
     "gsb_debug_download", "gsb_sort_pairs", "gsb_sort_pairs32", "gsb_set_graph", "gsb_host_alloc", "gsb_host_free",
     # reverse mode
-    "gsb_set_backward", "gsb_render_backward",
+    "gsb_set_backward", "gsb_render_backward", "gsb_render_backward_camera",
     # frame sharding over several GPUs
     "gsb_group_create", "gsb_group_destroy", "gsb_group_size", "gsb_group_context", "gsb_group_last_error",
     "gsb_group_scene_upload", "gsb_group_render", "gsb_group_render_async",
@@ -64,6 +64,25 @@ class Uniforms(C.Structure):
 
 
 assert C.sizeof(Uniforms) == 160
+
+# The float fields of gsb_uniforms in ABI order: camera_position[4], proj_mat[16], view_mat[16], tan_fovx, tan_fovy -- the
+# 4-byte words of the struct without width and height (words 36 and 37).
+UBO_FLOATS = 38
+UBO_FLOAT_WORDS = list(range(36)) + [38, 39]
+
+
+def pack_uniforms(u: Uniforms) -> np.ndarray:
+    """The UBO_FLOATS float fields of u, in ABI order, as a float32 array."""
+    return np.frombuffer(bytes(u), np.float32)[UBO_FLOAT_WORDS].copy()
+
+
+def unpack_uniforms(floats, width, height) -> Uniforms:
+    """The Uniforms whose float fields are `floats` (UBO_FLOATS values in ABI order) and whose size is width x height."""
+    f = _f32(floats, UBO_FLOATS)
+    words = np.zeros(40, np.float32)
+    words[UBO_FLOAT_WORDS] = f
+    words[36:38] = np.array([width, height], np.uint32).view(np.float32)
+    return Uniforms.from_buffer_copy(words.tobytes())
 
 
 class Stats(C.Structure):
@@ -122,6 +141,7 @@ lib.gsb_sort_pairs.argtypes = [_vp, _vp, _vp, _vp, _vp, C.c_uint64, C.c_uint32, 
 lib.gsb_sort_pairs32.argtypes = [_vp, _vp, _vp, _vp, _vp, C.c_uint64, C.c_uint32, _vp]
 lib.gsb_set_backward.argtypes = [_vp, C.c_int]
 lib.gsb_render_backward.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp]
+lib.gsb_render_backward_camera.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp]
 
 lib.gsb_group_create.argtypes = [C.c_int, C.POINTER(C.c_int), C.POINTER(_vp)]
 lib.gsb_group_destroy.argtypes = [_vp]
@@ -371,10 +391,17 @@ class Context:
         """gsb_set_backward: the next frames keep what gsb_render_backward needs (tile-cull level 2 falls back to 1)."""
         self._ck(lib.gsb_set_backward(self.h, int(on)))
 
-    def render_backward(self, vertices_ptr, grad_image_ptr, grad_vertices_ptr, stream=None, row_pitch_bytes=0):
-        """gsb_render_backward on device pointers: dL/d(image) (H x W float4) -> dL/d(vertices) (n x 60, overwritten)."""
-        self._ck(lib.gsb_render_backward(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
-                                         stream_ptr(stream)))
+    def render_backward(self, vertices_ptr, grad_image_ptr, grad_vertices_ptr, stream=None, row_pitch_bytes=0,
+                        grad_uniforms_ptr=None):
+        """gsb_render_backward on device pointers: dL/d(image) (H x W float4) -> dL/d(vertices) (n x 60, overwritten).
+        With grad_uniforms_ptr (160 B of device memory), gsb_render_backward_camera: also dL/d(the frame's gsb_uniforms),
+        overwritten; grad_vertices_ptr may then be None (a frozen scene)."""
+        if grad_uniforms_ptr is None:
+            self._ck(lib.gsb_render_backward(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
+                                             stream_ptr(stream)))
+        else:
+            self._ck(lib.gsb_render_backward_camera(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
+                                                    grad_uniforms_ptr, stream_ptr(stream)))
 
     def download(self, which) -> np.ndarray:
         nbytes = lib.gsb_debug_size(self.h, which)
@@ -418,8 +445,11 @@ def _render_fn():
 
         class RenderFn(torch.autograd.Function):
             @staticmethod
-            def forward(fctx, ctx, vertices, u):
+            def forward(fctx, ctx, vertices, u, ubo):
                 v = vertices.detach().contiguous()
+                if ubo is not None:  # the camera's float fields come from the tensor, the frame size from u
+                    u = unpack_uniforms(ubo.detach().to("cpu", torch.float32).numpy(), u.width, u.height)
+                    fctx.ubo_like = (ubo.dtype, ubo.device)
                 ctx.set_backward(True)
                 stream = torch.cuda.current_stream(v.device)
                 stream.synchronize()  # the upload runs on the context's own stream: v must be complete
@@ -438,23 +468,92 @@ def _render_fn():
                     raise RuntimeError("render_torch: another frame was rendered on this context between forward and backward")
                 v = fctx.vertices
                 g = grad_img.detach().to(torch.float32).contiguous()
-                grad_v = torch.empty_like(v)
-                # enqueued on torch's current stream (the engine runs backward on the forward's stream), so grad_v is
-                # complete for whatever torch enqueues after it
-                ctx._ck(lib.gsb_render_backward(ctx.h, v.data_ptr(), g.data_ptr(), 0, grad_v.data_ptr(),
-                                                _torch_stream_arg(torch.cuda.current_stream(v.device))))
-                return None, grad_v, None
+                need_v, need_ubo = fctx.needs_input_grad[1], fctx.needs_input_grad[3]
+                grad_v = torch.empty_like(v) if need_v else None
+                grad_ubo = None
+                # enqueued on torch's current stream (the engine runs backward on the forward's stream), so the gradients
+                # are complete for whatever torch enqueues after them
+                stream = _torch_stream_arg(torch.cuda.current_stream(v.device))
+                if need_ubo:
+                    gu = torch.empty(40, dtype=torch.float32, device=v.device)  # a whole gsb_uniforms
+                    ctx._ck(lib.gsb_render_backward_camera(ctx.h, v.data_ptr(), g.data_ptr(), 0,
+                                                           grad_v.data_ptr() if need_v else None, gu.data_ptr(), stream))
+                    dtype, device = fctx.ubo_like
+                    grad_ubo = gu[UBO_FLOAT_WORDS].to(device=device, dtype=dtype)
+                else:
+                    ctx._ck(lib.gsb_render_backward(ctx.h, v.data_ptr(), g.data_ptr(), 0, grad_v.data_ptr(), stream))
+                return None, grad_v, None, grad_ubo
 
         _RenderFn = RenderFn
     return _RenderFn
 
 
-def render_torch(ctx: "Context", vertices, u: Uniforms):
+def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None):
     """Differentiable frame: vertices is a CUDA float32 tensor (n, 60) of GSScene::Vertex records (activated parameters, as
     gsb_scene_upload takes them).  Uploads it from device memory, renders the whole frame as an (H, W, 4) RGBA32F tensor and,
     on backward, returns dL/dvertices through gsb_render_backward.  Turns gsb_set_backward on for `ctx`.  The frame on the
-    context must still be this one when backward runs."""
-    return _render_fn().apply(ctx, vertices, u)
+    context must still be this one when backward runs.
+
+    ubo (optional): a (UBO_FLOATS,) tensor of the camera's float fields in ABI order (uniforms_torch makes one from a pose);
+    its values replace u's, u still gives the frame size, and backward also returns dL/dubo (gsb_render_backward_camera).
+    Only the inputs that require grad are differentiated: frozen vertices cost no n x 60 gradient."""
+    return _render_fn().apply(ctx, vertices, u, ubo)
+
+
+def _uniforms_restated(position, rotation_wxyz, fov_deg, near, far, width, height):
+    """Renderer::makeUniforms and host/gsmath.h restated in float64 torch ops (differentiable in position, rotation and fov):
+    view = inverse(translate(position) mat4_cast(q)) with q as given (not normalised), tan_fovx = tan(radians(fov) / 2),
+    tan_fovy = tan_fovx H / W, proj = perspective(2 atan(tan_fovy), W / H, near, far) view, then rows y, z of view and row y
+    of proj negated.  Returns the UBO_FLOATS float fields in ABI order."""
+    import torch
+
+    p, q, fov = position, rotation_wxyz, fov_deg
+    w, x, y, z = q[0], q[1], q[2], q[3]
+    one, zero = torch.ones_like(w), torch.zeros_like(w)
+    R = torch.stack([  # mat4_cast: rows of the rotation
+        torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y)]),
+        torch.stack([2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x)]),
+        torch.stack([2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)]),
+    ])
+    M = torch.cat([torch.cat([R, p[:, None]], 1), torch.stack([zero, zero, zero, one])[None, :]], 0)  # translate * rotation
+    view = torch.linalg.inv(M)
+    tan_fovx = torch.tan(torch.deg2rad(fov) / 2)
+    tan_fovy = tan_fovx * float(height) / float(width)
+    aspect = float(width) / float(height)
+    persp = torch.stack([
+        torch.stack([1 / (aspect * tan_fovy), zero, zero, zero]),
+        torch.stack([zero, 1 / tan_fovy, zero, zero]),
+        torch.stack([zero, zero, -(far + near) / (far - near) * one, -(2 * far * near) / (far - near) * one]),
+        torch.stack([zero, zero, -one, zero]),
+    ])
+    proj = persp @ view
+    flip = torch.tensor([1.0, -1.0, -1.0, 1.0], dtype=view.dtype)[:, None]
+    view = view * flip
+    proj = proj * torch.tensor([1.0, -1.0, 1.0, 1.0], dtype=proj.dtype)[:, None]
+    return torch.cat([p, one[None], proj.T.reshape(16), view.T.reshape(16), tan_fovx[None], tan_fovy[None]])
+
+
+def uniforms_torch(position, rotation_wxyz, fov_deg, near, far, width, height):
+    """Differentiable gsb_uniforms of a camera pose, for render_torch(..., ubo=): a (UBO_FLOATS,) float32 tensor of the float
+    fields in ABI order (camera_position[4], proj_mat[16], view_mat[16], tan_fovx, tan_fovy) on position's device.
+
+    Its value is exactly what gsh_uniforms_from_camera (Renderer::makeUniforms) produces for the float32 inputs, bit for bit,
+    so a pose renders the viewer's image of that pose.  Its gradient is that of the float64 restatement of makeUniforms
+    (position (3,), rotation_wxyz (4,) used as given -- normalise it in torch if it is a free parameter -- and fov_deg may
+    each be a tensor that requires grad; near, far, width and height are constants)."""
+    import torch
+
+    position, rotation_wxyz, fov_deg = (torch.as_tensor(t) for t in (position, rotation_wxyz, fov_deg))
+    device = position.device
+    host = uniforms_from_camera(position.detach().to("cpu", torch.float32).numpy(),
+                                rotation_wxyz.detach().to("cpu", torch.float32).numpy(),
+                                float(fov_deg.detach().to(torch.float32)), near, far, width, height)
+    value = torch.from_numpy(pack_uniforms(host)).to(torch.float64)
+    r = _uniforms_restated(*(t.to("cpu", torch.float64) for t in (position, rotation_wxyz, fov_deg)),
+                           float(near), float(far), width, height)
+    # straight-through: the host's value with the restatement's gradient.  Written as value - (r' - r) rather than
+    # value + (r - r'): r' - r is +0, and x - (+0) keeps x's sign even when x is -0 (the flipped rows hold -0 entries).
+    return (value - (r.detach() - r)).to(torch.float32).to(device)
 
 
 # ---------------------------------------------------------------- one frame over several GPUs

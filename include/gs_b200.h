@@ -206,7 +206,7 @@ int gsb_render_async(gsb_ctx *ctx, const gsb_uniforms *ubo, uint32_t tile_row_be
 /* Waits for the last frame and fills stats (the retrieveTimestamps analogue, Renderer.cpp:85-100). */
 int gsb_get_stats(gsb_ctx *ctx, gsb_stats *out);
 
-/* ---- reverse mode: gradient of one rendered frame with respect to the scene (no reference counterpart) ----
+/* ---- reverse mode: gradient of one rendered frame with respect to the scene and the camera (no reference counterpart) ----
  * Keep what the next frames need for gsb_render_backward (default 0).  The image is unchanged.  Set before gsb_render.
  * While on, tile-cull level 2 falls back to 1, as under gsb_set_debug; every frame also stores 8 B per pixel (its final
  * transmittance and the list position of its last contributing Gaussian).  Sharded contexts: GSB_ERR_INVALID. */
@@ -224,6 +224,20 @@ int gsb_set_backward(gsb_ctx *ctx, int enabled);
  * the scene was uploaded again after it, if the scene stores fp16 SH, or on a sharded context. */
 int gsb_render_backward(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,
                         float *grad_vertices, void *stream);
+
+/* gsb_render_backward plus the gradient with respect to the last frame's camera: the same arguments, preconditions and error
+ * codes, and also GSB_ERR_INVALID for a NULL grad_uniforms.
+ *   grad_vertices  may be NULL (a frozen scene: only the camera is differentiated, no n x 60 store or memset); otherwise it
+ *                  receives exactly what gsb_render_backward writes
+ *   grad_uniforms  device memory, OVERWRITTEN with dL/d(each float field of the frame's gsb_uniforms), in fp32.  Non-zero only
+ *                  in camera_position[0..2], proj_mat rows 0, 1 and 3 (elements [c*4 + r], r != 2), view_mat rows 0-2
+ *                  ([c*4 + r], r != 3), tan_fovx and tan_fovy; every other word (camera_position[3], proj_mat row 2, view_mat
+ *                  row 3, width, height) is 0.  Depth order, culls, radii and tile AABBs are step functions of the camera.
+ * The gradient treats the UBO's fields as independent inputs: proj_mat already contains view_mat, and tan_fov enters the EWA
+ * Jacobian separately from proj_mat, so a caller chains it through its own camera model (gs_b200.uniforms_torch does so
+ * for Renderer::makeUniforms).  The camera gradient is reduced without global atomics, per CTA then in one fixed-order pass. */
+int gsb_render_backward_camera(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,
+                               float *grad_vertices, gsb_uniforms *grad_uniforms, void *stream);
 
 /* Size in bytes of a debug buffer for the last frame (0 if unavailable), and its download. */
 size_t gsb_debug_size(gsb_ctx *ctx, gsb_buffer which);
