@@ -564,6 +564,7 @@ void gsb_destroy(gsb_ctx* ctx) {
     dev_free(ctx->bw_record);
     dev_free(ctx->bw_scratch);
     dev_free(ctx->bw_cam_partials);
+    dev_free(ctx->bw_abs);
     for (auto& ev : ctx->ev)
         if (ev) cudaEventDestroy(ev);
     for (auto& ev : ctx->ev_sort)
@@ -916,10 +917,11 @@ int gsb_set_backward(gsb_ctx* ctx, int enabled) {
     return GSB_OK;
 }
 
-// The checks and the launch shared by gsb_render_backward and gsb_render_backward_camera (fn names the entry in messages).
-// grad_ubo == nullptr: the scene gradient only (grad_vertices required); otherwise also dL/d(UBO), grad_vertices optional.
+// The checks and the launch shared by gsb_render_backward, gsb_render_backward_camera and gsb_render_backward_density (fn
+// names the entry in messages).  grad_ubo == nullptr: no camera gradient; grad_vertices == nullptr: no scene gradient (each
+// entry's args_ok says which may be null).  density != nullptr: also accumulate the density statistics into it.
 static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const float* vertices, const float* grad_image, size_t pitch,
-                           float* grad_vertices, gsb_uniforms* grad_ubo, void* stream) {
+                           float* grad_vertices, gsb_uniforms* grad_ubo, float* density, void* stream) {
     if (!ctx) return GSB_ERR_INVALID;
     auto msg = [&](const char* what) { return std::string(fn) + ": " + what; };
     if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, msg("sharded contexts have no backward pass").c_str());
@@ -945,6 +947,14 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
         CK(cudaMemsetAsync(ctx->bw_scratch, 0, (size_t)n * 9 * sizeof(double), ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
         ctx->bw_scratch_n = n;
+    }
+    if (density && n > ctx->bw_abs_n) {  // zeroed once here; k_density_accumulate returns every entry it reads to zero
+        dev_free(ctx->bw_abs);
+        ctx->bw_abs_n = 0;
+        CK(dev_alloc(&ctx->bw_abs, (size_t)n * 2));
+        CK(cudaMemsetAsync(ctx->bw_abs, 0, (size_t)n * 2 * sizeof(double), ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        ctx->bw_abs_n = n;
     }
     if (grad_ubo && !ctx->bw_cam_partials)  // one row per CTA of k_preprocess_backward (4 per SM), fully overwritten by each call
         CK(dev_alloc(&ctx->bw_cam_partials, (size_t)ctx->num_sms * 4 * GSB_UBO_WORDS));
@@ -976,19 +986,27 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     bp.num_sms = ctx->num_sms;
     bp.cam_partials = grad_ubo ? ctx->bw_cam_partials : nullptr;
     bp.grad_ubo = grad_ubo;
+    bp.abs_scratch = density ? ctx->bw_abs : nullptr;
+    bp.density = density;
     CK(launch_backward(bp, s));
     return GSB_OK;
 }
 
 int gsb_render_backward(gsb_ctx* ctx, const float* vertices, const float* grad_image, size_t pitch, float* grad_vertices, void* stream) {
     return render_backward(ctx, "gsb_render_backward", vertices && grad_image && grad_vertices, vertices, grad_image, pitch, grad_vertices,
-                           nullptr, stream);
+                           nullptr, nullptr, stream);
 }
 
 int gsb_render_backward_camera(gsb_ctx* ctx, const float* vertices, const float* grad_image, size_t pitch, float* grad_vertices,
                                gsb_uniforms* grad_uniforms, void* stream) {
     return render_backward(ctx, "gsb_render_backward_camera", vertices && grad_image && grad_uniforms, vertices, grad_image, pitch,
-                           grad_vertices, grad_uniforms, stream);
+                           grad_vertices, grad_uniforms, nullptr, stream);
+}
+
+int gsb_render_backward_density(gsb_ctx* ctx, const float* vertices, const float* grad_image, size_t pitch, float* grad_vertices,
+                                gsb_uniforms* grad_uniforms, float* density, void* stream) {
+    return render_backward(ctx, "gsb_render_backward_density", vertices && grad_image && density && (grad_vertices || grad_uniforms),
+                           vertices, grad_image, pitch, grad_vertices, grad_uniforms, density, stream);
 }
 
 size_t gsb_debug_size(gsb_ctx* ctx, gsb_buffer which) {

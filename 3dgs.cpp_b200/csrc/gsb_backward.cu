@@ -11,6 +11,9 @@
 //                         Per survivor it accumulates d uv (2), d conic (3), d opacity (1), d colour (3): reduced over the warp
 //                         (fp32 shuffles), then over the CTA (fp64 shared-memory atomics), then one global fp64 atomic per value
 //                         and tile.  fp64 keeps the order-dependent rounding of the sums over warps and tiles ~1e-16 relative.
+//                         The ABSGRAD instantiation (gsb_render_backward_density) also sums |d u|, |d v| of each pixel.
+//   k_density_accumulate  one thread per survivor (gsb_render_backward_density only): adds the frame's screen-space gradient
+//                         norms, one view and the max pixel radius to the caller's n x 4 statistics.
 //   k_preprocess_backward one thread per survivor (grid-stride over N_v, read on the device): recomputes preprocess.comp for the
 //                         survivor's Gaussian from the scene and the frame's camera and chains colour -> SH + view direction,
 //                         conic -> cov2d -> (Sigma, J) -> position, uv -> ndc -> clip position -> position,
@@ -35,6 +38,7 @@ constexpr unsigned FULL = 0xffffffffu;
 constexpr int BW_THREADS = 256;  // one pixel per thread of a 16 x 16 tile
 constexpr int BW_BATCH = 256;    // list entries staged per batch (one per thread)
 constexpr int BW_NACC = 9;       // per-survivor accumulators: uv (2), conic (3), opacity, colour (3)
+constexpr int BW_NABS = 2;       // ABSGRAD: sum over pixels of |d u|, |d v| (gsb_render_backward_density)
 constexpr int PB_THREADS = 256;
 
 struct __align__(16) BwRec {  // the staged record in k_blend's pre-scaled form (render.comp:66 evaluated identically)
@@ -43,10 +47,14 @@ struct __align__(16) BwRec {  // the staged record in k_blend's pre-scaled form 
     float4 q2;                // b power_cut bits(compact id) -
 };
 
-template <int MODE>
+// ABSGRAD (gsb_render_backward_density): each lane's d u and d v -- one pixel's own terms -- also go through the same
+// reduction as absolute values, into P.abs_scratch.  ABSGRAD = false is the plain reverse walk: its code is the same as
+// before the density statistics existed.
+template <int MODE, bool ABSGRAD>
 __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_constant__ BackwardParams P) {
+    constexpr int NACC = BW_NACC + (ABSGRAD ? BW_NABS : 0);  // shared-memory columns: the extra two in ABSGRAD only
     __shared__ BwRec s_rec[BW_BATCH];
-    __shared__ double s_acc[BW_BATCH][BW_NACC];
+    __shared__ double s_acc[BW_BATCH][NACC];
     __shared__ uint32_t s_max;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -92,7 +100,7 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
             s_rec[tid].q1 = make_float4(-0.5f * b.x, b.y, col.x, col.y);
             s_rec[tid].q2 = make_float4(col.z, power_cut(b.y), __uint_as_float(cid), 0.f);
 #pragma unroll
-            for (int k = 0; k < BW_NACC; k++) s_acc[tid][k] = 0.0;
+            for (int k = 0; k < NACC; k++) s_acc[tid][k] = 0.0;
         }
         __syncthreads();
         for (int k = (int)cnt - 1; k >= 0; k--) {
@@ -135,15 +143,32 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
                     v[4] = dpw * (-0.5f * dy * dy);               // d C
                 }
             }
+            float va[BW_NABS];
+            if constexpr (ABSGRAD) {  // this pixel's own |d u|, |d v|, taken before the sum over pixels
+                va[0] = fabsf(v[0]);
+                va[1] = fabsf(v[1]);
+            }
 #pragma unroll
             for (int j = 0; j < BW_NACC; j++) {
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) v[j] += __shfl_xor_sync(FULL, v[j], o);
             }
+            if constexpr (ABSGRAD) {
+#pragma unroll
+                for (int j = 0; j < BW_NABS; j++) {
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) va[j] += __shfl_xor_sync(FULL, va[j], o);
+                }
+            }
             if (lane == 0) {
 #pragma unroll
                 for (int j = 0; j < BW_NACC; j++)
                     if (v[j] != 0.f) atomicAdd(&s_acc[k][j], (double)v[j]);
+                if constexpr (ABSGRAD) {
+#pragma unroll
+                    for (int j = 0; j < BW_NABS; j++)
+                        if (va[j] != 0.f) atomicAdd(&s_acc[k][BW_NACC + j], (double)va[j]);
+                }
             }
         }
         __syncthreads();
@@ -154,8 +179,41 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
                 const double a = s_acc[tid][j];
                 if (a != 0.0) atomicAdd(dst + j, a);
             }
+            if constexpr (ABSGRAD) {
+                double* dabs = P.abs_scratch + (size_t)__float_as_uint(s_rec[tid].q2.z) * BW_NABS;
+#pragma unroll
+                for (int j = 0; j < BW_NABS; j++) {
+                    const double a = s_acc[tid][BW_NACC + j];
+                    if (a != 0.0) atomicAdd(dabs + j, a);
+                }
+            }
         }
         hi = lo;
+    }
+}
+
+// gsb_render_backward_density, between k_blend_backward<MODE, true> and k_preprocess_backward: one thread per survivor
+// (grid-stride over N_v, read on the device) adds the frame's statistics to the Gaussian's row of P.density:
+// |d uv| and |sum_p |d uv_p|| in NDC units (d u / d ndc.x = W / 2 exactly), one view, and the max of the pixel radius.
+// Every survivor is counted, zero gradient or not -- which is why this is not folded into k_preprocess_backward, whose
+// threads skip such survivors.  It reads d uv without clearing it (k_preprocess_backward still consumes the scratch) and
+// returns abs_scratch to zero.  Plain loads and stores suffice: a Gaussian is at most one survivor of a frame.
+__global__ void __launch_bounds__(PB_THREADS) k_density_accumulate(const __grid_constant__ BackwardParams P) {
+    const uint32_t nv = P.ctl->num_visible;
+    const double hw = 0.5 * (double)P.width, hh = 0.5 * (double)P.height;
+    for (uint32_t cid = blockIdx.x * blockDim.x + threadIdx.x; cid < nv; cid += gridDim.x * blockDim.x) {
+        const double* sc = P.scratch + (size_t)cid * BW_NACC;
+        double* ab = P.abs_scratch + (size_t)cid * BW_NABS;
+        const double gx = sc[0] * hw, gy = sc[1] * hh;
+        const double ax = ab[0] * hw, ay = ab[1] * hh;
+        ab[0] = 0.0;
+        ab[1] = 0.0;
+        const float4 r3 = __ldg(P.recs + (size_t)cid * GSB_REC_F4 + 3);
+        float* d = P.density + (size_t)__float_as_uint(r3.y) * 4;
+        d[0] += (float)sqrt(gx * gx + gy * gy);
+        d[1] += (float)sqrt(ax * ax + ay * ay);
+        d[2] += 1.0f;
+        d[3] = fmaxf(d[3], r3.x);
     }
 }
 
@@ -458,14 +516,25 @@ __global__ void __launch_bounds__(CR_THREADS) k_camera_reduce(const double* __re
 }  // namespace
 
 cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s) {
+    const bool density = p.density != nullptr;
     if (p.num_tiles) {
-        if (p.mode == GSB_MODE_EXACT) k_blend_backward<GSB_MODE_EXACT><<<p.num_tiles, BW_THREADS, 0, s>>>(p);
-        else k_blend_backward<GSB_MODE_FAST><<<p.num_tiles, BW_THREADS, 0, s>>>(p);
+        if (p.mode == GSB_MODE_EXACT) {
+            if (density) k_blend_backward<GSB_MODE_EXACT, true><<<p.num_tiles, BW_THREADS, 0, s>>>(p);
+            else k_blend_backward<GSB_MODE_EXACT, false><<<p.num_tiles, BW_THREADS, 0, s>>>(p);
+        } else {
+            if (density) k_blend_backward<GSB_MODE_FAST, true><<<p.num_tiles, BW_THREADS, 0, s>>>(p);
+            else k_blend_backward<GSB_MODE_FAST, false><<<p.num_tiles, BW_THREADS, 0, s>>>(p);
+        }
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
     // grid-stride over N_v, which stays on the device: the grid comes from the SM count
     const unsigned grid = (unsigned)p.num_sms * 4u;
+    if (density) {  // reads d uv before k_preprocess_backward clears it
+        k_density_accumulate<<<grid, PB_THREADS, 0, s>>>(p);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
     if (!p.grad_ubo) {
         k_preprocess_backward<false><<<grid, PB_THREADS, 0, s>>>(p);
         return cudaGetLastError();

@@ -102,6 +102,8 @@ struct gsb_ctx {
     double* bw_scratch = nullptr;   // n x 9 per-survivor fp64 accumulators of the blend backward (kept zero between calls)
     uint64_t bw_scratch_n = 0;
     double* bw_cam_partials = nullptr;  // [4 * num_sms][GSB_UBO_WORDS] per-CTA fp64 partial sums of gsb_render_backward_camera
+    double* bw_abs = nullptr;       // n x 2 per-survivor fp64 sums of |d u|, |d v| of gsb_render_backward_density (kept zero)
+    uint64_t bw_abs_n = 0;
     uint64_t scene_gen = 0;         // bumped by every gsb_scene_upload
     bool any_frame = false;         // a frame has been rendered on this context since its creation
     bool frame_recorded = false;    // the last frame stored the backward state (whole frame, per-tile lists)

@@ -183,6 +183,9 @@ struct BackwardParams {
     // gsb_render_backward_camera (null otherwise).  Appended last so the other fields keep their offsets.
     double* cam_partials;     // [num_sms * 4][GSB_UBO_WORDS] per-CTA partial sums of dL/d(UBO), fully overwritten
     gsb_uniforms* grad_ubo;   // fp32 dL/d(UBO), fully overwritten
+    // gsb_render_backward_density (null otherwise).  Appended last so the other fields keep their offsets.
+    double* abs_scratch;      // n x 2 per survivor: sum over pixels of |d u|, |d v|; zero on entry, zero again on exit
+    float* density;           // n x 4 per Gaussian: |d uv|, |abs d uv| (NDC units), views, max radius; accumulated into
 };
 #define GSB_UBO_WORDS 40  // 4-byte words of gsb_uniforms; the camera gradient is reduced in this layout
 cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s);

@@ -41,7 +41,7 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_reserve_instances", "gsb_render", "gsb_render_async", "gsb_get_stats", "gsb_debug_size",
     "gsb_debug_download", "gsb_sort_pairs", "gsb_sort_pairs32", "gsb_set_graph", "gsb_host_alloc", "gsb_host_free",
     # reverse mode
-    "gsb_set_backward", "gsb_render_backward", "gsb_render_backward_camera",
+    "gsb_set_backward", "gsb_render_backward", "gsb_render_backward_camera", "gsb_render_backward_density",
     # frame sharding over several GPUs
     "gsb_group_create", "gsb_group_destroy", "gsb_group_size", "gsb_group_context", "gsb_group_last_error",
     "gsb_group_scene_upload", "gsb_group_render", "gsb_group_render_async",
@@ -142,6 +142,7 @@ lib.gsb_sort_pairs32.argtypes = [_vp, _vp, _vp, _vp, _vp, C.c_uint64, C.c_uint32
 lib.gsb_set_backward.argtypes = [_vp, C.c_int]
 lib.gsb_render_backward.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp]
 lib.gsb_render_backward_camera.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp]
+lib.gsb_render_backward_density.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp]
 
 lib.gsb_group_create.argtypes = [C.c_int, C.POINTER(C.c_int), C.POINTER(_vp)]
 lib.gsb_group_destroy.argtypes = [_vp]
@@ -392,11 +393,16 @@ class Context:
         self._ck(lib.gsb_set_backward(self.h, int(on)))
 
     def render_backward(self, vertices_ptr, grad_image_ptr, grad_vertices_ptr, stream=None, row_pitch_bytes=0,
-                        grad_uniforms_ptr=None):
+                        grad_uniforms_ptr=None, density_ptr=None):
         """gsb_render_backward on device pointers: dL/d(image) (H x W float4) -> dL/d(vertices) (n x 60, overwritten).
         With grad_uniforms_ptr (160 B of device memory), gsb_render_backward_camera: also dL/d(the frame's gsb_uniforms),
-        overwritten; grad_vertices_ptr may then be None (a frozen scene)."""
-        if grad_uniforms_ptr is None:
+        overwritten; grad_vertices_ptr may then be None (a frozen scene).
+        With density_ptr (n x 4 floats of device memory), gsb_render_backward_density: also accumulates the frame's
+        density-control statistics into it; either gradient output may then be None, but not both."""
+        if density_ptr is not None:
+            self._ck(lib.gsb_render_backward_density(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
+                                                     grad_uniforms_ptr, density_ptr, stream_ptr(stream)))
+        elif grad_uniforms_ptr is None:
             self._ck(lib.gsb_render_backward(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
                                              stream_ptr(stream)))
         else:
@@ -445,8 +451,12 @@ def _render_fn():
 
         class RenderFn(torch.autograd.Function):
             @staticmethod
-            def forward(fctx, ctx, vertices, u, ubo):
+            def forward(fctx, ctx, vertices, u, ubo, density):
                 v = vertices.detach().contiguous()
+                if density is not None and (density.dtype != torch.float32 or density.shape != (v.shape[0], 4)
+                                            or density.device != v.device or not density.is_contiguous()):
+                    raise ValueError("render_torch: density must be a contiguous (n, 4) float32 tensor on the vertices' device")
+                fctx.density = density
                 if ubo is not None:  # the camera's float fields come from the tensor, the frame size from u
                     u = unpack_uniforms(ubo.detach().to("cpu", torch.float32).numpy(), u.width, u.height)
                     fctx.ubo_like = (ubo.dtype, ubo.device)
@@ -474,21 +484,27 @@ def _render_fn():
                 # enqueued on torch's current stream (the engine runs backward on the forward's stream), so the gradients
                 # are complete for whatever torch enqueues after them
                 stream = _torch_stream_arg(torch.cuda.current_stream(v.device))
-                if need_ubo:
-                    gu = torch.empty(40, dtype=torch.float32, device=v.device)  # a whole gsb_uniforms
+                gu = torch.empty(40, dtype=torch.float32, device=v.device) if need_ubo else None  # a whole gsb_uniforms
+                if fctx.density is not None:
+                    ctx._ck(lib.gsb_render_backward_density(ctx.h, v.data_ptr(), g.data_ptr(), 0,
+                                                            grad_v.data_ptr() if need_v else None,
+                                                            gu.data_ptr() if need_ubo else None, fctx.density.data_ptr(),
+                                                            stream))
+                elif need_ubo:
                     ctx._ck(lib.gsb_render_backward_camera(ctx.h, v.data_ptr(), g.data_ptr(), 0,
                                                            grad_v.data_ptr() if need_v else None, gu.data_ptr(), stream))
-                    dtype, device = fctx.ubo_like
-                    grad_ubo = gu[UBO_FLOAT_WORDS].to(device=device, dtype=dtype)
                 else:
                     ctx._ck(lib.gsb_render_backward(ctx.h, v.data_ptr(), g.data_ptr(), 0, grad_v.data_ptr(), stream))
-                return None, grad_v, None, grad_ubo
+                if need_ubo:
+                    dtype, device = fctx.ubo_like
+                    grad_ubo = gu[UBO_FLOAT_WORDS].to(device=device, dtype=dtype)
+                return None, grad_v, None, grad_ubo, None
 
         _RenderFn = RenderFn
     return _RenderFn
 
 
-def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None):
+def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None):
     """Differentiable frame: vertices is a CUDA float32 tensor (n, 60) of GSScene::Vertex records (activated parameters, as
     gsb_scene_upload takes them).  Uploads it from device memory, renders the whole frame as an (H, W, 4) RGBA32F tensor and,
     on backward, returns dL/dvertices through gsb_render_backward.  Turns gsb_set_backward on for `ctx`.  The frame on the
@@ -496,8 +512,64 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None):
 
     ubo (optional): a (UBO_FLOATS,) tensor of the camera's float fields in ABI order (uniforms_torch makes one from a pose);
     its values replace u's, u still gives the frame size, and backward also returns dL/dubo (gsb_render_backward_camera).
-    Only the inputs that require grad are differentiated: frozen vertices cost no n x 60 gradient."""
-    return _render_fn().apply(ctx, vertices, u, ubo)
+    Only the inputs that require grad are differentiated: frozen vertices cost no n x 60 gradient.
+
+    density (optional): a contiguous (n, 4) float32 tensor on the vertices' device that backward accumulates this frame's
+    density-control statistics into (gsb_render_backward_density, on torch's stream): screen-space gradient norm and absolute
+    gradient norm in NDC units, the view count and the max pixel radius; see densify_and_prune.  Backward runs only when
+    vertices or ubo requires grad."""
+    return _render_fn().apply(ctx, vertices, u, ubo, density)
+
+
+def densify_and_prune(vertices, density, *, grad_threshold, scene_extent, percent_dense=0.01, min_opacity=0.005,
+                      max_screen_size=None, use_absgrad=False, generator=None):
+    """Adaptive density control (Kerbl et al. 2023, section 5) on activated (n, 60) GSScene::Vertex records, in torch on any
+    device.  density is the (n, 4) table render_torch(..., density=) accumulates; resetting it is the caller's job.
+
+    avg = density[:, 1 if use_absgrad else 0] / max(density[:, 2], 1), s_max = the largest of the row's three scales:
+      clone  avg >= grad_threshold and s_max <= percent_dense * scene_extent: the row is kept and appended again as it is;
+      split  avg >= grad_threshold and s_max >  percent_dense * scene_extent: the row is replaced by two children at
+             p + R(q) (s * eps) with scale s / 1.6, the rest of the row copied (R(q) from the quaternion as stored, eps ~ N(0, I)
+             drawn as one torch.randn((2 k, 3)) from `generator` for the k split rows, rows 0..k-1 for the first children);
+      prune  then, on the result, every row whose opacity < min_opacity and, when max_screen_size is given, every row whose
+             source's density[:, 3] (max pixel radius) > max_screen_size or whose own s_max > 0.1 * scene_extent.
+    Output order: the kept rows in their order, the clones, the first children, the second children, pruned rows removed.
+    Returns (new_vertices, source): source (int64, on vertices' device) is the old row each new row comes from, so the
+    caller can gather its optimizer state (and other per-row tensors) with it."""
+    import torch
+
+    v = vertices.detach()
+    n = v.shape[0]
+    if density.shape != (n, 4):
+        raise ValueError(f"densify_and_prune: density must be ({n}, 4), got {tuple(density.shape)}")
+    d = density.detach().to(device=v.device, dtype=torch.float32)
+    avg = d[:, 1 if use_absgrad else 0] / d[:, 2].clamp(min=1.0)
+    s_max = v[:, 4:7].max(1).values
+    hot = avg >= grad_threshold
+    small = s_max <= percent_dense * scene_extent
+    clone, split = hot & small, hot & ~small
+    rows = torch.arange(n, device=v.device)
+    split_rows = rows[split]
+    k = split_rows.numel()
+    eps = torch.randn((2 * k, 3), generator=generator, dtype=v.dtype, device=v.device)
+    parent = v[split_rows].repeat(2, 1)
+    q = parent[:, 8:12]
+    qw, qx, qy, qz = q[:, 0], q[:, 1], q[:, 2], q[:, 3]
+    R = torch.stack([  # the rotation whose columns are the Gaussian's axes: Sigma = R diag(s^2) R^T
+        torch.stack([1 - 2 * (qy * qy + qz * qz), 2 * (qx * qy - qw * qz), 2 * (qx * qz + qw * qy)], -1),
+        torch.stack([2 * (qx * qy + qw * qz), 1 - 2 * (qx * qx + qz * qz), 2 * (qy * qz - qw * qx)], -1),
+        torch.stack([2 * (qx * qz - qw * qy), 2 * (qy * qz + qw * qx), 1 - 2 * (qx * qx + qy * qy)], -1),
+    ], -2)
+    children = parent.clone()
+    children[:, 0:3] = parent[:, 0:3] + (R @ (parent[:, 4:7] * eps)[:, :, None])[:, :, 0]
+    children[:, 4:7] = parent[:, 4:7] / 1.6
+    source = torch.cat([rows[~split], rows[clone], split_rows, split_rows])
+    out = torch.cat([v[~split], v[clone], children])
+    prune = out[:, 7] < min_opacity
+    if max_screen_size is not None:
+        prune |= (d[source, 3] > max_screen_size) | (out[:, 4:7].max(1).values > 0.1 * scene_extent)
+    keep = ~prune
+    return out[keep].contiguous(), source[keep]
 
 
 def _uniforms_restated(position, rotation_wxyz, fov_deg, near, far, width, height):

@@ -239,6 +239,22 @@ int gsb_render_backward(gsb_ctx *ctx, const float *vertices, const float *grad_i
 int gsb_render_backward_camera(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,
                                float *grad_vertices, gsb_uniforms *grad_uniforms, void *stream);
 
+/* The backward pass plus the per-Gaussian statistics of adaptive density control (clone / split / prune): the same arguments,
+ * preconditions and error codes as gsb_render_backward, and also GSB_ERR_INVALID for a NULL density or when grad_vertices and
+ * grad_uniforms are both NULL.
+ *   grad_vertices  may be NULL; otherwise it receives exactly what gsb_render_backward writes
+ *   grad_uniforms  may be NULL; otherwise it receives exactly what gsb_render_backward_camera writes
+ *   density        device memory, n x 4 floats indexed by Gaussian (the upload's row order), ACCUMULATED INTO (the caller zeroes
+ *                  it when resetting its statistics).  For every Gaussian that survived the last frame's culls:
+ *                  [0] += |(dL/du W/2, dL/dv H/2)|, the screen-space gradient in NDC units (u = ((ndc + 1) W - 1) / 2);
+ *                  [1] += |(sum_p |dL_p/du| W/2, sum_p |dL_p/dv| H/2)|, the absolute gradient (absolute value per pixel and
+ *                         component before the sum over pixels);
+ *                  [2] += 1, zero gradient or not (the number of views);
+ *                  [3] = max([3], the frame's pixel radius ceil(3 sqrt(lambda_max))).
+ *                  Culled Gaussians' rows are not touched. */
+int gsb_render_backward_density(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,
+                                float *grad_vertices, gsb_uniforms *grad_uniforms, float *density, void *stream);
+
 /* Size in bytes of a debug buffer for the last frame (0 if unavailable), and its download. */
 size_t gsb_debug_size(gsb_ctx *ctx, gsb_buffer which);
 int gsb_debug_download(gsb_ctx *ctx, gsb_buffer which, void *dst, size_t bytes);

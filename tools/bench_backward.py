@@ -2,8 +2,8 @@
 """Times the reverse mode (DESIGN.md section 10) on bench.py's workloads: on one GPU at tile-cull level 1, device-event times
 of (a) the plain forward, (b) the recording forward (gsb_set_backward on) and (c) gsb_render_backward of a recorded whole
 frame with a seeded upstream gradient (RGBA32F layout), then gsb_render_backward_camera of such a frame (d) with both
-outputs and (e) with the camera gradient only (grad_vertices = NULL).  Prints one JSON line with the card name and its
-power limit.  Writes nothing.
+outputs and (e) with the camera gradient only (grad_vertices = NULL), then gsb_render_backward_density with the outputs of
+(d) and of (e) plus the density statistics.  Prints one JSON line with the card name and its power limit.  Writes nothing.
 
 usage: python tools/bench_backward.py [--steps K] [--warmup W] [--workload NAME] [--mode exact|fast]"""
 import argparse
@@ -82,14 +82,14 @@ def main():
     plain = forward_ms(False)
     recording = forward_ms(True)
 
-    def backward_ms(grad_vertices_ptr, grad_uniforms_ptr=None):
+    def backward_ms(grad_vertices_ptr, grad_uniforms_ptr=None, density_ptr=None):
         times = []
         for i in range(warmup + steps):
             ctx.render_into(cams[i % bench.NUM_CAMERAS], fb.data_ptr(), g.FORMAT_BGRA8, stream=stream)  # a recorded whole frame
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record(stream)
             ctx.render_backward(vtx_dev.data_ptr(), grad_img.data_ptr(), grad_vertices_ptr, stream=stream,
-                                grad_uniforms_ptr=grad_uniforms_ptr)
+                                grad_uniforms_ptr=grad_uniforms_ptr, density_ptr=density_ptr)
             e1.record(stream)
             e1.synchronize()
             if i >= warmup:
@@ -100,6 +100,10 @@ def main():
     back = backward_ms(grad_vtx.data_ptr())
     back_cam = backward_ms(grad_vtx.data_ptr(), grad_ubo.data_ptr())  # gsb_render_backward_camera, scene and camera
     back_cam_only = backward_ms(None, grad_ubo.data_ptr())  # a frozen scene: the camera only
+    density = torch.zeros((vtx_dev.shape[0], 4), dtype=torch.float32, device=dev)  # accumulated into across the calls
+    # gsb_render_backward_density with the same outputs as the two camera arms, plus the density statistics
+    back_dens = backward_ms(grad_vtx.data_ptr(), grad_ubo.data_ptr(), density.data_ptr())
+    back_dens_cam_only = backward_ms(None, grad_ubo.data_ptr(), density.data_ptr())
     ctx.set_backward(False)
     ctx.close()
     print(json.dumps({
@@ -110,6 +114,7 @@ def main():
         "recording_overhead": recording / plain - 1.0 if plain > 0 else None,
         "backward_ms": float(np.mean(back)), "backward_ms_median": float(np.median(back)),
         "camera_backward_ms": float(np.mean(back_cam)), "camera_only_backward_ms": float(np.mean(back_cam_only)),
+        "density_backward_ms": float(np.mean(back_dens)), "density_camera_only_backward_ms": float(np.mean(back_dens_cam_only)),
         "gpu":torch.cuda.get_device_properties(dev).name, "power_limit_w": power_limit_w(0),
         "how": "CUDA events on one stream: K back-to-back forwards per arm; the backward timed alone after each recorded frame",
     }))
