@@ -533,6 +533,8 @@ int gsb_create(int device, gsb_ctx** out) {
     return GSB_OK;
 }
 
+static void free_det_buffers(gsb_ctx* ctx);
+
 void gsb_destroy(gsb_ctx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
@@ -565,6 +567,7 @@ void gsb_destroy(gsb_ctx* ctx) {
     dev_free(ctx->bw_scratch);
     dev_free(ctx->bw_cam_partials);
     dev_free(ctx->bw_abs);
+    free_det_buffers(ctx);
     for (auto& ev : ctx->ev)
         if (ev) cudaEventDestroy(ev);
     for (auto& ev : ctx->ev_sort)
@@ -903,6 +906,20 @@ int gsb_get_stats(gsb_ctx* ctx, gsb_stats* out) {
     return GSB_OK;
 }
 
+static void free_det_buffers(gsb_ctx* ctx) {
+    dev_free(ctx->bw_det_slots);
+    dev_free(ctx->bw_det_keys[0]);
+    dev_free(ctx->bw_det_keys[1]);
+    dev_free(ctx->bw_det_pos[0]);
+    dev_free(ctx->bw_det_pos[1]);
+    dev_free(ctx->bw_det_status);
+    dev_free(ctx->bw_det_sc);
+    dev_free(ctx->bw_det_runs);
+    ctx->bw_det_capacity = 0;
+    ctx->bw_det_status_tiles = 0;
+    ctx->bw_det_runs_n = 0;
+}
+
 int gsb_set_backward(gsb_ctx* ctx, int enabled) {
     if (!ctx) return GSB_ERR_INVALID;
     if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, "gsb_set_backward: sharded contexts have no backward pass");
@@ -913,6 +930,39 @@ int gsb_set_backward(gsb_ctx* ctx, int enabled) {
         dev_free(ctx->bw_record);
         ctx->bw_record_pixels = 0;
         ctx->frame_recorded = false;
+        free_det_buffers(ctx);
+    }
+    return GSB_OK;
+}
+
+int gsb_set_backward_deterministic(gsb_ctx* ctx, int enabled) {
+    if (!ctx) return GSB_ERR_INVALID;
+    if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, "gsb_set_backward_deterministic: sharded contexts have no backward pass");
+    ctx->bw_deterministic = enabled != 0;
+    return GSB_OK;
+}
+
+// The buffers of the deterministic reduction for the current arena capacity and scene size (first use, then growth only).
+static int ensure_det_buffers(gsb_ctx* ctx, uint64_t n) {
+    if (ctx->capacity > ctx->bw_det_capacity || !ctx->bw_det_sc) {
+        const uint64_t cap = ctx->capacity;
+        free_det_buffers(ctx);
+        CK(dev_alloc(&ctx->bw_det_slots, (size_t)cap * 11));
+        CK(dev_alloc(&ctx->bw_det_keys[0], cap));
+        CK(dev_alloc(&ctx->bw_det_keys[1], cap));
+        CK(dev_alloc(&ctx->bw_det_pos[0], cap));
+        CK(dev_alloc(&ctx->bw_det_pos[1], cap));
+        const uint32_t tiles = (uint32_t)((cap + sort_tile_items() - 1) / sort_tile_items());
+        CK(dev_alloc(&ctx->bw_det_status, (size_t)std::max<uint32_t>(tiles, 1) * 256));
+        CK(dev_alloc(&ctx->bw_det_sc, 1));
+        ctx->bw_det_status_tiles = std::max<uint32_t>(tiles, 1);
+        ctx->bw_det_capacity = cap;
+    }
+    if (n > ctx->bw_det_runs_n) {
+        dev_free(ctx->bw_det_runs);
+        ctx->bw_det_runs_n = 0;
+        CK(dev_alloc(&ctx->bw_det_runs, (size_t)n));
+        ctx->bw_det_runs_n = n;
     }
     return GSB_OK;
 }
@@ -958,6 +1008,11 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     }
     if (grad_ubo && !ctx->bw_cam_partials)  // one row per CTA of k_preprocess_backward (4 per SM), fully overwritten by each call
         CK(dev_alloc(&ctx->bw_cam_partials, (size_t)ctx->num_sms * 4 * GSB_UBO_WORDS));
+    const bool det = ctx->bw_deterministic;
+    if (det) {
+        rc = ensure_det_buffers(ctx, n);
+        if (rc != GSB_OK) return rc;
+    }
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
     if (grad_vertices) CK(cudaMemsetAsync(grad_vertices, 0, (size_t)n * 60 * sizeof(float), s));
     if (n == 0) {
@@ -988,7 +1043,23 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     bp.grad_ubo = grad_ubo;
     bp.abs_scratch = density ? ctx->bw_abs : nullptr;
     bp.density = density;
-    CK(launch_backward(bp, s));
+    if (!det) {
+        CK(launch_backward(bp, s));
+        return GSB_OK;
+    }
+    bp.det_slots = ctx->bw_det_slots;
+    DetBackward db{};
+    db.keys[0] = ctx->bw_det_keys[0];
+    db.keys[1] = ctx->bw_det_keys[1];
+    db.pos[0] = ctx->bw_det_pos[0];
+    db.pos[1] = ctx->bw_det_pos[1];
+    db.runs = ctx->bw_det_runs;
+    db.sc = ctx->bw_det_sc;
+    db.status = ctx->bw_det_status;
+    db.status_tiles = ctx->bw_det_status_tiles;
+    db.m_hint = quantise_hint(ctx->m_hint);
+    db.key_bits = std::max<uint32_t>(bits_for((uint32_t)n), 1u);  // compact ids < N_v <= n
+    CK(launch_backward(bp, s, &db));
     return GSB_OK;
 }
 

@@ -23,8 +23,15 @@
 //                         projection matrix, camera position, tan_fov -- summed per thread, then per CTA into one fp64 row.
 //   k_camera_reduce       one CTA: sums those rows in a fixed order into the fp32 gsb_uniforms of gradients.
 //
-// The atomics make the sums depend on the order in which warps and CTAs add their partial sums: gradients are NOT guaranteed
-// to be bitwise reproducible from run to run (fp64 accumulation makes a difference in the final fp32 value rare).
+// The atomics make the sums depend on the order in which warps and CTAs add their partial sums: by default gradients are NOT
+// guaranteed to be bitwise reproducible from run to run (fp64 accumulation makes a difference in the final fp32 value rare).
+// gsb_set_backward_deterministic(ctx, 1) replaces that reduction, and only it (DESIGN.md section 10):
+//   k_blend_backward<MODE, ABSGRAD, DET = true>  the same walk; per-warp partials summed in warp order, one fp64 slot per
+//                         (tile, list entry) stored at the entry's list position, +0 for entries that contributed nothing.
+//   k_det_prepare + the Onesweep sort (k_sort_hist, k_onesweep_pass)  a stable sort of (compact id, list position) over the
+//                         frame's M entries; its last pass publishes each survivor's run, in tile order.
+//   k_det_reduce          one thread per survivor: the run's slots summed in order in fp64, stored into the scratch that
+//                         k_density_accumulate and k_preprocess_backward read.  Every output is then order-fixed.
 // Compiled with -fmad=false like the forward.
 #include "gsb_cull.cuh"
 #include "gsb_exp.cuh"
@@ -39,6 +46,10 @@ constexpr int BW_THREADS = 256;  // one pixel per thread of a 16 x 16 tile
 constexpr int BW_BATCH = 256;    // list entries staged per batch (one per thread)
 constexpr int BW_NACC = 9;       // per-survivor accumulators: uv (2), conic (3), opacity, colour (3)
 constexpr int BW_NABS = 2;       // ABSGRAD: sum over pixels of |d u|, |d v| (gsb_render_backward_density)
+constexpr int BW_DET_BATCH = 128;  // DET: list entries per batch, so that the per-warp partials fit 4-5 CTAs per SM
+constexpr int BW_WARPS = BW_THREADS / 32;
+template <bool DET>
+constexpr uint32_t bw_batch = DET ? BW_DET_BATCH : BW_BATCH;
 constexpr int PB_THREADS = 256;
 
 struct __align__(16) BwRec {  // the staged record in k_blend's pre-scaled form (render.comp:66 evaluated identically)
@@ -50,11 +61,22 @@ struct __align__(16) BwRec {  // the staged record in k_blend's pre-scaled form 
 // ABSGRAD (gsb_render_backward_density): each lane's d u and d v -- one pixel's own terms -- also go through the same
 // reduction as absolute values, into P.abs_scratch.  ABSGRAD = false is the plain reverse walk: its code is the same as
 // before the density statistics existed.
-template <int MODE, bool ABSGRAD>
+// DET (gsb_set_backward_deterministic): the same walk, reduced without atomics.  Lane 0 of each warp stores the warp's
+// shuffle sums into its own fp32 row of det_partials() (dynamic shared memory, [warp][NACC][BW_DET_BATCH]); at the flush
+// thread k sums the 8 warps in warp order in fp64 and stores the tile's partial of entry k into P.det_slots at its list
+// position.  Every position of the tile's list is stored, +0 for entries no pixel of the tile has as contributor.
+// DET = false is the atomic reduction, unchanged: its SASS is the same as before DET existed, which is why the DET-only
+// constants and the shared-memory pointer live outside the kernel (a new local, even unused, changes ptxas' allocation).
+__device__ __forceinline__ float* det_partials() {
+    extern __shared__ float s_dyn[];  // referenced by the DET instantiations only
+    return s_dyn;
+}
+
+template <int MODE, bool ABSGRAD, bool DET = false>
 __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_constant__ BackwardParams P) {
     constexpr int NACC = BW_NACC + (ABSGRAD ? BW_NABS : 0);  // shared-memory columns: the extra two in ABSGRAD only
-    __shared__ BwRec s_rec[BW_BATCH];
-    __shared__ double s_acc[BW_BATCH][NACC];
+    __shared__ BwRec s_rec[bw_batch<DET>];
+    __shared__ double s_acc[DET ? 1 : BW_BATCH][NACC];
     __shared__ uint32_t s_max;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -88,7 +110,7 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
 
     float acc_r = 0.f, acc_g = 0.f, acc_b = 0.f;  // colour behind the current entry, per unit of its transmittance
     for (uint32_t hi = max_last; hi > 0;) {
-        const uint32_t lo = hi > (uint32_t)BW_BATCH ? hi - (uint32_t)BW_BATCH : 0u;
+        const uint32_t lo = hi > bw_batch<DET> ? hi - bw_batch<DET> : 0u;
         const uint32_t cnt = hi - lo;
         __syncthreads();  // the previous batch's walk and flush are done with s_rec / s_acc
         if ((uint32_t)tid < cnt) {
@@ -99,8 +121,10 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
             s_rec[tid].q0 = make_float4(a.x, a.y, -0.5f * a.z, -a.w);
             s_rec[tid].q1 = make_float4(-0.5f * b.x, b.y, col.x, col.y);
             s_rec[tid].q2 = make_float4(col.z, power_cut(b.y), __uint_as_float(cid), 0.f);
+            if constexpr (!DET) {
 #pragma unroll
-            for (int k = 0; k < NACC; k++) s_acc[tid][k] = 0.0;
+                for (int k = 0; k < NACC; k++) s_acc[tid][k] = 0.0;
+            }
         }
         __syncthreads();
         for (int k = (int)cnt - 1; k >= 0; k--) {
@@ -118,7 +142,15 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
             const float raw = q1.y * e;
             const float al = fminf(0.99f, raw);
             const bool contrib = pos <= last && !(pw > 0.0f || pw < q2.y) && !(al < 1.0f / 255.0f);
-            if (!__any_sync(FULL, contrib)) continue;
+            if (!__any_sync(FULL, contrib)) {
+                if constexpr (DET) {
+                    if (lane == 0) {
+#pragma unroll
+                        for (int j = 0; j < NACC; j++) det_partials()[(warp * NACC + j) * bw_batch<true> + k] = 0.f;
+                    }
+                }
+                continue;
+            }
             float v[BW_NACC];
 #pragma unroll
             for (int j = 0; j < BW_NACC; j++) v[j] = 0.f;
@@ -160,7 +192,16 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
                     for (int o = 16; o > 0; o >>= 1) va[j] += __shfl_xor_sync(FULL, va[j], o);
                 }
             }
-            if (lane == 0) {
+            if constexpr (DET) {
+                if (lane == 0) {
+#pragma unroll
+                    for (int j = 0; j < BW_NACC; j++) det_partials()[(warp * NACC + j) * bw_batch<true> + k] = v[j];
+                    if constexpr (ABSGRAD) {
+#pragma unroll
+                        for (int j = 0; j < BW_NABS; j++) det_partials()[(warp * NACC + BW_NACC + j) * bw_batch<true> + k] = va[j];
+                    }
+                }
+            } else if (lane == 0) {
 #pragma unroll
                 for (int j = 0; j < BW_NACC; j++)
                     if (v[j] != 0.f) atomicAdd(&s_acc[k][j], (double)v[j]);
@@ -172,7 +213,18 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
             }
         }
         __syncthreads();
-        if ((uint32_t)tid < cnt) {
+        if constexpr (DET) {
+            if ((uint32_t)tid < cnt) {  // warps 0..7 in order, in fp64 from +0.0: the slot is never -0
+                double* dst = P.det_slots + (size_t)(range.x + lo + (uint32_t)tid) * NACC;
+#pragma unroll
+                for (int j = 0; j < NACC; j++) {
+                    double a = 0.0;
+#pragma unroll
+                    for (int w = 0; w < BW_WARPS; w++) a += (double)det_partials()[(w * NACC + j) * bw_batch<true> + tid];
+                    dst[j] = a;
+                }
+            }
+        } else if ((uint32_t)tid < cnt) {
             double* dst = P.scratch + (size_t)__float_as_uint(s_rec[tid].q2.z) * BW_NACC;
 #pragma unroll
             for (int j = 0; j < BW_NACC; j++) {
@@ -189,6 +241,14 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
             }
         }
         hi = lo;
+    }
+    if constexpr (DET) {  // the entries behind every pixel's last contributor: +0, so k_det_reduce reads no stale slot
+        const uint32_t len = range.y - range.x;
+        for (uint32_t p = max_last + (uint32_t)tid; p < len; p += BW_THREADS) {
+            double* dst = P.det_slots + (size_t)(range.x + p) * NACC;
+#pragma unroll
+            for (int j = 0; j < NACC; j++) dst[j] = 0.0;
+        }
     }
 }
 
@@ -214,6 +274,70 @@ __global__ void __launch_bounds__(PB_THREADS) k_density_accumulate(const __grid_
         d[1] += (float)sqrt(ax * ax + ay * ay);
         d[2] += 1.0f;
         d[3] = fmaxf(d[3], r3.x);
+    }
+}
+
+// gsb_set_backward_deterministic, before the sort that groups the slots by survivor: the sort's input pairs (compact id of
+// list position p, p) over the frame's M entries -- a copy, so the frame's lists survive for a repeated backward -- and the
+// per-survivor runs set to all ones (= no entry) for the sort's last pass to fill.  M and N_v are read on the device.
+__global__ void __launch_bounds__(PB_THREADS) k_det_prepare(const uint32_t* __restrict__ vals, const Control* ctl, uint32_t* __restrict__ keys,
+                                                            uint32_t* __restrict__ pos, uint2* __restrict__ runs) {
+    const uint32_t m = ctl->num_instances, nv = ctl->num_visible;
+    const uint32_t i0 = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
+    for (uint32_t p = i0; p < m; p += stride) {
+        keys[p] = __ldg(vals + p);
+        pos[p] = p;
+    }
+    for (uint32_t c = i0; c < nv; c += stride) runs[c] = make_uint2(0xffffffffu, 0xffffffffu);
+}
+
+// gsb_set_backward_deterministic, after the sort: one thread per survivor (grid-stride over N_v, read on the device) sums its
+// slots in run order -- ascending list position, which is tile order -- in fp64 from +0.0, and STORES the totals into
+// P.scratch (and P.abs_scratch), where k_density_accumulate and k_preprocess_backward read them as they read the atomic sums.
+// The sum is sequential so that an entry whose slot is +0 changes nothing: tile-cull level 1's list is level 0's with such
+// entries removed, and both give the same bits.  Loads run UNROLL entries ahead of the adds.
+template <bool ABSGRAD>
+__global__ void __launch_bounds__(PB_THREADS) k_det_reduce(const __grid_constant__ BackwardParams P, const uint32_t* __restrict__ pos,
+                                                           const uint2* __restrict__ runs) {
+    constexpr int NACC = BW_NACC + (ABSGRAD ? BW_NABS : 0);
+    constexpr uint32_t UNROLL = 4;
+    const uint32_t nv = P.ctl->num_visible;
+    const double* __restrict__ slots = P.det_slots;
+    for (uint32_t cid = blockIdx.x * blockDim.x + threadIdx.x; cid < nv; cid += gridDim.x * blockDim.x) {
+        double s[NACC];
+#pragma unroll
+        for (int k = 0; k < NACC; k++) s[k] = 0.0;
+        const uint2 r = __ldg(runs + cid);
+        if (r.x != 0xffffffffu) {  // a survivor in no list (level 1 culled it from every tile) keeps zeros
+            const uint32_t end = ~r.y;
+            uint32_t j = r.x;
+            for (; j + UNROLL <= end; j += UNROLL) {
+                double x[UNROLL][NACC];
+#pragma unroll
+                for (uint32_t u = 0; u < UNROLL; u++) {
+                    const double* sl = slots + (size_t)__ldg(pos + j + u) * NACC;
+#pragma unroll
+                    for (int k = 0; k < NACC; k++) x[u][k] = __ldg(sl + k);
+                }
+#pragma unroll
+                for (uint32_t u = 0; u < UNROLL; u++)
+#pragma unroll
+                    for (int k = 0; k < NACC; k++) s[k] += x[u][k];
+            }
+            for (; j < end; j++) {
+                const double* sl = slots + (size_t)__ldg(pos + j) * NACC;
+#pragma unroll
+                for (int k = 0; k < NACC; k++) s[k] += __ldg(sl + k);
+            }
+        }
+        double* sc = P.scratch + (size_t)cid * BW_NACC;
+#pragma unroll
+        for (int k = 0; k < BW_NACC; k++) sc[k] = s[k];
+        if constexpr (ABSGRAD) {
+            double* ab = P.abs_scratch + (size_t)cid * BW_NABS;
+#pragma unroll
+            for (int k = 0; k < BW_NABS; k++) ab[k] = s[BW_NACC + k];
+        }
     }
 }
 
@@ -513,11 +637,71 @@ __global__ void __launch_bounds__(CR_THREADS) k_camera_reduce(const double* __re
     }
 }
 
+template <int MODE, bool ABSGRAD>
+cudaError_t launch_blend_det(const BackwardParams& p, cudaStream_t s) {
+    constexpr int NACC = BW_NACC + (ABSGRAD ? BW_NABS : 0);
+    const size_t smem = (size_t)BW_WARPS * NACC * BW_DET_BATCH * sizeof(float);  // 36 KB, or 44 KB with ABSGRAD
+    cudaError_t e = cudaFuncSetAttribute(k_blend_backward<MODE, ABSGRAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    k_blend_backward<MODE, ABSGRAD, true><<<p.num_tiles, BW_THREADS, smem, s>>>(p);
+    return cudaGetLastError();
+}
+
+// gsb_set_backward_deterministic: the per-survivor sums of the blend backward without atomics.  The blend stores one slot
+// per (tile, entry); a stable sort of (compact id, list position) over the M entries groups each survivor's slots in tile
+// order, its last pass publishing each survivor's run; k_det_reduce sums every run in order.  Integer atomics remain
+// (the sort's counters and the runs' atomicMin), but their results do not depend on the order they land in.
+cudaError_t launch_det_sums(const BackwardParams& p, const DetBackward& d, unsigned grid, cudaStream_t s) {
+    const bool density = p.density != nullptr;
+    cudaError_t e = cudaMemsetAsync(d.sc, 0, sizeof(SortCtl), s);
+    if (e != cudaSuccess) return e;
+    // look-back words no earlier call has tagged: zeroed here, tagged 1.. by this sort's passes (epoch 0 = not published)
+    if ((e = cudaMemsetAsync(d.status, 0, (size_t)d.status_tiles * 256 * sizeof(unsigned long long), s)) != cudaSuccess) return e;
+    k_det_prepare<<<grid, PB_THREADS, 0, s>>>(p.vals, p.ctl, d.keys[0], d.pos[0], d.runs);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    SortParams sp{};
+    sp.keys[0] = d.keys[0];
+    sp.keys[1] = d.keys[1];
+    sp.vals[0] = d.pos[0];
+    sp.vals[1] = d.pos[1];
+    sp.key_bytes = 4;
+    sp.d_m = &p.ctl->num_instances;
+    sp.m_hint = d.m_hint;
+    sp.key_bits = d.key_bits;
+    sp.status = d.status;
+    sp.status_tiles = d.status_tiles;
+    sp.d_epoch = nullptr;
+    sp.epoch_base = 1;
+    sp.sc = d.sc;
+    sp.num_sms = p.num_sms;
+    sp.events = nullptr;
+    sp.ranges = d.runs;  // the last pass: (start, ~end) of each compact id's run
+    sp.range_key_mask = 0;
+    sp.discard_sorted_keys = true;
+    uint32_t passes = 0;
+    if ((e = launch_sort(sp, &passes, s)) != cudaSuccess) return e;
+    if (passes == 0) return cudaErrorInvalidValue;  // key_bits >= 1: the runs come from the last pass
+    if (p.num_tiles) {
+        if (p.mode == GSB_MODE_EXACT) e = density ? launch_blend_det<GSB_MODE_EXACT, true>(p, s) : launch_blend_det<GSB_MODE_EXACT, false>(p, s);
+        else e = density ? launch_blend_det<GSB_MODE_FAST, true>(p, s) : launch_blend_det<GSB_MODE_FAST, false>(p, s);
+        if (e != cudaSuccess) return e;
+    }
+    const uint32_t* sorted_pos = d.pos[passes & 1];
+    if (density) k_det_reduce<true><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs);
+    else k_det_reduce<false><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs);
+    return cudaGetLastError();
+}
+
 }  // namespace
 
-cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s) {
+cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s, const DetBackward* det) {
     const bool density = p.density != nullptr;
-    if (p.num_tiles) {
+    // grid-stride over N_v, which stays on the device: the grid comes from the SM count
+    const unsigned grid = (unsigned)p.num_sms * 4u;
+    if (det) {
+        cudaError_t e = launch_det_sums(p, *det, grid, s);
+        if (e != cudaSuccess) return e;
+    } else if (p.num_tiles) {
         if (p.mode == GSB_MODE_EXACT) {
             if (density) k_blend_backward<GSB_MODE_EXACT, true><<<p.num_tiles, BW_THREADS, 0, s>>>(p);
             else k_blend_backward<GSB_MODE_EXACT, false><<<p.num_tiles, BW_THREADS, 0, s>>>(p);
@@ -528,8 +712,6 @@ cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s) {
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
-    // grid-stride over N_v, which stays on the device: the grid comes from the SM count
-    const unsigned grid = (unsigned)p.num_sms * 4u;
     if (density) {  // reads d uv before k_preprocess_backward clears it
         k_density_accumulate<<<grid, PB_THREADS, 0, s>>>(p);
         cudaError_t e = cudaGetLastError();

@@ -104,6 +104,18 @@ struct gsb_ctx {
     double* bw_cam_partials = nullptr;  // [4 * num_sms][GSB_UBO_WORDS] per-CTA fp64 partial sums of gsb_render_backward_camera
     double* bw_abs = nullptr;       // n x 2 per-survivor fp64 sums of |d u|, |d v| of gsb_render_backward_density (kept zero)
     uint64_t bw_abs_n = 0;
+    // gsb_set_backward_deterministic: allocated on first deterministic use, grown with the arena and the scene, freed with
+    // bw_record.  bw_det_slots holds 11 fp64 per arena entry (the blend's per-(tile, entry) partials).
+    bool bw_deterministic = false;
+    double* bw_det_slots = nullptr;
+    uint32_t* bw_det_keys[2] = {nullptr, nullptr};
+    uint32_t* bw_det_pos[2] = {nullptr, nullptr};
+    unsigned long long* bw_det_status = nullptr;
+    uint32_t bw_det_status_tiles = 0;
+    gsb::SortCtl* bw_det_sc = nullptr;
+    uint64_t bw_det_capacity = 0;
+    uint2* bw_det_runs = nullptr;   // n (start, ~end) runs, one per possible survivor
+    uint64_t bw_det_runs_n = 0;
     uint64_t scene_gen = 0;         // bumped by every gsb_scene_upload
     bool any_frame = false;         // a frame has been rendered on this context since its creation
     bool frame_recorded = false;    // the last frame stored the backward state (whole frame, per-tile lists)

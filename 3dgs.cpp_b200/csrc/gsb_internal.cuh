@@ -186,8 +186,23 @@ struct BackwardParams {
     // gsb_render_backward_density (null otherwise).  Appended last so the other fields keep their offsets.
     double* abs_scratch;      // n x 2 per survivor: sum over pixels of |d u|, |d v|; zero on entry, zero again on exit
     float* density;           // n x 4 per Gaussian: |d uv|, |abs d uv| (NDC units), views, max radius; accumulated into
+    // gsb_set_backward_deterministic (null otherwise).  Appended last so the other fields keep their offsets.
+    double* det_slots;        // per list position: that tile's fp64 partial sums of the entry (9 columns, 11 with density)
 };
 #define GSB_UBO_WORDS 40  // 4-byte words of gsb_uniforms; the camera gradient is reduced in this layout
-cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s);
+
+// gsb_set_backward_deterministic: the buffers that group the per-(tile, entry) slots by survivor without atomics.  All
+// M-sized arrays hold the arena capacity; every one is fully rewritten (or zeroed) by each call.
+struct DetBackward {
+    uint32_t* keys[2];             // the sort's keys: compact id of each list position (a copy: the frame's lists stay intact)
+    uint32_t* pos[2];              // its payloads: the list position
+    uint2* runs;                   // per survivor: (start, ~end) of its run in the sorted positions; all ones = no entry
+    SortCtl* sc;                   // private sort control words, zeroed per call
+    unsigned long long* status;    // private look-back words, zeroed per call
+    uint32_t status_tiles;
+    uint32_t m_hint;               // sizes the sort's grids only
+    uint32_t key_bits;             // bits of the largest compact id
+};
+cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s, const DetBackward* det = nullptr);
 
 }  // namespace gsb

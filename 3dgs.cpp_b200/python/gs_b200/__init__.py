@@ -42,6 +42,7 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_debug_download", "gsb_sort_pairs", "gsb_sort_pairs32", "gsb_set_graph", "gsb_host_alloc", "gsb_host_free",
     # reverse mode
     "gsb_set_backward", "gsb_render_backward", "gsb_render_backward_camera", "gsb_render_backward_density",
+    "gsb_set_backward_deterministic",
     # frame sharding over several GPUs
     "gsb_group_create", "gsb_group_destroy", "gsb_group_size", "gsb_group_context", "gsb_group_last_error",
     "gsb_group_scene_upload", "gsb_group_render", "gsb_group_render_async",
@@ -140,6 +141,7 @@ lib.gsb_debug_download.argtypes = [_vp, C.c_int, _vp, C.c_size_t]
 lib.gsb_sort_pairs.argtypes = [_vp, _vp, _vp, _vp, _vp, C.c_uint64, C.c_uint32, _vp]
 lib.gsb_sort_pairs32.argtypes = [_vp, _vp, _vp, _vp, _vp, C.c_uint64, C.c_uint32, _vp]
 lib.gsb_set_backward.argtypes = [_vp, C.c_int]
+lib.gsb_set_backward_deterministic.argtypes = [_vp, C.c_int]
 lib.gsb_render_backward.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp]
 lib.gsb_render_backward_camera.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp]
 lib.gsb_render_backward_density.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp]
@@ -392,6 +394,11 @@ class Context:
         """gsb_set_backward: the next frames keep what gsb_render_backward needs (tile-cull level 2 falls back to 1)."""
         self._ck(lib.gsb_set_backward(self.h, int(on)))
 
+    def set_backward_deterministic(self, on=True):
+        """gsb_set_backward_deterministic: the next backward calls reduce without floating-point atomics, so their outputs
+        are bit-identical from call to call (and at tile-cull levels 0 and 1)."""
+        self._ck(lib.gsb_set_backward_deterministic(self.h, int(on)))
+
     def render_backward(self, vertices_ptr, grad_image_ptr, grad_vertices_ptr, stream=None, row_pitch_bytes=0,
                         grad_uniforms_ptr=None, density_ptr=None):
         """gsb_render_backward on device pointers: dL/d(image) (H x W float4) -> dL/d(vertices) (n x 60, overwritten).
@@ -485,6 +492,7 @@ def _render_fn():
                 # are complete for whatever torch enqueues after them
                 stream = _torch_stream_arg(torch.cuda.current_stream(v.device))
                 gu = torch.empty(40, dtype=torch.float32, device=v.device) if need_ubo else None  # a whole gsb_uniforms
+                ctx.set_backward_deterministic(torch.are_deterministic_algorithms_enabled())
                 if fctx.density is not None:
                     ctx._ck(lib.gsb_render_backward_density(ctx.h, v.data_ptr(), g.data_ptr(), 0,
                                                             grad_v.data_ptr() if need_v else None,
@@ -517,7 +525,11 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None):
     density (optional): a contiguous (n, 4) float32 tensor on the vertices' device that backward accumulates this frame's
     density-control statistics into (gsb_render_backward_density, on torch's stream): screen-space gradient norm and absolute
     gradient norm in NDC units, the view count and the max pixel radius; see densify_and_prune.  Backward runs only when
-    vertices or ubo requires grad."""
+    vertices or ubo requires grad.
+
+    Under torch.use_deterministic_algorithms(True), backward turns gsb_set_backward_deterministic on for `ctx` (otherwise
+    off): every gradient and density statistic is then bit-identical for the same inputs, at some cost in time.  With
+    torch's default settings backward takes the atomic path, whose results may differ in the last bit from run to run."""
     return _render_fn().apply(ctx, vertices, u, ubo, density)
 
 

@@ -212,14 +212,22 @@ int gsb_get_stats(gsb_ctx *ctx, gsb_stats *out);
  * transmittance and the list position of its last contributing Gaussian).  Sharded contexts: GSB_ERR_INVALID. */
 int gsb_set_backward(gsb_ctx *ctx, int enabled);
 
+/* Deterministic reverse mode (default 0).  While on, gsb_render_backward, gsb_render_backward_camera and
+ * gsb_render_backward_density use no floating-point atomics: every output word is a function of the frame, the
+ * vertices and grad_image alone, bit for bit -- the same on every call, on any stream, whatever the arena capacity,
+ * and the same at tile-cull levels 0 and 1.  Takes effect at the next backward call; the forward is unchanged.
+ * The first deterministic call allocates about 105 B per arena entry (gsb_reserve_instances) and 8 B per Gaussian, freed by
+ * gsb_set_backward(ctx, 0); GSB_ERR_OOM if that fails.  NULL ctx or a sharded context: GSB_ERR_INVALID. */
+int gsb_set_backward_deterministic(gsb_ctx *ctx, int enabled);
+
 /* Gradient of the last frame.  All pointers are device memory, enqueued on `stream` (NULL = the context's stream).
  *   vertices      n x 60 floats: the records last passed to gsb_scene_upload (scale and rotation are read from here)
  *   grad_image    H x W float4 (RGBA32F layout, row_pitch_bytes apart, 0 = tight); the A channel is ignored (the output is 1)
  *   grad_vertices n x 60 floats, OVERWRITTEN: d/d position xyz, scale xyz, opacity, rotation wxyz (as stored, no
  *                 normalisation), sh[48]; zero for position.w, for culled Gaussians and for Gaussians outside every list used
  * The parameters are the activated ones gsb_scene_upload receives (exp(s), sigmoid(o), the normalised quaternion); a caller
- * chains through its own activations.  Gradients are accumulated with (fp64) atomics, so they are not guaranteed to be bitwise
- * reproducible from run to run.  GSB_ERR_NO_SCENE before any upload or frame; GSB_ERR_INVALID if the last frame was rendered with
+ * chains through its own activations.  By default gradients are accumulated with (fp64) atomics, so they are not guaranteed to
+ * be bitwise reproducible from run to run; gsb_set_backward_deterministic makes them so.  GSB_ERR_NO_SCENE before any upload or frame; GSB_ERR_INVALID if the last frame was rendered with
  * gsb_set_backward off, was a band rather than the whole frame, or overflowed the instance arena (gsb_render_async), if
  * the scene was uploaded again after it, if the scene stores fp16 SH, or on a sharded context. */
 int gsb_render_backward(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,

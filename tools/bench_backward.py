@@ -3,7 +3,9 @@
 of (a) the plain forward, (b) the recording forward (gsb_set_backward on) and (c) gsb_render_backward of a recorded whole
 frame with a seeded upstream gradient (RGBA32F layout), then gsb_render_backward_camera of such a frame (d) with both
 outputs and (e) with the camera gradient only (grad_vertices = NULL), then gsb_render_backward_density with the outputs of
-(d) and of (e) plus the density statistics.  Prints one JSON line with the card name and its power limit.  Writes nothing.
+(d) and of (e) plus the density statistics.  The deterministic arms time (c), (d) and the density call with both outputs
+again with gsb_set_backward_deterministic on, on the same frames.  Prints one JSON line with the card name and its power
+limit.  Writes nothing.
 
 usage: python tools/bench_backward.py [--steps K] [--warmup W] [--workload NAME] [--mode exact|fast]"""
 import argparse
@@ -104,6 +106,11 @@ def main():
     # gsb_render_backward_density with the same outputs as the two camera arms, plus the density statistics
     back_dens = backward_ms(grad_vtx.data_ptr(), grad_ubo.data_ptr(), density.data_ptr())
     back_dens_cam_only = backward_ms(None, grad_ubo.data_ptr(), density.data_ptr())
+    ctx.set_backward_deterministic(True)  # the same calls without floating-point atomics
+    det_back = backward_ms(grad_vtx.data_ptr())
+    det_back_cam = backward_ms(grad_vtx.data_ptr(), grad_ubo.data_ptr())
+    det_back_dens = backward_ms(grad_vtx.data_ptr(), grad_ubo.data_ptr(), density.data_ptr())
+    ctx.set_backward_deterministic(False)
     ctx.set_backward(False)
     ctx.close()
     print(json.dumps({
@@ -115,6 +122,9 @@ def main():
         "backward_ms": float(np.mean(back)), "backward_ms_median": float(np.median(back)),
         "camera_backward_ms": float(np.mean(back_cam)), "camera_only_backward_ms": float(np.mean(back_cam_only)),
         "density_backward_ms": float(np.mean(back_dens)), "density_camera_only_backward_ms": float(np.mean(back_dens_cam_only)),
+        "deterministic_backward_ms": float(np.mean(det_back)), "deterministic_backward_ms_median": float(np.median(det_back)),
+        "deterministic_camera_backward_ms": float(np.mean(det_back_cam)),
+        "deterministic_density_backward_ms": float(np.mean(det_back_dens)),
         "gpu":torch.cuda.get_device_properties(dev).name, "power_limit_w": power_limit_w(0),
         "how": "CUDA events on one stream: K back-to-back forwards per arm; the backward timed alone after each recorded frame",
     }))
