@@ -35,6 +35,7 @@
 // Compiled with -fmad=false like the forward.
 #include "gsb_cull.cuh"
 #include "gsb_exp.cuh"
+#include "gsb_geom.cuh"
 #include "gsb_internal.cuh"
 
 namespace gsb {
@@ -59,14 +60,13 @@ struct __align__(16) BwRec {  // the staged record in k_blend's pre-scaled form 
 };
 
 // ABSGRAD (gsb_render_backward_density): each lane's d u and d v -- one pixel's own terms -- also go through the same
-// reduction as absolute values, into P.abs_scratch.  ABSGRAD = false is the plain reverse walk: its code is the same as
-// before the density statistics existed.
+// reduction as absolute values, into P.abs_scratch.
 // DET (gsb_set_backward_deterministic): the same walk, reduced without atomics.  Lane 0 of each warp stores the warp's
 // shuffle sums into its own fp32 row of det_partials() (dynamic shared memory, [warp][NACC][BW_DET_BATCH]); at the flush
 // thread k sums the 8 warps in warp order in fp64 and stores the tile's partial of entry k into P.det_slots at its list
 // position.  Every position of the tile's list is stored, +0 for entries no pixel of the tile has as contributor.
-// DET = false is the atomic reduction, unchanged: its SASS is the same as before DET existed, which is why the DET-only
-// constants and the shared-memory pointer live outside the kernel (a new local, even unused, changes ptxas' allocation).
+// DET = false is the atomic reduction.  The DET-only constants and the shared-memory pointer live outside the kernel: a new
+// local, even unused, changes ptxas' allocation of the DET = false instantiations.
 __device__ __forceinline__ float* det_partials() {
     extern __shared__ float s_dyn[];  // referenced by the DET instantiations only
     return s_dyn;
@@ -341,15 +341,6 @@ __global__ void __launch_bounds__(PB_THREADS) k_det_reduce(const __grid_constant
     }
 }
 
-// common.glsl:16-33
-__device__ constexpr float SH_C0 = 0.28209479177387814f;
-__device__ constexpr float SH_C1 = 0.4886025119029199f;
-__device__ constexpr float SH_C2_0 = 1.0925484305920792f, SH_C2_1 = -1.0925484305920792f, SH_C2_2 = 0.31539156525252005f,
-                           SH_C2_3 = -1.0925484305920792f, SH_C2_4 = 0.5462742152960396f;
-__device__ constexpr float SH_C3_0 = -0.5900435899266435f, SH_C3_1 = 2.890611442640554f, SH_C3_2 = -0.4570457994644658f,
-                           SH_C3_3 = 0.3731763325901154f, SH_C3_4 = -0.4570457994644658f, SH_C3_5 = 1.445305721320277f,
-                           SH_C3_6 = -0.5900435899266435f;
-
 // gsb_uniforms word offsets of the fields the camera gradient has
 constexpr int U_CAMPOS = 0, U_PROJ = 4, U_VIEW = 20, U_TANX = 38, U_TANY = 39;
 // Words of dL/d(UBO) that can be non-zero: camera_position.xyz, proj_mat rows 0, 1, 3, view_mat rows 0-2, tan_fovx / tan_fovy.
@@ -361,7 +352,6 @@ __host__ __device__ constexpr bool cam_word_live(int j) {
 // CAMERA (gsb_render_backward_camera): each thread also accumulates, over its survivors, their share of dL/d(UBO) in the
 // UBO's word layout (fp32), and each CTA writes one fp64 row of partial sums (warp shuffles, then a fixed-order sum over the
 // warps) into P.cam_partials for k_camera_reduce.  The vertex gradient is written only when P.grad_vertices is set.
-// CAMERA = false is the plain reverse pass: its code is the same as before the camera gradient existed.
 template <bool CAMERA>
 __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ BackwardParams P) {
     const uint32_t nv = P.ctl->num_visible;
@@ -393,41 +383,16 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         float* gv = P.grad_vertices + (size_t)i * 60;
         const float px = v[0], py = v[1], pz = v[2];
 
-        // ---- forward of preprocess.comp:130-157 (k_project's expressions) ----
-        const float hx = ((pm[0] * px + pm[4] * py) + pm[8] * pz) + pm[12];
-        const float hy = ((pm[1] * px + pm[5] * py) + pm[9] * pz) + pm[13];
-        const float hw = ((pm[3] * px + pm[7] * py) + pm[11] * pz) + pm[15];
-        const float p_w = 1.0f / hw;
-        const float ndcx = hx * p_w, ndcy = hy * p_w;
-        const float vx = ((vm[0] * px + vm[4] * py) + vm[8] * pz) + vm[12];
-        const float vy = ((vm[1] * px + vm[5] * py) + vm[9] * pz) + vm[13];
-        const float vz = ((vm[2] * px + vm[6] * py) + vm[10] * pz) + vm[14];
-        const float limx = 1.3f * U.tan_fovx, limy = 1.3f * U.tan_fovy;
-        const float txtz = vx / vz, tytz = vy / vz;
-        const float tx = fminf(limx, fmaxf(-limx, txtz)) * vz;
-        const float ty = fminf(limy, fmaxf(-limy, tytz)) * vz;
-        const float focal_x = (float)U.width / (2.0f * U.tan_fovx);
-        const float focal_y = (float)U.height / (2.0f * U.tan_fovy);
-        const float ja = focal_x / vz, jb = focal_y / vz;
-        const float g0 = -(focal_x * tx) / (vz * vz), g1 = -(focal_y * ty) / (vz * vz);
-        float T0[3], T1[3];  // rows of J W (W = the view rotation)
-#pragma unroll
-        for (int r = 0; r < 3; r++) {
-            T0[r] = vm[r * 4 + 0] * ja + vm[r * 4 + 2] * g0;
-            T1[r] = vm[r * 4 + 1] * jb + vm[r * 4 + 2] * g1;
-        }
-        const float4 ca = __ldg(P.cov_a + i);
-        const float2 cb = __ldg(P.cov_b + i);
-        const float S[3][3] = {{ca.x, ca.y, ca.z}, {ca.y, ca.w, cb.x}, {ca.z, cb.x, cb.y}};
-        float ST0[3], ST1[3];
-#pragma unroll
-        for (int k = 0; k < 3; k++) {
-            ST0[k] = (S[k][0] * T0[0] + S[k][1] * T0[1]) + S[k][2] * T0[2];
-            ST1[k] = (S[k][0] * T1[0] + S[k][1] * T1[1]) + S[k][2] * T1[2];
-        }
-        const float a = ((T0[0] * ST0[0] + T0[1] * ST0[1]) + T0[2] * ST0[2]) + 0.3f;
-        const float b = (T1[0] * ST0[0] + T1[1] * ST0[1]) + T1[2] * ST0[2];
-        const float c = ((T1[0] * ST1[0] + T1[1] * ST1[1]) + T1[2] * ST1[2]) + 0.3f;
+        // ---- forward of preprocess.comp:130-157 (k_project's values) ----
+        const ClipView cv = clip_view(U, px, py, pz);
+        const float p_w = cv.p_w, ndcx = cv.ndcx, ndcy = cv.ndcy, vz = cv.vz;
+        const Jacobian J = jacobian(U, cv.vx, cv.vy, vz);
+        const float limx = J.limx, limy = J.limy, txtz = J.txtz, tytz = J.tytz, tx = J.tx, ty = J.ty;
+        const float focal_x = J.focal_x, focal_y = J.focal_y, ja = J.ja, jb = J.jb, g0 = J.g0, g1 = J.g1;
+        const float(&T0)[3] = J.T0, (&T1)[3] = J.T1;  // rows of J W (W = the view rotation)
+        const Cov2d cov = cov2d(T0, T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
+        const float(&ST0)[3] = cov.tm0, (&ST1)[3] = cov.tm1;  // Sigma T0, Sigma T1
+        const float a = cov.m00, b = cov.m10, c = cov.m11;  // b: the [1][0] entry, rounded like k_project's m10
         const float det = a * c - b * b;
 
         // ---- conic = (c, -b, a) / det  ->  cov2d (a, b, c) ----
@@ -476,9 +441,8 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         // ---- colour (preprocess.comp:73-108) -> SH coefficients and the view direction ----
         const float dcr = r2.x > 0.0f ? d[6] : 0.0f;  // :102-104 red clamped at 0 (the record holds the clamped value)
         const float dcg = d[7], dcb = d[8];
-        const float ex = px - U.camera_position[0], ey = py - U.camera_position[1], ez = pz - U.camera_position[2];
-        const float len = sqrtf((ex * ex + ey * ey) + ez * ez);
-        const float x = ex / len, y = ey / len, z = ez / len;
+        float x, y, z;
+        const float len = view_direction(U.camera_position, px, py, pz, x, y, z);
         const float xx = x * x, yy = y * y, zz = z * z;
         const float basis[16] = {SH_C0,
                                  -SH_C1 * y,
@@ -561,15 +525,7 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         const float s[3] = {v[4], v[5], v[6]};
         const float qw = v[8], qx = v[9], qy = v[10], qz = v[11];
         float R[3][3];  // R[c][r] as in k_ingest_cov3d
-        R[0][0] = (1.0f - 2.0f * qy * qy) - 2.0f * qz * qz;
-        R[0][1] = (2.0f * qx) * qy - (2.0f * qz) * qw;
-        R[0][2] = (2.0f * qx) * qz + (2.0f * qy) * qw;
-        R[1][0] = (2.0f * qx) * qy + (2.0f * qz) * qw;
-        R[1][1] = (1.0f - 2.0f * qx * qx) - 2.0f * qz * qz;
-        R[1][2] = (2.0f * qy) * qz - (2.0f * qx) * qw;
-        R[2][0] = (2.0f * qx) * qz - (2.0f * qy) * qw;
-        R[2][1] = (2.0f * qy) * qz + (2.0f * qx) * qw;
-        R[2][2] = (1.0f - 2.0f * qx * qx) - 2.0f * qy * qy;
+        rotation_from_quaternion(qw, qx, qy, qz, R);
         float ds[3] = {0.f, 0.f, 0.f}, dR[3][3];
 #pragma unroll
         for (int r = 0; r < 3; r++) {  // row r of M: M_rc = s_r R[c][r];  dL/dM = 2 M G

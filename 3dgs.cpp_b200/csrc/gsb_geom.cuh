@@ -1,0 +1,106 @@
+// gsb_geom.cuh -- the forward's per-Gaussian geometry (preprocess.comp, precomp_cov3d.comp, common.glsl), stated once: k_project
+// and k_ingest_cov3d compute the frame with it and k_preprocess_backward recomputes the same values, which the reverse pass
+// needs bit for bit.  Every fp32 operation is a single IEEE op (-fmad=false) in the order of the GLSL source.
+#pragma once
+#include <cuda_runtime.h>
+
+#include "gs_b200.h"
+
+namespace gsb {
+
+// common.glsl:16-33
+__device__ constexpr float SH_C0 = 0.28209479177387814f;
+__device__ constexpr float SH_C1 = 0.4886025119029199f;
+__device__ constexpr float SH_C2_0 = 1.0925484305920792f, SH_C2_1 = -1.0925484305920792f, SH_C2_2 = 0.31539156525252005f,
+                           SH_C2_3 = -1.0925484305920792f, SH_C2_4 = 0.5462742152960396f;
+__device__ constexpr float SH_C3_0 = -0.5900435899266435f, SH_C3_1 = 2.890611442640554f, SH_C3_2 = -0.4570457994644658f,
+                           SH_C3_3 = 0.3731763325901154f, SH_C3_4 = -0.4570457994644658f, SH_C3_5 = 1.445305721320277f,
+                           SH_C3_6 = -0.5900435899266435f;
+
+// preprocess.comp:130-134: h = proj (p, 1) (p_w = 1 / h.w, ndc = h.xy p_w) and v = view (p, 1), each
+// mat4 * vec4(p, 1) = ((m0*x + m1*y) + m2*z) + m3*1
+struct ClipView {
+    float p_w, ndcx, ndcy, vx, vy, vz;
+};
+__device__ __forceinline__ ClipView clip_view(const gsb_uniforms& U, float px, float py, float pz) {
+    const float *pm = U.proj_mat, *vm = U.view_mat;
+    const float hx = ((pm[0] * px + pm[4] * py) + pm[8] * pz) + pm[12];
+    const float hy = ((pm[1] * px + pm[5] * py) + pm[9] * pz) + pm[13];
+    const float hw = ((pm[3] * px + pm[7] * py) + pm[11] * pz) + pm[15];
+    ClipView c;
+    c.p_w = 1.0f / hw;
+    c.ndcx = hx * c.p_w, c.ndcy = hy * c.p_w;
+    c.vx = ((vm[0] * px + vm[4] * py) + vm[8] * pz) + vm[12];
+    c.vy = ((vm[1] * px + vm[5] * py) + vm[9] * pz) + vm[13];
+    c.vz = ((vm[2] * px + vm[6] * py) + vm[10] * pz) + vm[14];
+    return c;
+}
+
+// get_projection_jacobian_approx (:34-50), t = clamp(v.xy / v.z, +-1.3 tan_fov) v.z, and the rows of T = J W (:55,:61), W the
+// view rotation: T0[r] = V[r][0]*ja + V[r][2]*g0, T1[r] = V[r][1]*jb + V[r][2]*g1
+struct Jacobian {
+    float limx, limy, txtz, tytz, tx, ty, focal_x, focal_y, ja, jb, g0, g1, T0[3], T1[3];
+};
+__device__ __forceinline__ Jacobian jacobian(const gsb_uniforms& U, float vx, float vy, float vz) {
+    const float* vm = U.view_mat;
+    Jacobian j;
+    j.limx = 1.3f * U.tan_fovx, j.limy = 1.3f * U.tan_fovy;
+    j.txtz = vx / vz, j.tytz = vy / vz;
+    j.tx = fminf(j.limx, fmaxf(-j.limx, j.txtz)) * vz;
+    j.ty = fminf(j.limy, fmaxf(-j.limy, j.tytz)) * vz;
+    j.focal_x = (float)U.width / (2.0f * U.tan_fovx);
+    j.focal_y = (float)U.height / (2.0f * U.tan_fovy);
+    j.ja = j.focal_x / vz, j.jb = j.focal_y / vz;
+    j.g0 = -(j.focal_x * j.tx) / (vz * vz), j.g1 = -(j.focal_y * j.ty) / (vz * vz);
+#pragma unroll
+    for (int r = 0; r < 3; r++) {
+        j.T0[r] = vm[r * 4 + 0] * j.ja + vm[r * 4 + 2] * j.g0;
+        j.T1[r] = vm[r * 4 + 1] * j.jb + vm[r * 4 + 2] * j.g1;
+    }
+    return j;
+}
+
+// cov2d = transpose(T) Sigma T + 0.3 I (:56-65), Sigma = the cov3d words ca.xyzw, cb.xy; tm0 / tm1 = Sigma T0 / Sigma T1 (S[k] =
+// column k).  m01 and m10 round differently, so each caller states its own determinant.
+struct Cov2d {
+    float tm0[3], tm1[3], m00, m01, m10, m11;
+};
+__device__ __forceinline__ Cov2d cov2d(const float (&T0)[3], const float (&T1)[3], float4 ca, float2 cb) {
+    const float S[3][3] = {{ca.x, ca.y, ca.z}, {ca.y, ca.w, cb.x}, {ca.z, cb.x, cb.y}};
+    Cov2d c;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        c.tm0[k] = (T0[0] * S[k][0] + T0[1] * S[k][1]) + T0[2] * S[k][2];
+        c.tm1[k] = (T1[0] * S[k][0] + T1[1] * S[k][1]) + T1[2] * S[k][2];
+    }
+    const float c00 = (c.tm0[0] * T0[0] + c.tm0[1] * T0[1]) + c.tm0[2] * T0[2];
+    const float c01 = (c.tm1[0] * T0[0] + c.tm1[1] * T0[1]) + c.tm1[2] * T0[2];  // [0][1]: col 0, row 1
+    const float c10 = (c.tm0[0] * T1[0] + c.tm0[1] * T1[1]) + c.tm0[2] * T1[2];  // [1][0]
+    const float c11 = (c.tm1[0] * T1[0] + c.tm1[1] * T1[1]) + c.tm1[2] * T1[2];
+    c.m00 = c00 + 0.3f, c.m01 = c01, c.m10 = c10, c.m11 = c11 + 0.3f;
+    return c;
+}
+
+// rotationFromQuaternion, common.glsl:51-75: R[c][r] of the quaternion as stored (not normalised)
+__device__ __forceinline__ void rotation_from_quaternion(float qw, float qx, float qy, float qz, float (&R)[3][3]) {
+    const float qx2 = qx * qx, qy2 = qy * qy, qz2 = qz * qz;
+    R[0][0] = (1.0f - 2.0f * qy2) - 2.0f * qz2;
+    R[0][1] = (2.0f * qx) * qy - (2.0f * qz) * qw;
+    R[0][2] = (2.0f * qx) * qz + (2.0f * qy) * qw;
+    R[1][0] = (2.0f * qx) * qy + (2.0f * qz) * qw;
+    R[1][1] = (1.0f - 2.0f * qx2) - 2.0f * qz2;
+    R[1][2] = (2.0f * qy) * qz - (2.0f * qx) * qw;
+    R[2][0] = (2.0f * qx) * qz - (2.0f * qy) * qw;
+    R[2][1] = (2.0f * qy) * qz + (2.0f * qx) * qw;
+    R[2][2] = (1.0f - 2.0f * qx2) - 2.0f * qy2;
+}
+
+// preprocess.comp:73-78: (x, y, z) = normalize(p - camera_position); returns |p - camera_position|
+__device__ __forceinline__ float view_direction(const float* cam, float px, float py, float pz, float& x, float& y, float& z) {
+    const float dx = px - cam[0], dy = py - cam[1], dz = pz - cam[2];
+    const float len = sqrtf((dx * dx + dy * dy) + dz * dz);
+    x = dx / len, y = dy / len, z = dz / len;
+    return len;
+}
+
+}  // namespace gsb

@@ -17,6 +17,7 @@
 #include <cuda_fp16.h>
 
 #include "gsb_cull.cuh"
+#include "gsb_geom.cuh"
 #include "gsb_internal.cuh"
 
 namespace gsb {
@@ -76,17 +77,6 @@ __device__ __forceinline__ W lookback_exclusive(W* status, uint32_t stride, uint
     return ex;
 }
 
-// common.glsl:16-33
-__device__ constexpr float SH_C0 = 0.28209479177387814f;
-__device__ constexpr float SH_C1 = 0.4886025119029199f;
-__device__ constexpr float SH_C2_0 = 1.0925484305920792f, SH_C2_1 = -1.0925484305920792f,
-                           SH_C2_2 = 0.31539156525252005f, SH_C2_3 = -1.0925484305920792f,
-                           SH_C2_4 = 0.5462742152960396f;
-__device__ constexpr float SH_C3_0 = -0.5900435899266435f, SH_C3_1 = 2.890611442640554f,
-                           SH_C3_2 = -0.4570457994644658f, SH_C3_3 = 0.3731763325901154f,
-                           SH_C3_4 = -0.4570457994644658f, SH_C3_5 = 1.445305721320277f,
-                           SH_C3_6 = -0.5900435899266435f;
-
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); }
 
 struct ShDir {
@@ -144,12 +134,8 @@ __device__ __forceinline__ void sh_group(const float4* __restrict__ sh4, float (
 template <bool SH16>
 __device__ __forceinline__ void compute_sh(const float4* __restrict__ sh4, float px, float py, float pz,
                                            const float* cam, float& r, float& g, float& b) {
-    const float dx = px - cam[0], dy = py - cam[1], dz = pz - cam[2];
-    const float len = sqrtf((dx * dx + dy * dy) + dz * dz);
     ShDir d;
-    d.x = dx / len;
-    d.y = dy / len;
-    d.z = dz / len;
+    view_direction(cam, px, py, pz, d.x, d.y, d.z);
     const float xx = d.x * d.x, yy = d.y * d.y;
     d.w6 = ((2.0f * d.z) * d.z - xx) - yy;
     d.w8 = xx - yy;
@@ -213,52 +199,13 @@ __global__ void __launch_bounds__(PRE_THREADS, GSB_PROJECT_MIN_BLOCKS) k_project
         py = po.y;
         pz = po.z;
         opac = po.w;
-        const float* pm = U.proj_mat;
-        const float* vm = U.view_mat;
-        // :130-134  mat4 * vec4(p, 1): ((m0*x + m1*y) + m2*z) + m3*1
-        const float hx = ((pm[0] * px + pm[4] * py) + pm[8] * pz) + pm[12];
-        const float hy = ((pm[1] * px + pm[5] * py) + pm[9] * pz) + pm[13];
-        const float hw = ((pm[3] * px + pm[7] * py) + pm[11] * pz) + pm[15];
-        const float p_w = 1.0f / hw;
-        const float ndcx = hx * p_w, ndcy = hy * p_w;
-        const float vx = ((vm[0] * px + vm[4] * py) + vm[8] * pz) + vm[12];
-        const float vy = ((vm[1] * px + vm[5] * py) + vm[9] * pz) + vm[13];
-        const float vz = ((vm[2] * px + vm[6] * py) + vm[10] * pz) + vm[14];
+        const ClipView cv = clip_view(U, px, py, pz);
+        const float ndcx = cv.ndcx, ndcy = cv.ndcy, vz = cv.vz;
         if (!(vz <= 0.2f)) {  // :135 (NaN is not culled by the shader's test either)
-            // get_projection_jacobian_approx :34-50
-            const float limx = 1.3f * U.tan_fovx, limy = 1.3f * U.tan_fovy;
-            const float txtz = vx / vz, tytz = vy / vz;
-            const float tx = fminf(limx, fmaxf(-limx, txtz)) * vz;
-            const float ty = fminf(limy, fmaxf(-limy, tytz)) * vz;
-            const float focal_x = (float)U.width / (2.0f * U.tan_fovx);
-            const float focal_y = (float)U.height / (2.0f * U.tan_fovy);
-            const float ja = focal_x / vz, jb = focal_y / vz;
-            const float g0 = -(focal_x * tx) / (vz * vz), g1 = -(focal_y * ty) / (vz * vz);
-            // T = transpose(mat3(view)) * J  (:55,:61): T[0][r] = V[r][0]*ja + V[r][2]*g0, T[1][r] = V[r][1]*jb + V[r][2]*g1
-            float T0[3], T1[3];
-#pragma unroll
-            for (int r = 0; r < 3; r++) {
-                T0[r] = vm[r * 4 + 0] * ja + vm[r * 4 + 2] * g0;
-                T1[r] = vm[r * 4 + 1] * jb + vm[r * 4 + 2] * g1;
-            }
-            const float4 ca = __ldg(P.cov_a + i);
-            const float2 cb = __ldg(P.cov_b + i);
-            // Sigma columns (:56-60): S[0]=(c0,c1,c2) S[1]=(c1,c3,c4) S[2]=(c2,c4,c5)
-            const float S[3][3] = {{ca.x, ca.y, ca.z}, {ca.y, ca.w, cb.x}, {ca.z, cb.x, cb.y}};
-            // tmp = transpose(T) * Sigma: tmp[k][r] = (T_r[0]*S[k][0] + T_r[1]*S[k][1]) + T_r[2]*S[k][2]
-            float tm0[3], tm1[3];
-#pragma unroll
-            for (int k = 0; k < 3; k++) {
-                tm0[k] = (T0[0] * S[k][0] + T0[1] * S[k][1]) + T0[2] * S[k][2];
-                tm1[k] = (T1[0] * S[k][0] + T1[1] * S[k][1]) + T1[2] * S[k][2];
-            }
-            // cov2d = tmp * T (:62): c[c][r] = (tmp[0][r]*T_c[0] + tmp[1][r]*T_c[1]) + tmp[2][r]*T_c[2]
-            const float c00 = (tm0[0] * T0[0] + tm0[1] * T0[1]) + tm0[2] * T0[2];
-            const float c01 = (tm1[0] * T0[0] + tm1[1] * T0[1]) + tm1[2] * T0[2];  // [0][1]: col 0, row 1
-            const float c10 = (tm0[0] * T1[0] + tm0[1] * T1[1]) + tm0[2] * T1[2];  // [1][0]
-            const float c11 = (tm1[0] * T1[0] + tm1[1] * T1[1]) + tm1[2] * T1[2];
-            const float m00 = c00 + 0.3f, m01 = c01, m10 = c10, m11 = c11 + 0.3f;  // :63-65
-            const float det = m00 * m11 - m10 * m01;                               // :138
+            const Jacobian J = jacobian(U, cv.vx, cv.vy, vz);
+            const Cov2d cov = cov2d(J.T0, J.T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
+            const float m00 = cov.m00, m01 = cov.m01, m10 = cov.m10, m11 = cov.m11;
+            const float det = m00 * m11 - m10 * m01;  // :138
             if (!(det <= 0.0f)) {                                                  // :139-141
                 const float ood = 1.0f / det;
                 conx = m11 * ood;

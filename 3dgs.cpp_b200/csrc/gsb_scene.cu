@@ -5,6 +5,7 @@
 // so the result equals the oracle's generic mat3 products (zero terms dropped: x + 0 == x).
 #include <cuda_fp16.h>
 
+#include "gsb_geom.cuh"
 #include "gsb_internal.cuh"
 
 namespace gsb {
@@ -22,19 +23,8 @@ __global__ void __launch_bounds__(256) k_ingest_cov3d(const float4* __restrict__
     const float4 q = v[2];           // rotation: x = w (common.glsl:52-55)
     const uint64_t o = dst_offset + i;
 
-    // rotationFromQuaternion, common.glsl:51-75: R[c][r]
-    const float qx = q.y, qy = q.z, qz = q.w, qw = q.x;
-    const float qx2 = qx * qx, qy2 = qy * qy, qz2 = qz * qz;
     float R[3][3];
-    R[0][0] = (1.0f - 2.0f * qy2) - 2.0f * qz2;
-    R[0][1] = (2.0f * qx) * qy - (2.0f * qz) * qw;
-    R[0][2] = (2.0f * qx) * qz + (2.0f * qy) * qw;
-    R[1][0] = (2.0f * qx) * qy + (2.0f * qz) * qw;
-    R[1][1] = (1.0f - 2.0f * qx2) - 2.0f * qz2;
-    R[1][2] = (2.0f * qy) * qz - (2.0f * qx) * qw;
-    R[2][0] = (2.0f * qx) * qz - (2.0f * qy) * qw;
-    R[2][1] = (2.0f * qy) * qz + (2.0f * qx) * qw;
-    R[2][2] = (1.0f - 2.0f * qx2) - 2.0f * qy2;
+    rotation_from_quaternion(q.x, q.y, q.z, q.w, R);
     // M = S * R  (precomp_cov3d.comp:39), S diagonal => M[c][r] = s_r * R[c][r]
     const float s[3] = {so.x * scale_factor, so.y * scale_factor, so.z * scale_factor};
     float M[3][3];

@@ -123,46 +123,25 @@ def walk_coverage(vtx, u, frame, grad_image):
       max_last (tiles,)     the largest last-contributor list position + 1 over the tile's pixels: where the walk starts
       break_pos (H, W)      list position + 1 of the entry at which the pixel breaks (T' < 1e-4), 0 if it never does
       clamped (n,)          bool: contributor to some pixel with a non-zero upstream gradient at raw alpha > 0.99"""
-    v_all = np.asarray(vtx, np.float32)
-    n = v_all.shape[0]
-    W, H = int(u.width), int(u.height)
-    tiles_x = (W + 15) // 16
-    ranges = frame["ranges"]
-    vals = frame["vals"].astype(np.int64)
-    used = np.unique(vals)
-    local = np.full(n, -1, np.int64)
-    local[used] = np.arange(used.size)
+    v_all, used, local = grad_ref.survivors(vtx, frame)
     with torch.no_grad():
         uv, conic, op, col, _ = grad_ref.preprocess(torch.tensor(v_all[used].astype(np.float64)), u)
     gimg = np.asarray(grad_image)[..., :3]
-    max_last = np.zeros(ranges.shape[0], np.int64)
-    break_pos = np.zeros((H, W), np.int64)
-    clamped = np.zeros(n, bool)
-    for t in range(ranges.shape[0]):
-        s, e = int(ranges[t, 0]), int(ranges[t, 1])
-        if e <= s:
-            continue
-        tx, ty = t % tiles_x, t // tiles_x
-        xs = np.arange(tx * 16, min(W, tx * 16 + 16))
-        ys = np.arange(ty * 16, min(H, ty * 16 + 16))
-        gy, gx = np.meshgrid(ys, xs, indexing="ij")
-        fx, fy = torch.tensor(gx.ravel(), dtype=torch.float64), torch.tensor(gy.ravel(), dtype=torch.float64)
-        idx = torch.tensor(local[vals[s:e]])
+    max_last = np.zeros(frame["ranges"].shape[0], np.int64)
+    break_pos = np.zeros((int(u.height), int(u.width)), np.int64)
+    clamped = np.zeros(v_all.shape[0], bool)
+    for tl in grad_ref.tiles(u, frame, local):
         with torch.no_grad():
-            _, contrib, raw = grad_ref._blend_tile(uv[idx], conic[idx], op[idx], col[idx], fx, fy)
-            c = conic[idx]
-            dx, dy = uv[idx, 0][None, :] - fx[:, None], uv[idx, 1][None, :] - fy[:, None]
-            power = -0.5 * (c[None, :, 0] * dx * dx + c[None, :, 2] * dy * dy) - c[None, :, 1] * dx * dy
-            valid = (power <= 0) & (torch.clamp(raw, max=0.99) >= 1.0 / 255.0)
+            _, contrib, raw, valid = grad_ref.blend_tile(uv[tl.idx], conic[tl.idx], op[tl.idx], col[tl.idx], tl.fx, tl.fy)
         contrib, valid, raw = contrib.numpy(), valid.numpy(), raw.numpy()
         L = contrib.shape[1]
         pos1 = np.arange(1, L + 1)
         last = np.where(contrib, pos1[None, :], 0).max(1)
-        max_last[t] = last.max()
+        max_last[tl.t] = last.max()
         broken = valid & ~contrib  # the break entry and the valid entries behind it
         first_broken = np.where(broken, pos1[None, :], L + 1).min(1)
-        break_pos[gy.ravel(), gx.ravel()] = np.where(first_broken <= L, first_broken, 0)
-        live = (gimg[gy.ravel(), gx.ravel()] != 0).any(1)
+        break_pos[tl.py, tl.px] = np.where(first_broken <= L, first_broken, 0)
+        live = (gimg[tl.py, tl.px] != 0).any(1)
         hit = (contrib & (raw > 0.99) & live[:, None]).any(0)
-        clamped[vals[s:e][hit]] = True
+        clamped[tl.ids[hit]] = True
     return {"max_last": max_last, "break_pos": break_pos, "clamped": clamped}

@@ -1,13 +1,13 @@
 """The camera side of reverse mode, on the CPU: gs_b200.uniforms_torch (the differentiable gsb_uniforms of a pose), the
-UBO pack / unpack helpers, and the camera gradient of the float64 reference (tests/grad_ref_camera.py) that the GPU's
+UBO pack / unpack helpers, and the camera gradient of the float64 reference (tests/grad_ref.py) that the GPU's
 gsb_render_backward_camera is compared against."""
 import numpy as np
 import pytest
 import torch
 
 import grad_ref
-import grad_ref_camera
 import scenes
+from backward_util import translation_identity
 
 
 def _random_poses(n=20, seed=11):
@@ -62,28 +62,13 @@ def test_uniforms_torch_carries_the_restatements_gradient(gs):
         assert torch.allclose(a.grad.double(), b.grad, rtol=1e-6, atol=1e-9)
 
 
-def translation_identity(grad_pos_sum, grad_pos_abs, u, g_ubo):
-    """Moving every Gaussian by delta equals t_view += V3 delta, t_proj += P3 delta, campos -= delta, so
-    sum_i dL/dp_i = V3^T g(view_mat[12..14]) + P3^T g(proj_mat[12, 13, 15]) - g(camera_position).  g_ubo: the 38 float fields.
-    Returns the residual and, per component, the sum of the absolute values of every term."""
-    P = np.asarray(list(u.proj_mat), np.float64).reshape(4, 4).T
-    V = np.asarray(list(u.view_mat), np.float64).reshape(4, 4).T
-    g_c, g_p, g_v = g_ubo[0:3], g_ubo[4:20], g_ubo[20:36]
-    rows = [0, 1, 3]
-    tv = V[:3, :3].T * g_v[12:15][None, :]  # tv[k, r] = V[r, k] g(t_view[r])
-    tp = P[rows, :3].T * g_p[[12, 13, 15]][None, :]
-    rhs = tv.sum(1) + tp.sum(1) - g_c
-    scale = grad_pos_abs + np.abs(tv).sum(1) + np.abs(tp).sum(1) + np.abs(g_c)
-    return grad_pos_sum - rhs, scale
-
-
 def test_reference_camera_gradient_obeys_the_translation_identity(oracle):
     _, vtx, u = scenes.c1()
     oracle.set_exp_mode(0)
     frame, steps = oracle.render_frame_probed(vtx, oracle.cov3d(vtx), u)
     g = np.random.default_rng(5).standard_normal((u.height, u.width, 4)).astype(np.float32)
     g[steps] = 0.0
-    ref = grad_ref_camera.reference(vtx, u, frame, g)
+    ref = grad_ref.reference(vtx, u, frame, g, camera=True)
     gu = ref["grad_ubo"]
     assert gu.shape == (38,) and np.abs(gu).max() > 0
     # the fields the forward does not read, or reads only through step functions, have no gradient
@@ -91,7 +76,7 @@ def test_reference_camera_gradient_obeys_the_translation_identity(oracle):
     gp = ref["grad"][:, 0:3]
     res, scale = translation_identity(gp.sum(0), np.abs(gp).sum(0), u, gu)
     assert (np.abs(res) <= 1e-9 * scale).all(), (res, scale)
-    # the camera restatement differentiates the same function as grad_ref: same vertex gradient and exclusions
+    # with the camera as leaves the reference differentiates the same function: same vertex gradient and exclusions
     plain = grad_ref.reference(vtx, u, frame, g)
     assert np.linalg.norm(plain["grad"] - ref["grad"]) <= 1e-12 * np.linalg.norm(plain["grad"])
     assert np.array_equal(plain["exclude"], ref["exclude"])
@@ -99,13 +84,13 @@ def test_reference_camera_gradient_obeys_the_translation_identity(oracle):
 
 @pytest.mark.parametrize("cam", ["c1", "odd_size", "inside"])
 def test_camera_restatement_is_grad_refs_preprocess(cam):
-    """grad_ref_camera.preprocess with the camera as tensors computes what grad_ref.preprocess computes from the UBO."""
+    """grad_ref.preprocess with the camera as tensors (camera_leaves) computes what it computes from the UBO."""
     _, vtx, _ = scenes.c1()
     u = scenes.camera(cam)
     v = torch.from_numpy(vtx.astype(np.float64))
     with torch.no_grad():
         want = grad_ref.preprocess(v, u)
-        got = grad_ref_camera.preprocess(v, u, grad_ref_camera.camera_leaves(u))
+        got = grad_ref.preprocess(v, u, grad_ref.camera_leaves(u))
     for name, a, b in zip(("uv", "conic", "opacity", "colour", "red"), got, want):
         ok = torch.isfinite(b)
         assert torch.equal(ok, torch.isfinite(a)), name

@@ -1,48 +1,28 @@
-"""The density-control statistics' float64 reference (tests/density_ref.py) and gs_b200.densify_and_prune.  CPU only.
+"""The density-control statistics' float64 reference (grad_ref.density_reference) and gs_b200.densify_and_prune.  CPU only.
 
-density_ref restates grad_ref's blend with per-(pixel, entry) offsets as leaves; summed over pixels its uv gradient must be
-grad_ref's own, and its absolute gradient can only be larger (triangle inequality).  densify_and_prune is checked on a
+density_reference takes grad_ref's blend with per-(pixel, entry) offsets as leaves; summed over pixels its uv gradient must
+be grad_ref's own, and its absolute gradient can only be larger (triangle inequality).  densify_and_prune is checked on a
 hand-built statistics table: which rows clone, split and prune, the source index, and the children's geometry."""
 import numpy as np
 import pytest
 import torch
 
-import density_ref
 import grad_ref
 import scenes
-
-
-def _grad_image(u, steps, seed=7):
-    g = np.random.default_rng(seed).standard_normal((u.height, u.width, 4)).astype(np.float32)
-    g[steps] = 0.0
-    return g
+from backward_util import grad_image
 
 
 def _grad_ref_uv(vtx, u, frame, g):
     """dL/d uv (n, 2) through grad_ref's own tile blend, uv as one float64 leaf (the loop of grad_ref.reference)."""
-    v_all = np.asarray(vtx, np.float32)
-    n = v_all.shape[0]
-    W, H = int(u.width), int(u.height)
-    tiles_x = (W + 15) // 16
-    ranges, vals = frame["ranges"], frame["vals"].astype(np.int64)
-    used = np.unique(vals)
-    local = np.full(n, -1, np.int64)
-    local[used] = np.arange(used.size)
+    v_all, used, local = grad_ref.survivors(vtx, frame)
     with torch.no_grad():
         uv, conic, op, col, _ = grad_ref.preprocess(torch.tensor(v_all[used].astype(np.float64)), u)
     uv = uv.clone().requires_grad_()
     gimg = torch.tensor(np.asarray(g, np.float64)[..., :3])
-    for t in range(ranges.shape[0]):
-        s, e = int(ranges[t, 0]), int(ranges[t, 1])
-        if e <= s:
-            continue
-        tx, ty = t % tiles_x, t // tiles_x
-        gy, gx = np.meshgrid(np.arange(ty * 16, min(H, ty * 16 + 16)), np.arange(tx * 16, min(W, tx * 16 + 16)), indexing="ij")
-        fx, fy = torch.tensor(gx.ravel(), dtype=torch.float64), torch.tensor(gy.ravel(), dtype=torch.float64)
-        idx = torch.tensor(local[vals[s:e]])
-        rgb, _, _ = grad_ref._blend_tile(uv[idx], conic[idx], op[idx], col[idx], fx, fy)
-        (rgb * gimg[gy.ravel(), gx.ravel()]).sum().backward()
-    out = np.zeros((n, 2))
+    for tl in grad_ref.tiles(u, frame, local):
+        rgb = grad_ref.blend_tile(uv[tl.idx], conic[tl.idx], op[tl.idx], col[tl.idx], tl.fx, tl.fy)[0]
+        (rgb * gimg[tl.py, tl.px]).sum().backward()
+    out = np.zeros((v_all.shape[0], 2))
     out[used] = uv.grad.numpy()
     return out
 
@@ -53,8 +33,8 @@ def test_per_pixel_leaves_sum_to_grad_ref(oracle, cam):
     u = scenes.camera(cam)
     oracle.set_exp_mode(0)
     frame, steps = oracle.render_frame_probed(vtx, oracle.cov3d(vtx), u)
-    g = _grad_image(u, steps)
-    ref = density_ref.reference(vtx, u, frame, g)
+    g = grad_image(u, steps)
+    ref = grad_ref.density_reference(vtx, u, frame, g)
     want = _grad_ref_uv(vtx, u, frame, g)
     assert np.abs(want).max() > 0
     err = np.abs(ref["duv"] - want).max()

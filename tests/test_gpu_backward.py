@@ -5,24 +5,15 @@ import pytest
 
 import grad_ref
 import scenes
+from backward_util import GROUPS, expect, grad_image, rel, render
 
 pytestmark = pytest.mark.gpu
-
-GROUPS = {"position": slice(0, 3), "scale": slice(4, 7), "opacity": slice(7, 8), "rotation": slice(8, 12),
-          "sh_dc": slice(12, 15), "sh_rest": slice(15, 60)}
-
 
 @pytest.fixture
 def bctx(gs):
     c = gs.Context(0)
     yield c
     c.close()
-
-
-def _grad_image(u, steps, seed=7):
-    g = np.random.default_rng(seed).standard_normal((u.height, u.width, 4)).astype(np.float32)
-    g[steps] = 0.0
-    return g
 
 
 def _backward(ctx, vtx, g):
@@ -36,15 +27,8 @@ def _backward(ctx, vtx, g):
     return out.cpu().numpy().astype(np.float64)
 
 
-def _rel(a, b):
-    return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-30))
-
-
 def _frame_grad(ctx, vtx, u, g, level=0, mode=0):
-    ctx.set_mode(mode)
-    ctx.set_tile_cull(level)
-    ctx.set_backward(True)
-    ctx.render(u)
+    render(ctx, u, level, mode)
     return _backward(ctx, vtx, g)
 
 
@@ -71,7 +55,7 @@ def test_gradient_matches_float64_reference(oracle, bctx, cam):
     u = scenes.camera(cam)
     oracle.set_exp_mode(0)
     frame, steps = oracle.render_frame_probed(vtx, oracle.cov3d(vtx), u)
-    g = _grad_image(u, steps)
+    g = grad_image(u, steps)
     ref = grad_ref.reference(vtx, u, frame, g)
     bctx.upload(vtx)
     got = _frame_grad(bctx, vtx, u, g)
@@ -79,31 +63,31 @@ def test_gradient_matches_float64_reference(oracle, bctx, cam):
     keep = ~ref["exclude"]
     assert keep.sum() > 100
     for name, cols in GROUPS.items():
-        r = _rel(got[keep, cols], ref["grad"][keep, cols])
+        r = rel(got[keep, cols], ref["grad"][keep, cols])
         assert r <= 1e-3, (cam, name, r)
     assert not got[:, 3].any()  # position.w
 
 
 def test_levels_0_and_1_agree(bctx):
     _, vtx, u = scenes.c1()
-    g = _grad_image(u, np.zeros((u.height, u.width), bool))
+    g = grad_image(u, np.zeros((u.height, u.width), bool))
     bctx.upload(vtx)
     g0 = _frame_grad(bctx, vtx, u, g, level=0)
     g1 = _frame_grad(bctx, vtx, u, g, level=1)
     g2 = _frame_grad(bctx, vtx, u, g, level=2)  # falls back to level 1 while recording
-    assert _rel(g1, g0) <= 1e-6
-    assert _rel(g2, g0) <= 1e-6
+    assert rel(g1, g0) <= 1e-6
+    assert rel(g2, g0) <= 1e-6
 
 
 def test_fast_mode_close_to_exact(oracle, bctx):
     _, vtx, u = scenes.c1()
     oracle.set_exp_mode(0)
     _, steps = oracle.render_frame_probed(vtx, oracle.cov3d(vtx), u)
-    g = _grad_image(u, steps)
+    g = grad_image(u, steps)
     bctx.upload(vtx)
     ge = _frame_grad(bctx, vtx, u, g, mode=0)
     gf = _frame_grad(bctx, vtx, u, g, mode=1)
-    assert _rel(gf, ge) <= 1e-3
+    assert rel(gf, ge) <= 1e-3
 
 
 def test_nothing_visible_gives_zero(bctx):
@@ -112,13 +96,6 @@ def test_nothing_visible_gives_zero(bctx):
     bctx.upload(vtx)
     got = _frame_grad(bctx, vtx, u, np.ones((u.height, u.width, 4), np.float32))
     assert not got.any()
-
-
-def _expect(gs, ctx, code, fn):
-    with pytest.raises(gs.GsbError) as ei:
-        fn()
-    assert ei.value.code == code
-    assert gs.lib.gsb_last_error(ctx.h).decode() != ""
 
 
 def test_error_cases(gs, bctx):
@@ -132,19 +109,19 @@ def test_error_cases(gs, bctx):
     def bw(c):
         return lambda: c.render_backward(v.data_ptr(), gi.data_ptr(), out.data_ptr())
 
-    _expect(gs, bctx, gs.ERR_NO_SCENE, bw(bctx))  # nothing uploaded
+    expect(gs, bctx, gs.ERR_NO_SCENE, bw(bctx))  # nothing uploaded
     bctx.upload(vtx)
-    _expect(gs, bctx, gs.ERR_NO_SCENE, bw(bctx))  # no frame yet
+    expect(gs, bctx, gs.ERR_NO_SCENE, bw(bctx))  # no frame yet
     bctx.set_backward(False)
     bctx.render(u)
-    _expect(gs, bctx, gs.ERR_INVALID, bw(bctx))  # switch off
+    expect(gs, bctx, gs.ERR_INVALID, bw(bctx))  # switch off
     bctx.set_backward(True)
     bctx.render(u, rows=(0, 2))
-    _expect(gs, bctx, gs.ERR_INVALID, bw(bctx))  # a band
+    expect(gs, bctx, gs.ERR_INVALID, bw(bctx))  # a band
     bctx.render(u)
     bctx.render_backward(v.data_ptr(), gi.data_ptr(), out.data_ptr())  # the whole frame: fine
     bctx.upload(vtx)
-    _expect(gs, bctx, gs.ERR_INVALID, bw(bctx))  # uploaded again after the frame
+    expect(gs, bctx, gs.ERR_INVALID, bw(bctx))  # uploaded again after the frame
     # a pipelined frame that overflowed its arena (gsb_render_async never regrows; a fresh context holds N = 10 k instances)
     fresh = gs.Context(0)
     try:
@@ -154,7 +131,7 @@ def test_error_cases(gs, bctx):
         dev = torch.empty((ui.height, ui.width, 4), dtype=torch.float32, device="cuda")
         fresh.render_into(ui, dev.data_ptr(), gs.FORMAT_RGBA32F, sync=False)
         torch.cuda.synchronize()
-        _expect(gs, fresh, gs.ERR_INVALID, bw(fresh))
+        expect(gs, fresh, gs.ERR_INVALID, bw(fresh))
         with pytest.raises(gs.GsbError):
             fresh.stats()  # reports (and clears) the overflow
     finally:
@@ -163,13 +140,13 @@ def test_error_cases(gs, bctx):
     bctx.set_sh_storage(True)
     bctx.upload(vtx)
     bctx.render(u)
-    _expect(gs, bctx, gs.ERR_INVALID, bw(bctx))
+    expect(gs, bctx, gs.ERR_INVALID, bw(bctx))
     # a sharded context (two ranks on one GPU)
     grp = gs.Group([0, 0])
     try:
         c0 = grp.context(0)
-        _expect(gs, c0, gs.ERR_INVALID, lambda: c0.set_backward(True))
-        _expect(gs, c0, gs.ERR_INVALID, bw(c0))
+        expect(gs, c0, gs.ERR_INVALID, lambda: c0.set_backward(True))
+        expect(gs, c0, gs.ERR_INVALID, bw(c0))
     finally:
         grp.close()
 
@@ -221,11 +198,11 @@ def test_render_torch_gradient_is_ordered_on_torchs_stream(gs, bctx):
     import torch
 
     _, vtx, u = scenes.c1()
-    g = _grad_image(u, np.zeros((u.height, u.width), bool))
+    g = grad_image(u, np.zeros((u.height, u.width), bool))
     v = torch.from_numpy(vtx).cuda().requires_grad_()
     img = gs.render_torch(bctx, v, u)
     (img * torch.from_numpy(g).cuda()).sum().backward()
     got = v.grad.cpu().numpy().astype(np.float64)
     want = _backward(bctx, vtx, g)  # the same frame, differentiated again and synchronised
     assert np.abs(want).max() > 0
-    assert _rel(got, want) <= 1e-6
+    assert rel(got, want) <= 1e-6

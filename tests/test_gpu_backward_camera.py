@@ -1,5 +1,5 @@
 """gsb_render_backward_camera / render_torch(..., ubo=) / uniforms_torch: the gradient of a frame with respect to its camera
-matches the float64 restatement of the forward (tests/grad_ref_camera.py), obeys the translation identity at full
+matches the float64 restatement of the forward (tests/grad_ref.py), obeys the translation identity at full
 size, and refines a perturbed camera pose."""
 import math
 
@@ -7,23 +7,13 @@ import numpy as np
 import pytest
 
 import grad_ref
-import grad_ref_camera
 import scenes
-from test_camera_grad import translation_identity
+from backward_util import CAMERA_GROUPS, DEAD, expect, grad_image, rel, render, translation_identity
 
 pytestmark = pytest.mark.gpu
 
+ENTRY = "gsb_render_backward_camera"  # what its error messages start with
 REF_CAMERAS = ("c1", "odd_size", "inside")
-# gsb_uniforms word groups of the camera gradient (the struct as 40 4-byte words; proj_mat at 4, view_mat at 20, column-major)
-GROUPS = {
-    "camera_position": [0, 1, 2],
-    "view_3x3": [20 + c * 4 + r for c in range(3) for r in range(3)],
-    "view_translation": [32, 33, 34],
-    "proj_013x3": [4 + c * 4 + k for c in range(3) for k in (0, 1, 3)],
-    "proj_translation": [16, 17, 19],
-    "tan_fov": [38, 39],
-}
-LIVE = sorted(sum(GROUPS.values(), []))
 # pose refinement: Adam step sizes (position, quaternion) and step count
 POSE_LR_POS, POSE_LR_ROT, POSE_STEPS = 2e-3, 5e-4, 100
 
@@ -63,16 +53,6 @@ def bctx(gs):
     c.close()
 
 
-def _grad_image(u, steps, seed=7):
-    g = np.random.default_rng(seed).standard_normal((u.height, u.width, 4)).astype(np.float32)
-    g[steps] = 0.0
-    return g
-
-
-def _rel(a, b):
-    return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-30))
-
-
 def _camera_backward(ctx, vtx, g, with_vertices=True):
     """gsb_render_backward_camera of the context's last frame: (grad_vertices or None, the 40 words of dL/d(UBO)) in float64."""
     import torch
@@ -97,13 +77,6 @@ def _vertex_backward(ctx, vtx, g):
     return out.cpu().numpy().astype(np.float64)
 
 
-def _render(ctx, u, level=0, mode=0):
-    ctx.set_mode(mode)
-    ctx.set_tile_cull(level)
-    ctx.set_backward(True)
-    ctx.render(u)
-
-
 def _words(gs, floats38):
     w = np.zeros(40)
     w[gs.UBO_FLOAT_WORDS] = floats38
@@ -115,67 +88,59 @@ def test_camera_gradient_matches_float64_reference(gs, oracle, bctx, cam_vtx, ca
     u = scenes.camera(cam)
     oracle.set_exp_mode(0)
     frame, steps = oracle.render_frame_probed(cam_vtx, oracle.cov3d(cam_vtx), u)
-    g = _grad_image(u, steps)
-    ref = grad_ref_camera.reference(cam_vtx, u, frame, g)
+    g = grad_image(u, steps)
+    ref = grad_ref.reference(cam_vtx, u, frame, g, camera=True)
     assert not ref["exclude"].any()
     want = _words(gs, ref["grad_ubo"])
     bctx.upload(cam_vtx)
-    _render(bctx, u)
+    render(bctx, u)
     gv, got = _camera_backward(bctx, cam_vtx, g)
     assert np.isfinite(got).all() and np.isfinite(gv).all()
-    for name, idx in GROUPS.items():
-        r = _rel(got[idx], want[idx])
+    for name, idx in CAMERA_GROUPS.items():
+        r = rel(got[idx], want[idx])
         assert r <= 1e-3, (cam, name, r, got[idx], want[idx])
-    dead = np.setdiff1d(np.arange(40), LIVE)
-    assert not got[dead].any()  # camera_position.w, proj row 2, view row 3, width, height
+    assert not got[DEAD].any()  # camera_position.w, proj row 2, view row 3, width, height
     # the vertex gradient is gsb_render_backward's, and a frozen scene gives the same camera gradient
-    assert _rel(gv, _vertex_backward(bctx, cam_vtx, g)) <= 1e-6
+    assert rel(gv, _vertex_backward(bctx, cam_vtx, g)) <= 1e-6
     _, frozen = _camera_backward(bctx, cam_vtx, g, with_vertices=False)
-    assert _rel(frozen, got) <= 1e-6
+    assert rel(frozen, got) <= 1e-6
 
 
 def test_levels_agree(bctx, cam_vtx):
     u = scenes.camera("c1")
-    g = _grad_image(u, np.zeros((u.height, u.width), bool))
+    g = grad_image(u, np.zeros((u.height, u.width), bool))
     bctx.upload(cam_vtx)
     got = []
     for level in (0, 1, 2):  # 2 falls back to 1 while recording
-        _render(bctx, u, level=level)
+        render(bctx, u, level=level)
         got.append(_camera_backward(bctx, cam_vtx, g)[1])
     assert np.abs(got[0]).max() > 0
-    assert _rel(got[1], got[0]) <= 1e-6
-    assert _rel(got[2], got[0]) <= 1e-6
+    assert rel(got[1], got[0]) <= 1e-6
+    assert rel(got[2], got[0]) <= 1e-6
 
 
 def test_fast_mode_close_to_exact(oracle, bctx, cam_vtx):
     u = scenes.camera("c1")
     oracle.set_exp_mode(0)
     _, steps = oracle.render_frame_probed(cam_vtx, oracle.cov3d(cam_vtx), u)
-    g = _grad_image(u, steps)
+    g = grad_image(u, steps)
     bctx.upload(cam_vtx)
-    _render(bctx, u, mode=0)
+    render(bctx, u, mode=0)
     ge = _camera_backward(bctx, cam_vtx, g)[1]
-    _render(bctx, u, mode=1)
+    render(bctx, u, mode=1)
     gf = _camera_backward(bctx, cam_vtx, g)[1]
-    assert _rel(gf, ge) <= 1e-3
+    assert rel(gf, ge) <= 1e-3
 
 
 def test_nothing_visible_gives_zero(bctx):
     _, vtx, _ = scenes.c1()
     u = scenes.camera("away")
     bctx.upload(vtx)
-    _render(bctx, u)
+    render(bctx, u)
     g = np.ones((u.height, u.width, 4), np.float32)
     gv, gu = _camera_backward(bctx, vtx, g)
     assert not gv.any() and not gu.any()
     assert not _camera_backward(bctx, vtx, g, with_vertices=False)[1].any()
-
-
-def _expect(gs, ctx, code, fn):
-    with pytest.raises(gs.GsbError) as ei:
-        fn()
-    assert ei.value.code == code
-    assert gs.lib.gsb_last_error(ctx.h).decode().startswith("gsb_render_backward_camera")
 
 
 def test_error_cases(gs, bctx):
@@ -191,22 +156,23 @@ def test_error_cases(gs, bctx):
         return lambda: c.render_backward(v.data_ptr(), gi.data_ptr(), out.data_ptr() if vertices else None,
                                          grad_uniforms_ptr=gu.data_ptr())
 
-    _expect(gs, bctx, gs.ERR_NO_SCENE, bw(bctx))  # nothing uploaded
+    expect(gs, bctx, gs.ERR_NO_SCENE, bw(bctx), ENTRY)  # nothing uploaded
     bctx.upload(vtx)
-    _expect(gs, bctx, gs.ERR_NO_SCENE, bw(bctx))  # no frame yet
+    expect(gs, bctx, gs.ERR_NO_SCENE, bw(bctx), ENTRY)  # no frame yet
     bctx.set_backward(False)
     bctx.render(u)
-    _expect(gs, bctx, gs.ERR_INVALID, bw(bctx, vertices=False))  # switch off
+    expect(gs, bctx, gs.ERR_INVALID, bw(bctx, vertices=False), ENTRY)  # switch off
     bctx.set_backward(True)
     bctx.render(u, rows=(0, 2))
-    _expect(gs, bctx, gs.ERR_INVALID, bw(bctx))  # a band
+    expect(gs, bctx, gs.ERR_INVALID, bw(bctx), ENTRY)  # a band
     bctx.render(u)
-    _expect(gs, bctx, gs.ERR_INVALID,  # a NULL grad_uniforms
-            lambda: bctx._ck(gs.lib.gsb_render_backward_camera(bctx.h, v.data_ptr(), gi.data_ptr(), 0, out.data_ptr(), None, None)))
+    expect(gs, bctx, gs.ERR_INVALID,  # a NULL grad_uniforms
+           lambda: bctx._ck(gs.lib.gsb_render_backward_camera(bctx.h, v.data_ptr(), gi.data_ptr(), 0, out.data_ptr(), None, None)),
+           ENTRY)
     bw(bctx)()  # the whole frame: fine
     bw(bctx, vertices=False)()
     bctx.upload(vtx)
-    _expect(gs, bctx, gs.ERR_INVALID, bw(bctx))  # uploaded again after the frame
+    expect(gs, bctx, gs.ERR_INVALID, bw(bctx), ENTRY)  # uploaded again after the frame
     # a pipelined frame that overflowed its arena (gsb_render_async never regrows; a fresh context holds N = 10 k instances)
     fresh = gs.Context(0)
     try:
@@ -216,7 +182,7 @@ def test_error_cases(gs, bctx):
         dev = torch.empty((ui.height, ui.width, 4), dtype=torch.float32, device="cuda")
         fresh.render_into(ui, dev.data_ptr(), gs.FORMAT_RGBA32F, sync=False)
         torch.cuda.synchronize()
-        _expect(gs, fresh, gs.ERR_INVALID, bw(fresh))
+        expect(gs, fresh, gs.ERR_INVALID, bw(fresh), ENTRY)
         with pytest.raises(gs.GsbError):
             fresh.stats()  # reports (and clears) the overflow
     finally:
@@ -225,12 +191,12 @@ def test_error_cases(gs, bctx):
     bctx.set_sh_storage(True)
     bctx.upload(vtx)
     bctx.render(u)
-    _expect(gs, bctx, gs.ERR_INVALID, bw(bctx))
+    expect(gs, bctx, gs.ERR_INVALID, bw(bctx), ENTRY)
     # a sharded context (two ranks on one GPU)
     grp = gs.Group([0, 0])
     try:
         c0 = grp.context(0)
-        _expect(gs, c0, gs.ERR_INVALID, bw(c0))
+        expect(gs, c0, gs.ERR_INVALID, bw(c0), ENTRY)
     finally:
         grp.close()
 
@@ -275,7 +241,7 @@ def test_render_torch_ubo_gradient_is_ordered_on_torchs_stream(gs, bctx, cam_vtx
     import torch
 
     u = scenes.camera("c1")
-    g = _grad_image(u, np.zeros((u.height, u.width), bool))
+    g = grad_image(u, np.zeros((u.height, u.width), bool))
     gt = torch.from_numpy(g).cuda()
     v = torch.from_numpy(cam_vtx).cuda().requires_grad_()
     ubo = torch.from_numpy(gs.pack_uniforms(u)).cuda().requires_grad_()
@@ -285,15 +251,15 @@ def test_render_torch_ubo_gradient_is_ordered_on_torchs_stream(gs, bctx, cam_vtx
     got_u = ubo.grad.cpu().numpy().astype(np.float64)
     want_v, want_u = _camera_backward(bctx, cam_vtx, g)  # the same frame, differentiated again and synchronised
     assert np.abs(want_u).max() > 0
-    assert _rel(got_u, want_u[gs.UBO_FLOAT_WORDS]) <= 1e-6
-    assert _rel(got_v, want_v) <= 1e-6
+    assert rel(got_u, want_u[gs.UBO_FLOAT_WORDS]) <= 1e-6
+    assert rel(got_v, want_v) <= 1e-6
     # frozen vertices: no vertex gradient, the same camera gradient
     vf = torch.from_numpy(cam_vtx).cuda()
     ubo2 = torch.from_numpy(gs.pack_uniforms(u)).cuda().requires_grad_()
     img = gs.render_torch(bctx, vf, u, ubo2)
     (img * gt).sum().backward()
     assert vf.grad is None
-    assert _rel(ubo2.grad.cpu().numpy().astype(np.float64), want_u[gs.UBO_FLOAT_WORDS]) <= 1e-6
+    assert rel(ubo2.grad.cpu().numpy().astype(np.float64), want_u[gs.UBO_FLOAT_WORDS]) <= 1e-6
     # a ubo that needs no gradient renders its camera and differentiates the scene only
     u2 = scenes.camera("odd_size")
     v2 = torch.from_numpy(cam_vtx).cuda().requires_grad_()

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 import scenes
+from backward_util import CAMERA_GROUPS, DEAD, GROUPS, grad_image, rel
 
 pytestmark = pytest.mark.gpu
 
@@ -21,10 +22,8 @@ def _torch():
     return torch
 
 
-def _grad_image(u, seed=7):
-    torch = _torch()
-    g = np.random.default_rng(seed).standard_normal((u.height, u.width, 4)).astype(np.float32)
-    return torch.from_numpy(g).cuda()
+def _grad_image(u):
+    return _torch().from_numpy(grad_image(u)).cuda()
 
 
 def _backward(ctx, v, gi, entry, stream=None):
@@ -171,16 +170,6 @@ def test_levels_bit_for_bit(gs, c1, cam):
         ctx.close()
 
 
-def _rel(a, b):
-    a, b = a.double().cpu().numpy(), b.double().cpu().numpy()
-    return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-30))
-
-
-VERTEX_GROUPS = {"position": slice(0, 3), "scale": slice(4, 7), "opacity": slice(7, 8), "rotation": slice(8, 12),
-                 "sh": slice(12, 60)}
-CAMERA_GROUPS = {"camera_position": slice(0, 3), "proj_mat": slice(4, 20), "view_mat": slice(20, 36), "tan_fov": slice(38, 40)}
-
-
 @pytest.mark.parametrize("mode", [0, 1], ids=["exact", "fast"])
 @pytest.mark.parametrize("scene", ["c1", "garden"])
 def test_close_to_the_atomic_path(gs, request, scene, mode):
@@ -195,15 +184,16 @@ def test_close_to_the_atomic_path(gs, request, scene, mode):
         atom = _backward(ctx, v, gi, "density")
     finally:
         ctx.close()
-    for name, s in VERTEX_GROUPS.items():
+    for name, s in GROUPS.items():
         assert atom["vertices"][:, s].abs().max() > 0, name
-        r = _rel(det["vertices"][:, s], atom["vertices"][:, s])
+        r = rel(det["vertices"][:, s], atom["vertices"][:, s])
         assert r <= 1e-6, (name, r)
     for name, s in CAMERA_GROUPS.items():
-        r = _rel(det["uniforms"][s], atom["uniforms"][s])
+        r = rel(det["uniforms"][s], atom["uniforms"][s])
         assert r <= 1e-6, (name, r)
+    assert not det["uniforms"][DEAD].any() and not atom["uniforms"][DEAD].any()
     for c in (0, 1):
-        r = _rel(det["density"][:, c], atom["density"][:, c])
+        r = rel(det["density"][:, c], atom["density"][:, c])
         assert r <= 1e-6, (c, r)
     for c in (2, 3):
         assert torch.equal(det["density"][:, c], atom["density"][:, c]), c
@@ -284,8 +274,8 @@ def test_render_torch_honours_deterministic_mode(gs, c1):
         # the switch follows torch's setting: outside deterministic mode the result is the atomic path's
         c = _torch_pass(gs, ctx, v, u, g)
         want = _backward(ctx, v, g, "density")  # the same frame again: the context's switch is off now
-        assert _rel(c["vertices"], want["vertices"]) <= 1e-6
-        assert _rel(c["density"][:, :2], want["density"][:, :2]) <= 1e-6
+        assert rel(c["vertices"], want["vertices"]) <= 1e-6
+        assert rel(c["density"][:, :2], want["density"][:, :2]) <= 1e-6
         assert torch.equal(c["density"][:, 2:], want["density"][:, 2:])
         # and inside it, the deterministic words of gsb_render_backward_density
         ctx.set_backward_deterministic(True)

@@ -13,17 +13,12 @@ from pathlib import Path
 import numpy as np
 import pytest
 
-import density_ref
 import grad_ref
-import grad_ref_camera
 import stress_scene
-from test_gpu_backward_camera import GROUPS as CAMERA_GROUPS
-from test_gpu_backward_camera import LIVE as CAMERA_LIVE
+from backward_util import CAMERA_GROUPS, DEAD, GROUPS, grad_image, rel
 
 pytestmark = pytest.mark.gpu
 
-GROUPS = {"position": slice(0, 3), "scale": slice(4, 7), "opacity": slice(7, 8), "rotation": slice(8, 12),
-          "sh_dc": slice(12, 15), "sh_rest": slice(15, 60)}
 # Measured on an H100 80GB HBM3 (700 W limit), over all Gaussians of both paths and levels: the largest ||got_i - ref_i|| is
 # 3.3e-4 ||ref_i|| among the rows above a tenth of the 99th percentile, and 2.1e-4 x the 99th percentile among all rows
 # (the stress scene's position and scale, the garden band's density column 0).  With these two the largest
@@ -38,16 +33,6 @@ def _torch():
     import torch
 
     return torch
-
-
-def _grad_image(u, steps, seed=7):
-    g = np.random.default_rng(seed).standard_normal((u.height, u.width, 4)).astype(np.float32)
-    g[steps] = 0.0
-    return g
-
-
-def _rel(a, b):
-    return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-30))
 
 
 def _atol(ref, rows, cols):
@@ -72,12 +57,12 @@ def _check_vertices(got, ref, keep, sets, what):
     worst = {}
     for name, cols in GROUPS.items():
         atol = _atol(ref, keep, cols)
-        r = _rel(got[keep, cols], ref[keep, cols])
+        r = rel(got[keep, cols], ref[keep, cols])
         assert r <= 1e-3, (what, name, r)
         worst[name] = _row_ratio(got, ref, keep, cols, atol)
         for sname, rows in sets.items():
             if np.linalg.norm(ref[rows][:, cols]) > 0:
-                rs = _rel(got[rows][:, cols], ref[rows][:, cols])
+                rs = rel(got[rows][:, cols], ref[rows][:, cols])
                 assert rs <= 1e-3, (what, sname, name, rs)
             worst[f"{sname}/{name}"] = _row_ratio(got, ref, rows, cols, atol)
     print(what, "max per-Gaussian error / tolerance:", {k: f"{v:.3g}" for k, v in worst.items()})
@@ -93,7 +78,7 @@ def _check_density(got, ref, keep, what):
     worst = {}
     for c in (0, 1):
         want = ref["density"][:, c:c + 1]
-        r = _rel(got[keep, c], want[keep, 0])
+        r = rel(got[keep, c], want[keep, 0])
         assert r <= 1e-3, (what, c, r)
         worst[c] = _row_ratio(got[:, c:c + 1], want, keep, slice(0, 1), _atol(want, keep, slice(0, 1)))
     print(what, "density: max per-Gaussian error / tolerance:", {k: f"{v:.3g}" for k, v in worst.items()})
@@ -141,21 +126,21 @@ def stress(oracle):
         u = stress_scene.camera(cam)
         oracle.set_exp_mode(0)
         frame, steps = oracle.render_frame_probed(vtx, oracle.cov3d(vtx), u)
-        g = _grad_image(u, steps)
+        g = grad_image(u, steps)
         ref = grad_ref.reference(vtx, u, frame, g)
         keep = ~ref["exclude"]
         survivor = frame["attr"]["color_radii"][:, 3] != 0
         sets = {"clamped_alpha": keep & stress_scene.walk_coverage(vtx, u, frame, g)["clamped"],
                 "red_below_0": keep & survivor & (stress_scene.red(vtx, u) < 0),
                 "fov_clamped": keep & survivor & stress_scene.fov_clamped(vtx, u)}
-        return {"u": u, "g": g, "ref": ref, "keep": keep, "sets": sets, "density": density_ref.reference(vtx, u, frame, g)}
+        return {"u": u, "g": g, "ref": ref, "keep": keep, "sets": sets, "density": grad_ref.density_reference(vtx, u, frame, g)}
 
     return vtx, at
 
 
 @pytest.fixture(scope="module")
 def stress_camera(oracle):
-    """stress_scene.camera_vertices() and, once per camera, its upstream gradient and grad_ref_camera's reference."""
+    """stress_scene.camera_vertices() and, once per camera, its upstream gradient and grad_ref's camera reference."""
     vtx = stress_scene.camera_vertices()
 
     @functools.lru_cache(maxsize=None)
@@ -163,8 +148,8 @@ def stress_camera(oracle):
         u = stress_scene.camera(cam)
         oracle.set_exp_mode(0)
         frame, steps = oracle.render_frame_probed(vtx, oracle.cov3d(vtx), u)
-        g = _grad_image(u, steps)
-        return {"u": u, "g": g, "ref": grad_ref_camera.reference(vtx, u, frame, g)}
+        g = grad_image(u, steps)
+        return {"u": u, "g": g, "ref": grad_ref.reference(vtx, u, frame, g, camera=True)}
 
     return vtx, at
 
@@ -205,11 +190,11 @@ def test_camera_gradient_matches_reference(gs, stress_camera, cam, level, path):
     _, _, got = _backward(gs, vtx, r["u"], r["g"], level=level, deterministic=PATHS[path], camera=True)
     got = got.astype(np.float64)
     assert np.isfinite(got).all()
-    rels = {name: _rel(got[idx], want[idx]) for name, idx in CAMERA_GROUPS.items()}
+    rels = {name: rel(got[idx], want[idx]) for name, idx in CAMERA_GROUPS.items()}
     print((cam, level, path), "camera gradient relative error:", {k: f"{v:.3g}" for k, v in rels.items()})
     for name, r_ in rels.items():
         assert r_ <= 1e-3, (cam, level, path, name, r_)
-    assert not got[np.setdiff1d(np.arange(40), CAMERA_LIVE)].any()
+    assert not got[DEAD].any()
 
 
 @pytest.mark.parametrize("cam", stress_scene.CAMERAS)
@@ -221,10 +206,10 @@ def test_fast_mode_close_to_exact(gs, stress, cam):
     keep = r["keep"]
     gf, ge, df, de = (a.astype(np.float64) for a in (gf, ge, df, de))
     for name, cols in GROUPS.items():
-        rel = _rel(gf[keep, cols], ge[keep, cols])
-        assert rel <= 1e-3, (cam, name, rel)
+        err = rel(gf[keep, cols], ge[keep, cols])
+        assert err <= 1e-3, (cam, name, err)
     for c in (0, 1):
-        assert _rel(df[keep, c], de[keep, c]) <= 1e-3, (cam, c)
+        assert rel(df[keep, c], de[keep, c]) <= 1e-3, (cam, c)
 
 
 @pytest.fixture(scope="module")
@@ -247,7 +232,7 @@ def garden_band(gs, oracle):
     g[y0:y1] = np.random.default_rng(11).standard_normal((y1 - y0, u.width, 4))
     g[steps] = 0.0
     ref = grad_ref.reference(vtx, u, frame, g)
-    dens = density_ref.reference(vtx, u, frame, g)
+    dens = grad_ref.density_reference(vtx, u, frame, g)
     used = np.zeros(vtx.shape[0], bool)
     used[np.unique(frame["vals"])] = True
     print("garden band: tile rows", rows, "instances", frame["m"], "Gaussians in the band", int(used.sum()),

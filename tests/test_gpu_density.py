@@ -1,15 +1,16 @@
 """gsb_render_backward_density / render_torch(..., density=) / densify_and_prune: the per-Gaussian statistics of adaptive
-density control match the float64 reference (tests/density_ref.py) and the oracle's survivors and radii, accumulate over
+density control match the float64 reference (tests/grad_ref.py) and the oracle's survivors and radii, accumulate over
 frames, leave the gradients of the other two entries unchanged, and let a sparse scene grow while it trains."""
 import numpy as np
 import pytest
 
-import density_ref
 import grad_ref
 import scenes
+from backward_util import expect, grad_image, rel, render
 
 pytestmark = pytest.mark.gpu
 
+ENTRY = "gsb_render_backward_density"  # what its error messages start with
 REF_CAMERAS = ("c1", "odd_size", "inside")
 
 
@@ -18,23 +19,6 @@ def bctx(gs):
     c = gs.Context(0)
     yield c
     c.close()
-
-
-def _grad_image(u, steps, seed=7):
-    g = np.random.default_rng(seed).standard_normal((u.height, u.width, 4)).astype(np.float32)
-    g[steps] = 0.0
-    return g
-
-
-def _rel(a, b):
-    return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-30))
-
-
-def _render(ctx, u, level=0, mode=0):
-    ctx.set_mode(mode)
-    ctx.set_tile_cull(level)
-    ctx.set_backward(True)
-    ctx.render(u)
 
 
 def _density_backward(ctx, vtx, g, density=None, vertices=True, camera=False):
@@ -58,12 +42,12 @@ def _density_backward(ctx, vtx, g, density=None, vertices=True, camera=False):
 
 
 def _frame_density(ctx, vtx, u, g, level=0, mode=0):
-    _render(ctx, u, level, mode)
+    render(ctx, u, level, mode)
     return _density_backward(ctx, vtx, g)[0]
 
 
 def _same_stats(a, b, tol):
-    assert _rel(a[:, 0], b[:, 0]) <= tol and _rel(a[:, 1], b[:, 1]) <= tol
+    assert rel(a[:, 0], b[:, 0]) <= tol and rel(a[:, 1], b[:, 1]) <= tol
     assert np.array_equal(a[:, 2], b[:, 2]) and np.array_equal(a[:, 3], b[:, 3])
 
 
@@ -73,15 +57,15 @@ def test_density_matches_float64_reference(oracle, bctx, cam):
     u = scenes.camera(cam)
     oracle.set_exp_mode(0)
     frame, steps = oracle.render_frame_probed(vtx, oracle.cov3d(vtx), u)
-    g = _grad_image(u, steps)
-    ref = density_ref.reference(vtx, u, frame, g)
+    g = grad_image(u, steps)
+    ref = grad_ref.density_reference(vtx, u, frame, g)
     keep = ~grad_ref.reference(vtx, u, frame, g)["exclude"]
     bctx.upload(vtx)
     got = _frame_density(bctx, vtx, u, g)
     assert np.isfinite(got).all()
     assert keep.sum() > 100 and got[keep, 0].max() > 0
     for c in (0, 1):
-        r = _rel(got[keep, c], ref["density"][keep, c])
+        r = rel(got[keep, c], ref["density"][keep, c])
         assert r <= 1e-3, (cam, c, r)
     assert np.array_equal(got[:, 2], ref["survivor"].astype(np.float64))
     assert np.array_equal(got[:, 3].astype(np.float32).view(np.uint32), ref["radii"].astype(np.float32).view(np.uint32))
@@ -95,7 +79,7 @@ def test_density_accumulates_over_frames(gs, bctx):
     frames = []
     for i, cam in enumerate(REF_CAMERAS):
         u = scenes.camera(cam)
-        frames.append((u, _grad_image(u, np.zeros((u.height, u.width), bool), seed=i)))
+        frames.append((u, grad_image(u, np.zeros((u.height, u.width), bool), seed=i)))
     single = []
     for u, g in frames:  # each frame alone, each on a fresh context
         c = gs.Context(0)
@@ -107,11 +91,11 @@ def test_density_accumulates_over_frames(gs, bctx):
     acc = torch.zeros((n, 4), dtype=torch.float32, device="cuda")
     bctx.upload(vtx)
     for u, g in frames:  # one context, one buffer: its abs scratch must be back at zero after every call
-        _render(bctx, u)
+        render(bctx, u)
         _density_backward(bctx, vtx, g, density=acc)
     got = acc.cpu().numpy().astype(np.float64)
     want01 = sum(s[:, :2] for s in single)
-    assert _rel(got[:, 0], want01[:, 0]) <= 1e-6 and _rel(got[:, 1], want01[:, 1]) <= 1e-6
+    assert rel(got[:, 0], want01[:, 0]) <= 1e-6 and rel(got[:, 1], want01[:, 1]) <= 1e-6
     assert np.array_equal(got[:, 2], sum(s[:, 2] for s in single))
     assert got[:, 2].max() == 3
     assert np.array_equal(got[:, 3], np.maximum.reduce([s[:, 3] for s in single]))
@@ -121,9 +105,9 @@ def test_gradient_outputs_are_the_other_entries(bctx):
     import torch
 
     _, vtx, u = scenes.c1()
-    g = _grad_image(u, np.zeros((u.height, u.width), bool))
+    g = grad_image(u, np.zeros((u.height, u.width), bool))
     bctx.upload(vtx)
-    _render(bctx, u)
+    render(bctx, u)
     v = torch.from_numpy(vtx).cuda()
     gi = torch.from_numpy(g).cuda()
     want_v = torch.empty_like(v)
@@ -134,18 +118,18 @@ def test_gradient_outputs_are_the_other_entries(bctx):
     want_v, want_u = want_v.cpu().numpy().astype(np.float64), want_u.cpu().numpy().astype(np.float64)
     assert np.abs(want_v).max() > 0 and np.abs(want_u).max() > 0
     d_both, gv, gu = _density_backward(bctx, vtx, g, vertices=True, camera=True)
-    assert _rel(gv, want_v) <= 1e-6 and _rel(gu, want_u) <= 1e-6
+    assert rel(gv, want_v) <= 1e-6 and rel(gu, want_u) <= 1e-6
     d_v, gv, gu = _density_backward(bctx, vtx, g, vertices=True, camera=False)
-    assert gu is None and _rel(gv, want_v) <= 1e-6
+    assert gu is None and rel(gv, want_v) <= 1e-6
     d_u, gv, gu = _density_backward(bctx, vtx, g, vertices=False, camera=True)
-    assert gv is None and _rel(gu, want_u) <= 1e-6
+    assert gv is None and rel(gu, want_u) <= 1e-6
     for d in (d_v, d_u):
         _same_stats(d, d_both, 1e-6)
 
 
 def test_levels_agree(bctx):
     _, vtx, u = scenes.c1()
-    g = _grad_image(u, np.zeros((u.height, u.width), bool))
+    g = grad_image(u, np.zeros((u.height, u.width), bool))
     bctx.upload(vtx)
     d0 = _frame_density(bctx, vtx, u, g, level=0)
     d1 = _frame_density(bctx, vtx, u, g, level=1)
@@ -159,7 +143,7 @@ def test_fast_mode_close_to_exact(oracle, bctx):
     _, vtx, u = scenes.c1()
     oracle.set_exp_mode(0)
     _, steps = oracle.render_frame_probed(vtx, oracle.cov3d(vtx), u)
-    g = _grad_image(u, steps)
+    g = grad_image(u, steps)
     bctx.upload(vtx)
     de = _frame_density(bctx, vtx, u, g, mode=0)
     df = _frame_density(bctx, vtx, u, g, mode=1)
@@ -172,13 +156,6 @@ def test_nothing_visible_leaves_the_buffer_zero(bctx):
     bctx.upload(vtx)
     got = _frame_density(bctx, vtx, u, np.ones((u.height, u.width, 4), np.float32))
     assert not got.any()
-
-
-def _expect(gs, ctx, code, fn):
-    with pytest.raises(gs.GsbError) as ei:
-        fn()
-    assert ei.value.code == code
-    assert gs.lib.gsb_last_error(ctx.h).decode().startswith("gsb_render_backward_density")
 
 
 def test_error_cases(gs, bctx):
@@ -196,21 +173,21 @@ def test_error_cases(gs, bctx):
     def bw(c):
         return raw(c, out.data_ptr(), None, dens.data_ptr())
 
-    _expect(gs, bctx, gs.ERR_NO_SCENE, bw(bctx))  # nothing uploaded
+    expect(gs, bctx, gs.ERR_NO_SCENE, bw(bctx), ENTRY)  # nothing uploaded
     bctx.upload(vtx)
-    _expect(gs, bctx, gs.ERR_NO_SCENE, bw(bctx))  # no frame yet
+    expect(gs, bctx, gs.ERR_NO_SCENE, bw(bctx), ENTRY)  # no frame yet
     bctx.set_backward(False)
     bctx.render(u)
-    _expect(gs, bctx, gs.ERR_INVALID, bw(bctx))  # switch off
+    expect(gs, bctx, gs.ERR_INVALID, bw(bctx), ENTRY)  # switch off
     bctx.set_backward(True)
     bctx.render(u, rows=(0, 2))
-    _expect(gs, bctx, gs.ERR_INVALID, bw(bctx))  # a band
+    expect(gs, bctx, gs.ERR_INVALID, bw(bctx), ENTRY)  # a band
     bctx.render(u)
-    _expect(gs, bctx, gs.ERR_INVALID, raw(bctx, out.data_ptr(), None, None))  # a NULL density
-    _expect(gs, bctx, gs.ERR_INVALID, raw(bctx, None, None, dens.data_ptr()))  # no gradient output
+    expect(gs, bctx, gs.ERR_INVALID, raw(bctx, out.data_ptr(), None, None), ENTRY)  # a NULL density
+    expect(gs, bctx, gs.ERR_INVALID, raw(bctx, None, None, dens.data_ptr()), ENTRY)  # no gradient output
     bw(bctx)()  # the whole frame: fine
     bctx.upload(vtx)
-    _expect(gs, bctx, gs.ERR_INVALID, bw(bctx))  # uploaded again after the frame
+    expect(gs, bctx, gs.ERR_INVALID, bw(bctx), ENTRY)  # uploaded again after the frame
     # a pipelined frame that overflowed its arena (gsb_render_async never regrows; a fresh context holds N = 10 k instances)
     fresh = gs.Context(0)
     try:
@@ -220,7 +197,7 @@ def test_error_cases(gs, bctx):
         dev = torch.empty((ui.height, ui.width, 4), dtype=torch.float32, device="cuda")
         fresh.render_into(ui, dev.data_ptr(), gs.FORMAT_RGBA32F, sync=False)
         torch.cuda.synchronize()
-        _expect(gs, fresh, gs.ERR_INVALID, bw(fresh))
+        expect(gs, fresh, gs.ERR_INVALID, bw(fresh), ENTRY)
         with pytest.raises(gs.GsbError):
             fresh.stats()  # reports (and clears) the overflow
     finally:
@@ -229,12 +206,12 @@ def test_error_cases(gs, bctx):
     bctx.set_sh_storage(True)
     bctx.upload(vtx)
     bctx.render(u)
-    _expect(gs, bctx, gs.ERR_INVALID, bw(bctx))
+    expect(gs, bctx, gs.ERR_INVALID, bw(bctx), ENTRY)
     # a sharded context (two ranks on one GPU)
     grp = gs.Group([0, 0])
     try:
         c0 = grp.context(0)
-        _expect(gs, c0, gs.ERR_INVALID, bw(c0))
+        expect(gs, c0, gs.ERR_INVALID, bw(c0), ENTRY)
     finally:
         grp.close()
 
@@ -280,7 +257,7 @@ def test_render_torch_density_equals_the_context_call(gs, bctx):
     import torch
 
     _, vtx, u = scenes.c1()
-    g = torch.from_numpy(_grad_image(u, np.zeros((u.height, u.width), bool))).cuda()
+    g = torch.from_numpy(grad_image(u, np.zeros((u.height, u.width), bool))).cuda()
     v = torch.from_numpy(vtx).cuda().requires_grad_()
     dens = torch.zeros((v.shape[0], 4), dtype=torch.float32, device="cuda")
     img = gs.render_torch(bctx, v, u, density=dens)
@@ -289,7 +266,7 @@ def test_render_torch_density_equals_the_context_call(gs, bctx):
     want, want_v, _ = _density_backward(bctx, vtx, g.cpu().numpy())  # the same frame, again, into a zeroed buffer
     assert got[:, 0].max() > 0
     _same_stats(got, want, 1e-6)
-    assert _rel(v.grad.cpu().numpy().astype(np.float64), want_v) <= 1e-6
+    assert rel(v.grad.cpu().numpy().astype(np.float64), want_v) <= 1e-6
     with pytest.raises(ValueError):
         gs.render_torch(bctx, v, u, density=torch.zeros((3, 4), device="cuda"))
 
