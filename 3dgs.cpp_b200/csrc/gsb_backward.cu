@@ -615,24 +615,20 @@ cudaError_t launch_det_sums(const BackwardParams& p, const DetBackward& d, unsig
     if ((e = cudaMemsetAsync(d.status, 0, (size_t)d.status_tiles * 256 * sizeof(unsigned long long), s)) != cudaSuccess) return e;
     k_det_prepare<<<grid, PB_THREADS, 0, s>>>(p.vals, p.ctl, d.keys[0], d.pos[0], d.runs);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    SortParams sp{};
+    SortParams sp;
     sp.keys[0] = d.keys[0];
     sp.keys[1] = d.keys[1];
     sp.vals[0] = d.pos[0];
     sp.vals[1] = d.pos[1];
-    sp.key_bytes = 4;
     sp.d_m = &p.ctl->num_instances;
     sp.m_hint = d.m_hint;
     sp.key_bits = d.key_bits;
     sp.status = d.status;
     sp.status_tiles = d.status_tiles;
-    sp.d_epoch = nullptr;
     sp.epoch_base = 1;
     sp.sc = d.sc;
     sp.num_sms = p.num_sms;
-    sp.events = nullptr;
     sp.ranges = d.runs;  // the last pass: (start, ~end) of each compact id's run
-    sp.range_key_mask = 0;
     sp.discard_sorted_keys = true;
     uint32_t passes = 0;
     if ((e = launch_sort(sp, &passes, s)) != cudaSuccess) return e;

@@ -3,22 +3,93 @@
 #pragma once
 #include <algorithm>
 #include <string>
+#include <utility>
 
 #include "gsb_internal.cuh"
 
 namespace gsb {
 struct ShardState;  // gsb_shard.cu
+
+template <typename T>
+cudaError_t dev_alloc(T** p, size_t count) {
+    return cudaMalloc(reinterpret_cast<void**>(p), std::max<size_t>(count, 1) * sizeof(T));
 }
+
+// A device array owned by a context: freed with it or by reset(), and grown, never shrunk, by grow().  Memory is given back
+// only then: a smaller scene upload, for one, keeps the larger buffers.  Moving an array (`group = {}` frees a struct of
+// them) leaves the source empty.
+template <typename T>
+struct DevArray {
+    T* p = nullptr;
+    uint64_t count = 0;  // elements asked for by the last grow() that allocated
+
+    DevArray() = default;
+    DevArray(const DevArray&) = delete;
+    DevArray& operator=(DevArray&& o) noexcept {
+        if (this != &o) {
+            reset();
+            p = std::exchange(o.p, nullptr);
+            count = std::exchange(o.count, 0);
+        }
+        return *this;
+    }
+    ~DevArray() { reset(); }
+    operator T*() const { return p; }
+
+    // cudaFree waits for all work on the device
+    void reset() {
+        if (p) cudaFree(p);
+        p = nullptr;
+        count = 0;
+    }
+    // Room for n elements: unless that many are allocated, frees, then allocates max(n, 1).  A failed allocation leaves the
+    // array empty (count 0), so that the next call tries again.
+    cudaError_t grow(uint64_t n) {
+        if (p && n <= count) return cudaSuccess;
+        reset();
+        const cudaError_t e = dev_alloc(&p, n);
+        if (e != cudaSuccess) p = nullptr;
+        else count = n;
+        return e;
+    }
+};
+
+// The survivor arrays the middle of a frame and the blend read: the context's own, or on a sharded context the band's
+// (the exchange buffers of the frame's parity and the destination-side sort arrays of ShardState).
+struct Survivors {
+    const float4* recs;
+    uint32_t* dkeys[2];  // Gaussian-level sort: depth bits
+    uint32_t* dvals[2];  //                       compact ids
+    unsigned long long* emit_status;  // k_emit look-back words
+    bool operator==(const Survivors& o) const {
+        return recs == o.recs && dkeys[0] == o.dkeys[0] && dkeys[1] == o.dkeys[1] && dvals[0] == o.dvals[0] && dvals[1] == o.dvals[1] &&
+               emit_status == o.emit_status;
+    }
+};
+
+// gsb_set_backward_deterministic: the buffers behind DetBackward, allocated on first deterministic use, grown with the arena
+// and the scene, and freed with bw_record.
+struct DetBuffers {
+    DevArray<double> slots;  // 11 fp64 per arena entry (the blend's per-(tile, entry) partials)
+    DevArray<uint32_t> keys[2];
+    DevArray<uint32_t> pos[2];
+    DevArray<unsigned long long> status;
+    DevArray<SortCtl> sc;
+    DevArray<uint2> runs;    // n (start, ~end) runs, one per possible survivor
+};
+}  // namespace gsb
 using gsb::Control;
+using gsb::DevArray;
 
 // Captured CUDA graph of the "middle" of a frame (depth sort, key emission, tile sort: 9-10 kernels whose arguments do
 // not depend on the camera).  Replaces recordRenderCommandBuffer's pre-recorded command buffer (src/Renderer.cpp:532-717).
 struct MiddleKey {
-    uint32_t tiles_x = 0, num_tiles = 0, nv_q = 0, m_q = 0, cull = 0, tag = 0, cs = 0;
+    uint32_t tiles_x = 0, num_tiles = 0, nv_q = 0, m_q = 0, cull = 0, cs = 0;
     uint64_t alloc_gen = 0;
+    gsb::Survivors sv{};  // the survivor arrays the graph reads (on a sharded context they depend on the frame's parity)
     bool operator==(const MiddleKey& o) const {
-        return tiles_x == o.tiles_x && num_tiles == o.num_tiles && nv_q == o.nv_q && m_q == o.m_q && cull == o.cull && tag == o.tag &&
-               cs == o.cs && alloc_gen == o.alloc_gen;
+        return tiles_x == o.tiles_x && num_tiles == o.num_tiles && nv_q == o.nv_q && m_q == o.m_q && cull == o.cull && cs == o.cs &&
+               alloc_gen == o.alloc_gen && sv == o.sv;
     }
 };
 struct MiddleGraph {
@@ -36,31 +107,27 @@ struct gsb_ctx {
 
     // scene
     uint64_t n = 0;
-    float4* pos_op = nullptr;
-    float4* cov_a = nullptr;
-    float2* cov_b = nullptr;
-    float* sh = nullptr;        // [n][48] fp32, or [n][48] fp16 when sh_half
+    DevArray<float4> pos_op;
+    DevArray<float4> cov_a;
+    DevArray<float2> cov_b;
+    DevArray<float> sh;         // [n][48] fp32, or [n][48] fp16 when sh_half
     bool sh_half = false;       // gsb_set_sh_storage(1): takes effect at the next gsb_scene_upload
     bool scene_sh_half = false; // storage of the uploaded scene
 
     // frame state
     Control* ctl = nullptr;
     Control* ctl_host = nullptr;  // pinned mirror, filled at the end of each frame
-    uint32_t* project_status = nullptr;        // k_project look-back words (one per 256-Gaussian chunk)
-    unsigned long long* emit_status = nullptr;  // k_emit look-back words
-    float4* recs = nullptr;
-    uint32_t* dkeys[2] = {nullptr, nullptr};  // Gaussian-level sort: depth bits
-    uint32_t* dvals[2] = {nullptr, nullptr};  //                       compact ids
+    DevArray<uint32_t> project_status;        // k_project look-back words (one per 256-Gaussian chunk)
+    DevArray<unsigned long long> emit_status;  // k_emit look-back words
+    DevArray<float4> recs;
+    DevArray<uint32_t> dkeys[2];  // Gaussian-level sort: depth bits
+    DevArray<uint32_t> dvals[2];  //                       compact ids
     uint64_t capacity = 0;
-    uint32_t* keys[2] = {nullptr, nullptr};   // instance-level sort: tile ids
-    uint32_t* vals[2] = {nullptr, nullptr};   //                      compact ids
-    unsigned long long* sort_status = nullptr;
-    uint32_t sort_status_tiles = 0;
-    uint32_t epoch = 8;
-    uint2* ranges = nullptr;
-    uint32_t ranges_tiles = 0;
-    void* fb = nullptr;
-    size_t fb_bytes = 0;
+    DevArray<uint32_t> keys[2];   // instance-level sort: tile ids (capacity + 16 entries)
+    DevArray<uint32_t> vals[2];   //                      compact ids
+    DevArray<unsigned long long> sort_status;  // [tiles][256] look-back words of the frame's sorts
+    DevArray<uint2> ranges;
+    DevArray<unsigned char> fb;   // staging frame of gsb_render to pageable host memory
 
     int mode = GSB_MODE_EXACT;
     bool debug = false;
@@ -85,37 +152,23 @@ struct gsb_ctx {
     uint32_t regrow_count = 0;
 
     // description of the last frame (for stats / debug download)
-    uint32_t last_w = 0, last_h = 0, last_tiles_x = 0, last_tiles_y = 0, last_passes = 0, last_depth_passes = 0, last_final = 0;
+    uint32_t last_tiles_x = 0, last_tiles_y = 0, last_passes = 0, last_depth_passes = 0, last_final = 0;
 
     // debug copies
-    uint32_t* dbg_tiles = nullptr;
-    uint4* dbg_aabb = nullptr;
-    uint32_t* dbg_keys_unsorted = nullptr;
-    uint32_t* dbg_vals_unsorted = nullptr;
-    uint64_t dbg_m = 0;
-    unsigned long long* dbg_offsets = nullptr;  // N: k_emit's exclusive scan value per depth-sorted survivor
+    DevArray<uint32_t> dbg_tiles;
+    DevArray<uint4> dbg_aabb;
+    DevArray<uint32_t> dbg_keys_unsorted;
+    DevArray<uint32_t> dbg_vals_unsorted;
+    DevArray<unsigned long long> dbg_offsets;  // N: k_emit's exclusive scan value per depth-sorted survivor
 
     // reverse mode (gsb_set_backward / gsb_render_backward)
     bool backward = false;          // frames record the per-pixel state the backward needs
-    uint2* bw_record = nullptr;     // W x H (bits(final T), last contributor position + 1) of the last recorded frame
-    size_t bw_record_pixels = 0;
-    double* bw_scratch = nullptr;   // n x 9 per-survivor fp64 accumulators of the blend backward (kept zero between calls)
-    uint64_t bw_scratch_n = 0;
-    double* bw_cam_partials = nullptr;  // [4 * num_sms][GSB_UBO_WORDS] per-CTA fp64 partial sums of gsb_render_backward_camera
-    double* bw_abs = nullptr;       // n x 2 per-survivor fp64 sums of |d u|, |d v| of gsb_render_backward_density (kept zero)
-    uint64_t bw_abs_n = 0;
-    // gsb_set_backward_deterministic: allocated on first deterministic use, grown with the arena and the scene, freed with
-    // bw_record.  bw_det_slots holds 11 fp64 per arena entry (the blend's per-(tile, entry) partials).
-    bool bw_deterministic = false;
-    double* bw_det_slots = nullptr;
-    uint32_t* bw_det_keys[2] = {nullptr, nullptr};
-    uint32_t* bw_det_pos[2] = {nullptr, nullptr};
-    unsigned long long* bw_det_status = nullptr;
-    uint32_t bw_det_status_tiles = 0;
-    gsb::SortCtl* bw_det_sc = nullptr;
-    uint64_t bw_det_capacity = 0;
-    uint2* bw_det_runs = nullptr;   // n (start, ~end) runs, one per possible survivor
-    uint64_t bw_det_runs_n = 0;
+    DevArray<uint2> bw_record;      // W x H (bits(final T), last contributor position + 1) of the last recorded frame
+    DevArray<double> bw_scratch;    // n x 9 per-survivor fp64 accumulators of the blend backward (kept zero between calls)
+    DevArray<double> bw_cam_partials;  // [4 * num_sms][GSB_UBO_WORDS] per-CTA fp64 partial sums of gsb_render_backward_camera
+    DevArray<double> bw_abs;        // n x 2 per-survivor fp64 sums of |d u|, |d v| of gsb_render_backward_density (kept zero)
+    bool bw_deterministic = false;  // gsb_set_backward_deterministic
+    gsb::DetBuffers bw_det;
     uint64_t scene_gen = 0;         // bumped by every gsb_scene_upload
     bool any_frame = false;         // a frame has been rendered on this context since its creation
     bool frame_recorded = false;    // the last frame stored the backward state (whole frame, per-tile lists)
@@ -126,7 +179,6 @@ struct gsb_ctx {
 
     // frame sharding over several GPUs (gsb_shard.cu); null for a plain context
     gsb::ShardState* shard = nullptr;
-    uint32_t middle_tag = 0;  // distinguishes captured graphs that read different record buffers (the shard exchange parity)
 };
 
 
@@ -139,16 +191,6 @@ int fail(gsb_ctx* c, int code, const char* what, cudaError_t e = cudaSuccess);
         cudaError_t e_ = (call);                                       \
         if (e_ != cudaSuccess) return gsb::fail(ctx, e_ == cudaErrorMemoryAllocation ? GSB_ERR_OOM : GSB_ERR_CUDA, #call, e_); \
     } while (0)
-
-template <typename T>
-cudaError_t dev_alloc(T** p, size_t count) {
-    return cudaMalloc(reinterpret_cast<void**>(p), std::max<size_t>(count, 1) * sizeof(T));
-}
-template <typename T>
-void dev_free(T*& p) {
-    if (p) cudaFree(p);
-    p = nullptr;
-}
 
 struct FramePlan {
     uint32_t W, H, tiles_x, tiles_y, T, rb, re;
@@ -164,14 +206,18 @@ uint32_t bits_for(uint32_t count);
 uint32_t quantise_hint(uint64_t hint);
 size_t bytes_per_pixel(int fmt);
 int wait_frame(gsb_ctx* ctx);
+void poll_frame(gsb_ctx* ctx);
+int regrow_after_overflow(gsb_ctx* ctx, cudaStream_t stream);
 int ensure_ranges(gsb_ctx* ctx, uint32_t W, uint32_t H);
 // fills the size-derived fields of a plan, (re)allocates the tile ranges and handles the look-back epoch wrap
 int plan_frame(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, cudaStream_t stream, FramePlan* out);
-int enqueue_middle(gsb_ctx* ctx, const FramePlan& fp, cudaStream_t stream, bool events);
-int launch_middle_graph(gsb_ctx* ctx, const FramePlan& fp, cudaStream_t stream);
-int enqueue_blend(gsb_ctx* ctx, const FramePlan& fp, uint32_t b0, uint32_t b1, void* band_out, size_t pitch, int fmt,
-                  cudaStream_t stream, void* const* peer_frames = nullptr, int num_peer_frames = 0);
+ProjectParams project_params(const gsb_ctx* ctx, const gsb_uniforms& ubo, uint32_t rb, uint32_t re);
+int enqueue_middle(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, cudaStream_t stream, bool events);
+int launch_middle_graph(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, cudaStream_t stream);
+int enqueue_blend(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, uint32_t b0, uint32_t b1, void* band_out, size_t pitch,
+                  int fmt, cudaStream_t stream, void* const* peer_frames = nullptr, int num_peer_frames = 0);
 int enqueue_tail(gsb_ctx* ctx, const FramePlan& fp, cudaStream_t stream);
+int check_image(gsb_ctx* ctx, const gsb_uniforms* ubo, int fmt);
 int check_render_args(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t& rb, uint32_t& re, const void* out, size_t& pitch, int fmt);
 
 // gsb_shard.cu

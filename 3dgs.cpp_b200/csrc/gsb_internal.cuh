@@ -105,23 +105,23 @@ cudaError_t launch_cov3d(const float* vtx_aos, uint64_t count, uint64_t dst_offs
 cudaError_t launch_project(const ProjectParams& p, bool debug, cudaStream_t s);
 cudaError_t launch_emit(const EmitParams& p, cudaStream_t s);
 
-struct SortParams {
-    void* keys[2];             // u32 or u64 keys (key_bytes)
-    uint32_t* vals[2];
-    int key_bytes;             // 4 or 8
-    const uint32_t* d_m;       // device pointer to the element count
-    uint32_t m_hint;           // host estimate of the count (sizes the grids only; any value is correct)
-    uint32_t key_bits;
-    unsigned long long* status;  // epoch-tagged look-back words [tiles][256]
-    uint32_t status_tiles;     // capacity of status in tiles
-    const uint32_t* d_epoch;   // device word added to the epoch (the frame counter of Control; null = 0)
-    uint32_t epoch_base;       // pass p tags its look-back words with *d_epoch + epoch_base + p: unique per (frame, sort, pass)
-    SortCtl* sc;               // must be zero on entry
-    int num_sms;
-    cudaEvent_t* events;       // optional: events[0] after the histogram, events[1 + p] after pass p
-    uint2* ranges;             // optional (u32 keys): the last pass also produces the tile ranges (start, ~end)
-    uint32_t range_key_mask;   // bits of a key that index `ranges` (0 = all; coarse bins keep a tile mask above bit 15)
-    bool discard_sorted_keys;  // the last pass writes payloads only (the caller never reads the sorted keys)
+struct SortParams {  // host-side arguments of launch_sort
+    void* keys[2] = {};        // u32 or u64 keys (key_bytes)
+    uint32_t* vals[2] = {};
+    int key_bytes = 4;         // 4 or 8
+    const uint32_t* d_m = nullptr;  // device pointer to the element count
+    uint32_t m_hint = 0;       // host estimate of the count (sizes the grids only; any value is correct)
+    uint32_t key_bits = 0;
+    unsigned long long* status = nullptr;  // epoch-tagged look-back words [tiles][256]
+    uint32_t status_tiles = 0;  // capacity of status in tiles
+    const uint32_t* d_epoch = nullptr;  // device word added to the epoch (the frame counter of Control; null = 0)
+    uint32_t epoch_base = 0;   // pass p tags its look-back words with *d_epoch + epoch_base + p: unique per (frame, sort, pass)
+    SortCtl* sc = nullptr;     // must be zero on entry
+    int num_sms = 0;
+    cudaEvent_t* events = nullptr;  // optional: events[0] after the histogram, events[1 + p] after pass p
+    uint2* ranges = nullptr;   // optional (u32 keys): the last pass also produces the tile ranges (start, ~end)
+    uint32_t range_key_mask = 0;  // bits of a key that index `ranges` (0 = all; coarse bins keep a tile mask above bit 15)
+    bool discard_sorted_keys = false;  // the last pass writes payloads only (the caller never reads the sorted keys)
 };
 // Returns the number of passes P via *passes; sorted data ends in keys[P & 1].
 cudaError_t launch_sort(const SortParams& p, uint32_t* passes, cudaStream_t s);

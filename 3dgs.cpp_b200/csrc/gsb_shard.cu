@@ -79,10 +79,10 @@ struct ShardState {
     unsigned char* peer_window[GSB_MAX_SHARDS] = {};  // this rank's view of every rank's window (own included)
 
     // destination-side dense survivor arrays (the plain context's are the source-side ones)
-    uint32_t* dkeys_d[2] = {nullptr, nullptr};
-    uint32_t* dvals_d[2] = {nullptr, nullptr};
-    unsigned long long* emit_status_d = nullptr;
-    uint32_t* route_status = nullptr;  // [chunks of the slice][GSB_MAX_SHARDS]
+    DevArray<uint32_t> dkeys_d[2];
+    DevArray<uint32_t> dvals_d[2];
+    DevArray<unsigned long long> emit_status_d;
+    DevArray<uint32_t> route_status;   // [chunks of the slice][GSB_MAX_SHARDS]
     Mailbox* mailbox_host = nullptr;   // pinned copy of the own mailbox (overflow flags, error) at the end of a frame
     uint32_t last_parity = 0;
 
@@ -367,22 +367,8 @@ int enqueue_sharded_phase(gsb_ctx* ctx, ShardFrame& F, int phase) {
         if (ctx->timers) CK(cudaEventRecord(ctx->ev[0], stream));
         // ---- k_project over the local slice (whole frame, no band clip) delivers every survivor straight into the exchange
         // buffers (parity f & 1: last read in frame f - 2, see the header) of the ranks whose band it touches, and announces it ----
-        ProjectParams pp{};
-        pp.pos_op = ctx->pos_op;
-        pp.cov_a = ctx->cov_a;
-        pp.cov_b = ctx->cov_b;
-        pp.sh = ctx->sh;
-        pp.sh_half = ctx->scene_sh_half ? 1 : 0;
-        pp.n = (uint32_t)ctx->n;
+        ProjectParams pp = project_params(ctx, F.ubo, 0, F.tiles_y);  // its recs, dkeys and dvals are unused by the routed kernel
         pp.index_base = (uint32_t)((uint64_t)r * sh->slice);
-        pp.ubo = F.ubo;
-        pp.tile_row_begin = 0;
-        pp.tile_row_end = F.tiles_y;
-        pp.recs = ctx->recs;      // unused by the routed kernel
-        pp.dkeys = ctx->dkeys[0];
-        pp.dvals = ctx->dvals[0];
-        pp.status = ctx->project_status;
-        pp.ctl = ctx->ctl;
         pp.route_world = G;
         pp.band_rows = std::max(F.R, 1u);
         pp.route_status = sh->route_status;
@@ -410,42 +396,20 @@ int enqueue_sharded_phase(gsb_ctx* ctx, ShardFrame& F, int phase) {
         k_shard_gather<<<std::min<uint32_t>((F.fp.nv_q + 255) / 256, (uint32_t)ctx->num_sms * 8u), 256, 0, stream>>>(gp);
         CK(cudaGetLastError());
 
-        // ---- the middle of the frame and the blend run on the destination-side arrays ----
-        struct Swap {
-            gsb_ctx* c;
-            float4* recs;
-            uint32_t* dk[2];
-            uint32_t* dv[2];
-            unsigned long long* es;
-            uint32_t tag;
-            ~Swap() {
-                c->recs = recs;
-                c->dkeys[0] = dk[0];
-                c->dkeys[1] = dk[1];
-                c->dvals[0] = dv[0];
-                c->dvals[1] = dv[1];
-                c->emit_status = es;
-                c->middle_tag = tag;
-            }
-        } swap{ctx, ctx->recs, {ctx->dkeys[0], ctx->dkeys[1]}, {ctx->dvals[0], ctx->dvals[1]}, ctx->emit_status, ctx->middle_tag};
-        ctx->recs = sh->recs_x(r, F.par);
-        ctx->dkeys[0] = sh->dkeys_d[0];
-        ctx->dkeys[1] = sh->dkeys_d[1];
-        ctx->dvals[0] = sh->dvals_d[0];
-        ctx->dvals[1] = sh->dvals_d[1];
-        ctx->emit_status = sh->emit_status_d;
-        ctx->middle_tag = 1u + (uint32_t)F.par;
+        // ---- the middle of the frame and the blend run on the band's survivors: this parity's exchange buffers and the
+        // destination-side arrays ----
+        const Survivors sv{sh->recs_x(r, F.par), {sh->dkeys_d[0], sh->dkeys_d[1]}, {sh->dvals_d[0], sh->dvals_d[1]}, sh->emit_status_d};
         int rc;
-        if (ctx->use_graph && !ctx->timers && !ctx->debug) rc = launch_middle_graph(ctx, F.fp, stream);
-        else rc = enqueue_middle(ctx, F.fp, stream, ctx->timers);
+        if (ctx->use_graph && !ctx->timers && !ctx->debug) rc = launch_middle_graph(ctx, F.fp, sv, stream);
+        else rc = enqueue_middle(ctx, F.fp, sv, stream, ctx->timers);
         if (rc != GSB_OK) return rc;
 
         const size_t pitch = (size_t)F.ubo.width * bytes_per_pixel(F.fmt);
         void* frames[GSB_MAX_SHARDS];
         for (int p = 0; p < G; p++) frames[p] = sh->frame_x(p, F.par);
         if (F.rb < F.re) {
-            if (sh->gather_nccl) rc = enqueue_blend(ctx, F.fp, F.rb, F.re, nullptr, pitch, F.fmt, stream, &frames[r], 1);
-            else rc = enqueue_blend(ctx, F.fp, F.rb, F.re, nullptr, pitch, F.fmt, stream, frames, G);
+            if (sh->gather_nccl) rc = enqueue_blend(ctx, F.fp, sv, F.rb, F.re, nullptr, pitch, F.fmt, stream, &frames[r], 1);
+            else rc = enqueue_blend(ctx, F.fp, sv, F.rb, F.re, nullptr, pitch, F.fmt, stream, frames, G);
             if (rc != GSB_OK) return rc;
         }
         if (sh->gather_nccl && sh->comm) {  // the baseline: one in-place all-gather of the equal-height bands
@@ -497,16 +461,6 @@ int sharded_frame_status(gsb_ctx* ctx, bool* any_overflow) {
     return GSB_OK;
 }
 
-int regrow_after_overflow(gsb_ctx* ctx) {
-    if (!ctx->ctl_host->overflow) return GSB_OK;
-    const uint64_t want = ctx->ctl_host->instances_total + ctx->ctl_host->instances_total / 4 + 4096;
-    int rc = ensure_arena(ctx, want);
-    if (rc != GSB_OK) return rc;
-    CK(cudaMemsetAsync(&ctx->ctl->overflow_sticky, 0, sizeof(uint32_t), ctx->stream));
-    ctx->regrow_count++;
-    return GSB_OK;
-}
-
 int copy_frame_out(gsb_ctx* ctx, const gsb_uniforms* ubo, void* out, size_t pitch, gsb_memory out_mem, int fmt, cudaStream_t s) {
     ShardState* sh = ctx->shard;
     const size_t tight = (size_t)ubo->width * bytes_per_pixel(fmt);
@@ -539,18 +493,12 @@ int upload_slice(gsb_ctx* ctx, const float* vertices, uint64_t n_total, gsb_memo
     const uint64_t first = std::min(n_total, (uint64_t)sh->rank * sh->slice), count = std::min(sh->slice, n_total - first);
     int rc = gsb_scene_upload(ctx, count ? vertices : nullptr, count, mem);
     if (rc != GSB_OK) return rc;
-    dev_free(sh->dkeys_d[0]);
-    dev_free(sh->dkeys_d[1]);
-    dev_free(sh->dvals_d[0]);
-    dev_free(sh->dvals_d[1]);
-    dev_free(sh->emit_status_d);
-    dev_free(sh->route_status);
-    CK(dev_alloc(&sh->dkeys_d[0], sh->cap));
-    CK(dev_alloc(&sh->dkeys_d[1], sh->cap));
-    CK(dev_alloc(&sh->dvals_d[0], sh->cap));
-    CK(dev_alloc(&sh->dvals_d[1], sh->cap));
-    CK(dev_alloc(&sh->emit_status_d, (sh->cap + 255) / 256));
-    CK(dev_alloc(&sh->route_status, ((sh->slice + 255) / 256) * GSB_MAX_SHARDS));
+    CK(sh->dkeys_d[0].grow(sh->cap));
+    CK(sh->dkeys_d[1].grow(sh->cap));
+    CK(sh->dvals_d[0].grow(sh->cap));
+    CK(sh->dvals_d[1].grow(sh->cap));
+    CK(sh->emit_status_d.grow((sh->cap + 255) / 256));
+    CK(sh->route_status.grow(((sh->slice + 255) / 256) * GSB_MAX_SHARDS));
     ctx->alloc_gen++;
     rc = ensure_sort_status(ctx, std::max<uint64_t>(sh->cap, ctx->capacity));
     if (rc != GSB_OK) return rc;
@@ -567,8 +515,8 @@ int check_sharded_args(gsb_ctx* ctx, const gsb_uniforms* ubo, int fmt) {
     if (!ctx->shard) return fail(ctx, GSB_ERR_INVALID, "not a sharded context (gsb_create_sharded / gsb_group_create)");
     if (!ubo) return fail(ctx, GSB_ERR_INVALID, "null argument");
     if (!ctx->shard->n_total || !ctx->pos_op) return fail(ctx, GSB_ERR_NO_SCENE, "no scene uploaded");
-    if (fmt < GSB_FORMAT_RGBA32F || fmt > GSB_FORMAT_BGRA8) return fail(ctx, GSB_ERR_INVALID, "bad format");
-    if (ubo->width == 0 || ubo->height == 0 || ubo->width > 16u * 65535u || ubo->height > 16u * 65535u) return fail(ctx, GSB_ERR_INVALID, "bad image size");
+    const int rc = check_image(ctx, ubo, fmt);
+    if (rc != GSB_OK) return rc;
     if (ctx->debug) return fail(ctx, GSB_ERR_INVALID, "gsb_set_debug is not available on a sharded context");
     return GSB_OK;
 }
@@ -606,15 +554,9 @@ void shard_destroy(gsb_ctx* ctx) {
     if (!sh) return;
     close_peers(ctx);
     if (sh->window) cudaFree(sh->window);
-    dev_free(sh->dkeys_d[0]);
-    dev_free(sh->dkeys_d[1]);
-    dev_free(sh->dvals_d[0]);
-    dev_free(sh->dvals_d[1]);
-    dev_free(sh->emit_status_d);
-    dev_free(sh->route_status);
     if (sh->mailbox_host) cudaFreeHost(sh->mailbox_host);
     if (sh->comm) sh->nccl.CommDestroy(sh->comm);
-    delete sh;
+    delete sh;  // frees the device arrays
     ctx->shard = nullptr;
 }
 
@@ -716,11 +658,7 @@ int gsb_render_sharded_async(gsb_ctx* ctx, const gsb_uniforms* ubo, gsb_format f
     CK(cudaSetDevice(ctx->device));
     rc = ensure_frame_ipc(ctx, ubo, fmt);
     if (rc != GSB_OK) return rc;
-    if (ctx->frame_pending && cudaEventQuery(ctx->ev_done) == cudaSuccess) {
-        ctx->frame_pending = false;
-        ctx->m_hint = ctx->ctl_host->num_instances;
-        ctx->nv_hint = ctx->ctl_host->num_visible;
-    }
+    poll_frame(ctx);
     return enqueue_sharded(ctx, ubo, fmt, stream ? static_cast<cudaStream_t>(stream) : ctx->stream);
 }
 
@@ -743,7 +681,7 @@ int gsb_render_sharded(gsb_ctx* ctx, const gsb_uniforms* ubo, void* out, size_t 
         if (!any) break;
         // some rank's arena overflowed: every rank sees the same flags, so all of them re-render together
         if (attempt >= 3) return fail(ctx, GSB_ERR_OVERFLOW, "instance arena overflow persists after regrow");
-        rc = regrow_after_overflow(ctx);
+        rc = regrow_after_overflow(ctx, ctx->stream);
         if (rc != GSB_OK) return rc;
     }
     if (out) return copy_frame_out(ctx, ubo, out, pitch, out_mem, fmt, s);
@@ -849,11 +787,7 @@ static int group_enqueue(gsb_group* g, const gsb_uniforms* ubo, int fmt) {
     for (size_t i = 0; i < g->ctx.size(); i++) {
         gsb_ctx* c = g->ctx[i];
         cudaSetDevice(c->device);
-        if (c->frame_pending && cudaEventQuery(c->ev_done) == cudaSuccess) {
-            c->frame_pending = false;
-            c->m_hint = c->ctl_host->num_instances;
-            c->nv_hint = c->ctl_host->num_visible;
-        }
+        poll_frame(c);
         F[i].ubo = *ubo;
         F[i].fmt = fmt;
         F[i].stream = c->stream;
@@ -892,7 +826,7 @@ int gsb_group_render(gsb_group* g, const gsb_uniforms* ubo, void* out, size_t pi
         if (attempt >= 3) return group_fail(g, GSB_ERR_OVERFLOW, "instance arena overflow persists after regrow");
         for (gsb_ctx* c : g->ctx) {
             cudaSetDevice(c->device);
-            rc = regrow_after_overflow(c);
+            rc = regrow_after_overflow(c, c->stream);
             if (rc != GSB_OK) return group_fail(g, rc, c->err);
         }
     }
