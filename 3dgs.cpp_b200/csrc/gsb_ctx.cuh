@@ -177,6 +177,10 @@ struct gsb_ctx {
     int frame_mode = GSB_MODE_EXACT;
     gsb_uniforms last_ubo{};        // the last frame's camera
 
+    // gsb_image_loss (gsb_loss.cu): allocated on first use, grown with the frame size
+    DevArray<float> loss_abc;        // 9 x W x H: the gather terms A, B, C of each RGB channel (only for a gradient)
+    DevArray<double> loss_partials;  // 3 x tiles: per-tile fp64 sums of |x - y|, (x - y)^2 and the SSIM map
+
     // frame sharding over several GPUs (gsb_shard.cu); null for a plain context
     gsb::ShardState* shard = nullptr;
 };

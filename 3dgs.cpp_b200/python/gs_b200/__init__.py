@@ -43,6 +43,8 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     # reverse mode
     "gsb_set_backward", "gsb_render_backward", "gsb_render_backward_camera", "gsb_render_backward_density",
     "gsb_set_backward_deterministic",
+    # training loss
+    "gsb_image_loss",
     # frame sharding over several GPUs
     "gsb_group_create", "gsb_group_destroy", "gsb_group_size", "gsb_group_context", "gsb_group_last_error",
     "gsb_group_scene_upload", "gsb_group_render", "gsb_group_render_async",
@@ -145,6 +147,8 @@ lib.gsb_set_backward_deterministic.argtypes = [_vp, C.c_int]
 lib.gsb_render_backward.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp]
 lib.gsb_render_backward_camera.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp]
 lib.gsb_render_backward_density.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp]
+lib.gsb_image_loss.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_float, _vp,
+                               C.c_size_t, _vp, _vp]
 
 lib.gsb_group_create.argtypes = [C.c_int, C.POINTER(C.c_int), C.POINTER(_vp)]
 lib.gsb_group_destroy.argtypes = [_vp]
@@ -416,6 +420,41 @@ class Context:
             self._ck(lib.gsb_render_backward_camera(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
                                                     grad_uniforms_ptr, stream_ptr(stream)))
 
+    def image_loss(self, image, target, lambda_dssim=0.2, grad_image=None, stream=None):
+        """gsb_image_loss on torch tensors: the photometric loss (1 - lambda) L1 + lambda (1 - SSIM) of `image` against
+        `target`, and, when grad_image is given, d loss / d image written into it (A = 0).  Returns the (4,) float64 device
+        tensor (loss, L1, SSIM, MSE) without waiting for it.
+
+        image and grad_image are (H, W, 4) float32 and target (H, W, 4) float32 or uint8 (read as v / 255), all CUDA tensors
+        on the context's device; pixels are dense, rows may be padded (a view of wider rows).  Runs on `stream` (a torch
+        stream), by default torch's current stream.  Bad shapes, dtypes or devices raise ValueError."""
+        import torch
+
+        image_pitch = self._frame_pitch("image", image, (torch.float32,), image.shape[:2] if image.dim() == 3 else None)
+        H, W = image.shape[0], image.shape[1]
+        target_pitch = self._frame_pitch("target", target, (torch.float32, torch.uint8), (H, W))
+        grad_pitch = 0 if grad_image is None else self._frame_pitch("grad_image", grad_image, (torch.float32,), (H, W))
+        result = torch.empty(4, dtype=torch.float64, device=image.device)
+        s = _torch_stream_arg(torch.cuda.current_stream(image.device) if stream is None else stream)
+        self._ck(lib.gsb_image_loss(self.h, W, H, image.data_ptr(), image_pitch, target.data_ptr(), target_pitch,
+                                    FORMAT_RGBA8 if target.dtype == torch.uint8 else FORMAT_RGBA32F, float(lambda_dssim),
+                                    None if grad_image is None else grad_image.data_ptr(), grad_pitch, result.data_ptr(), s))
+        return result
+
+    def _frame_pitch(self, name, t, dtypes, hw):
+        """Row pitch in bytes of an (H, W, 4) CUDA tensor with dense pixels on this context's device; ValueError otherwise."""
+        import torch
+
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
+            raise ValueError(f"image_loss: {name} must be a CUDA tensor on device {self.device}")
+        if t.dim() != 3 or t.shape[2] != 4 or hw is None or tuple(t.shape[:2]) != tuple(hw) or t.numel() == 0:
+            raise ValueError(f"image_loss: {name} must be (H, W, 4) with the image's H and W >= 1, got {tuple(t.shape)}")
+        if t.dtype not in dtypes:
+            raise ValueError(f"image_loss: {name} must be {' or '.join(str(d) for d in dtypes)}, got {t.dtype}")
+        if t.stride(2) != 1 or t.stride(1) != 4 or t.stride(0) < 4 * t.shape[1]:
+            raise ValueError(f"image_loss: {name} must have dense pixels and rows in order, got strides {t.stride()}")
+        return t.stride(0) * t.element_size()
+
     def download(self, which) -> np.ndarray:
         nbytes = lib.gsb_debug_size(self.h, which)
         dt = {BUF_COV3D: np.float32, BUF_ATTR: ATTR_DTYPE, BUF_TILES_OVERLAP: np.uint32, BUF_PREFIX_SUM: np.uint32,
@@ -531,6 +570,51 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None):
     off): every gradient and density statistic is then bit-identical for the same inputs, at some cost in time.  With
     torch's default settings backward takes the atomic path, whose results may differ in the last bit from run to run."""
     return _render_fn().apply(ctx, vertices, u, ubo, density)
+
+
+_LossFn = None
+
+
+def _loss_fn():
+    global _LossFn
+    if _LossFn is None:
+        import torch
+
+        class LossFn(torch.autograd.Function):
+            @staticmethod
+            def forward(fctx, ctx, image, target, lambda_dssim):
+                img = image.detach()
+                # the loss and its gradient in one call; only the loss when the image needs no gradient
+                grad = torch.empty(img.shape, dtype=torch.float32, device=img.device) if fctx.needs_input_grad[1] else None
+                result = ctx.image_loss(img, target.detach(), lambda_dssim, grad)  # on torch's current stream
+                fctx.grad = grad
+                return result[0].to(torch.float32)
+
+            @staticmethod
+            def backward(fctx, grad_loss):
+                return None, fctx.grad * grad_loss, None, None
+
+        _LossFn = LossFn
+    return _LossFn
+
+
+def image_loss_torch(ctx: "Context", image, target, lambda_dssim=0.2):
+    """Differentiable photometric loss of 3DGS training (Kerbl et al. 2023) through gsb_image_loss, as a float32 scalar tensor:
+    (1 - lambda_dssim) L1 + lambda_dssim (1 - SSIM), means over the RGB values, SSIM with an 11 x 11 Gaussian window
+    (sigma 1.5) and zero padding.  image is the (H, W, 4) float32 CUDA tensor render_torch returns, target an (H, W, 4) float32
+    or uint8 (read as v / 255) tensor on the same device; A is ignored.  Runs on torch's current stream and never waits on the
+    host; backward returns the gradient the forward computed, scaled by the upstream gradient.  The result and the gradient
+    are bitwise reproducible for the same inputs.  Bad shapes, dtypes or devices raise ValueError."""
+    return _loss_fn().apply(ctx, image, target, float(lambda_dssim))
+
+
+def image_metrics(ctx: "Context", image, target):
+    """Evaluation metrics of an (H, W, 4) float32 CUDA frame against a float32 or uint8 target through gsb_image_loss, on the
+    host: {"l1", "ssim", "mse", "psnr"} with PSNR = -10 log10(MSE) for values in [0, 1] (inf for identical RGB)."""
+    import math
+
+    _, l1, ssim, mse = (float(v) for v in ctx.image_loss(image, target).cpu())
+    return {"l1": l1, "ssim": ssim, "mse": mse, "psnr": -10.0 * math.log10(mse) if mse > 0 else math.inf}
 
 
 def densify_and_prune(vertices, density, *, grad_threshold, scene_extent, percent_dense=0.01, min_opacity=0.005,

@@ -263,6 +263,26 @@ int gsb_render_backward_camera(gsb_ctx *ctx, const float *vertices, const float 
 int gsb_render_backward_density(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,
                                 float *grad_vertices, gsb_uniforms *grad_uniforms, float *density, void *stream);
 
+/* Photometric loss of a frame against a target, and its gradient (no reference counterpart): the loss of 3DGS training,
+ * loss = (1 - lambda) L1 + lambda (1 - SSIM), with SSIM over an 11 x 11 Gaussian window (sigma 1.5) applied with zero
+ * padding, C1 = 0.01^2, C2 = 0.03^2 (DESIGN.md section 11).  All pointers are device memory, enqueued on `stream` (NULL = the
+ * context's stream); never synchronises.
+ *   image        H x W float4, RGBA32F layout (render_torch's / gsb_render's float output), image_pitch apart (0 = tight)
+ *   target       H x W in target_fmt: GSB_FORMAT_RGBA32F or GSB_FORMAT_RGBA8 (UNORM8, read as v / 255.0f); A is ignored
+ *   lambda_dssim in [0, 1]
+ *   grad_image   may be NULL (metrics only); otherwise OVERWRITTEN with d loss / d image, A = 0 -- exactly the grad_image
+ *                gsb_render_backward takes
+ *   result       4 doubles, OVERWRITTEN: loss, L1, SSIM, MSE (means over the 3 W H RGB values)
+ * Needs no scene and leaves the last frame's backward state alone.  No atomics: the result and the gradient are bitwise
+ * reproducible for the same inputs, whatever the stream or the pitches.  The context keeps a scratch of 24 B per 32 x 16 tile
+ * and, with a gradient, 36 B per pixel, grown with the frame size and freed with the context; calls on different streams
+ * share it, so the caller orders them.  GSB_ERR_INVALID for a NULL ctx, image, target or result, W or H of 0, lambda outside
+ * [0, 1] or NaN, any other target format, a pitch below the row size, or a pointer or pitch not aligned to 16 B (float4
+ * buffers) or 4 B (an RGBA8 target). */
+int gsb_image_loss(gsb_ctx *ctx, uint32_t width, uint32_t height, const float *image, size_t image_pitch,
+                   const void *target, size_t target_pitch, gsb_format target_fmt, float lambda_dssim,
+                   float *grad_image, size_t grad_pitch, double *result, void *stream);
+
 /* Size in bytes of a debug buffer for the last frame (0 if unavailable), and its download. */
 size_t gsb_debug_size(gsb_ctx *ctx, gsb_buffer which);
 int gsb_debug_download(gsb_ctx *ctx, gsb_buffer which, void *dst, size_t bytes);
