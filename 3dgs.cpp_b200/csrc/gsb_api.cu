@@ -1012,6 +1012,60 @@ int gsb_render_backward_density(gsb_ctx* ctx, const float* vertices, const float
                            vertices, grad_image, pitch, grad_vertices, grad_uniforms, density, stream);
 }
 
+int gsb_adam_step(gsb_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* grad_vertices, float* vertices,
+                  const gsb_adam_config* cfg, void* stream) {
+    if (!ctx) return GSB_ERR_INVALID;
+    auto bad = [&](const char* what) { return fail(ctx, GSB_ERR_INVALID, (std::string("gsb_adam_step: ") + what).c_str()); };
+    if (ctx->shard) return bad("sharded contexts have no training step");
+    if (!ctx->pos_op) return fail(ctx, GSB_ERR_NO_SCENE, "gsb_adam_step: no scene uploaded");
+    if (ctx->scene_sh_half) return bad("fp16 SH storage has no training step");
+    if (!params || !exp_avg || !exp_avg_sq || !grad_vertices || !vertices || !cfg) return bad("null argument");
+    for (const void* p : {(const void*)params, (const void*)exp_avg, (const void*)exp_avg_sq, (const void*)grad_vertices, (const void*)vertices})
+        if (reinterpret_cast<uintptr_t>(p) % 16) return bad("array not aligned to 16 B");
+    for (float lr : cfg->lr)
+        if (!(lr >= 0.0f)) return bad("learning rate below 0 or NaN");
+    if (!(cfg->beta1 >= 0.0f && cfg->beta1 < 1.0f) || !(cfg->beta2 >= 0.0f && cfg->beta2 < 1.0f)) return bad("beta outside [0, 1)");
+    if (!(cfg->eps >= 0.0f)) return bad("eps below 0 or NaN");
+    if (!(cfg->bias_correction1 > 0.0f && cfg->bias_correction1 <= 1.0f) ||
+        !(cfg->bias_correction2_sqrt > 0.0f && cfg->bias_correction2_sqrt <= 1.0f))
+        return bad("bias correction outside (0, 1]");
+    if (cfg->selective > 1) return bad("selective is neither 0 nor 1");
+    CK(cudaSetDevice(ctx->device));
+    if (cfg->selective) {  // the survivors of the last frame: what gsb_render_backward differentiates
+        if (!ctx->any_frame || ctx->frame_scene_gen != ctx->scene_gen) return bad("selective: no frame of the scene as it is now");
+        if (!ctx->frame_recorded) return bad("selective: the last frame was rendered with gsb_set_backward off");
+        if (ctx->frame_band) return bad("selective: the last frame was a band of tile rows, not the whole frame");
+        int rc = wait_frame(ctx);
+        if (rc != GSB_OK) return rc;
+        if (ctx->ctl_host->overflow) return bad("selective: the last frame overflowed the instance arena (its survivors are incomplete)");
+    }
+    AdamParams P{};
+    P.params = reinterpret_cast<float4*>(params);
+    P.exp_avg = reinterpret_cast<float4*>(exp_avg);
+    P.exp_avg_sq = reinterpret_cast<float4*>(exp_avg_sq);
+    P.grad = reinterpret_cast<const float4*>(grad_vertices);
+    P.vertices = reinterpret_cast<float4*>(vertices);
+    P.pos_op = ctx->pos_op;
+    P.cov_a = ctx->cov_a;
+    P.cov_b = ctx->cov_b;
+    P.sh = reinterpret_cast<float4*>(ctx->sh.p);
+    P.n = ctx->n;
+    P.recs = cfg->selective ? ctx->recs.p : nullptr;
+    P.ctl = ctx->ctl;
+    for (int g = 0; g < 6; g++) P.lr[g] = cfg->lr[g];
+    P.beta1 = cfg->beta1;
+    P.beta2 = cfg->beta2;
+    P.eps = cfg->eps;
+    P.bias_correction1 = cfg->bias_correction1;
+    P.bias_correction2_sqrt = cfg->bias_correction2_sqrt;
+    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    // the scene changes in place: the last frame no longer describes it (gsb_render_backward, a second selective step).  The
+    // buffers keep their addresses, so the captured graphs, the arena and the grid hints stay.
+    ctx->scene_gen++;
+    CK(launch_adam(P, ctx->num_sms, s));
+    return GSB_OK;
+}
+
 size_t gsb_debug_size(gsb_ctx* ctx, gsb_buffer which) {
     if (!ctx) return 0;
     const uint64_t n = ctx->n;

@@ -95,6 +95,30 @@ __device__ __forceinline__ void rotation_from_quaternion(float qw, float qx, flo
     R[2][2] = (1.0f - 2.0f * qx2) - 2.0f * qy2;
 }
 
+// The scene words of one record (GSScene.cpp:157-184, precomp_cov3d.comp:25-48): pos_op[o] = (p.xyz, opacity) and Sigma =
+// transpose(M) M with M = S R, S = diag(scale * scale_factor), stored as cov_a[o], cov_b[o].  p, so, q are the record's first
+// three float4 (position, scale_opacity, rotation wxyz as stored).  k_ingest_cov3d and k_adam_step both store through it, so a
+// step leaves the words a gsb_scene_upload of the same records would.
+__device__ __forceinline__ void store_cov3d(float4 p, float4 so, float4 q, uint64_t o, float4* __restrict__ pos_op,
+                                            float4* __restrict__ cov_a, float2* __restrict__ cov_b, float scale_factor) {
+    float R[3][3];
+    rotation_from_quaternion(q.x, q.y, q.z, q.w, R);
+    // M = S * R  (precomp_cov3d.comp:39), S diagonal => M[c][r] = s_r * R[c][r]
+    const float s[3] = {so.x * scale_factor, so.y * scale_factor, so.z * scale_factor};
+    float M[3][3];
+#pragma unroll
+    for (int c = 0; c < 3; c++)
+#pragma unroll
+        for (int r = 0; r < 3; r++) M[c][r] = s[r] * R[c][r];
+        // cov3d = transpose(M) * M (:40): cov[c][r] = sum_k M[r][k] * M[c][k]
+#define COV(c, r) ((M[r][0] * M[c][0] + M[r][1] * M[c][1]) + M[r][2] * M[c][2])
+    const float c0 = COV(0, 0), c1 = COV(0, 1), c2 = COV(0, 2), c3 = COV(1, 1), c4 = COV(1, 2), c5 = COV(2, 2);
+#undef COV
+    pos_op[o] = make_float4(p.x, p.y, p.z, so.w);
+    cov_a[o] = make_float4(c0, c1, c2, c3);
+    cov_b[o] = make_float2(c4, c5);
+}
+
 // preprocess.comp:73-78: (x, y, z) = normalize(p - camera_position); returns |p - camera_position|
 __device__ __forceinline__ float view_direction(const float* cam, float px, float py, float pz, float& x, float& y, float& z) {
     const float dx = px - cam[0], dy = py - cam[1], dz = pz - cam[2];

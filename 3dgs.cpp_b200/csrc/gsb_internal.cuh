@@ -205,4 +205,23 @@ struct DetBackward {
 };
 cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s, const DetBackward* det = nullptr);
 
+// gsb_optim.cu: one Adam step over the scene's rows (gsb_adam_step).  Every per-row array is n x 60 floats = 15 float4 per row.
+struct AdamParams {
+    float4* params;            // raw parameters: position, -, log scale, opacity logit, quaternion wxyz, SH
+    float4* exp_avg;
+    float4* exp_avg_sq;
+    const float4* grad;        // dL/d(activated record), as gsb_render_backward writes it
+    float4* vertices;          // OUT: the activated records
+    float4* pos_op;            // OUT: the scene words k_ingest_cov3d would store for them
+    float4* cov_a;
+    float2* cov_b;
+    float4* sh;
+    uint64_t n;
+    const float4* recs;        // selective: the last frame's survivor records (index in q3.y); null: every row
+    const Control* ctl;        // selective: num_visible
+    float lr[6];               // position, scale, opacity, rotation, SH DC, SH rest
+    float beta1, beta2, eps, bias_correction1, bias_correction2_sqrt;
+};
+cudaError_t launch_adam(const AdamParams& p, int num_sms, cudaStream_t s);
+
 }  // namespace gsb

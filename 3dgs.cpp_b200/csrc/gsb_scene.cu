@@ -22,23 +22,7 @@ __global__ void __launch_bounds__(256) k_ingest_cov3d(const float4* __restrict__
     const float4 so = v[1];          // scale_opacity
     const float4 q = v[2];           // rotation: x = w (common.glsl:52-55)
     const uint64_t o = dst_offset + i;
-
-    float R[3][3];
-    rotation_from_quaternion(q.x, q.y, q.z, q.w, R);
-    // M = S * R  (precomp_cov3d.comp:39), S diagonal => M[c][r] = s_r * R[c][r]
-    const float s[3] = {so.x * scale_factor, so.y * scale_factor, so.z * scale_factor};
-    float M[3][3];
-#pragma unroll
-    for (int c = 0; c < 3; c++)
-#pragma unroll
-        for (int r = 0; r < 3; r++) M[c][r] = s[r] * R[c][r];
-        // cov3d = transpose(M) * M (:40): cov[c][r] = sum_k M[r][k] * M[c][k]
-#define COV(c, r) ((M[r][0] * M[c][0] + M[r][1] * M[c][1]) + M[r][2] * M[c][2])
-    const float c0 = COV(0, 0), c1 = COV(0, 1), c2 = COV(0, 2), c3 = COV(1, 1), c4 = COV(1, 2), c5 = COV(2, 2);
-#undef COV
-    pos_op[o] = make_float4(p.x, p.y, p.z, so.w);
-    cov_a[o] = make_float4(c0, c1, c2, c3);
-    cov_b[o] = make_float2(c4, c5);
+    store_cov3d(p, so, q, o, pos_op, cov_a, cov_b, scale_factor);
     if constexpr (SH16) {  // gsb_set_sh_storage(1): 48 halves = 6 x 16 B per Gaussian (non-parity)
         uint4* dsh = reinterpret_cast<uint4*>(sh) + o * 6;
 #pragma unroll

@@ -43,8 +43,8 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     # reverse mode
     "gsb_set_backward", "gsb_render_backward", "gsb_render_backward_camera", "gsb_render_backward_density",
     "gsb_set_backward_deterministic",
-    # training loss
-    "gsb_image_loss",
+    # training loss and optimizer step
+    "gsb_image_loss", "gsb_adam_step",
     # frame sharding over several GPUs
     "gsb_group_create", "gsb_group_destroy", "gsb_group_size", "gsb_group_context", "gsb_group_last_error",
     "gsb_group_scene_upload", "gsb_group_render", "gsb_group_render_async",
@@ -109,6 +109,27 @@ class SynthParams(C.Structure):
                 ("sh_dc_range", C.c_float), ("sh_rest_sigma", C.c_float)]
 
 
+class AdamConfig(C.Structure):
+    """gsb_adam_config."""
+    _fields_ = [("lr", C.c_float * 6), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float),
+                ("bias_correction1", C.c_float), ("bias_correction2_sqrt", C.c_float), ("selective", C.c_uint32)]
+
+
+# the learning-rate groups of gsb_adam_config.lr, in order: columns 0-2, 4-6, 7, 8-11, 12-14 and 15-59 of the record
+ADAM_GROUPS = ("position", "scale", "opacity", "rotation", "sh_dc", "sh_rest")
+
+
+def adam_config(lr, betas=(0.9, 0.999), eps=1e-15, step=1, selective=False) -> AdamConfig:
+    """The gsb_adam_config of Adam's step number `step` (1 for the first): lr is six learning rates in ADAM_GROUPS order;
+    the bias corrections 1 - beta1^step and sqrt(1 - beta2^step) are computed in double, as torch.optim.Adam does."""
+    lr = [float(x) for x in lr]
+    if len(lr) != 6:
+        raise ValueError(f"adam_config: lr must hold 6 learning rates ({', '.join(ADAM_GROUPS)}), got {len(lr)}")
+    beta1, beta2 = (float(b) for b in betas)
+    return AdamConfig((C.c_float * 6)(*lr), beta1, beta2, float(eps), 1 - beta1 ** step, (1 - beta2 ** step) ** 0.5,
+                      int(bool(selective)))
+
+
 ATTR_DTYPE = np.dtype([("conic_opacity", "<f4", 4), ("color_radii", "<f4", 4), ("aabb", "<u4", 4),
                        ("uv", "<f4", 2), ("depth", "<f4"), ("magic", "<u4")])
 assert ATTR_DTYPE.itemsize == 64
@@ -149,6 +170,7 @@ lib.gsb_render_backward_camera.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, 
 lib.gsb_render_backward_density.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp]
 lib.gsb_image_loss.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_float, _vp,
                                C.c_size_t, _vp, _vp]
+lib.gsb_adam_step.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(AdamConfig), _vp]
 
 lib.gsb_group_create.argtypes = [C.c_int, C.POINTER(C.c_int), C.POINTER(_vp)]
 lib.gsb_group_destroy.argtypes = [_vp]
@@ -441,6 +463,28 @@ class Context:
                                     None if grad_image is None else grad_image.data_ptr(), grad_pitch, result.data_ptr(), s))
         return result
 
+    def adam_step(self, params, exp_avg, exp_avg_sq, grad_vertices, vertices, cfg: AdamConfig, stream=None):
+        """gsb_adam_step on torch tensors: one Adam step of the raw parameters `params` from grad_vertices (dL/d(activated
+        record)), updating params, exp_avg and exp_avg_sq in place and writing the activated records into `vertices` and the
+        context's scene (no upload needed).  All five are contiguous (n, 60) float32 CUDA tensors on the context's device,
+        n the scene's size; cfg is an adam_config(...).  Runs on `stream` (a torch stream), by default torch's current
+        stream, and does not wait for it.  Bad shapes, dtypes, devices or layouts raise ValueError."""
+        import torch
+
+        n = self.num_gaussians
+        arrays = {"params": params, "exp_avg": exp_avg, "exp_avg_sq": exp_avg_sq, "grad_vertices": grad_vertices,
+                  "vertices": vertices}
+        for name, t in arrays.items():
+            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
+                raise ValueError(f"adam_step: {name} must be a CUDA tensor on device {self.device}")
+            if t.dtype != torch.float32 or tuple(t.shape) != (n, 60) or not t.is_contiguous():
+                raise ValueError(f"adam_step: {name} must be a contiguous ({n}, 60) float32 tensor, got {tuple(t.shape)} "
+                                 f"{t.dtype}{'' if t.is_contiguous() else ' (not contiguous)'}")
+        s = _torch_stream_arg(torch.cuda.current_stream(params.device) if stream is None else stream)
+        self._ck(lib.gsb_adam_step(self.h, params.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(),
+                                   grad_vertices.data_ptr(), vertices.data_ptr(), C.byref(cfg), s))
+        self.frames += 1  # the scene changed: the last frame can no longer be differentiated
+
     def _frame_pitch(self, name, t, dtypes, hw):
         """Row pitch in bytes of an (H, W, 4) CUDA tensor with dense pixels on this context's device; ValueError otherwise."""
         import torch
@@ -666,6 +710,116 @@ def densify_and_prune(vertices, density, *, grad_threshold, scene_extent, percen
         prune |= (d[source, 3] > max_screen_size) | (out[:, 4:7].max(1).values > 0.1 * scene_extent)
     keep = ~prune
     return out[keep].contiguous(), source[keep]
+
+
+def raw_parameters(vertices):
+    """The raw parameters gsb_adam_step optimises, of activated (n, 60) records: position, column 3 as given, log(scale),
+    logit(opacity) (opacity clamped to [1e-6, 1 - 1e-6]), the quaternion and SH as given."""
+    import torch
+
+    p = vertices.detach().clone()
+    p[:, 4:7] = p[:, 4:7].log()
+    p[:, 7] = torch.logit(p[:, 7], eps=1e-6)
+    return p
+
+
+def adam_state_after_densify(params, exp_avg, exp_avg_sq, vertices, new_vertices, source):
+    """The raw parameters and Adam moments of densify_and_prune's output (new_vertices, source) of `vertices`: every row's
+    are gathered from its source row; a split child -- recognised by scale columns that differ from its source's (s / 1.6 !=
+    s for every finite s > 0) -- takes its raw position and log scale from new_vertices and starts with zero moments
+    (gsplat's convention).  Returns (params, exp_avg, exp_avg_sq)."""
+    import torch
+
+    p, m, v = params[source], exp_avg[source], exp_avg_sq[source]
+    child = (new_vertices[:, 4:7] != vertices[source, 4:7]).any(1)
+    p[child, 0:3] = new_vertices[child, 0:3]
+    p[child, 4:7] = new_vertices[child, 4:7].log()
+    m[child] = 0.0
+    v[child] = 0.0
+    return p.contiguous(), m.contiguous(), v.contiguous()
+
+
+class SceneAdam:
+    """Trains the scene resident on `ctx` with gsb_adam_step: the fused chain rule through the activations, Adam and the
+    scene update in one kernel, so a step needs no upload and waits on nothing.  A training step reads
+
+        img = opt.render(u); ctx.image_loss(img, target, 0.2, grad_image=g); opt.step(g)
+
+    with one host wait per step, inside gsb_render's arena check.  Owns, as (n, 60) float32 tensors on ctx's device:
+    `params` (raw_parameters(vertices)), `exp_avg`, `exp_avg_sq`, `vertices` (the activated records the frames and the
+    backward pass read; at first the given ones) and `grad` (the last step's dL/d vertices).
+
+    lr: six learning rates in ADAM_GROUPS order (position, scale, opacity, rotation, SH DC, SH rest), read at every step,
+    so the caller may change them (a schedule).  selective=True updates only the rows of the Gaussians that survived the
+    frame's culls (the "selective Adam" of Mallick et al. 2024); False is torch.optim.Adam's dense update of every row.
+    Turns gsb_set_backward on for ctx and uploads `vertices` once; under torch.use_deterministic_algorithms(True) the
+    backward pass runs deterministically, as in render_torch."""
+
+    def __init__(self, ctx: "Context", vertices, lr, betas=(0.9, 0.999), eps=1e-15, selective=True):
+        import torch
+
+        if not isinstance(vertices, torch.Tensor) or not vertices.is_cuda or vertices.dim() != 2 or vertices.shape[1] != 60:
+            raise ValueError("SceneAdam: vertices must be an (n, 60) CUDA tensor")
+        self.ctx, self.lr, self.betas, self.eps, self.selective = ctx, list(lr), tuple(betas), float(eps), bool(selective)
+        self.steps = 0
+        self._adopt(vertices.detach().to(torch.float32).contiguous().clone(), None)
+        ctx.set_backward(True)
+        self._upload()
+
+    def _adopt(self, vertices, state):
+        import torch
+
+        self.vertices = vertices
+        if state is None:
+            state = (raw_parameters(vertices), torch.zeros_like(vertices), torch.zeros_like(vertices))
+        self.params, self.exp_avg, self.exp_avg_sq = state
+        self.grad = torch.empty_like(vertices)
+
+    def _upload(self):
+        import torch
+
+        torch.cuda.current_stream(self.vertices.device).synchronize()  # the upload runs on the context's own stream
+        self.ctx.upload(self.vertices)
+
+    def render(self, u: Uniforms):
+        """The resident scene's frame of u as an (H, W, 4) float32 tensor, rendered on torch's current stream with the
+        backward state recorded.  No upload."""
+        import torch
+
+        img = torch.empty((u.height, u.width, 4), dtype=torch.float32, device=self.vertices.device)
+        self.ctx.frames += 1
+        self.ctx._ck(lib.gsb_render(self.ctx.h, C.byref(u), 0, ALL_ROWS, img.data_ptr(), 0, MEM_DEVICE, FORMAT_RGBA32F,
+                                    _torch_stream_arg(torch.cuda.current_stream(img.device))))
+        return img
+
+    def step(self, grad_image, density=None):
+        """One training step from dL/d(the last render()'s image), an (H, W, 4) float32 tensor: gsb_render_backward into
+        `grad` (gsb_render_backward_density, accumulating into `density`, an (n, 4) float32 tensor, when given), then
+        gsb_adam_step.  Everything runs on torch's current stream; nothing waits on the host."""
+        import torch
+
+        ctx, v = self.ctx, self.vertices
+        g = grad_image.detach().to(torch.float32).contiguous()
+        stream = _torch_stream_arg(torch.cuda.current_stream(v.device))
+        ctx.set_backward_deterministic(torch.are_deterministic_algorithms_enabled())
+        if density is None:
+            ctx._ck(lib.gsb_render_backward(ctx.h, v.data_ptr(), g.data_ptr(), 0, self.grad.data_ptr(), stream))
+        else:
+            if density.dtype != torch.float32 or tuple(density.shape) != (v.shape[0], 4) or not density.is_contiguous():
+                raise ValueError(f"SceneAdam.step: density must be a contiguous ({v.shape[0]}, 4) float32 tensor")
+            ctx._ck(lib.gsb_render_backward_density(ctx.h, v.data_ptr(), g.data_ptr(), 0, self.grad.data_ptr(), None,
+                                                    density.data_ptr(), stream))
+        self.steps += 1
+        ctx.adam_step(self.params, self.exp_avg, self.exp_avg_sq, self.grad, v,
+                      adam_config(self.lr, self.betas, self.eps, self.steps, self.selective))
+
+    def densify(self, density, **kwargs):
+        """densify_and_prune(vertices, density, **kwargs) of the resident scene: `vertices` becomes its output, params and
+        the moments follow through adam_state_after_densify, and the new scene is uploaded.  Returns `source`."""
+        new, source = densify_and_prune(self.vertices, density, **kwargs)
+        self._adopt(new, adam_state_after_densify(self.params, self.exp_avg, self.exp_avg_sq, self.vertices, new, source))
+        self._upload()
+        return source
 
 
 def _uniforms_restated(position, rotation_wxyz, fov_deg, near, far, width, height):

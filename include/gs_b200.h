@@ -283,6 +283,38 @@ int gsb_image_loss(gsb_ctx *ctx, uint32_t width, uint32_t height, const float *i
                    const void *target, size_t target_pitch, gsb_format target_fmt, float lambda_dssim,
                    float *grad_image, size_t grad_pitch, double *result, void *stream);
 
+/* ---- training: one fused Adam step of the resident scene (no reference counterpart; DESIGN.md section 12) ---- */
+typedef struct gsb_adam_config {
+    float lr[6];                  /* position, scale, opacity, rotation, sh dc (columns 12-14), sh rest (15-59); >= 0 */
+    float beta1, beta2, eps;      /* beta in [0, 1), eps >= 0 */
+    float bias_correction1;       /* 1 - beta1^t, computed in double and rounded; in (0, 1] */
+    float bias_correction2_sqrt;  /* sqrt(1 - beta2^t), likewise */
+    uint32_t selective;           /* 0: all n rows; 1: the last frame's survivors only */
+} gsb_adam_config;
+
+/* One torch.optim.Adam step (no weight decay) of the scene's raw parameters, which also writes the activated records and
+ * the scene words the next frame reads, so no gsb_scene_upload follows it.  All arrays are device memory of n =
+ * gsb_scene_size rows of 60 floats in the column layout of the records; enqueued on `stream` (NULL = the context's stream);
+ * never synchronises.
+ *   params        raw parameters, UPDATED: position (0-2), log scale (4-6), opacity logit (7), quaternion wxyz (8-11, any
+ *                 norm), SH (12-59); column 3 is neither read as a parameter nor written
+ *   exp_avg, exp_avg_sq  Adam's moments in the same layout, UPDATED (column 3 untouched)
+ *   grad_vertices dL/d(activated record) as gsb_render_backward writes it; the step chains it through exp, sigmoid and
+ *                 q / |q| of the parameters before the update (a sum of several frames' gradients is fine in dense mode)
+ *   vertices      OVERWRITTEN with the activated records of the updated parameters: (p, 1), exp(log s), sigmoid(logit),
+ *                 q / |q|, SH -- what the next gsb_render_backward takes
+ * The scene words (position, opacity, Sigma, SH) of each updated row become bit-identical to what gsb_scene_upload of that
+ * `vertices` row stores.  selective = 0 updates all n rows (torch's semantics: zero-gradient rows decay their moments and
+ * move); selective = 1 only the survivors of the last frame, read on the device, and leaves every other row of all five
+ * arrays and of the scene untouched; it needs what gsb_render_backward needs of the last frame (recorded, whole, of this
+ * scene, not overflowed) and waits for that frame if it is still pending.  No atomics: every output word is a function of
+ * the inputs.  The step changes the scene, so the last frame no longer describes it: gsb_render_backward and a second
+ * selective step return GSB_ERR_INVALID until the next frame.  Keeps the captured graphs, the instance arena and the grid
+ * hints.  GSB_ERR_NO_SCENE before any upload; GSB_ERR_INVALID for a NULL ctx, array or cfg, a sharded context, fp16 SH
+ * storage, a learning rate below 0 or NaN, a beta outside [0, 1), eps < 0 or NaN, or a bias correction outside (0, 1]. */
+int gsb_adam_step(gsb_ctx *ctx, float *params, float *exp_avg, float *exp_avg_sq, const float *grad_vertices,
+                  float *vertices, const gsb_adam_config *cfg, void *stream);
+
 /* Size in bytes of a debug buffer for the last frame (0 if unavailable), and its download. */
 size_t gsb_debug_size(gsb_ctx *ctx, gsb_buffer which);
 int gsb_debug_download(gsb_ctx *ctx, gsb_buffer which, void *dst, size_t bytes);
