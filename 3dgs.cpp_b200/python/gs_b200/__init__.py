@@ -43,8 +43,8 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     # reverse mode
     "gsb_set_backward", "gsb_render_backward", "gsb_render_backward_camera", "gsb_render_backward_density",
     "gsb_set_backward_deterministic",
-    # training loss and optimizer step
-    "gsb_image_loss", "gsb_adam_step",
+    # training loss, optimizer step and initialisation from a point cloud
+    "gsb_image_loss", "gsb_adam_step", "gsb_init_from_points",
     # frame sharding over several GPUs
     "gsb_group_create", "gsb_group_destroy", "gsb_group_size", "gsb_group_context", "gsb_group_last_error",
     "gsb_group_scene_upload", "gsb_group_render", "gsb_group_render_async",
@@ -171,6 +171,7 @@ lib.gsb_render_backward_density.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp,
 lib.gsb_image_loss.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_float, _vp,
                                C.c_size_t, _vp, _vp]
 lib.gsb_adam_step.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(AdamConfig), _vp]
+lib.gsb_init_from_points.argtypes = [_vp, _vp, _vp, C.c_uint64, C.c_float, _vp, _vp]
 
 lib.gsb_group_create.argtypes = [C.c_int, C.POINTER(C.c_int), C.POINTER(_vp)]
 lib.gsb_group_destroy.argtypes = [_vp]
@@ -283,6 +284,81 @@ def write_ply(path, records: np.ndarray):
     rec = _f32(records).reshape(-1, 62)
     if host.gsh_write_ply(str(path).encode(), rec.ctypes.data, rec.shape[0]) != 0:
         raise RuntimeError(host.gsh_last_error().decode())
+
+
+def ply_records(params) -> np.ndarray:
+    """The (n, 62) float32 PLY records write_ply takes, of raw parameters in the record's column layout (SceneAdam.params:
+    position 0-2, column 3 ignored, log scale 4-6, opacity logit 7, quaternion wxyz 8-11, SH 12-59 RGB-interleaved): x, y, z,
+    zero normals, f_dc = sh[0..2], f_rest[15 c + j - 1] = sh[3 j + c] (channel-major), opacity, scale_0..2, rot_0..3, copied
+    without any activation -- the exact inverse of the loader's layout.  params is a numpy array or a tensor (copied to the
+    host).  A trained scene is saved with write_ply(path, ply_records(opt.params))."""
+    if not isinstance(params, np.ndarray):
+        params = params.detach().cpu().numpy()
+    p = _f32(params).reshape(-1, 60)
+    out = np.zeros((p.shape[0], 62), np.float32)
+    out[:, 0:3] = p[:, 0:3]
+    out[:, 6:9] = p[:, 12:15]
+    sh_rest = p[:, 15:60].reshape(-1, 15, 3)  # [row, j - 1, c] = sh[3 j + c]
+    out[:, 9:54] = sh_rest.transpose(0, 2, 1).reshape(-1, 45)  # [row, 15 c + j - 1]
+    out[:, 54] = p[:, 7]
+    out[:, 55:58] = p[:, 4:7]
+    out[:, 58:62] = p[:, 8:12]
+    return out
+
+
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2", "ushort": "u2",
+              "uint16": "u2", "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4", "float": "f4", "float32": "f4",
+              "double": "f8", "float64": "f8"}
+
+
+def load_points_ply(path):
+    """(xyz, rgb) of a point-cloud PLY as Inria's storePly writes it (COLMAP's points3D as x, y, z, nx, ny, nz, red, green,
+    blue): binary little-endian, a single `vertex` element of scalar properties.  x, y, z (float or double) become float32,
+    red, green, blue (uchar) float32 / 255; other properties are skipped.  Both are (n, 3) float32 numpy arrays.  ascii or
+    big-endian files, list properties, other elements and a missing coordinate or colour raise ValueError."""
+    data = Path(path).read_bytes()
+    end = data.find(b"end_header")
+    if not data.startswith(b"ply") or end < 0:
+        raise ValueError(f"{path}: not a PLY file")
+    body = data.index(b"\n", end) + 1
+    fmt, elements = None, []
+    for line in data[:body].decode("ascii", "replace").splitlines()[1:]:
+        tok = line.split()
+        if not tok or tok[0] in ("comment", "obj_info", "end_header"):
+            continue
+        if tok[0] == "format":
+            fmt = tok[1] if len(tok) > 1 else None
+        elif tok[0] == "element":
+            elements.append((tok[1], int(tok[2]), []))
+        elif tok[0] == "property":
+            if not elements:
+                raise ValueError(f"{path}: property before any element")
+            if tok[1] == "list":
+                raise ValueError(f"{path}: list property '{tok[-1]}' (scalar properties only)")
+            if tok[1] not in _PLY_TYPES:
+                raise ValueError(f"{path}: unknown property type '{tok[1]}'")
+            elements[-1][2].append((tok[2], "<" + _PLY_TYPES[tok[1]]))
+        else:
+            raise ValueError(f"{path}: unexpected header line '{line}'")
+    if fmt != "binary_little_endian":
+        raise ValueError(f"{path}: format '{fmt}' (binary_little_endian only)")
+    if len(elements) != 1 or elements[0][0] != "vertex":
+        raise ValueError(f"{path}: elements {[e[0] for e in elements]} (a single 'vertex' element only)")
+    _, n, props = elements[0]
+    dtype = np.dtype(props)
+    names = dict(props)
+    for k in ("x", "y", "z"):
+        if names.get(k) not in ("<f4", "<f8"):
+            raise ValueError(f"{path}: property '{k}' missing or not float / double")
+    for k in ("red", "green", "blue"):
+        if names.get(k) != "<u1":
+            raise ValueError(f"{path}: property '{k}' missing or not uchar")
+    if len(data) - body < n * dtype.itemsize:
+        raise ValueError(f"{path}: truncated ({len(data) - body} bytes of vertex data, {n * dtype.itemsize} expected)")
+    v = np.frombuffer(data, dtype, count=n, offset=body)
+    xyz = np.stack([v[k].astype(np.float32) for k in ("x", "y", "z")], 1)
+    rgb = np.stack([v[k].astype(np.float32) for k in ("red", "green", "blue")], 1) / np.float32(255)
+    return xyz, rgb
 
 
 def synth_params(**kw) -> SynthParams:
@@ -484,6 +560,30 @@ class Context:
         self._ck(lib.gsb_adam_step(self.h, params.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(),
                                    grad_vertices.data_ptr(), vertices.data_ptr(), C.byref(cfg), s))
         self.frames += 1  # the scene changed: the last frame can no longer be differentiated
+
+    def init_from_points(self, xyz, rgb, opacity=0.1):
+        """gsb_init_from_points on torch tensors: the (n, 60) float32 activated records of a point cloud, one isotropic
+        Gaussian per point (Kerbl et al. 2023): scale sqrt of the mean squared distance to its three nearest neighbours
+        (floored at 1e-7), `opacity`, identity rotation, SH DC (rgb - 0.5) / C0 and zero higher bands.  xyz is (n, 3)
+        float32, rgb (n, 3) float32 in [0, 1] or uint8 (read as v / 255), both CUDA tensors on the context's device.  Runs
+        on torch's current stream and returns when the records are written; needs no scene and leaves the context's scene
+        and last frame alone.  Bad shapes, dtypes or devices raise ValueError."""
+        import torch
+
+        for name, t, dtypes in (("xyz", xyz, (torch.float32,)), ("rgb", rgb, (torch.float32, torch.uint8))):
+            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
+                raise ValueError(f"init_from_points: {name} must be a CUDA tensor on device {self.device}")
+            if t.dim() != 2 or t.shape[1] != 3 or t.shape[0] != xyz.shape[0]:
+                raise ValueError(f"init_from_points: {name} must be (n, 3) with xyz's n, got {tuple(t.shape)}")
+            if t.dtype not in dtypes:
+                raise ValueError(f"init_from_points: {name} must be {' or '.join(str(d) for d in dtypes)}, got {t.dtype}")
+        n = xyz.shape[0]
+        out = torch.empty((n, 60), dtype=torch.float32, device=xyz.device)
+        xyz = xyz.contiguous()
+        rgb = (rgb.to(torch.float32) / 255 if rgb.dtype == torch.uint8 else rgb).contiguous()
+        s = _torch_stream_arg(torch.cuda.current_stream(xyz.device))
+        self._ck(lib.gsb_init_from_points(self.h, xyz.data_ptr(), rgb.data_ptr(), n, float(opacity), out.data_ptr(), s))
+        return out
 
     def _frame_pitch(self, name, t, dtypes, hw):
         """Row pitch in bytes of an (H, W, 4) CUDA tensor with dense pixels on this context's device; ValueError otherwise."""

@@ -315,6 +315,28 @@ typedef struct gsb_adam_config {
 int gsb_adam_step(gsb_ctx *ctx, float *params, float *exp_avg, float *exp_avg_sq, const float *grad_vertices,
                   float *vertices, const gsb_adam_config *cfg, void *stream);
 
+/* ---- training: a scene initialised from a point cloud (no reference counterpart; DESIGN.md section 13) ---- */
+/* Kerbl et al. 2023's initialisation from SfM points: every point becomes an isotropic Gaussian.  All pointers are device
+ * memory: xyz and rgb are n x 3 floats, tightly packed; vertices (n x 60 floats) is OVERWRITTEN with activated
+ * GSScene::Vertex records, what gsb_scene_upload takes.  Row i:
+ *   position    (x, y, z, 1), copied bit for bit
+ *   scale       columns 4-6 all hold s = sqrtf(fmaxf(D, 1e-7f)); column 7 is `opacity`
+ *   rotation    (1, 0, 0, 0)
+ *   SH          sh[c] = (rgb[c] - 0.5f) / SH_C0 for c = 0, 1, 2 (two IEEE operations, rgb not clamped); sh[3..47] = 0
+ * D: with d = (dx*dx + dy*dy) + dz*dz, dx = x_j - x_i (likewise y, z), one IEEE fp32 operation each in this order, over the
+ * other rows j != i (by index: a duplicate point counts, at distance 0), m = min(3, n - 1) and d_1 <= ... <= d_m the m
+ * smallest values of d: D = ((d_1 + d_2) + d_3) / 3.0f, summed in ascending order (for m < 3 the same sum over m terms
+ * divided by (float)m); D = 0 for n = 1.  The multiset of the m smallest values is unique, so every output word is a
+ * function of the inputs alone: bitwise reproducible on any stream, in any context, on any grid.
+ * Enqueued on `stream` (NULL = the context's stream); returns when the records are written.  Needs no scene and leaves the
+ * context's scene and frame state alone (control block, arena, captured graphs, backward recording): a gsb_render_backward
+ * of the last frame still works after it and gives the same words.  Scratch is allocated and freed inside the call.
+ * n == 0 returns GSB_OK and writes nothing.  GSB_ERR_INVALID for a NULL ctx, a NULL pointer, a pointer not aligned to 4 B,
+ * n >= 2^30, an opacity outside (0, 1) or NaN, and a coordinate that is not finite (found on the device; nothing is written
+ * then). */
+int gsb_init_from_points(gsb_ctx *ctx, const float *xyz, const float *rgb, uint64_t n, float opacity, float *vertices,
+                         void *stream);
+
 /* Size in bytes of a debug buffer for the last frame (0 if unavailable), and its download. */
 size_t gsb_debug_size(gsb_ctx *ctx, gsb_buffer which);
 int gsb_debug_download(gsb_ctx *ctx, gsb_buffer which, void *dst, size_t bytes);
