@@ -74,7 +74,7 @@ int ensure_arena(gsb_ctx* ctx, uint64_t capacity) {
     if (capacity >= (1ull << 30)) return fail(ctx, GSB_ERR_OVERFLOW, "instance arena limited to 2^30 - 1 entries");
     ctx->capacity = 0;
     ctx->alloc_gen++;
-    ctx->frame_recorded = false;  // the last frame's sorted lists are gone: nothing left to differentiate
+    ctx->frame.recorded = false;  // the last frame's sorted lists are gone: nothing left to differentiate
     // + 16 entries: the blend's TMA segments are 16-B granular and may read up to 3 entries past the end of the last run
     CK(ctx->keys[0].grow(capacity + 16));
     CK(ctx->keys[1].grow(capacity + 16));
@@ -105,13 +105,13 @@ size_t bytes_per_pixel(int fmt) { return fmt == GSB_FORMAT_RGBA32F ? 16 : 4; }
 
 // the finished frame's counts size the next frame's grids
 static void take_hints(gsb_ctx* ctx) {
-    ctx->frame_pending = false;
+    ctx->frame.pending = false;
     ctx->m_hint = ctx->ctl_host->num_instances;
     ctx->nv_hint = ctx->ctl_host->num_visible;
 }
 
 int wait_frame(gsb_ctx* ctx) {
-    if (ctx->frame_pending) {
+    if (ctx->frame.pending) {
         CK(cudaEventSynchronize(ctx->ev_done));
         take_hints(ctx);
     }
@@ -120,7 +120,7 @@ int wait_frame(gsb_ctx* ctx) {
 
 // opportunistic hint refresh: takes the hints only if the last frame has already finished
 void poll_frame(gsb_ctx* ctx) {
-    if (ctx->frame_pending && cudaEventQuery(ctx->ev_done) == cudaSuccess) take_hints(ctx);
+    if (ctx->frame.pending && cudaEventQuery(ctx->ev_done) == cudaSuccess) take_hints(ctx);
 }
 
 // After wait_frame: if the last frame overflowed the instance arena, grow it like the reference's sortBufferSizeMultiplier
@@ -415,27 +415,29 @@ int enqueue_blend(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, uint32
     return GSB_OK;
 }
 
-// stats copy + completion event; latches what gsb_get_stats / gsb_debug_download may read about this frame
-int enqueue_tail(gsb_ctx* ctx, const FramePlan& fp, cudaStream_t stream) {
+// stats copy + completion event; records the frame in ctx->frame
+int enqueue_tail(gsb_ctx* ctx, const FramePlan& fp, const gsb_uniforms& ubo, cudaStream_t stream) {
     if (ctx->timers) CK(cudaEventRecord(ctx->ev[6], stream));
     CK(cudaMemcpyAsync(ctx->ctl_host, ctx->ctl, offsetof(Control, sort_depth), cudaMemcpyDeviceToHost, stream));
     CK(cudaEventRecord(ctx->ev_done, stream));
-    ctx->frame_pending = true;
-    ctx->have_frame = true;
-    ctx->frame_debug = ctx->debug;
-    ctx->frame_timers = ctx->timers;
-    ctx->last_tiles_x = fp.tiles_x;
-    ctx->last_tiles_y = fp.tiles_y;
-    ctx->last_passes = fp.passes;
-    ctx->last_depth_passes = fp.depth_passes;
-    ctx->last_final = (uint32_t)fp.fin;
+    LastFrame& f = ctx->frame;
+    f.plan = fp;
+    f.ubo = ubo;
+    f.mode = ctx->mode;
+    f.scene_gen = ctx->scene_gen;
+    f.pending = true;
+    f.exists = true;
+    f.debug = ctx->debug;
+    f.timers = ctx->timers;
+    f.recorded = ctx->backward && fp.cs == 0;  // what enqueue_blend records (a sharded context never has the switch on)
+    f.band = !(fp.rb == 0 && fp.re == fp.tiles_y);
     return GSB_OK;
 }
 
 // Enqueue one whole frame on `stream`; out_dev is device memory.
 static int enqueue_frame(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, void* out_dev, size_t pitch, int fmt,
                   cudaStream_t stream) {
-    ctx->frame_recorded = false;
+    ctx->frame.recorded = false;  // the frame overwrites the record and the lists the last one left
     // W x H per-pixel state of the reverse pass, grown on demand while gsb_set_backward is on
     if (ctx->backward) CK(ctx->bw_record.grow((size_t)ubo->width * ubo->height));
     const Survivors sv{ctx->recs, {ctx->dkeys[0], ctx->dkeys[1]}, {ctx->dvals[0], ctx->dvals[1]}, ctx->emit_status};
@@ -444,16 +446,7 @@ static int enqueue_frame(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uin
     if (rc != GSB_OK) return rc;
     rc = enqueue_blend(ctx, fp, sv, rb, re, out_dev, pitch, fmt, stream);
     if (rc != GSB_OK) return rc;
-    rc = enqueue_tail(ctx, fp, stream);
-    if (rc != GSB_OK) return rc;
-    // what gsb_render_backward checks and reads about this frame
-    ctx->any_frame = true;
-    ctx->frame_recorded = ctx->backward && fp.cs == 0;
-    ctx->frame_band = !(rb == 0 && re == fp.tiles_y);
-    ctx->frame_scene_gen = ctx->scene_gen;
-    ctx->frame_mode = ctx->mode;
-    ctx->last_ubo = *ubo;
-    return GSB_OK;
+    return enqueue_tail(ctx, fp, *ubo, stream);
 }
 
 // the pixel format and image size checks of every render entry point
@@ -576,11 +569,11 @@ int gsb_scene_upload(gsb_ctx* ctx, const float* vertices, uint64_t n, gsb_memory
     // A frame (gsb_render_async) or a backward pass on a caller's stream may still read the scene buffers, which are
     // rewritten in place when the new scene fits: wait for the whole device, not only for ctx->stream.
     if (ctx->pos_op) CK(cudaDeviceSynchronize());
-    ctx->frame_pending = false;
-    ctx->have_frame = false;
+    // nothing of the last frame is left to read; its scene_gen, now behind, tells the backward pass why
+    ctx->frame.pending = ctx->frame.exists = false;
     ctx->n = 0;
     ctx->alloc_gen++;
-    ctx->scene_gen++;  // the last frame no longer describes this scene (gsb_render_backward)
+    ctx->scene_gen++;
     drop_graphs(ctx);
     CK(ctx->pos_op.grow(n));
     CK(ctx->cov_a.grow(n));
@@ -750,8 +743,7 @@ int gsb_render_async(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_
     if (rc != GSB_OK) return rc;
     CK(cudaSetDevice(ctx->device));
     poll_frame(ctx);
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-    return enqueue_frame(ctx, ubo, rb, re, out_device, pitch, fmt, s);
+    return enqueue_frame(ctx, ubo, rb, re, out_device, pitch, fmt, stream_or_own(ctx, stream));
 }
 
 int gsb_render(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, void* out, size_t pitch, gsb_memory out_mem,
@@ -759,7 +751,7 @@ int gsb_render(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, 
     int rc = check_render_args(ctx, ubo, rb, re, out, pitch, fmt);
     if (rc != GSB_OK) return rc;
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s = stream_or_own(ctx, stream);
     const uint32_t H = ubo->height;
     const uint32_t rows = std::min(H, re * GSB_TILE) - rb * GSB_TILE;
     const size_t tight = (size_t)ubo->width * bytes_per_pixel(fmt);
@@ -806,14 +798,10 @@ int gsb_render(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, 
 int gsb_get_stats(gsb_ctx* ctx, gsb_stats* out) {
     if (!ctx || !out) return GSB_ERR_INVALID;
     memset(out, 0, sizeof *out);
-    if (!ctx->have_frame) return fail(ctx, GSB_ERR_INVALID, "no frame rendered yet");
+    if (!ctx->frame.exists) return fail(ctx, GSB_ERR_INVALID, "no frame rendered yet");
     CK(cudaSetDevice(ctx->device));
-    if (ctx->frame_pending) {
-        int rc = wait_frame(ctx);
-        if (rc != GSB_OK) return rc;
-    } else {
-        CK(cudaEventSynchronize(ctx->ev_done));
-    }
+    const int rc = wait_frame(ctx);  // a frame no longer pending has been waited for already
+    if (rc != GSB_OK) return rc;
     const Control* c = ctx->ctl_host;
     out->num_gaussians = ctx->n;
     out->num_visible = c->num_visible;
@@ -824,10 +812,10 @@ int gsb_get_stats(gsb_ctx* ctx, gsb_stats* out) {
     out->blend_pixel_hits = c->blend_hits;
     out->blend_staged = c->blend_staged;
     out->instance_capacity = ctx->capacity;
-    out->sort_passes = ctx->last_passes;
-    out->sort_depth_passes = ctx->last_depth_passes;
+    out->sort_passes = ctx->frame.plan.passes;
+    out->sort_depth_passes = ctx->frame.plan.depth_passes;
     out->regrow_count = ctx->regrow_count;
-    if (ctx->frame_timers) {  // latched per frame: toggling gsb_set_timers between frames must not read stale events
+    if (ctx->frame.timers) {  // latched per frame: toggling gsb_set_timers between frames must not read stale events
         float ms = 0.f;
         CK(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
         out->preprocess_ms = ms;  // k_project
@@ -838,10 +826,10 @@ int gsb_get_stats(gsb_ctx* ctx, gsb_stats* out) {
         CK(cudaEventElapsedTime(&ms, ctx->ev[3], ctx->ev[4]));
         out->sort_tile_ms = ms;  // instance-level Onesweep
         out->sort_ms = out->sort_depth_ms + out->sort_tile_ms;
-        if (ctx->last_passes) {
+        if (ctx->frame.plan.passes) {
             CK(cudaEventElapsedTime(&ms, ctx->ev[3], ctx->ev_sort[0]));
             out->sort_hist_ms = ms;
-            for (uint32_t p = 0; p < ctx->last_passes && p < 8; p++) {
+            for (uint32_t p = 0; p < ctx->frame.plan.passes && p < 8; p++) {
                 CK(cudaEventElapsedTime(&ms, ctx->ev_sort[p], ctx->ev_sort[p + 1]));
                 out->sort_pass_ms[p] = ms;
             }
@@ -878,7 +866,7 @@ int gsb_set_backward(gsb_ctx* ctx, int enabled) {
     if (!ctx->backward) {  // the per-pixel state exists only while the switch is on
         CK(cudaStreamSynchronize(ctx->stream));
         ctx->bw_record.reset();
-        ctx->frame_recorded = false;
+        ctx->frame.recorded = false;
         ctx->bw_det = {};
     }
     return GSB_OK;
@@ -907,6 +895,22 @@ static int ensure_det_buffers(gsb_ctx* ctx, uint64_t n) {
     return GSB_OK;
 }
 
+// What gsb_render_backward and the selective gsb_adam_step read of the last frame must hold: a frame of the scene as it is
+// now, recorded over the whole image, that did not overflow the instance arena (waited for here; the caller has set the
+// device).  `no_frame` is the code when no frame has been rendered yet; `fn` starts every message.
+static int check_recorded_frame(gsb_ctx* ctx, int no_frame, const char* fn) {
+    const LastFrame& f = ctx->frame;
+    auto bad = [&](int code, const char* what) { return fail(ctx, code, (std::string(fn) + ": " + what).c_str()); };
+    if (f.scene_gen == 0) return bad(no_frame, "no frame rendered yet");
+    if (f.scene_gen != ctx->scene_gen) return bad(GSB_ERR_INVALID, "the scene was uploaded or stepped after the last frame");
+    if (!f.recorded) return bad(GSB_ERR_INVALID, "the last frame was rendered with gsb_set_backward off, or the arena grew since");
+    if (f.band) return bad(GSB_ERR_INVALID, "the last frame was a band of tile rows, not the whole frame");
+    const int rc = wait_frame(ctx);
+    if (rc != GSB_OK) return rc;
+    if (ctx->ctl_host->overflow) return bad(GSB_ERR_INVALID, "the last frame overflowed the instance arena (its lists are incomplete)");
+    return GSB_OK;
+}
+
 // The checks and the launch shared by gsb_render_backward, gsb_render_backward_camera and gsb_render_backward_density (fn
 // names the entry in messages).  grad_ubo == nullptr: no camera gradient; grad_vertices == nullptr: no scene gradient (each
 // entry's args_ok says which may be null).  density != nullptr: also accumulate the density statistics into it.
@@ -915,20 +919,16 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     if (!ctx) return GSB_ERR_INVALID;
     auto msg = [&](const char* what) { return std::string(fn) + ": " + what; };
     if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, msg("sharded contexts have no backward pass").c_str());
-    if (!ctx->pos_op || !ctx->any_frame) return fail(ctx, GSB_ERR_NO_SCENE, msg("no scene uploaded or no frame rendered").c_str());
-    if (ctx->frame_scene_gen != ctx->scene_gen) return fail(ctx, GSB_ERR_INVALID, msg("the scene was uploaded again after the last frame").c_str());
+    if (!ctx->pos_op) return fail(ctx, GSB_ERR_NO_SCENE, msg("no scene uploaded").c_str());
+    CK(cudaSetDevice(ctx->device));
+    int rc = check_recorded_frame(ctx, GSB_ERR_NO_SCENE, fn);
+    if (rc != GSB_OK) return rc;
     if (ctx->scene_sh_half) return fail(ctx, GSB_ERR_INVALID, msg("fp16 SH storage has no backward pass").c_str());
-    if (!ctx->frame_recorded) return fail(ctx, GSB_ERR_INVALID, msg("the last frame was rendered with gsb_set_backward off").c_str());
-    if (ctx->frame_band) return fail(ctx, GSB_ERR_INVALID, msg("the last frame was a band of tile rows, not the whole frame").c_str());
     if (!args_ok) return fail(ctx, GSB_ERR_INVALID, msg("null argument").c_str());
-    const gsb_uniforms& U = ctx->last_ubo;
-    const size_t tight = (size_t)U.width * sizeof(float4);
+    const LastFrame& f = ctx->frame;
+    const size_t tight = (size_t)f.ubo.width * sizeof(float4);
     if (pitch == 0) pitch = tight;
     if (pitch < tight || pitch % sizeof(float4) != 0) return fail(ctx, GSB_ERR_INVALID, msg("bad row pitch").c_str());
-    CK(cudaSetDevice(ctx->device));
-    int rc = wait_frame(ctx);
-    if (rc != GSB_OK) return rc;
-    if (ctx->ctl_host->overflow) return fail(ctx, GSB_ERR_INVALID, msg("the last frame overflowed the instance arena (its lists are incomplete)").c_str());
     const uint64_t n = ctx->n;
     // zeroed once here; k_preprocess_backward returns every entry it reads to zero
     rc = grow_zeroed(ctx, ctx->bw_scratch, n * 9, "ctx->bw_scratch");
@@ -944,7 +944,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
         rc = ensure_det_buffers(ctx, n);
         if (rc != GSB_OK) return rc;
     }
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s = stream_or_own(ctx, stream);
     if (grad_vertices) CK(cudaMemsetAsync(grad_vertices, 0, (size_t)n * 60 * sizeof(float), s));
     if (n == 0) {
         if (grad_ubo) CK(cudaMemsetAsync(grad_ubo, 0, sizeof(gsb_uniforms), s));
@@ -952,16 +952,16 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     }
     BackwardParams bp{};
     bp.recs = ctx->recs;
-    bp.vals = ctx->vals[ctx->last_final];
+    bp.vals = ctx->vals[f.plan.fin];
     bp.ranges = ctx->ranges;
     bp.record = ctx->bw_record;
     bp.ctl = ctx->ctl;
-    bp.width = U.width;
-    bp.height = U.height;
-    bp.tiles_x = ctx->last_tiles_x;
-    bp.num_tiles = ctx->last_tiles_x * ctx->last_tiles_y;
-    bp.mode = ctx->frame_mode;
-    bp.ubo = U;
+    bp.width = f.ubo.width;
+    bp.height = f.ubo.height;
+    bp.tiles_x = f.plan.tiles_x;
+    bp.num_tiles = f.plan.T;
+    bp.mode = f.mode;
+    bp.ubo = f.ubo;
     bp.vertices = vertices;
     bp.cov_a = ctx->cov_a;
     bp.cov_b = ctx->cov_b;
@@ -1032,12 +1032,8 @@ int gsb_adam_step(gsb_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq
     if (cfg->selective > 1) return bad("selective is neither 0 nor 1");
     CK(cudaSetDevice(ctx->device));
     if (cfg->selective) {  // the survivors of the last frame: what gsb_render_backward differentiates
-        if (!ctx->any_frame || ctx->frame_scene_gen != ctx->scene_gen) return bad("selective: no frame of the scene as it is now");
-        if (!ctx->frame_recorded) return bad("selective: the last frame was rendered with gsb_set_backward off");
-        if (ctx->frame_band) return bad("selective: the last frame was a band of tile rows, not the whole frame");
-        int rc = wait_frame(ctx);
+        const int rc = check_recorded_frame(ctx, GSB_ERR_INVALID, "gsb_adam_step: selective");
         if (rc != GSB_OK) return rc;
-        if (ctx->ctl_host->overflow) return bad("selective: the last frame overflowed the instance arena (its survivors are incomplete)");
     }
     AdamParams P{};
     P.params = reinterpret_cast<float4*>(params);
@@ -1058,7 +1054,7 @@ int gsb_adam_step(gsb_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq
     P.eps = cfg->eps;
     P.bias_correction1 = cfg->bias_correction1;
     P.bias_correction2_sqrt = cfg->bias_correction2_sqrt;
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s = stream_or_own(ctx, stream);
     // the scene changes in place: the last frame no longer describes it (gsb_render_backward, a second selective step).  The
     // buffers keep their addresses, so the captured graphs, the arena and the grid hints stay.
     ctx->scene_gen++;
@@ -1070,7 +1066,7 @@ size_t gsb_debug_size(gsb_ctx* ctx, gsb_buffer which) {
     if (!ctx) return 0;
     const uint64_t n = ctx->n;
     if (which == GSB_BUF_COV3D) return (size_t)n * 6 * sizeof(float);
-    if (!ctx->have_frame || !ctx->debug || !ctx->frame_debug) return 0;
+    if (!ctx->frame.exists || !ctx->debug || !ctx->frame.debug) return 0;
     if (wait_frame(ctx) != GSB_OK) return 0;
     const uint64_t m = ctx->ctl_host->num_instances;
     switch (which) {
@@ -1081,7 +1077,7 @@ size_t gsb_debug_size(gsb_ctx* ctx, gsb_buffer which) {
         case GSB_BUF_KEYS_SORTED: return (size_t)m * 8;
         case GSB_BUF_VALS_UNSORTED:
         case GSB_BUF_VALS_SORTED: return (size_t)m * 4;
-        case GSB_BUF_TILE_BOUNDARY: return (size_t)ctx->last_tiles_x * ctx->last_tiles_y * 8;
+        case GSB_BUF_TILE_BOUNDARY: return (size_t)ctx->frame.plan.T * 8;
         case GSB_BUF_DEPTH_ORDER: return (size_t)ctx->ctl_host->num_visible * 4;
         case GSB_BUF_EMIT_OFFSETS: return (size_t)ctx->ctl_host->num_visible * 8;
         default: return 0;
@@ -1097,8 +1093,8 @@ int gsb_debug_download(gsb_ctx* ctx, gsb_buffer which, void* dst, size_t bytes) 
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaDeviceSynchronize());
     const uint64_t n = ctx->n;
-    const uint32_t nv = ctx->have_frame ? ctx->ctl_host->num_visible : 0;
-    const uint64_t m = ctx->have_frame ? ctx->ctl_host->num_instances : 0;
+    const uint32_t nv = ctx->frame.exists ? ctx->ctl_host->num_visible : 0;
+    const uint64_t m = ctx->frame.exists ? ctx->ctl_host->num_instances : 0;
     switch (which) {
         case GSB_BUF_COV3D: {
             std::vector<float4> a(n);
@@ -1174,8 +1170,8 @@ int gsb_debug_download(gsb_ctx* ctx, gsb_buffer which, void* dst, size_t bytes) 
             std::vector<float4> recs((size_t)nv * GSB_REC_F4);
             if (nv) CK(cudaMemcpy(recs.data(), ctx->recs, recs.size() * sizeof(float4), cudaMemcpyDeviceToHost));
             std::vector<uint32_t> tk(m), cv(m);
-            const uint32_t* ksrc = sorted ? ctx->keys[ctx->last_final] : ctx->dbg_keys_unsorted;
-            const uint32_t* vsrc = sorted ? ctx->vals[ctx->last_final] : ctx->dbg_vals_unsorted;
+            const uint32_t* ksrc = sorted ? ctx->keys[ctx->frame.plan.fin] : ctx->dbg_keys_unsorted;
+            const uint32_t* vsrc = sorted ? ctx->vals[ctx->frame.plan.fin] : ctx->dbg_vals_unsorted;
             if (m) {
                 CK(cudaMemcpy(tk.data(), ksrc, m * 4, cudaMemcpyDeviceToHost));
                 CK(cudaMemcpy(cv.data(), vsrc, m * 4, cudaMemcpyDeviceToHost));
@@ -1196,7 +1192,7 @@ int gsb_debug_download(gsb_ctx* ctx, gsb_buffer which, void* dst, size_t bytes) 
             std::vector<uint32_t> cid(nv);
             if (nv) {
                 CK(cudaMemcpy(recs.data(), ctx->recs, recs.size() * sizeof(float4), cudaMemcpyDeviceToHost));
-                CK(cudaMemcpy(cid.data(), ctx->dvals[ctx->last_depth_passes & 1], (size_t)nv * 4, cudaMemcpyDeviceToHost));
+                CK(cudaMemcpy(cid.data(), ctx->dvals[ctx->frame.plan.depth_passes & 1], (size_t)nv * 4, cudaMemcpyDeviceToHost));
             }
             for (uint32_t j = 0; j < nv; j++) {
                 if (cid[j] >= nv) return fail(ctx, GSB_ERR_CUDA, "corrupt depth order");
@@ -1228,30 +1224,31 @@ static int sort_pairs_impl(gsb_ctx* ctx, void* keys, uint32_t* vals, void* keys_
     if (!keys || !vals || !keys_tmp || !vals_tmp || key_bits == 0 || key_bits > 8u * (uint32_t)key_bytes) return fail(ctx, GSB_ERR_INVALID, "bad argument");
     if (m >= (1ull << 30)) return fail(ctx, GSB_ERR_INVALID, "sort limited to 2^30 - 1 pairs");
     CK(cudaSetDevice(ctx->device));
-    int rc = wait_frame(ctx);
-    if (rc != GSB_OK) return rc;
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-    // private look-back storage sized for m (the frame path uses the arena's)
+    cudaStream_t s = stream_or_own(ctx, stream);
+    // private look-back words, sort control words and pair count: the frame's control block is left alone
     const uint32_t tiles = (uint32_t)((m + sort_tile_items() - 1) / sort_tile_items());
-    unsigned long long* status = nullptr;
-    CK(dev_alloc(&status, (size_t)tiles * 256));
-    cudaError_t e = cudaMemsetAsync(status, 0, (size_t)tiles * 256 * 8, s);
-    if (e == cudaSuccess) e = cudaMemsetAsync(&ctx->ctl->sort_tile, 0, sizeof(SortCtl), s);  // not the whole block: epoch / overflow_sticky persist
+    const size_t status_bytes = (size_t)tiles * 256 * 8;
+    unsigned char* scratch = nullptr;
+    CK(dev_alloc(&scratch, status_bytes + sizeof(SortCtl) + 4));
+    unsigned long long* status = reinterpret_cast<unsigned long long*>(scratch);
+    SortCtl* sc = reinterpret_cast<SortCtl*>(scratch + status_bytes);
+    uint32_t* d_m = reinterpret_cast<uint32_t*>(sc + 1);
+    cudaError_t e = cudaMemsetAsync(scratch, 0, status_bytes + sizeof(SortCtl), s);
     const uint32_t m32 = (uint32_t)m;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&ctx->ctl->num_instances, &m32, 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_m, &m32, 4, cudaMemcpyHostToDevice, s);
     SortParams sp;
     sp.keys[0] = keys;
     sp.keys[1] = keys_tmp;
     sp.key_bytes = key_bytes;
     sp.vals[0] = vals;
     sp.vals[1] = vals_tmp;
-    sp.d_m = &ctx->ctl->num_instances;
+    sp.d_m = d_m;
     sp.m_hint = m32;
     sp.key_bits = key_bits;
     sp.status = status;
     sp.status_tiles = tiles;
     sp.epoch_base = 8;
-    sp.sc = &ctx->ctl->sort_tile;
+    sp.sc = sc;
     sp.num_sms = ctx->num_sms;
     uint32_t passes = 0;
     if (e == cudaSuccess) e = launch_sort(sp, &passes, s);
@@ -1259,8 +1256,8 @@ static int sort_pairs_impl(gsb_ctx* ctx, void* keys, uint32_t* vals, void* keys_
         e = cudaMemcpyAsync(keys, keys_tmp, m * (size_t)key_bytes, cudaMemcpyDeviceToDevice, s);
         if (e == cudaSuccess) e = cudaMemcpyAsync(vals, vals_tmp, m * 4, cudaMemcpyDeviceToDevice, s);
     }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);  // m32/status lifetime
-    cudaFree(status);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);  // m32/scratch lifetime
+    cudaFree(scratch);
     if (e != cudaSuccess) return fail(ctx, GSB_ERR_CUDA, what, e);
     return GSB_OK;
 }

@@ -77,6 +77,29 @@ struct DetBuffers {
     DevArray<SortCtl> sc;
     DevArray<uint2> runs;    // n (start, ~end) runs, one per possible survivor
 };
+
+struct FramePlan {
+    uint32_t W, H, tiles_x, tiles_y, T, rb, re;
+    uint32_t cs, bins_x, bins;  // instance-sort bins: 2^cs x 2^cs tile blocks (cs = 0: the tiles themselves, bins == T)
+    uint32_t nv_q, m_q, depth_passes, passes;
+    int fin;
+};
+
+// The last frame enqueued on a context, plain or sharded: what gsb_get_stats, gsb_debug_size / _download, the backward pass
+// and the selective gsb_adam_step read about it.  Filled by enqueue_tail only; what ends part of its use (a new frame's
+// enqueue, an arena regrow, gsb_set_backward(0), a scene upload) clears `recorded` or `exists`.
+struct LastFrame {
+    FramePlan plan{};
+    gsb_uniforms ubo{};      // its camera
+    int mode = GSB_MODE_EXACT;
+    uint64_t scene_gen = 0;  // gsb_ctx::scene_gen when enqueued; 0: no frame yet (a frame needs an upload, which bumps it)
+    bool pending = false;    // its completion event and stats copy have not been waited for (wait_frame)
+    bool exists = false;     // its stats and debug buffers may be read (a scene upload clears it)
+    bool debug = false;      // ran with gsb_set_debug on (its debug buffers and sorted keys exist)
+    bool timers = false;     // recorded the stage events (gsb_get_stats may read them)
+    bool recorded = false;   // its backward state is stored: per-pixel record and per-tile lists (gsb_set_backward, cs == 0)
+    bool band = false;       // a band of tile rows, not the whole frame
+};
 }  // namespace gsb
 using gsb::Control;
 using gsb::DevArray;
@@ -137,10 +160,7 @@ struct gsb_ctx {
     cudaEvent_t ev[8] = {};
     cudaEvent_t ev_sort[9] = {};  // instance sort: after hist, after each pass
     cudaEvent_t ev_done = nullptr;
-    bool frame_pending = false;
-    bool have_frame = false;
-    bool frame_debug = false;   // the last frame ran with gsb_set_debug on (its debug buffers and sorted keys exist)
-    bool frame_timers = false;  // the last frame recorded the stage events (gsb_get_stats may read them)
+    gsb::LastFrame frame;
     bool host_direct = true;    // gsb_render to page-locked host memory: blend straight into it (GSB_HOST_DIRECT=0: always stage)
     bool use_graph = true;      // replay the sorts + key emission from a captured CUDA graph when timers and debug are off
     uint64_t alloc_gen = 0;     // bumped by every (re)allocation a captured graph could point into
@@ -150,9 +170,6 @@ struct gsb_ctx {
     uint32_t m_hint = 0;
     uint32_t nv_hint = 0;
     uint32_t regrow_count = 0;
-
-    // description of the last frame (for stats / debug download)
-    uint32_t last_tiles_x = 0, last_tiles_y = 0, last_passes = 0, last_depth_passes = 0, last_final = 0;
 
     // debug copies
     DevArray<uint32_t> dbg_tiles;
@@ -169,13 +186,7 @@ struct gsb_ctx {
     DevArray<double> bw_abs;        // n x 2 per-survivor fp64 sums of |d u|, |d v| of gsb_render_backward_density (kept zero)
     bool bw_deterministic = false;  // gsb_set_backward_deterministic
     gsb::DetBuffers bw_det;
-    uint64_t scene_gen = 0;         // bumped by every gsb_scene_upload
-    bool any_frame = false;         // a frame has been rendered on this context since its creation
-    bool frame_recorded = false;    // the last frame stored the backward state (whole frame, per-tile lists)
-    bool frame_band = false;        // the last frame was a band of tile rows
-    uint64_t frame_scene_gen = 0;   // scene_gen of the last frame
-    int frame_mode = GSB_MODE_EXACT;
-    gsb_uniforms last_ubo{};        // the last frame's camera
+    uint64_t scene_gen = 0;         // bumped by every gsb_scene_upload and gsb_adam_step
 
     // gsb_image_loss (gsb_loss.cu): allocated on first use, grown with the frame size
     DevArray<float> loss_abc;        // 9 x W x H: the gather terms A, B, C of each RGB channel (only for a gradient)
@@ -196,12 +207,8 @@ int fail(gsb_ctx* c, int code, const char* what, cudaError_t e = cudaSuccess);
         if (e_ != cudaSuccess) return gsb::fail(ctx, e_ == cudaErrorMemoryAllocation ? GSB_ERR_OOM : GSB_ERR_CUDA, #call, e_); \
     } while (0)
 
-struct FramePlan {
-    uint32_t W, H, tiles_x, tiles_y, T, rb, re;
-    uint32_t cs, bins_x, bins;  // instance-sort bins: 2^cs x 2^cs tile blocks (cs = 0: the tiles themselves, bins == T)
-    uint32_t nv_q, m_q, depth_passes, passes;
-    int fin;
-};
+// the caller's stream of an entry point, or the context's own for NULL
+inline cudaStream_t stream_or_own(const gsb_ctx* ctx, void* s) { return s ? static_cast<cudaStream_t>(s) : ctx->stream; }
 
 void drop_graphs(gsb_ctx* ctx);
 int ensure_sort_status(gsb_ctx* ctx, uint64_t items);
@@ -220,7 +227,7 @@ int enqueue_middle(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, cudaS
 int launch_middle_graph(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, cudaStream_t stream);
 int enqueue_blend(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, uint32_t b0, uint32_t b1, void* band_out, size_t pitch,
                   int fmt, cudaStream_t stream, void* const* peer_frames = nullptr, int num_peer_frames = 0);
-int enqueue_tail(gsb_ctx* ctx, const FramePlan& fp, cudaStream_t stream);
+int enqueue_tail(gsb_ctx* ctx, const FramePlan& fp, const gsb_uniforms& ubo, cudaStream_t stream);
 int check_image(gsb_ctx* ctx, const gsb_uniforms* ubo, int fmt);
 int check_render_args(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t& rb, uint32_t& re, const void* out, size_t& pitch, int fmt);
 

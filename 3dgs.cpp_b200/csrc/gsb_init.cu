@@ -339,7 +339,7 @@ extern "C" int gsb_init_from_points(gsb_ctx* ctx, const float* xyz, const float*
     if (n >= (1ull << 30)) return bad("limited to 2^30 - 1 points");
     if (!(opacity > 0.0f && opacity < 1.0f)) return bad("opacity outside (0, 1) or NaN");
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s = stream_or_own(ctx, stream);
 
     // the implicit tree: level 0 = leaves of 32 sorted points, level l + 1 groups 32 nodes of level l
     Tree T{};

@@ -50,7 +50,7 @@ struct Control {
     unsigned long long blend_hits;        // (pixel, Gaussian) pairs of those visits that passed the shader's tests
     unsigned long long blend_staged;      // records gathered into shared memory by the blend
     SortCtl sort_depth;        // Gaussian-level sort (32-bit depth keys)
-    SortCtl sort_tile;         // instance-level sort (tile-id keys); also used by gsb_sort_pairs
+    SortCtl sort_tile;         // instance-level sort (tile-id keys)
     // frame sharding (gsb_shard.cu): per-destination-band survivor totals of the routed k_project
     uint32_t route_total[GSB_MAX_SHARDS];
 };

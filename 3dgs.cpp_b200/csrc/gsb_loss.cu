@@ -309,7 +309,7 @@ extern "C" int gsb_image_loss(gsb_ctx* ctx, uint32_t width, uint32_t height, con
     const double n = 3.0 * (double)pixels;
     P.k_l1 = (float)((1.0 - (double)lambda_dssim) / n);
     P.k_ssim = (float)((double)lambda_dssim / n);
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s = stream_or_own(ctx, stream);
     k_loss_forward<<<tiles, L_THREADS, 0, s>>>(P);
     CK(cudaGetLastError());
     if (grad_image) {

@@ -429,7 +429,7 @@ int enqueue_sharded_phase(gsb_ctx* ctx, ShardFrame& F, int phase) {
     k_shard_wait<<<1, 32, 0, stream>>>(mb->framed, F.f, G, &mb->error, WAIT_TIMEOUT_CYCLES);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(sh->mailbox_host, mb, sizeof(Mailbox), cudaMemcpyDeviceToHost, stream));
-    return enqueue_tail(ctx, F.fp, stream);
+    return enqueue_tail(ctx, F.fp, F.ubo, stream);
 }
 
 // Enqueue one sharded frame of ONE rank on `stream`.  Collective: every rank enqueues the same frame; never blocks the host.
@@ -659,7 +659,7 @@ int gsb_render_sharded_async(gsb_ctx* ctx, const gsb_uniforms* ubo, gsb_format f
     rc = ensure_frame_ipc(ctx, ubo, fmt);
     if (rc != GSB_OK) return rc;
     poll_frame(ctx);
-    return enqueue_sharded(ctx, ubo, fmt, stream ? static_cast<cudaStream_t>(stream) : ctx->stream);
+    return enqueue_sharded(ctx, ubo, fmt, stream_or_own(ctx, stream));
 }
 
 int gsb_render_sharded(gsb_ctx* ctx, const gsb_uniforms* ubo, void* out, size_t pitch, gsb_memory out_mem, gsb_format fmt, void* stream) {
@@ -669,7 +669,7 @@ int gsb_render_sharded(gsb_ctx* ctx, const gsb_uniforms* ubo, void* out, size_t 
     CK(cudaSetDevice(ctx->device));
     rc = ensure_frame_ipc(ctx, ubo, fmt);
     if (rc != GSB_OK) return rc;
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s = stream_or_own(ctx, stream);
     for (int attempt = 0;; attempt++) {
         rc = enqueue_sharded(ctx, ubo, fmt, s);
         if (rc != GSB_OK) return rc;

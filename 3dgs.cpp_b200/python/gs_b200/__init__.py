@@ -508,15 +508,30 @@ class Context:
         overwritten; grad_vertices_ptr may then be None (a frozen scene).
         With density_ptr (n x 4 floats of device memory), gsb_render_backward_density: also accumulates the frame's
         density-control statistics into it; either gradient output may then be None, but not both."""
+        self._backward(vertices_ptr, grad_image_ptr, grad_vertices_ptr, stream_ptr(stream), row_pitch_bytes,
+                       grad_uniforms_ptr, density_ptr)
+
+    def _backward(self, vertices_ptr, grad_image_ptr, grad_vertices_ptr, stream, row_pitch_bytes=0, grad_uniforms_ptr=None,
+                  density_ptr=None):
+        """render_backward with `stream` already the C ABI's cudaStream_t argument."""
         if density_ptr is not None:
             self._ck(lib.gsb_render_backward_density(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
-                                                     grad_uniforms_ptr, density_ptr, stream_ptr(stream)))
+                                                     grad_uniforms_ptr, density_ptr, stream))
         elif grad_uniforms_ptr is None:
-            self._ck(lib.gsb_render_backward(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
-                                             stream_ptr(stream)))
+            self._ck(lib.gsb_render_backward(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr, stream))
         else:
             self._ck(lib.gsb_render_backward_camera(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
-                                                    grad_uniforms_ptr, stream_ptr(stream)))
+                                                    grad_uniforms_ptr, stream))
+
+    def _render_whole_frame(self, u: Uniforms, device):
+        """The whole frame of u, recorded while gsb_set_backward is on, as a new tensor on torch's current stream."""
+        import torch
+
+        img = torch.empty((u.height, u.width, 4), dtype=torch.float32, device=device)
+        self.frames += 1
+        self._ck(lib.gsb_render(self.h, C.byref(u), 0, ALL_ROWS, img.data_ptr(), 0, MEM_DEVICE, FORMAT_RGBA32F,
+                                _torch_stream_arg(torch.cuda.current_stream(device))))
+        return img
 
     def image_loss(self, image, target, lambda_dssim=0.2, grad_image=None, stream=None):
         """gsb_image_loss on torch tensors: the photometric loss (1 - lambda) L1 + lambda (1 - SSIM) of `image` against
@@ -634,6 +649,16 @@ def _torch_stream_arg(torch_stream):
     return C.c_void_p(torch_stream.cuda_stream or CUDA_STREAM_LEGACY)
 
 
+def _check_density(caller, density, vertices):
+    """ValueError unless density is None or the contiguous (n, 4) float32 table of the (n, 60) vertices, on their device."""
+    import torch
+
+    n = vertices.shape[0]
+    if density is not None and (density.dtype != torch.float32 or tuple(density.shape) != (n, 4)
+                                or density.device != vertices.device or not density.is_contiguous()):
+        raise ValueError(f"{caller}: density must be a contiguous ({n}, 4) float32 tensor on the vertices' device")
+
+
 def _render_fn():
     global _RenderFn
     if _RenderFn is None:
@@ -643,21 +668,15 @@ def _render_fn():
             @staticmethod
             def forward(fctx, ctx, vertices, u, ubo, density):
                 v = vertices.detach().contiguous()
-                if density is not None and (density.dtype != torch.float32 or density.shape != (v.shape[0], 4)
-                                            or density.device != v.device or not density.is_contiguous()):
-                    raise ValueError("render_torch: density must be a contiguous (n, 4) float32 tensor on the vertices' device")
+                _check_density("render_torch", density, v)
                 fctx.density = density
                 if ubo is not None:  # the camera's float fields come from the tensor, the frame size from u
                     u = unpack_uniforms(ubo.detach().to("cpu", torch.float32).numpy(), u.width, u.height)
                     fctx.ubo_like = (ubo.dtype, ubo.device)
                 ctx.set_backward(True)
-                stream = torch.cuda.current_stream(v.device)
-                stream.synchronize()  # the upload runs on the context's own stream: v must be complete
+                torch.cuda.current_stream(v.device).synchronize()  # the upload runs on the context's stream: v must be complete
                 ctx.upload(v)
-                img = torch.empty((u.height, u.width, 4), dtype=torch.float32, device=v.device)
-                ctx.frames += 1
-                ctx._ck(lib.gsb_render(ctx.h, C.byref(u), 0, ALL_ROWS, img.data_ptr(), 0, MEM_DEVICE, FORMAT_RGBA32F,
-                                       _torch_stream_arg(stream)))
+                img = ctx._render_whole_frame(u, v.device)
                 fctx.gs_ctx, fctx.frame, fctx.vertices = ctx, ctx.frames, v
                 return img
 
@@ -676,16 +695,9 @@ def _render_fn():
                 stream = _torch_stream_arg(torch.cuda.current_stream(v.device))
                 gu = torch.empty(40, dtype=torch.float32, device=v.device) if need_ubo else None  # a whole gsb_uniforms
                 ctx.set_backward_deterministic(torch.are_deterministic_algorithms_enabled())
-                if fctx.density is not None:
-                    ctx._ck(lib.gsb_render_backward_density(ctx.h, v.data_ptr(), g.data_ptr(), 0,
-                                                            grad_v.data_ptr() if need_v else None,
-                                                            gu.data_ptr() if need_ubo else None, fctx.density.data_ptr(),
-                                                            stream))
-                elif need_ubo:
-                    ctx._ck(lib.gsb_render_backward_camera(ctx.h, v.data_ptr(), g.data_ptr(), 0,
-                                                           grad_v.data_ptr() if need_v else None, gu.data_ptr(), stream))
-                else:
-                    ctx._ck(lib.gsb_render_backward(ctx.h, v.data_ptr(), g.data_ptr(), 0, grad_v.data_ptr(), stream))
+                ctx._backward(v.data_ptr(), g.data_ptr(), grad_v.data_ptr() if need_v else None, stream,
+                              grad_uniforms_ptr=gu.data_ptr() if need_ubo else None,
+                              density_ptr=None if fctx.density is None else fctx.density.data_ptr())
                 if need_ubo:
                     dtype, device = fctx.ubo_like
                     grad_ubo = gu[UBO_FLOAT_WORDS].to(device=device, dtype=dtype)
@@ -884,13 +896,7 @@ class SceneAdam:
     def render(self, u: Uniforms):
         """The resident scene's frame of u as an (H, W, 4) float32 tensor, rendered on torch's current stream with the
         backward state recorded.  No upload."""
-        import torch
-
-        img = torch.empty((u.height, u.width, 4), dtype=torch.float32, device=self.vertices.device)
-        self.ctx.frames += 1
-        self.ctx._ck(lib.gsb_render(self.ctx.h, C.byref(u), 0, ALL_ROWS, img.data_ptr(), 0, MEM_DEVICE, FORMAT_RGBA32F,
-                                    _torch_stream_arg(torch.cuda.current_stream(img.device))))
-        return img
+        return self.ctx._render_whole_frame(u, self.vertices.device)
 
     def step(self, grad_image, density=None):
         """One training step from dL/d(the last render()'s image), an (H, W, 4) float32 tensor: gsb_render_backward into
@@ -902,13 +908,9 @@ class SceneAdam:
         g = grad_image.detach().to(torch.float32).contiguous()
         stream = _torch_stream_arg(torch.cuda.current_stream(v.device))
         ctx.set_backward_deterministic(torch.are_deterministic_algorithms_enabled())
-        if density is None:
-            ctx._ck(lib.gsb_render_backward(ctx.h, v.data_ptr(), g.data_ptr(), 0, self.grad.data_ptr(), stream))
-        else:
-            if density.dtype != torch.float32 or tuple(density.shape) != (v.shape[0], 4) or not density.is_contiguous():
-                raise ValueError(f"SceneAdam.step: density must be a contiguous ({v.shape[0]}, 4) float32 tensor")
-            ctx._ck(lib.gsb_render_backward_density(ctx.h, v.data_ptr(), g.data_ptr(), 0, self.grad.data_ptr(), None,
-                                                    density.data_ptr(), stream))
+        _check_density("SceneAdam.step", density, v)
+        ctx._backward(v.data_ptr(), g.data_ptr(), self.grad.data_ptr(), stream,
+                      density_ptr=None if density is None else density.data_ptr())
         self.steps += 1
         ctx.adam_step(self.params, self.exp_avg, self.exp_avg_sq, self.grad, v,
                       adam_config(self.lr, self.betas, self.eps, self.steps, self.selective))

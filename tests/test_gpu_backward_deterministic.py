@@ -226,6 +226,29 @@ def test_nothing_visible_and_empty_scene(gs, c1):
         ctx.close()
 
 
+def test_standalone_sort_leaves_the_frame_alone(gs, c1):
+    """gsb_sort_pairs32 of unrelated pairs between a recorded frame and its deterministic backward changes no output word:
+    the sort keeps its own control words and pair count, so the backward still groups the frame's whole instance list."""
+    torch = _torch()
+    v, u, _ = c1
+    gi = _grad_image(u)
+    ctx = _new_ctx(gs, v)
+    try:
+        _frame(ctx, u, 0, 0)
+        want = _backward(ctx, v, gi, "plain")
+        m = ctx.stats().num_instances // 3  # well below the frame's M: no read past the arena whatever the sort does
+        assert m >= 16
+        keys = torch.randint(0, 1 << 16, (m,), dtype=torch.int32, device="cuda")
+        vals = torch.arange(m, dtype=torch.int32, device="cuda")
+        keys_tmp, vals_tmp = torch.empty_like(keys), torch.empty_like(vals)
+        torch.cuda.synchronize()  # the sort runs on the context's stream
+        ctx.sort_pairs32(keys.data_ptr(), vals.data_ptr(), keys_tmp.data_ptr(), vals_tmp.data_ptr(), m, 16)
+        assert bool((keys[1:] >= keys[:-1]).all())
+        _same_words(_backward(ctx, v, gi, "plain"), want)
+    finally:
+        ctx.close()
+
+
 def test_switch_error_codes(gs):
     assert gs.lib.gsb_set_backward_deterministic(None, 1) == gs.ERR_INVALID
     grp = gs.Group([0, 0])
