@@ -395,12 +395,15 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         const float a = cov.m00, b = cov.m10, c = cov.m11;  // b: the [1][0] entry, rounded like k_project's m10
         const float det = a * c - b * b;
 
-        // ---- conic = (c, -b, a) / det  ->  cov2d (a, b, c) ----
-        const float id2 = 1.0f / (det * det);
+        // ---- conic K = (c, -b, a) / det  ->  cov2d (a, b, c): dL/dcov2d = -K dL/dK K ----
+        // From k_project's conic (ood = 1 / det) rather than 1 / det^2: det^2 overflows past det ~ 1.8e19 (an isotropic sigma of
+        // ~6.5e4 px), while the products of K stay normal from the 0.3 dilation floor to sigma ~ 1e9 px.
+        const float ood = 1.0f / det;
+        const float k00 = c * ood, k01 = -b * ood, k11 = a * ood;
         const float dA = d[2], dB = d[3], dC = d[4];
-        const float da = id2 * ((-c * c * dA + b * c * dB) - b * b * dC);
-        const float db = id2 * ((2.0f * b * c * dA - (det + 2.0f * b * b) * dB) + 2.0f * a * b * dC);
-        const float dc = id2 * ((-b * b * dA + a * b * dB) - a * a * dC);
+        const float da = -((k00 * k00 * dA + k00 * k01 * dB) + k01 * k01 * dC);
+        const float db = -((2.0f * k00 * k01 * dA + (k00 * k11 + k01 * k01) * dB) + 2.0f * k01 * k11 * dC);
+        const float dc = -((k01 * k01 * dA + k01 * k11 * dB) + k11 * k11 * dC);
         // cov2d = (J W) Sigma (J W)^T: dL/dSigma (symmetric) and dL/d(J W)
         float G[3][3];
 #pragma unroll

@@ -165,12 +165,14 @@ def tiles(u, frame, local):
                    torch.tensor(local[ids]))
 
 
-def reference(vertices, u, frame, grad_image=None, camera=False):
+def reference(vertices, u, frame, grad_image=None, camera=False, cut_conic=None):
     """Float64 image (H, W, 3) of the frame whose oracle lists are `frame` (oracle.render_frame of the same vertices / u) and,
     if grad_image (H, W, >= 3) is given, dL/dvertices (n, 60) for L = sum(grad_image[..., :3] * image) plus `exclude` (n,):
     Gaussians whose gradient is ill-posed at float64 / fp32 resolution (unclamped red within 1e-4 of 0, or raw alpha within
     1e-4 of the 0.99 clamp on a pixel with a non-zero upstream gradient).  camera=True also returns grad_ubo: dL/d(the 38
-    float fields of u in ABI order: camera_position[4], proj_mat[16], view_mat[16], tan_fovx, tan_fovy)."""
+    float fields of u in ABI order: camera_position[4], proj_mat[16], view_mat[16], tan_fovx, tan_fovy).  cut_conic (n,)
+    bool: the conics of these Gaussians are detached, so no gradient flows through them (what a backward pass that drops
+    the conic path of those rows would compute)."""
     v_all, used, local = survivors(vertices, frame)
     n = v_all.shape[0]
     W, H = int(u.width), int(u.height)
@@ -178,6 +180,9 @@ def reference(vertices, u, frame, grad_image=None, camera=False):
     cam = camera_leaves(u) if camera else None
     with torch.set_grad_enabled(grad_image is not None):
         uv, conic, op, col, red = preprocess(leaf, u, cam)
+        if cut_conic is not None:
+            cut = torch.from_numpy(np.asarray(cut_conic, bool)[used])[:, None]
+            conic = torch.where(cut, conic.detach(), conic)
     # per-tile blends against detached copies; their gradients are chained through preprocess once at the end
     parts = [t.detach().clone().requires_grad_(grad_image is not None) for t in (uv, conic, op, col)]
     image = np.zeros((H, W, 3), np.float64)

@@ -49,9 +49,11 @@ def _row_ratio(got, ref, rows, cols, atol):
     return float((d / (RTOL * r + atol)).max()) if k else 0.0
 
 
-def _check_vertices(got, ref, keep, sets, what):
+def _check_vertices(got, ref, keep, sets, what, set_atol=False, min_rows=10):
     """The per-group norm check over `keep` at 1e-3, the per-Gaussian check over `keep`, and both again over each named
-    subset of `keep` in `sets` (name -> bool mask), each of which must hold Gaussians with a gradient."""
+    subset of `keep` in `sets` (name -> bool mask), each of which must hold min_rows Gaussians with a gradient.  The per-Gaussian
+    check's absolute tolerance comes from the rows of `keep`, or with set_atol=True from each set's own rows: a set whose
+    gradients are all far below the others' (sub-pixel or huge Gaussians) is then held to its own scale."""
     assert np.isfinite(got).all(), what
     assert not got[:, 3].any(), what  # position.w
     worst = {}
@@ -61,15 +63,17 @@ def _check_vertices(got, ref, keep, sets, what):
         assert r <= 1e-3, (what, name, r)
         worst[name] = _row_ratio(got, ref, keep, cols, atol)
         for sname, rows in sets.items():
-            if np.linalg.norm(ref[rows][:, cols]) > 0:
+            live = np.linalg.norm(ref[rows][:, cols]) > 0
+            if live:
                 rs = rel(got[rows][:, cols], ref[rows][:, cols])
                 assert rs <= 1e-3, (what, sname, name, rs)
-            worst[f"{sname}/{name}"] = _row_ratio(got, ref, rows, cols, atol)
+            tol = _atol(ref, rows, cols) if set_atol and live else atol
+            worst[f"{sname}/{name}"] = _row_ratio(got, ref, rows, cols, tol)
     print(what, "max per-Gaussian error / tolerance:", {k: f"{v:.3g}" for k, v in worst.items()})
     for k, v in worst.items():
         assert v <= 1.0, (what, k, v)
     for sname, rows in sets.items():
-        assert (np.abs(ref[rows]).sum(1) > 0).sum() >= 10, (what, sname)
+        assert (np.abs(ref[rows]).sum(1) > 0).sum() >= min_rows, (what, sname)
 
 
 def _check_density(got, ref, keep, what):
