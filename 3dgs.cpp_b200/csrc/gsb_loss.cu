@@ -8,14 +8,15 @@
 //                    give the five moments of every pixel.  Per pixel it evaluates S, |x - y| and (x - y)^2 and, when a
 //                    gradient is wanted, the gather terms A, B, C of S's derivative into the context's scratch.  Per CTA it
 //                    stores fp64 sums of |d|, d^2 and S, reduced in a fixed order.
-//   k_loss_backward  one CTA per tile (gradient only): stages A, B, C with a halo of 5, blurs them with the same window and
-//                    stores d loss / d x = (1 - lambda)/N sign(x - y) - lambda/N (w*A + 2 x (w*B) + y (w*C)) as float4(r, g, b, 0).
+//   k_loss_backward  one CTA per tile (gradient only): stages A, B, C and x, y with a halo of 5, blurs A, B, x B, C and y C
+//                    with the same window and stores d loss / d x = (1 - lambda)/N sign(x - y) - lambda/N d S / d x as
+//                    float4(r, g, b, 0).
 //   k_loss_reduce    one CTA: sums the per-tile rows in a fixed order in fp64 and writes loss, L1, SSIM, MSE.
 //
-// The moments are taken of x - 1/2 and y - 1/2 (the zero padding then reads -1/2): sigma^2 = E[x^2] - mu^2 cancels less in
-// fp32 around 0 than around 1/2, and the variances and covariance do not depend on the shift (mu is corrected back).  The
-// gather terms use the shifted values as well, which keeps w*A and 2 x (w*B) small.  No atomics: every output word is a
-// function of the inputs alone.  Compiled with -fmad=false like the rest of the library; fused ops are spelled fmaf.
+// The window passes and everything per pixel run in fp64: sigma^2 = E[x^2] - mu^2 cancels completely over a flat window,
+// and in fp32 the residue (~1e-7 x^2, of one sign over a whole flat region) divided by C2 = 9e-4 biased S by up to 6e-5 on
+// sky, backgrounds and saturated areas.  A, B and C are stored as fp32.  No atomics: every output word is a function of
+// the inputs alone.  Compiled with -fmad=false like the rest of the library; fused ops are spelled fma / fmaf.
 #include "gsb_ctx.cuh"
 
 namespace gsb {
@@ -31,13 +32,25 @@ constexpr int LH_N = LS_H * LT_W;            // horizontal pass output: 26 rows 
 constexpr int L_THREADS = 256;               // two output pixels per thread: rows r and r + 8 of column lane
 constexpr int L_PIX = LT_W * LT_H / L_THREADS;
 constexpr int LR_THREADS = 1024;
-constexpr float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;
+constexpr double C1 = 0.01 * 0.01, C2 = 0.03 * 0.03;
 constexpr unsigned FULL = 0xffffffffu;
 
-// g[i] = exp(-(i - 5)^2 / 4.5) / sum, rounded once from the float64 values
-__constant__ float c_win[L_K] = {1.028380124e-03f, 7.598758209e-03f, 3.600077331e-02f, 1.093606874e-01f, 2.130055428e-01f,
-                                 2.660117149e-01f, 2.130055428e-01f, 1.093606874e-01f, 3.600077331e-02f, 7.598758209e-03f,
-                                 1.028380124e-03f};
+// g[i] = exp(-(i - 5)^2 / 4.5) / sum in float64
+__constant__ double c_win[L_K] = {0.00102838008447911, 0.007598758135239185, 0.03600077212843083, 0.10936068950970002,
+                                  0.2130055377112537,  0.26601172486179436,  0.2130055377112537,  0.10936068950970002,
+                                  0.03600077212843083, 0.007598758135239185, 0.00102838008447911};
+
+// dynamic shared memory of the two tile kernels (more than the 48 KB of static shared memory)
+struct ForwardSmem {
+    double h[5][LH_N];                 // horizontal pass: x, y, x^2, y^2, x y
+    float x[3][LS_N], y[3][LS_N];      // 0 outside the frame
+    double warp[L_THREADS / 32];
+};
+struct BackwardSmem {
+    double h[5][LH_N];                 // horizontal pass: A, B, x B, C, y C
+    float x[3][LS_N], y[3][LS_N];      // 0 outside the frame
+    float t[3][LS_N];                  // A, B, C of one channel, 0 outside the frame
+};
 
 struct LossParams {
     const float4* image;
@@ -52,7 +65,7 @@ struct LossParams {
     uint32_t num_tiles;
     float4* grad;
     size_t grad_pitch;
-    float k_l1, k_ssim;       // (1 - lambda) / N, lambda / N
+    double k_l1, k_ssim;      // (1 - lambda) / N, lambda / N
 };
 
 __device__ __forceinline__ float4 load_target(const LossParams& P, uint32_t x, uint32_t y) {
@@ -68,7 +81,19 @@ __device__ __forceinline__ float4 load_image(const LossParams& P, uint32_t x, ui
     return reinterpret_cast<const float4*>(reinterpret_cast<const unsigned char*>(P.image) + (size_t)y * P.image_pitch)[x];
 }
 
-__device__ __forceinline__ float chan(const float4& v, int c) { return c == 0 ? v.x : (c == 1 ? v.y : v.z); }
+// Stages the tile's x and y with a halo of L_R (0 outside the frame) as three planes each.
+__device__ __forceinline__ void stage_xy(const LossParams& P, int x0, int y0, float (*s_x)[LS_N], float (*s_y)[LS_N]) {
+    for (int i = threadIdx.x; i < LS_N; i += L_THREADS) {
+        const int gx = x0 + i % LS_W, gy = y0 + i / LS_W;
+        float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
+        if (gx >= 0 && gy >= 0 && gx < (int)P.width && gy < (int)P.height) {
+            a = load_image(P, gx, gy);
+            b = load_target(P, gx, gy);
+        }
+        s_x[0][i] = a.x; s_x[1][i] = a.y; s_x[2][i] = a.z;
+        s_y[0][i] = b.x; s_y[1][i] = b.y; s_y[2][i] = b.z;
+    }
+}
 
 // Sums v over the CTA in a fixed order: a shuffle tree per warp, then the warps in order by thread 0.
 __device__ __forceinline__ double cta_sum(double v, double* s_warp) {
@@ -84,41 +109,30 @@ __device__ __forceinline__ double cta_sum(double v, double* s_warp) {
 }
 
 __global__ void __launch_bounds__(L_THREADS) k_loss_forward(const __grid_constant__ LossParams P) {
-    __shared__ float s_x[3][LS_N], s_y[3][LS_N];  // unshifted values, 0 outside the frame
-    __shared__ float s_h[5][LH_N];                 // horizontal pass: x, y, x^2, y^2, x y (shifted)
-    __shared__ double s_warp[L_THREADS / 32];
+    extern __shared__ __align__(16) unsigned char l_smem[];
+    ForwardSmem& S = *reinterpret_cast<ForwardSmem*>(l_smem);
     const uint32_t tx = blockIdx.x % P.tiles_x, ty = blockIdx.x / P.tiles_x;
-    const int x0 = (int)(tx * LT_W) - L_R, y0 = (int)(ty * LT_H) - L_R;
-    for (int i = threadIdx.x; i < LS_N; i += L_THREADS) {
-        const int gx = x0 + i % LS_W, gy = y0 + i / LS_W;
-        float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
-        if (gx >= 0 && gy >= 0 && gx < (int)P.width && gy < (int)P.height) {
-            a = load_image(P, gx, gy);
-            b = load_target(P, gx, gy);
-        }
-        s_x[0][i] = a.x; s_x[1][i] = a.y; s_x[2][i] = a.z;
-        s_y[0][i] = b.x; s_y[1][i] = b.y; s_y[2][i] = b.z;
-    }
+    stage_xy(P, (int)(tx * LT_W) - L_R, (int)(ty * LT_H) - L_R, S.x, S.y);
     const int col = threadIdx.x & 31, row0 = threadIdx.x >> 5;
     double sum_abs = 0.0, sum_sq = 0.0, sum_s = 0.0;
     for (int c = 0; c < 3; c++) {
-        __syncthreads();  // staging done / the previous channel's vertical pass has read s_h
+        __syncthreads();  // staging done / the previous channel's vertical pass has read S.h
         for (int i = threadIdx.x; i < LH_N; i += L_THREADS) {
             const int r = i / LT_W, cc = i % LT_W;
-            const float* px = &s_x[c][r * LS_W + cc];
-            const float* py = &s_y[c][r * LS_W + cc];
-            float m0 = 0.f, m1 = 0.f, m2 = 0.f, m3 = 0.f, m4 = 0.f;
+            const float* px = &S.x[c][r * LS_W + cc];
+            const float* py = &S.y[c][r * LS_W + cc];
+            double m0 = 0.0, m1 = 0.0, m2 = 0.0, m3 = 0.0, m4 = 0.0;
 #pragma unroll
             for (int k = 0; k < L_K; k++) {
-                const float w = c_win[k], a = px[k] - 0.5f, b = py[k] - 0.5f;
-                const float wa = w * a, wb = w * b;
+                const double w = c_win[k], a = px[k], b = py[k];
+                const double wa = w * a, wb = w * b;
                 m0 += wa;
                 m1 += wb;
-                m2 = fmaf(wa, a, m2);
-                m3 = fmaf(wb, b, m3);
-                m4 = fmaf(wa, b, m4);
+                m2 = fma(wa, a, m2);
+                m3 = fma(wb, b, m3);
+                m4 = fma(wa, b, m4);
             }
-            s_h[0][i] = m0; s_h[1][i] = m1; s_h[2][i] = m2; s_h[3][i] = m3; s_h[4][i] = m4;
+            S.h[0][i] = m0; S.h[1][i] = m1; S.h[2][i] = m2; S.h[3][i] = m3; S.h[4][i] = m4;
         }
         __syncthreads();
 #pragma unroll
@@ -126,38 +140,38 @@ __global__ void __launch_bounds__(L_THREADS) k_loss_forward(const __grid_constan
             const int r = row0 + j * (L_THREADS / 32);
             const uint32_t gx = tx * LT_W + col, gy = ty * LT_H + r;
             if (gx >= P.width || gy >= P.height) continue;
-            float m[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+            double m[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
 #pragma unroll
             for (int k = 0; k < L_K; k++) {
-                const float w = c_win[k];
+                const double w = c_win[k];
 #pragma unroll
-                for (int q = 0; q < 5; q++) m[q] = fmaf(w, s_h[q][(r + k) * LT_W + col], m[q]);
+                for (int q = 0; q < 5; q++) m[q] = fma(w, S.h[q][(r + k) * LT_W + col], m[q]);
             }
-            const float mx = m[0], my = m[1];                      // shifted means
-            const float vx = fmaf(-mx, mx, m[2]), vy = fmaf(-my, my, m[3]), cxy = fmaf(-mx, my, m[4]);
-            const float ux = mx + 0.5f, uy = my + 0.5f;            // the means themselves
-            const float a1 = fmaf(2.0f * ux, uy, C1), a2 = fmaf(2.0f, cxy, C2);
-            const float b1 = fmaf(ux, ux, fmaf(uy, uy, C1)), b2 = vx + vy + C2;
-            const float inv = 1.0f / (b1 * b2);
-            const float s = a1 * a2 * inv;
+            const double ux = m[0], uy = m[1];
+            const double vx = fma(-ux, ux, m[2]), vy = fma(-uy, uy, m[3]), cxy = fma(-ux, uy, m[4]);
+            const double a1 = fma(2.0 * ux, uy, C1), a2 = fma(2.0, cxy, C2);
+            const double b1 = fma(ux, ux, fma(uy, uy, C1)), b2 = vx + vy + C2;
+            const double r1 = 1.0 / b1, r2 = 1.0 / b2;
+            const double s = a1 * a2 * (r1 * r2);
             const int si = (r + L_R) * LS_W + col + L_R;
-            const float xv = s_x[c][si], yv = s_y[c][si], d = xv - yv;
+            const float xv = S.x[c][si], yv = S.y[c][si], d = xv - yv;
             sum_abs += (double)fabsf(d);
             sum_sq += (double)d * (double)d;
-            sum_s += (double)s;
+            sum_s += s;
             if (P.abc) {
-                const float dmx = 2.0f * uy * a2 * inv - 2.0f * ux * s / b1;  // dS / d mu_x
-                const float B = -s / b2;                                     // dS / d sigma_x^2
-                const float Cc = 2.0f * a1 * inv;                            // dS / d sigma_xy
-                const float A = dmx - 2.0f * mx * B - my * Cc;
+                const double dmx = 2.0 * uy * a2 * (r1 * r2) - 2.0 * ux * s * r1;  // dS / d mu_x
+                const double B = -s * r2;                                           // dS / d sigma_x^2
+                const double Cc = 2.0 * a1 * (r1 * r2);                             // dS / d sigma_xy
+                // A relative to the pixel's own values: small where the window is flat (section 11)
+                const double A = dmx - 2.0 * (ux - (double)xv) * B - (uy - (double)yv) * Cc;
                 const size_t p = (size_t)gy * P.width + gx;
-                P.abc[(3 * c + 0) * P.plane + p] = A;
-                P.abc[(3 * c + 1) * P.plane + p] = B;
-                P.abc[(3 * c + 2) * P.plane + p] = Cc;
+                P.abc[(3 * c + 0) * P.plane + p] = (float)A;
+                P.abc[(3 * c + 1) * P.plane + p] = (float)B;
+                P.abc[(3 * c + 2) * P.plane + p] = (float)Cc;
             }
         }
     }
-    const double t0 = cta_sum(sum_abs, s_warp), t1 = cta_sum(sum_sq, s_warp), t2 = cta_sum(sum_s, s_warp);
+    const double t0 = cta_sum(sum_abs, S.warp), t1 = cta_sum(sum_sq, S.warp), t2 = cta_sum(sum_s, S.warp);
     if (threadIdx.x == 0) {
         P.partials[blockIdx.x] = t0;
         P.partials[P.num_tiles + blockIdx.x] = t1;
@@ -165,58 +179,58 @@ __global__ void __launch_bounds__(L_THREADS) k_loss_forward(const __grid_constan
     }
 }
 
+// d S / d x_q = sum_p w(q - p) (A_p + 2 (x_q - x_p) B_p + (y_q - y_p) C_p), gathered as
+// w*A + 2 (x_q (w*B) - w*(x B)) + (y_q (w*C) - w*(y C)) in fp64: the two differences cancel where the window is flat, and
+// the rounding of B and C to fp32 is common to both of their terms.
 __global__ void __launch_bounds__(L_THREADS) k_loss_backward(const __grid_constant__ LossParams P) {
-    __shared__ float s_t[3][LS_N];   // A, B, C of one channel, 0 outside the frame
-    __shared__ float s_h[3][LH_N];
+    extern __shared__ __align__(16) unsigned char l_smem[];
+    BackwardSmem& S = *reinterpret_cast<BackwardSmem*>(l_smem);
     const uint32_t tx = blockIdx.x % P.tiles_x, ty = blockIdx.x / P.tiles_x;
     const int x0 = (int)(tx * LT_W) - L_R, y0 = (int)(ty * LT_H) - L_R;
     const int col = threadIdx.x & 31, row0 = threadIdx.x >> 5;
-    float4 xs[L_PIX], ys[L_PIX], out[L_PIX];
-#pragma unroll
-    for (int j = 0; j < L_PIX; j++) {
-        const uint32_t gx = tx * LT_W + col, gy = ty * LT_H + row0 + j * (L_THREADS / 32);
-        const bool in = gx < P.width && gy < P.height;
-        xs[j] = in ? load_image(P, gx, gy) : make_float4(0.f, 0.f, 0.f, 0.f);
-        ys[j] = in ? load_target(P, gx, gy) : make_float4(0.f, 0.f, 0.f, 0.f);
-        out[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
+    stage_xy(P, x0, y0, S.x, S.y);
+    float4 out[L_PIX];
     for (int c = 0; c < 3; c++) {
-        if (c) __syncthreads();  // the previous channel's passes have read s_t and s_h
+        if (c) __syncthreads();  // the previous channel's passes have read S.t and S.h
         for (int i = threadIdx.x; i < LS_N; i += L_THREADS) {
             const int gx = x0 + i % LS_W, gy = y0 + i / LS_W;
             const bool in = gx >= 0 && gy >= 0 && gx < (int)P.width && gy < (int)P.height;
             const size_t p = in ? (size_t)gy * P.width + gx : 0;
 #pragma unroll
-            for (int q = 0; q < 3; q++) s_t[q][i] = in ? P.abc[(3 * c + q) * P.plane + p] : 0.0f;
+            for (int q = 0; q < 3; q++) S.t[q][i] = in ? P.abc[(3 * c + q) * P.plane + p] : 0.0f;
         }
         __syncthreads();
         for (int i = threadIdx.x; i < LH_N; i += L_THREADS) {
-            const int r = i / LT_W, cc = i % LT_W;
+            const int r = i / LT_W, cc = i % LT_W, o = r * LS_W + cc;
+            double hA = 0.0, hB = 0.0, hxB = 0.0, hC = 0.0, hyC = 0.0;
 #pragma unroll
-            for (int q = 0; q < 3; q++) {
-                const float* pt = &s_t[q][r * LS_W + cc];
-                float m = 0.f;
-#pragma unroll
-                for (int k = 0; k < L_K; k++) m = fmaf(c_win[k], pt[k], m);
-                s_h[q][i] = m;
+            for (int k = 0; k < L_K; k++) {
+                const double w = c_win[k];
+                const double wb = w * S.t[1][o + k], wc = w * S.t[2][o + k];
+                hA = fma(w, (double)S.t[0][o + k], hA);
+                hB += wb;
+                hxB = fma(wb, (double)S.x[c][o + k], hxB);
+                hC += wc;
+                hyC = fma(wc, (double)S.y[c][o + k], hyC);
             }
+            S.h[0][i] = hA; S.h[1][i] = hB; S.h[2][i] = hxB; S.h[3][i] = hC; S.h[4][i] = hyC;
         }
         __syncthreads();
 #pragma unroll
         for (int j = 0; j < L_PIX; j++) {
             const int r = row0 + j * (L_THREADS / 32);
-            float m[3] = {0.f, 0.f, 0.f};
+            double m[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
 #pragma unroll
             for (int k = 0; k < L_K; k++) {
-                const float w = c_win[k];
+                const double w = c_win[k];
 #pragma unroll
-                for (int q = 0; q < 3; q++) m[q] = fmaf(w, s_h[q][(r + k) * LT_W + col], m[q]);
+                for (int q = 0; q < 5; q++) m[q] = fma(w, S.h[q][(r + k) * LT_W + col], m[q]);
             }
-            const float xv = chan(xs[j], c), yv = chan(ys[j], c);
-            const float a = xv - 0.5f, b = yv - 0.5f;
-            const float g = fmaf(2.0f * a, m[1], fmaf(b, m[2], m[0]));
-            const float sgn = xv > yv ? 1.0f : (xv < yv ? -1.0f : 0.0f);
-            const float v = fmaf(P.k_l1, sgn, -P.k_ssim * g);
+            const int si = (r + L_R) * LS_W + col + L_R;
+            const float xv = S.x[c][si], yv = S.y[c][si];
+            const double g = m[0] + 2.0 * fma((double)xv, m[1], -m[2]) + fma((double)yv, m[3], -m[4]);
+            const double sgn = xv > yv ? 1.0 : (xv < yv ? -1.0 : 0.0);
+            const float v = (float)(P.k_l1 * sgn - P.k_ssim * g);
             if (c == 0) out[j].x = v;
             else if (c == 1) out[j].y = v;
             else out[j].z = v;
@@ -226,7 +240,8 @@ __global__ void __launch_bounds__(L_THREADS) k_loss_backward(const __grid_consta
     for (int j = 0; j < L_PIX; j++) {
         const uint32_t gx = tx * LT_W + col, gy = ty * LT_H + row0 + j * (L_THREADS / 32);
         if (gx < P.width && gy < P.height)
-            reinterpret_cast<float4*>(reinterpret_cast<unsigned char*>(P.grad) + (size_t)gy * P.grad_pitch)[gx] = out[j];
+            reinterpret_cast<float4*>(reinterpret_cast<unsigned char*>(P.grad) + (size_t)gy * P.grad_pitch)[gx] =
+                make_float4(out[j].x, out[j].y, out[j].z, 0.0f);
     }
 }
 
@@ -307,13 +322,15 @@ extern "C" int gsb_image_loss(gsb_ctx* ctx, uint32_t width, uint32_t height, con
     P.grad = reinterpret_cast<float4*>(grad_image);
     P.grad_pitch = grad_pitch;
     const double n = 3.0 * (double)pixels;
-    P.k_l1 = (float)((1.0 - (double)lambda_dssim) / n);
-    P.k_ssim = (float)((double)lambda_dssim / n);
+    P.k_l1 = (1.0 - (double)lambda_dssim) / n;
+    P.k_ssim = (double)lambda_dssim / n;
+    CK(cudaFuncSetAttribute(k_loss_forward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ForwardSmem)));
+    CK(cudaFuncSetAttribute(k_loss_backward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BackwardSmem)));
     cudaStream_t s = stream_or_own(ctx, stream);
-    k_loss_forward<<<tiles, L_THREADS, 0, s>>>(P);
+    k_loss_forward<<<tiles, L_THREADS, sizeof(ForwardSmem), s>>>(P);
     CK(cudaGetLastError());
     if (grad_image) {
-        k_loss_backward<<<tiles, L_THREADS, 0, s>>>(P);
+        k_loss_backward<<<tiles, L_THREADS, sizeof(BackwardSmem), s>>>(P);
         CK(cudaGetLastError());
     }
     k_loss_reduce<<<1, LR_THREADS, 0, s>>>(ctx->loss_partials, tiles, 1.0 / n, (double)lambda_dssim, result);
