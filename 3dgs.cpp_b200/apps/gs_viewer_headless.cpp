@@ -1,7 +1,8 @@
 // gs_viewer_headless -- the reference viewer's command line (apps/viewer/main.cpp:12-98) without a window:
 //   gs_viewer_headless [-d DEVICE] [-w WIDTH] [-h HEIGHT] [-v] [--frames N] [--camera x,y,z[,qw,qx,qy,qz]]
-//                      [--fov DEG] [--camera-path poses.txt] [--mode exact|fast] [--cull [LEVEL]] [--out image.ppm]
-//                      [--float-out image.pfm] scene.ply
+//                      [--fov DEG] [--camera-path poses.txt] [--mode exact|fast] [--cull [LEVEL]] [--antialiased]
+//                      [--out image.ppm] [--float-out image.pfm] scene.ply
+// --antialiased: gsb_set_antialiased (opacity compensated for the 0.3 px dilation, as scenes trained that way expect).
 // --camera-path: one pose per line `x y z qw qx qy qz [fov]` (# comments); `--frames` frames are rendered at each pose
 // and one JSON line is printed per pose (SURVEY 8d: record M for every timed camera).
 // Loads the .ply through GSScene, renders N frames through Renderer::draw() (B8G8R8A8 like the swapchain),
@@ -22,8 +23,8 @@
 
 static void usage() {
     std::puts("usage: gs_viewer_headless [-d device] [-w width] [-h height] [-v] [--frames n] [--camera x,y,z[,qw,qx,qy,qz]]\n"
-              "                          [--fov deg] [--camera-path poses.txt] [--mode exact|fast] [--cull [0|1|2]] [--out image.ppm]\n"
-              "                          [--float-out image.pfm] scene.ply");
+              "                          [--fov deg] [--camera-path poses.txt] [--mode exact|fast] [--cull [0|1|2]] [--antialiased]\n"
+              "                          [--out image.ppm] [--float-out image.pfm] scene.ply");
 }
 
 int main(int argc, char** argv) {
@@ -31,7 +32,7 @@ int main(int argc, char** argv) {
     std::string out_path, float_path, scene, path_file;
     int cull_level = 0;
     uint32_t frames = 1;
-    bool verbose = false, cull = false;
+    bool verbose = false, cull = false, antialiased = false;
     float cam[7] = {0, 0, 0, 1, 0, 0, 0};
     float fov = 45.0f;
     if (const char* env = std::getenv("VKGS_PHYSICAL_DEVICE")) cfg.physicalDeviceId = static_cast<uint8_t>(std::atoi(env));
@@ -55,7 +56,8 @@ int main(int argc, char** argv) {
             cull = true;
             cull_level = 1;
             if (i + 1 < argc && std::strlen(argv[i + 1]) == 1 && argv[i + 1][0] >= '0' && argv[i + 1][0] <= '2') cull_level = argv[++i][0] - '0';
-        } else if (a == "--float-out") float_path = next();
+        } else if (a == "--antialiased") antialiased = true;
+        else if (a == "--float-out") float_path = next();
         else if (a == "--out") out_path = next();
         else if (a == "--camera-path") path_file = next();
         else if (a == "--camera") {
@@ -77,6 +79,7 @@ int main(int argc, char** argv) {
         renderer.initialize();
         const double load_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
         if (cull && gsb_set_tile_cull(renderer.context(), cull_level) != GSB_OK) throw std::runtime_error("gsb_set_tile_cull failed");
+        if (antialiased && gsb_set_antialiased(renderer.context(), 1) != GSB_OK) throw std::runtime_error("gsb_set_antialiased failed");
         struct Pose {
             float v[7];
             float fov;

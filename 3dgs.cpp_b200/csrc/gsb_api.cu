@@ -373,7 +373,7 @@ static int enqueue_front(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uin
     if (timers) CK(cudaEventRecord(ctx->ev[0], stream));
 
     // ---- k_project: preprocess.comp + survivor compaction ----
-    CK(launch_project(project_params(ctx, *ubo, rb, re), ctx->debug, stream));
+    CK(launch_project(project_params(ctx, *ubo, rb, re), ctx->debug, ctx->antialiased, stream));
     if (timers) CK(cudaEventRecord(ctx->ev[1], stream));
 
     if (ctx->use_graph && !timers && !ctx->debug) rc = launch_middle_graph(ctx, fp, sv, stream);
@@ -424,6 +424,7 @@ int enqueue_tail(gsb_ctx* ctx, const FramePlan& fp, const gsb_uniforms& ubo, cud
     f.plan = fp;
     f.ubo = ubo;
     f.mode = ctx->mode;
+    f.antialiased = ctx->antialiased;
     f.scene_gen = ctx->scene_gen;
     f.pending = true;
     f.exists = true;
@@ -872,6 +873,14 @@ int gsb_set_backward(gsb_ctx* ctx, int enabled) {
     return GSB_OK;
 }
 
+int gsb_set_antialiased(gsb_ctx* ctx, int enabled) {
+    if (!ctx) return GSB_ERR_INVALID;
+    if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, "gsb_set_antialiased: sharded contexts have no anti-aliased mode");
+    // k_project is launched outside the captured middle graph and the survivor set does not change: graphs and hints stay
+    ctx->antialiased = enabled != 0;
+    return GSB_OK;
+}
+
 int gsb_set_backward_deterministic(gsb_ctx* ctx, int enabled) {
     if (!ctx) return GSB_ERR_INVALID;
     if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, "gsb_set_backward_deterministic: sharded contexts have no backward pass");
@@ -975,7 +984,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     bp.abs_scratch = density ? ctx->bw_abs.p : nullptr;
     bp.density = density;
     if (!det) {
-        CK(launch_backward(bp, s));
+        CK(launch_backward(bp, f.antialiased, s));
         return GSB_OK;
     }
     const DetBuffers& d = ctx->bw_det;
@@ -991,7 +1000,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     db.status_tiles = (uint32_t)(d.status.count / 256);
     db.m_hint = quantise_hint(ctx->m_hint);
     db.key_bits = std::max<uint32_t>(bits_for((uint32_t)n), 1u);  // compact ids < N_v <= n
-    CK(launch_backward(bp, s, &db));
+    CK(launch_backward(bp, f.antialiased, s, &db));
     return GSB_OK;
 }
 

@@ -352,7 +352,9 @@ __host__ __device__ constexpr bool cam_word_live(int j) {
 // CAMERA (gsb_render_backward_camera): each thread also accumulates, over its survivors, their share of dL/d(UBO) in the
 // UBO's word layout (fp32), and each CTA writes one fp64 row of partial sums (warp shuffles, then a fixed-order sum over the
 // warps) into P.cam_partials for k_camera_reduce.  The vertex gradient is written only when P.grad_vertices is set.
-template <bool CAMERA>
+// AA (a frame of gsb_set_antialiased): d[5] is dL/d(o comp), comp = sqrt(det0 / det).  The opacity gets d[5] comp, and
+// g = d[5] o reaches both determinants: dL/d det0 = g comp / (2 det0), dL/d det = -g comp / (2 det), 0 where comp = 0.
+template <bool CAMERA, bool AA>
 __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ BackwardParams P) {
     const uint32_t nv = P.ctl->num_visible;
     const gsb_uniforms& U = P.ubo;
@@ -401,9 +403,21 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         const float ood = 1.0f / det;
         const float k00 = c * ood, k01 = -b * ood, k11 = a * ood;
         const float dA = d[2], dB = d[3], dC = d[4];
-        const float da = -((k00 * k00 * dA + k00 * k01 * dB) + k01 * k01 * dC);
-        const float db = -((2.0f * k00 * k01 * dA + (k00 * k11 + k01 * k01) * dB) + 2.0f * k01 * k11 * dC);
-        const float dc = -((k01 * k01 * dA + k01 * k11 * dB) + k11 * k11 * dC);
+        float da = -((k00 * k00 * dA + k00 * k01 * dB) + k01 * k01 * dC);
+        float db = -((2.0f * k00 * k01 * dA + (k00 * k11 + k01 * k01) * dB) + 2.0f * k01 * k11 * dC);
+        float dc = -((k01 * k01 * dA + k01 * k11 * dB) + k11 * k11 * dC);
+        float comp = 1.0f;
+        if constexpr (AA) {  // det0 = c00 c11 - b^2, det = a c - b^2 (a = c00 + 0.3, c = c11 + 0.3): k_project's own values
+            const float det_f = a * c - cov.m10 * cov.m01, det0 = aa_det0(cov);
+            comp = aa_compensation(det0, det_f);
+            if (comp > 0.0f) {
+                const float h = 0.5f * (d[5] * v[7]) * comp;
+                const float gdet0 = h / det0, gdet = -h / det_f;  // dL/d det0, dL/d det
+                da += gdet0 * cov.c11 + gdet * c;
+                dc += gdet0 * cov.c00 + gdet * a;
+                db -= 2.0f * b * (gdet0 + gdet);
+            }
+        }
         // cov2d = (J W) Sigma (J W)^T: dL/dSigma (symmetric) and dL/d(J W)
         float G[3][3];
 #pragma unroll
@@ -553,7 +567,7 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         gv[4] = ds[0];
         gv[5] = ds[1];
         gv[6] = ds[2];
-        gv[7] = d[5];
+        gv[7] = AA ? d[5] * comp : d[5];
         gv[8] = dqw;
         gv[9] = dqx;
         gv[10] = dqy;
@@ -649,7 +663,7 @@ cudaError_t launch_det_sums(const BackwardParams& p, const DetBackward& d, unsig
 
 }  // namespace
 
-cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s, const DetBackward* det) {
+cudaError_t launch_backward(const BackwardParams& p, bool antialiased, cudaStream_t s, const DetBackward* det) {
     const bool density = p.density != nullptr;
     // grid-stride over N_v, which stays on the device: the grid comes from the SM count
     const unsigned grid = (unsigned)p.num_sms * 4u;
@@ -673,10 +687,12 @@ cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s, const DetBa
         if (e != cudaSuccess) return e;
     }
     if (!p.grad_ubo) {
-        k_preprocess_backward<false><<<grid, PB_THREADS, 0, s>>>(p);
+        if (antialiased) k_preprocess_backward<false, true><<<grid, PB_THREADS, 0, s>>>(p);
+        else k_preprocess_backward<false, false><<<grid, PB_THREADS, 0, s>>>(p);
         return cudaGetLastError();
     }
-    k_preprocess_backward<true><<<grid, PB_THREADS, 0, s>>>(p);
+    if (antialiased) k_preprocess_backward<true, true><<<grid, PB_THREADS, 0, s>>>(p);
+    else k_preprocess_backward<true, false><<<grid, PB_THREADS, 0, s>>>(p);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     k_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo);

@@ -92,6 +92,7 @@ struct LastFrame {
     FramePlan plan{};
     gsb_uniforms ubo{};      // its camera
     int mode = GSB_MODE_EXACT;
+    bool antialiased = false;  // gsb_set_antialiased when enqueued: its opacities carry the compensation
     uint64_t scene_gen = 0;  // gsb_ctx::scene_gen when enqueued; 0: no frame yet (a frame needs an upload, which bumps it)
     bool pending = false;    // its completion event and stats copy have not been waited for (wait_frame)
     bool exists = false;     // its stats and debug buffers may be read (a scene upload clears it)
@@ -155,6 +156,7 @@ struct gsb_ctx {
     int mode = GSB_MODE_EXACT;
     bool debug = false;
     bool timers = true;
+    bool antialiased = false;   // gsb_set_antialiased: k_project scales opacities by the dilation's compensation
     int tile_cull = 0;          // gsb_set_tile_cull level: 0 reference-equivalent lists, 1 exact per-tile culling, 2 coarse bins
     uint32_t coarse_shift = 2;  // level 2 bins are 2^shift x 2^shift tiles (GSB_COARSE_SHIFT)
     cudaEvent_t ev[8] = {};

@@ -61,9 +61,10 @@ __device__ __forceinline__ Jacobian jacobian(const gsb_uniforms& U, float vx, fl
 }
 
 // cov2d = transpose(T) Sigma T + 0.3 I (:56-65), Sigma = the cov3d words ca.xyzw, cb.xy; tm0 / tm1 = Sigma T0 / Sigma T1 (S[k] =
-// column k).  m01 and m10 round differently, so each caller states its own determinant.
+// column k).  m01 and m10 round differently, so each caller states its own determinant.  c00 and c11 are the diagonal before
+// the dilation (the anti-aliased mode's opacity compensation reads them; m01 and m10 are not dilated).
 struct Cov2d {
-    float tm0[3], tm1[3], m00, m01, m10, m11;
+    float tm0[3], tm1[3], m00, m01, m10, m11, c00, c11;
 };
 __device__ __forceinline__ Cov2d cov2d(const float (&T0)[3], const float (&T1)[3], float4 ca, float2 cb) {
     const float S[3][3] = {{ca.x, ca.y, ca.z}, {ca.y, ca.w, cb.x}, {ca.z, cb.x, cb.y}};
@@ -78,8 +79,15 @@ __device__ __forceinline__ Cov2d cov2d(const float (&T0)[3], const float (&T1)[3
     const float c10 = (c.tm0[0] * T1[0] + c.tm0[1] * T1[1]) + c.tm0[2] * T1[2];  // [1][0]
     const float c11 = (c.tm1[0] * T1[0] + c.tm1[1] * T1[1]) + c.tm1[2] * T1[2];
     c.m00 = c00 + 0.3f, c.m01 = c01, c.m10 = c10, c.m11 = c11 + 0.3f;
+    c.c00 = c00, c.c11 = c11;
     return c;
 }
+
+// The anti-aliased mode (gsb_set_antialiased): the opacity factor sqrt(det(cov2d) / det(cov2d + 0.3 I)) that keeps a
+// Gaussian's integral what it was before the dilation.  det is the caller's dilated determinant (m00 m11 - m10 m01, > 0);
+// det0 is the same product order over the undilated entries.  A NaN ratio gives 0.
+__device__ __forceinline__ float aa_det0(const Cov2d& c) { return c.c00 * c.c11 - c.m10 * c.m01; }
+__device__ __forceinline__ float aa_compensation(float det0, float det) { return sqrtf(fmaxf(0.0f, det0 / det)); }
 
 // rotationFromQuaternion, common.glsl:51-75: R[c][r] of the quaternion as stored (not normalised)
 __device__ __forceinline__ void rotation_from_quaternion(float qw, float qx, float qy, float qz, float (&R)[3][3]) {

@@ -102,7 +102,8 @@ struct EmitParams {
 
 cudaError_t launch_cov3d(const float* vtx_aos, uint64_t count, uint64_t dst_offset, float4* pos_op,
                          float4* cov_a, float2* cov_b, float* sh, float scale_factor, cudaStream_t s, bool sh_half = false);
-cudaError_t launch_project(const ProjectParams& p, bool debug, cudaStream_t s);
+// antialiased: gsb_set_antialiased's opacity compensation (not on the routed kernel of a sharded frame)
+cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s);
 cudaError_t launch_emit(const EmitParams& p, cudaStream_t s);
 
 struct SortParams {  // host-side arguments of launch_sort
@@ -203,7 +204,8 @@ struct DetBackward {
     uint32_t m_hint;               // sizes the sort's grids only
     uint32_t key_bits;             // bits of the largest compact id
 };
-cudaError_t launch_backward(const BackwardParams& p, cudaStream_t s, const DetBackward* det = nullptr);
+// antialiased: the frame ran with gsb_set_antialiased on (its opacities carry the compensation, whose chain rule is added)
+cudaError_t launch_backward(const BackwardParams& p, bool antialiased, cudaStream_t s, const DetBackward* det = nullptr);
 
 // gsb_optim.cu: one Adam step over the scene's rows (gsb_adam_step).  Every per-row array is n x 60 floats = 15 float4 per row.
 struct AdamParams {

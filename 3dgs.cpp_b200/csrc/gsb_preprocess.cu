@@ -167,8 +167,11 @@ __device__ __forceinline__ void compute_sh(const float4* __restrict__ sh4, float
 // from registers into the exchange buffer of every rank whose band the AABB touches (stores into peer-mapped memory over
 // NVLink).  Slots are deterministic (Gaussian-index order inside this source's region), so every band's survivor list is
 // ordered exactly like the single-GPU compaction and the band's pixels are bit-identical.
-template <bool DEBUG, bool ROUTED, bool SH16>
+// AA (gsb_set_antialiased, plain contexts only): the stored opacity is scaled by sqrt(det(cov2d) / det(cov2d + 0.3 I)); the
+// conic, radius, AABB and survivor set are those of AA = false.
+template <bool DEBUG, bool ROUTED, bool SH16, bool AA>
 __global__ void __launch_bounds__(PRE_THREADS, GSB_PROJECT_MIN_BLOCKS) k_project(const __grid_constant__ ProjectParams P) {
+    static_assert(!(ROUTED && AA), "sharded contexts have no anti-aliased mode");
     __shared__ uint32_t s_chunk;
     __shared__ uint32_t s_wsurv[PRE_THREADS / 32];
     __shared__ uint32_t s_base_surv;
@@ -211,6 +214,7 @@ __global__ void __launch_bounds__(PRE_THREADS, GSB_PROJECT_MIN_BLOCKS) k_project
                 conx = m11 * ood;
                 cony = -m01 * ood;
                 conz = m00 * ood;  // :142-143
+                if constexpr (AA) opac = opac * aa_compensation(aa_det0(cov), det);
                 const float mid = 0.5f * (m00 + m11);
                 const float sq = sqrtf(fmaxf(0.1f, mid * mid - det));
                 const float lambda = fmaxf(mid + sq, mid - sq);
@@ -790,16 +794,27 @@ __global__ void __launch_bounds__(PRE_THREADS) k_emit_coarse(const __grid_consta
 
 }  // namespace
 
-cudaError_t launch_project(const ProjectParams& p, bool debug, cudaStream_t s) {
+template <bool AA>
+void launch_project_plain(const ProjectParams& p, bool debug, unsigned blocks, cudaStream_t s) {
+    if (p.sh_half) {  // fp16 SH storage (non-parity)
+        if (debug) k_project<true, false, true, AA><<<blocks, PRE_THREADS, 0, s>>>(p);
+        else k_project<false, false, true, AA><<<blocks, PRE_THREADS, 0, s>>>(p);
+    } else if (debug) k_project<true, false, false, AA><<<blocks, PRE_THREADS, 0, s>>>(p);
+    else k_project<false, false, false, AA><<<blocks, PRE_THREADS, 0, s>>>(p);
+}
+
+cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s) {
     if (p.n == 0) return cudaSuccess;
     const unsigned blocks = (p.n + PRE_THREADS - 1) / PRE_THREADS;
-    if (p.sh_half) {  // fp16 SH storage (non-parity)
-        if (p.route_world > 0) k_project<false, true, true><<<blocks, PRE_THREADS, 0, s>>>(p);
-        else if (debug) k_project<true, false, true><<<blocks, PRE_THREADS, 0, s>>>(p);
-        else k_project<false, false, true><<<blocks, PRE_THREADS, 0, s>>>(p);
-    } else if (p.route_world > 0) k_project<false, true, false><<<blocks, PRE_THREADS, 0, s>>>(p);
-    else if (debug) k_project<true, false, false><<<blocks, PRE_THREADS, 0, s>>>(p);
-    else k_project<false, false, false><<<blocks, PRE_THREADS, 0, s>>>(p);
+    if (p.route_world > 0) {
+        if (antialiased) return cudaErrorInvalidValue;  // the routed kernel has no AA instantiation
+        if (p.sh_half) k_project<false, true, true, false><<<blocks, PRE_THREADS, 0, s>>>(p);
+        else k_project<false, true, false, false><<<blocks, PRE_THREADS, 0, s>>>(p);
+    } else if (antialiased) {
+        launch_project_plain<true>(p, debug, blocks, s);
+    } else {
+        launch_project_plain<false>(p, debug, blocks, s);
+    }
     return cudaGetLastError();
 }
 

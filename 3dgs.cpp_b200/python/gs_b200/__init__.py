@@ -38,6 +38,7 @@ ALL_ROWS = 0xFFFFFFFF
 EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_abi_version", "gsb_device_count", "gsb_create", "gsb_destroy", "gsb_last_error",
     "gsb_scene_upload", "gsb_scene_size", "gsb_set_mode", "gsb_set_debug", "gsb_set_timers", "gsb_set_tile_cull", "gsb_set_sh_storage",
+    "gsb_set_antialiased",
     "gsb_reserve_instances", "gsb_render", "gsb_render_async", "gsb_get_stats", "gsb_debug_size",
     "gsb_debug_download", "gsb_sort_pairs", "gsb_sort_pairs32", "gsb_set_graph", "gsb_host_alloc", "gsb_host_free",
     # reverse mode
@@ -149,6 +150,7 @@ lib.gsb_set_mode.argtypes = [_vp, C.c_int]
 lib.gsb_set_debug.argtypes = [_vp, C.c_int]
 lib.gsb_set_timers.argtypes = [_vp, C.c_int]
 lib.gsb_set_tile_cull.argtypes = [_vp, C.c_int]
+lib.gsb_set_antialiased.argtypes = [_vp, C.c_int]
 lib.gsb_set_sh_storage.argtypes = [_vp, C.c_int]
 lib.gsb_set_graph.argtypes = [_vp, C.c_int]
 lib.gsb_host_alloc.argtypes = [C.POINTER(_vp), C.c_size_t]
@@ -449,6 +451,12 @@ class Context:
     def set_tile_cull(self, level=1):
         """gsb_set_tile_cull: 0 reference lists, 1 (True) exact per-tile instance culling, 2 coarse 4x4-tile bins."""
         self._ck(lib.gsb_set_tile_cull(self.h, int(level)))
+
+    def set_antialiased(self, on=True):
+        """gsb_set_antialiased: from the next frame, opacities are scaled by sqrt(det(cov2d) / det(cov2d + 0.3 I)), the
+        compensation for the 0.3 px dilation (gsplat's antialiased mode).  render_torch, SceneAdam, image_metrics and the
+        backward pass follow it (the backward uses the setting of the frame it differentiates)."""
+        self._ck(lib.gsb_set_antialiased(self.h, int(on)))
 
     def set_sh_storage(self, half=True):
         """gsb_set_sh_storage: fp16 SH coefficients from the next upload on (NOT a parity mode)."""

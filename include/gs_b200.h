@@ -169,6 +169,20 @@ int gsb_set_debug(gsb_ctx *ctx, int debug);
  *      stays the reference's count.  Unavailable (falls back to 1) with gsb_set_debug, whose downloads are per tile,
  *      and for frames of more than 65536 blocks. */
 int gsb_set_tile_cull(gsb_ctx *ctx, int level);
+/* Anti-aliased rendering (default 0; no reference counterpart).  preprocess.comp:63-65 dilates the screen-space covariance
+ * by 0.3 px^2 and keeps the opacity, so a Gaussian smaller than a pixel is drawn as a blob of at least 0.3 px^2 at full
+ * opacity, and thin structure thickens and brightens when a scene is rendered farther away or at a lower resolution than
+ * it was trained at.  While on, every Gaussian that passes the det > 0 test keeps the dilated covariance for its conic,
+ * radius and tiles and has its opacity scaled, in fp32 in this order (the rule of gsplat's rasterize_mode="antialiased"):
+ *     det0 = c00 * c11 - c10 * c01            the undilated cov2d, in the product order of the dilated det
+ *     comp = sqrt(max(0, det0 / det))         det = the dilated determinant; a NaN ratio gives 0
+ *     opacity = opacity * comp
+ * so opacity * sqrt(det) -- a Gaussian's integrated weight -- is that of the undilated footprint.  The blend, tile-cull
+ * levels 1 and 2 and the backward pass see the compensated opacity, which is what GSB_BUF_ATTR's conic_opacity[3] holds;
+ * conic, radius, tile AABB, depth, colour and the survivor set are those of the default mode.  Takes effect at the next
+ * frame; the backward entries and the selective gsb_adam_step follow the setting the last frame was rendered with and
+ * differentiate through comp.  NULL ctx or a sharded context (gsb_create_sharded, a gsb_group rank): GSB_ERR_INVALID. */
+int gsb_set_antialiased(gsb_ctx *ctx, int enabled);
 /* per-stage cudaEvent timers (the QueryManager analogue, Renderer.cpp:85-100). Default on. */
 int gsb_set_timers(gsb_ctx *ctx, int enabled);
 /* Replay the camera-independent middle of the frame (both sorts + key emission) from a captured CUDA graph instead of
