@@ -1,8 +1,9 @@
 // gs_viewer_headless -- the reference viewer's command line (apps/viewer/main.cpp:12-98) without a window:
 //   gs_viewer_headless [-d DEVICE] [-w WIDTH] [-h HEIGHT] [-v] [--frames N] [--camera x,y,z[,qw,qx,qy,qz]]
 //                      [--fov DEG] [--camera-path poses.txt] [--mode exact|fast] [--cull [LEVEL]] [--antialiased]
-//                      [--out image.ppm] [--float-out image.pfm] scene.ply
+//                      [--background r,g,b] [--out image.ppm] [--float-out image.pfm] scene.ply
 // --antialiased: gsb_set_antialiased (opacity compensated for the 0.3 px dilation, as scenes trained that way expect).
+// --background r,g,b: gsb_set_background (e.g. 1,1,1 for an object scene trained over white; default black).
 // --camera-path: one pose per line `x y z qw qx qy qz [fov]` (# comments); `--frames` frames are rendered at each pose
 // and one JSON line is printed per pose (SURVEY 8d: record M for every timed camera).
 // Loads the .ply through GSScene, renders N frames through Renderer::draw() (B8G8R8A8 like the swapchain),
@@ -24,7 +25,7 @@
 static void usage() {
     std::puts("usage: gs_viewer_headless [-d device] [-w width] [-h height] [-v] [--frames n] [--camera x,y,z[,qw,qx,qy,qz]]\n"
               "                          [--fov deg] [--camera-path poses.txt] [--mode exact|fast] [--cull [0|1|2]] [--antialiased]\n"
-              "                          [--out image.ppm] [--float-out image.pfm] scene.ply");
+              "                          [--background r,g,b] [--out image.ppm] [--float-out image.pfm] scene.ply");
 }
 
 int main(int argc, char** argv) {
@@ -32,7 +33,8 @@ int main(int argc, char** argv) {
     std::string out_path, float_path, scene, path_file;
     int cull_level = 0;
     uint32_t frames = 1;
-    bool verbose = false, cull = false, antialiased = false;
+    bool verbose = false, cull = false, antialiased = false, background = false;
+    float bg[3] = {0, 0, 0};
     float cam[7] = {0, 0, 0, 1, 0, 0, 0};
     float fov = 45.0f;
     if (const char* env = std::getenv("VKGS_PHYSICAL_DEVICE")) cfg.physicalDeviceId = static_cast<uint8_t>(std::atoi(env));
@@ -57,6 +59,11 @@ int main(int argc, char** argv) {
             cull_level = 1;
             if (i + 1 < argc && std::strlen(argv[i + 1]) == 1 && argv[i + 1][0] >= '0' && argv[i + 1][0] <= '2') cull_level = argv[++i][0] - '0';
         } else if (a == "--antialiased") antialiased = true;
+        else if (a == "--background") {
+            background = true;
+            int k = 0;
+            for (char* tok = std::strtok(const_cast<char*>(next()), ","); tok && k < 3; tok = std::strtok(nullptr, ",")) bg[k++] = static_cast<float>(std::atof(tok));
+        }
         else if (a == "--float-out") float_path = next();
         else if (a == "--out") out_path = next();
         else if (a == "--camera-path") path_file = next();
@@ -80,6 +87,7 @@ int main(int argc, char** argv) {
         const double load_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
         if (cull && gsb_set_tile_cull(renderer.context(), cull_level) != GSB_OK) throw std::runtime_error("gsb_set_tile_cull failed");
         if (antialiased && gsb_set_antialiased(renderer.context(), 1) != GSB_OK) throw std::runtime_error("gsb_set_antialiased failed");
+        if (background && gsb_set_background(renderer.context(), bg) != GSB_OK) throw std::runtime_error("gsb_set_background failed");
         struct Pose {
             float v[7];
             float fov;

@@ -411,6 +411,7 @@ int enqueue_blend(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, uint32
     bp.ctl = ctx->ctl;
     // gsb_set_backward: the per-pixel state of gsb_render_backward (plain contexts, per-tile lists)
     bp.record = (ctx->backward && fp.cs == 0 && num_peer_frames == 0) ? ctx->bw_record.p : nullptr;
+    for (int c = 0; c < 3; c++) bp.background[c] = ctx->background[c];  // gsb_set_background (every context, sharded or not)
     CK(launch_blend(bp, stream));
     return GSB_OK;
 }
@@ -425,6 +426,7 @@ int enqueue_tail(gsb_ctx* ctx, const FramePlan& fp, const gsb_uniforms& ubo, cud
     f.ubo = ubo;
     f.mode = ctx->mode;
     f.antialiased = ctx->antialiased;
+    for (int c = 0; c < 3; c++) f.background[c] = ctx->background[c];
     f.scene_gen = ctx->scene_gen;
     f.pending = true;
     f.exists = true;
@@ -881,6 +883,16 @@ int gsb_set_antialiased(gsb_ctx* ctx, int enabled) {
     return GSB_OK;
 }
 
+int gsb_set_background(gsb_ctx* ctx, const float* rgb) {
+    if (!ctx) return GSB_ERR_INVALID;
+    const float v[3] = {rgb ? rgb[0] : 0.0f, rgb ? rgb[1] : 0.0f, rgb ? rgb[2] : 0.0f};
+    for (float x : v)
+        if (!isfinite(x)) return fail(ctx, GSB_ERR_INVALID, "gsb_set_background: the colour must be finite");
+    // k_blend runs outside the captured middle graph and reads the colour from its arguments: graphs and hints stay
+    for (int c = 0; c < 3; c++) ctx->background[c] = v[c];
+    return GSB_OK;
+}
+
 int gsb_set_backward_deterministic(gsb_ctx* ctx, int enabled) {
     if (!ctx) return GSB_ERR_INVALID;
     if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, "gsb_set_backward_deterministic: sharded contexts have no backward pass");
@@ -983,8 +995,9 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     bp.grad_ubo = grad_ubo;
     bp.abs_scratch = density ? ctx->bw_abs.p : nullptr;
     bp.density = density;
+    const float3 bg = make_float3(f.background[0], f.background[1], f.background[2]);  // the frame's, not the current setting
     if (!det) {
-        CK(launch_backward(bp, f.antialiased, s));
+        CK(launch_backward(bp, f.antialiased, bg, s));
         return GSB_OK;
     }
     const DetBuffers& d = ctx->bw_det;
@@ -1000,7 +1013,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     db.status_tiles = (uint32_t)(d.status.count / 256);
     db.m_hint = quantise_hint(ctx->m_hint);
     db.key_bits = std::max<uint32_t>(bits_for((uint32_t)n), 1u);  // compact ids < N_v <= n
-    CK(launch_backward(bp, f.antialiased, s, &db));
+    CK(launch_backward(bp, f.antialiased, bg, s, &db));
     return GSB_OK;
 }
 
@@ -1019,6 +1032,27 @@ int gsb_render_backward_density(gsb_ctx* ctx, const float* vertices, const float
                                 gsb_uniforms* grad_uniforms, float* density, void* stream) {
     return render_backward(ctx, "gsb_render_backward_density", vertices && grad_image && density && (grad_vertices || grad_uniforms),
                            vertices, grad_image, pitch, grad_vertices, grad_uniforms, density, stream);
+}
+
+int gsb_background_gradient(gsb_ctx* ctx, const float* grad_image, size_t pitch, float* grad_background, void* stream) {
+    if (!ctx) return GSB_ERR_INVALID;
+    const char* fn = "gsb_background_gradient";
+    auto msg = [&](const char* what) { return std::string(fn) + ": " + what; };
+    if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, msg("sharded contexts have no backward pass").c_str());
+    if (!ctx->pos_op) return fail(ctx, GSB_ERR_NO_SCENE, msg("no scene uploaded").c_str());
+    CK(cudaSetDevice(ctx->device));
+    const int rc = check_recorded_frame(ctx, GSB_ERR_NO_SCENE, fn);
+    if (rc != GSB_OK) return rc;
+    if (!grad_image || !grad_background) return fail(ctx, GSB_ERR_INVALID, msg("null argument").c_str());
+    const LastFrame& f = ctx->frame;
+    const size_t tight = (size_t)f.ubo.width * sizeof(float4);
+    if (pitch == 0) pitch = tight;
+    if (pitch < tight || pitch % sizeof(float4) != 0) return fail(ctx, GSB_ERR_INVALID, msg("bad row pitch").c_str());
+    // one row of partials per CTA, fully overwritten by each call; runs for an empty scene too (every T_final is 1)
+    CK(ctx->bg_partials.grow((uint64_t)background_grad_rows(f.ubo.height) * 3));
+    CK(launch_background_grad(ctx->bw_record, grad_image, pitch, f.ubo.width, f.ubo.height, ctx->bg_partials, grad_background,
+                              stream_or_own(ctx, stream)));
+    return GSB_OK;
 }
 
 int gsb_adam_step(gsb_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* grad_vertices, float* vertices,

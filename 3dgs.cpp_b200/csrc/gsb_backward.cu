@@ -1,7 +1,10 @@
 // gsb_backward.cu -- reverse mode of one whole frame: dL/d(image) -> dL/d(GSScene::Vertex records).  No reference counterpart
 // (3DGS.cpp only renders); this differentiates the function the forward computes, quirks included (DESIGN.md section 10):
-// no background term, only the red channel clamped at 0, integer pixel centres, alpha = min(0.99, .), the T' < 1e-4 break and
-// the per-tile lists of the frame.
+// only the red channel clamped at 0, integer pixel centres, alpha = min(0.99, .), the T' < 1e-4 break and the per-tile lists
+// of the frame.  A frame of gsb_set_background composites c + T_final bg (DESIGN.md section 15): the BG instantiations of
+// k_blend_backward start the colour behind every pixel's last contributor at bg instead of 0, and
+//   k_background_grad + k_background_reduce  (gsb_background_gradient) sum T_final g over the frame's pixels for dL/d bg, in
+//                         fp64 in an order fixed by the frame size: one row of partials per CTA, then one CTA.
 //
 //   k_blend_backward      one CTA per 16 x 16 tile, one pixel per thread.  The tile's list is walked back to front from the
 //                         largest last-contributor position among its pixels (recorded by k_blend<..., RECORD>), in batches
@@ -33,6 +36,9 @@
 //   k_det_reduce          one thread per survivor: the run's slots summed in order in fp64, stored into the scratch that
 //                         k_density_accumulate and k_preprocess_backward read.  Every output is then order-fixed.
 // Compiled with -fmad=false like the forward.
+#include <algorithm>
+#include <type_traits>
+
 #include "gsb_cull.cuh"
 #include "gsb_exp.cuh"
 #include "gsb_geom.cuh"
@@ -72,8 +78,21 @@ __device__ __forceinline__ float* det_partials() {
     return s_dyn;
 }
 
-template <int MODE, bool ABSGRAD, bool DET = false>
-__global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_constant__ BackwardParams P) {
+// BG (a frame of gsb_set_background): the colour behind every pixel's last contributor is P.bg instead of 0.  Only the BG
+// instantiations take the larger argument: the others keep BackwardParams as it was, and with it their code.
+struct BackwardBgParams : BackwardParams {
+    float3 bg;
+};
+template <bool BG>
+using BwParams = std::conditional_t<BG, BackwardBgParams, BackwardParams>;
+template <bool BG>
+BwParams<BG> bw_params(const BackwardParams& p, float3 bg) {
+    if constexpr (BG) return BackwardBgParams{p, bg};
+    else return p;
+}
+
+template <int MODE, bool ABSGRAD, bool DET = false, bool BG = false>
+__global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_constant__ BwParams<BG> P) {
     constexpr int NACC = BW_NACC + (ABSGRAD ? BW_NABS : 0);  // shared-memory columns: the extra two in ABSGRAD only
     __shared__ BwRec s_rec[bw_batch<DET>];
     __shared__ double s_acc[DET ? 1 : BW_BATCH][NACC];
@@ -109,6 +128,11 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
     if (range.x >= range.y) return;  // empty list: every pixel has last == 0
 
     float acc_r = 0.f, acc_g = 0.f, acc_b = 0.f;  // colour behind the current entry, per unit of its transmittance
+    if constexpr (BG) {  // the background is behind every pixel's last contributor
+        acc_r = P.bg.x;
+        acc_g = P.bg.y;
+        acc_b = P.bg.z;
+    }
     for (uint32_t hi = max_last; hi > 0;) {
         const uint32_t lo = hi > bw_batch<DET> ? hi - bw_batch<DET> : 0u;
         const uint32_t cnt = hi - lo;
@@ -610,21 +634,90 @@ __global__ void __launch_bounds__(CR_THREADS) k_camera_reduce(const double* __re
     }
 }
 
-template <int MODE, bool ABSGRAD>
-cudaError_t launch_blend_det(const BackwardParams& p, cudaStream_t s) {
+template <int MODE, bool ABSGRAD, bool BG>
+cudaError_t launch_blend_det(const BackwardParams& p, float3 bg, cudaStream_t s) {
     constexpr int NACC = BW_NACC + (ABSGRAD ? BW_NABS : 0);
     const size_t smem = (size_t)BW_WARPS * NACC * BW_DET_BATCH * sizeof(float);  // 36 KB, or 44 KB with ABSGRAD
-    cudaError_t e = cudaFuncSetAttribute(k_blend_backward<MODE, ABSGRAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(k_blend_backward<MODE, ABSGRAD, true, BG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    k_blend_backward<MODE, ABSGRAD, true><<<p.num_tiles, BW_THREADS, smem, s>>>(p);
+    k_blend_backward<MODE, ABSGRAD, true, BG><<<p.num_tiles, BW_THREADS, smem, s>>>(bw_params<BG>(p, bg));
     return cudaGetLastError();
+}
+
+template <int MODE, bool ABSGRAD>
+cudaError_t launch_blend_det(const BackwardParams& p, float3 bg, cudaStream_t s) {
+    return has_background(bg) ? launch_blend_det<MODE, ABSGRAD, true>(p, bg, s) : launch_blend_det<MODE, ABSGRAD, false>(p, bg, s);
+}
+
+template <bool BG>
+void launch_blend_backward(const BackwardParams& p, float3 bg, cudaStream_t s) {
+    const bool density = p.density != nullptr;
+    if (p.mode == GSB_MODE_EXACT) {
+        if (density) k_blend_backward<GSB_MODE_EXACT, true, false, BG><<<p.num_tiles, BW_THREADS, 0, s>>>(bw_params<BG>(p, bg));
+        else k_blend_backward<GSB_MODE_EXACT, false, false, BG><<<p.num_tiles, BW_THREADS, 0, s>>>(bw_params<BG>(p, bg));
+    } else {
+        if (density) k_blend_backward<GSB_MODE_FAST, true, false, BG><<<p.num_tiles, BW_THREADS, 0, s>>>(bw_params<BG>(p, bg));
+        else k_blend_backward<GSB_MODE_FAST, false, false, BG><<<p.num_tiles, BW_THREADS, 0, s>>>(bw_params<BG>(p, bg));
+    }
+}
+
+// gsb_background_gradient: one CTA per row r, r + grid, ... of the frame (grid = background_grad_rows(H)); each thread sums
+// T_final * g of its pixels x = tid, tid + 256, ... in fp64 (the products of two floats are exact), then a shuffle tree and
+// the 8 warps in order give the CTA's row of 3 partials.  k_background_reduce sums the rows in a fixed order.
+constexpr int BG_THREADS = 256;
+constexpr uint32_t BG_MAX_ROWS = 2048;
+__global__ void __launch_bounds__(BG_THREADS) k_background_grad(const uint2* __restrict__ record, const unsigned char* __restrict__ grad_image,
+                                                                size_t pitch, uint32_t width, uint32_t height, double* __restrict__ partials) {
+    __shared__ double s_w[BG_THREADS / 32][3];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    double a0 = 0.0, a1 = 0.0, a2 = 0.0;
+    for (uint32_t y = blockIdx.x; y < height; y += gridDim.x) {
+        const uint2* rec = record + (size_t)y * width;
+        const float4* g = reinterpret_cast<const float4*>(grad_image + (size_t)y * pitch);
+        for (uint32_t x = threadIdx.x; x < width; x += BG_THREADS) {
+            const double t = (double)__uint_as_float(__ldg(&rec[x].x));
+            const float4 v = __ldg(g + x);  // A is ignored: the output's A is constant
+            a0 = __dadd_rn(a0, __dmul_rn(t, (double)v.x));
+            a1 = __dadd_rn(a1, __dmul_rn(t, (double)v.y));
+            a2 = __dadd_rn(a2, __dmul_rn(t, (double)v.z));
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        a0 += __shfl_xor_sync(FULL, a0, o);
+        a1 += __shfl_xor_sync(FULL, a1, o);
+        a2 += __shfl_xor_sync(FULL, a2, o);
+    }
+    if (lane == 0) {
+        s_w[warp][0] = a0;
+        s_w[warp][1] = a1;
+        s_w[warp][2] = a2;
+    }
+    __syncthreads();
+    if (threadIdx.x < 3) {
+        double a = 0.0;
+#pragma unroll
+        for (int w = 0; w < BG_THREADS / 32; w++) a += s_w[w][threadIdx.x];
+        partials[(size_t)blockIdx.x * 3 + threadIdx.x] = a;
+    }
+}
+
+// One CTA of three warps: warp c sums column c of the `rows` partial rows (lane-strided, then a shuffle tree) and stores it,
+// rounded once, into out[c].
+__global__ void __launch_bounds__(96) k_background_reduce(const double* __restrict__ partials, uint32_t rows, float* out) {
+    const int lane = threadIdx.x & 31, c = threadIdx.x >> 5;
+    double a = 0.0;
+    for (uint32_t r = lane; r < rows; r += 32) a += partials[(size_t)r * 3 + c];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(FULL, a, o);
+    if (lane == 0) out[c] = (float)a;
 }
 
 // gsb_set_backward_deterministic: the per-survivor sums of the blend backward without atomics.  The blend stores one slot
 // per (tile, entry); a stable sort of (compact id, list position) over the M entries groups each survivor's slots in tile
 // order, its last pass publishing each survivor's run; k_det_reduce sums every run in order.  Integer atomics remain
 // (the sort's counters and the runs' atomicMin), but their results do not depend on the order they land in.
-cudaError_t launch_det_sums(const BackwardParams& p, const DetBackward& d, unsigned grid, cudaStream_t s) {
+cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackward& d, unsigned grid, cudaStream_t s) {
     const bool density = p.density != nullptr;
     cudaError_t e = cudaMemsetAsync(d.sc, 0, sizeof(SortCtl), s);
     if (e != cudaSuccess) return e;
@@ -651,8 +744,8 @@ cudaError_t launch_det_sums(const BackwardParams& p, const DetBackward& d, unsig
     if ((e = launch_sort(sp, &passes, s)) != cudaSuccess) return e;
     if (passes == 0) return cudaErrorInvalidValue;  // key_bits >= 1: the runs come from the last pass
     if (p.num_tiles) {
-        if (p.mode == GSB_MODE_EXACT) e = density ? launch_blend_det<GSB_MODE_EXACT, true>(p, s) : launch_blend_det<GSB_MODE_EXACT, false>(p, s);
-        else e = density ? launch_blend_det<GSB_MODE_FAST, true>(p, s) : launch_blend_det<GSB_MODE_FAST, false>(p, s);
+        if (p.mode == GSB_MODE_EXACT) e = density ? launch_blend_det<GSB_MODE_EXACT, true>(p, bg, s) : launch_blend_det<GSB_MODE_EXACT, false>(p, bg, s);
+        else e = density ? launch_blend_det<GSB_MODE_FAST, true>(p, bg, s) : launch_blend_det<GSB_MODE_FAST, false>(p, bg, s);
         if (e != cudaSuccess) return e;
     }
     const uint32_t* sorted_pos = d.pos[passes & 1];
@@ -663,21 +756,16 @@ cudaError_t launch_det_sums(const BackwardParams& p, const DetBackward& d, unsig
 
 }  // namespace
 
-cudaError_t launch_backward(const BackwardParams& p, bool antialiased, cudaStream_t s, const DetBackward* det) {
+cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det) {
     const bool density = p.density != nullptr;
     // grid-stride over N_v, which stays on the device: the grid comes from the SM count
     const unsigned grid = (unsigned)p.num_sms * 4u;
     if (det) {
-        cudaError_t e = launch_det_sums(p, *det, grid, s);
+        cudaError_t e = launch_det_sums(p, background, *det, grid, s);
         if (e != cudaSuccess) return e;
     } else if (p.num_tiles) {
-        if (p.mode == GSB_MODE_EXACT) {
-            if (density) k_blend_backward<GSB_MODE_EXACT, true><<<p.num_tiles, BW_THREADS, 0, s>>>(p);
-            else k_blend_backward<GSB_MODE_EXACT, false><<<p.num_tiles, BW_THREADS, 0, s>>>(p);
-        } else {
-            if (density) k_blend_backward<GSB_MODE_FAST, true><<<p.num_tiles, BW_THREADS, 0, s>>>(p);
-            else k_blend_backward<GSB_MODE_FAST, false><<<p.num_tiles, BW_THREADS, 0, s>>>(p);
-        }
+        if (has_background(background)) launch_blend_backward<true>(p, background, s);  // a frame of gsb_set_background
+        else launch_blend_backward<false>(p, background, s);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
@@ -696,6 +784,19 @@ cudaError_t launch_backward(const BackwardParams& p, bool antialiased, cudaStrea
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     k_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo);
+    return cudaGetLastError();
+}
+
+uint32_t background_grad_rows(uint32_t height) { return std::min(height, BG_MAX_ROWS); }
+
+cudaError_t launch_background_grad(const uint2* record, const float* grad_image, size_t row_pitch_bytes, uint32_t width,
+                                   uint32_t height, double* partials, float* out, cudaStream_t s) {
+    const uint32_t rows = background_grad_rows(height);
+    k_background_grad<<<rows, BG_THREADS, 0, s>>>(record, reinterpret_cast<const unsigned char*>(grad_image), row_pitch_bytes, width,
+                                                  height, partials);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    k_background_reduce<<<1, 96, 0, s>>>(partials, rows, out);
     return cudaGetLastError();
 }
 

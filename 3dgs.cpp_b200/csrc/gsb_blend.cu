@@ -89,8 +89,8 @@ __device__ __forceinline__ uint32_t block_mask(float ux, float uy, float A, floa
 }
 
 // Per-pixel state of gsb_set_backward frames (k_blend<..., RECORD = true>): for each of the thread's two pixels, the
-// transmittance after its last contributor and that contributor's list position + 1 (0 = none).  Empty otherwise, so the
-// plain instantiations carry no trace of it.
+// transmittance after its last contributor and that contributor's list position + 1 (0 = none).  The BG instantiations keep
+// the same state for their background term.  Empty otherwise, so the plain instantiations carry no trace of it.
 template <bool ON>
 struct BlendRecord {
     float t0 = 1.0f, t1 = 1.0f;
@@ -124,7 +124,10 @@ struct BlendRecord<false> {
 // RECORD (gsb_set_backward, per-tile lists only): each pixel also stores its final transmittance (the product of 1 - alpha
 // over its contributors: the T the shader holds at its break or at the end of the list) and the list position + 1 of its
 // last contributor into P.record -- what gsb_backward.cu needs to walk the list back to front.  The image is unchanged.
-template <int MODE, bool STATS, bool COARSE, bool RECORD = false>
+// BG (gsb_set_background, a non-zero P.background): the pixels keep the same final transmittance (BlendRecord's note, stored
+// only when RECORD) and every colour channel is stored as c + T_final * bg (one multiply, one add, both rounded), in both
+// store paths.  A pixel no entry reaches keeps T_final = 1 and is stored as bg exactly.
+template <int MODE, bool STATS, bool COARSE, bool RECORD = false, bool BG = false>
 __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(const __grid_constant__ BlendParams P) {
     static_assert(!(RECORD && COARSE), "the backward state is recorded on per-tile lists only");
     __shared__ StagedRec s_rec[BLEND_BATCH];
@@ -169,7 +172,7 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
     float T0 = in0 ? 1.0f : 0.0f, T1 = in1 ? 1.0f : 0.0f, ca0 = 0.f, ca1 = 0.f, cb0 = 0.f, cb1 = 0.f, cc0 = 0.f, cc1 = 0.f;
 #define BLEND_DONE (T0 == 0.0f && T1 == 0.0f)
     uint32_t used = 0, walked = 0, hits = 0, staged = 0;
-    BlendRecord<RECORD> brec;
+    BlendRecord<RECORD || BG> brec;
     const uint32_t rec_sh = (uint32_t)__cvta_generic_to_shared(&s_rec[0]);
     const uint32_t list_sh = (uint32_t)__cvta_generic_to_shared(&s_list[warp][0]);
 
@@ -348,7 +351,7 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
                         cb1 = __fadd_rn(cb1, w1b);
                         cc1 = __fadd_rn(cc1, w1c);
                     }
-                    if constexpr (RECORD) brec.note(ok0, ok1, tt0, tt1, base_off + __float_as_uint(q2.z) + 1u);
+                    if constexpr (RECORD || BG) brec.note(ok0, ok1, tt0, tt1, base_off + __float_as_uint(q2.z) + 1u);
                     if (in0k) T0 = ok0 ? tt0 : 0.0f;  // :88, or the break
                     if (in1k) T1 = ok1 ? tt1 : 0.0f;
                 }
@@ -363,6 +366,14 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
 #undef BLEND_DONE
     if (COARSE && seg_pending) mbar_wait(&s_bar, seg_parity);  // never leave with a bulk copy still writing this CTA's shared memory
     if constexpr (RECORD) brec.store(P, in0, in1, px, py0, py1);
+    if constexpr (BG) {  // what both store paths below write: c + T_final * bg
+        ca0 = __fadd_rn(ca0, __fmul_rn(brec.t0, P.background[0]));
+        cb0 = __fadd_rn(cb0, __fmul_rn(brec.t0, P.background[1]));
+        cc0 = __fadd_rn(cc0, __fmul_rn(brec.t0, P.background[2]));
+        ca1 = __fadd_rn(ca1, __fmul_rn(brec.t1, P.background[0]));
+        cb1 = __fadd_rn(cb1, __fmul_rn(brec.t1, P.background[1]));
+        cc1 = __fadd_rn(cc1, __fmul_rn(brec.t1, P.background[2]));
+    }
 
     if (STATS) {
         if (in0 || in1) atomicMax(&s_used, used);
@@ -423,35 +434,41 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
     }
 }
 
+template <bool BG>
+void launch_blend_as(const BlendParams& p, uint32_t blocks, cudaStream_t s) {
+    if (p.coarse_shift) {
+        if (p.stats) {
+            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, true, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            else k_blend<GSB_MODE_FAST, true, true, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        } else {
+            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, true, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            else k_blend<GSB_MODE_FAST, false, true, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        }
+    } else if (p.record) {  // gsb_set_backward
+        if (p.stats) {
+            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, false, true, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            else k_blend<GSB_MODE_FAST, true, false, true, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        } else {
+            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, false, true, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            else k_blend<GSB_MODE_FAST, false, false, true, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        }
+    } else if (p.stats) {
+        if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, false, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        else k_blend<GSB_MODE_FAST, true, false, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+    } else {
+        if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, false, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        else k_blend<GSB_MODE_FAST, false, false, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+    }
+}
+
 }  // namespace
 
 cudaError_t launch_blend(const BlendParams& p, cudaStream_t s) {
     const uint32_t rows = p.tile_row_end - p.tile_row_begin;
     const uint32_t blocks = rows * p.tiles_x;
     if (blocks == 0) return cudaSuccess;
-    if (p.coarse_shift) {
-        if (p.stats) {
-            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
-            else k_blend<GSB_MODE_FAST, true, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
-        } else {
-            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
-            else k_blend<GSB_MODE_FAST, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
-        }
-    } else if (p.record) {  // gsb_set_backward
-        if (p.stats) {
-            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
-            else k_blend<GSB_MODE_FAST, true, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
-        } else {
-            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
-            else k_blend<GSB_MODE_FAST, false, false, true><<<blocks, BLEND_THREADS, 0, s>>>(p);
-        }
-    } else if (p.stats) {
-        if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, false><<<blocks, BLEND_THREADS, 0, s>>>(p);
-        else k_blend<GSB_MODE_FAST, true, false><<<blocks, BLEND_THREADS, 0, s>>>(p);
-    } else {
-        if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, false><<<blocks, BLEND_THREADS, 0, s>>>(p);
-        else k_blend<GSB_MODE_FAST, false, false><<<blocks, BLEND_THREADS, 0, s>>>(p);
-    }
+    if (has_background(p.background)) launch_blend_as<true>(p, blocks, s);  // gsb_set_background
+    else launch_blend_as<false>(p, blocks, s);
     return cudaGetLastError();
 }
 

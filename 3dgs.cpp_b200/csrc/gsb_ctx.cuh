@@ -93,6 +93,7 @@ struct LastFrame {
     gsb_uniforms ubo{};      // its camera
     int mode = GSB_MODE_EXACT;
     bool antialiased = false;  // gsb_set_antialiased when enqueued: its opacities carry the compensation
+    float background[3] = {};  // gsb_set_background when enqueued: the colour its pixels were composited over
     uint64_t scene_gen = 0;  // gsb_ctx::scene_gen when enqueued; 0: no frame yet (a frame needs an upload, which bumps it)
     bool pending = false;    // its completion event and stats copy have not been waited for (wait_frame)
     bool exists = false;     // its stats and debug buffers may be read (a scene upload clears it)
@@ -157,6 +158,7 @@ struct gsb_ctx {
     bool debug = false;
     bool timers = true;
     bool antialiased = false;   // gsb_set_antialiased: k_project scales opacities by the dilation's compensation
+    float background[3] = {};   // gsb_set_background: k_blend composites every pixel over this colour (zeros: no term)
     int tile_cull = 0;          // gsb_set_tile_cull level: 0 reference-equivalent lists, 1 exact per-tile culling, 2 coarse bins
     uint32_t coarse_shift = 2;  // level 2 bins are 2^shift x 2^shift tiles (GSB_COARSE_SHIFT)
     cudaEvent_t ev[8] = {};
@@ -188,7 +190,8 @@ struct gsb_ctx {
     DevArray<double> bw_abs;        // n x 2 per-survivor fp64 sums of |d u|, |d v| of gsb_render_backward_density (kept zero)
     bool bw_deterministic = false;  // gsb_set_backward_deterministic
     gsb::DetBuffers bw_det;
-    uint64_t scene_gen = 0;         // bumped by every gsb_scene_upload and gsb_adam_step
+    DevArray<double> bg_partials;   // [background_grad_rows(H)][3] per-CTA fp64 partial sums of gsb_background_gradient
+    uint64_t scene_gen = 0;        // bumped by every gsb_scene_upload and gsb_adam_step
 
     // gsb_image_loss (gsb_loss.cu): allocated on first use, grown with the frame size
     DevArray<float> loss_abc;        // 9 x W x H: the gather terms A, B, C of each RGB channel (only for a gradient)

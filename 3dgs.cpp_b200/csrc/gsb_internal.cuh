@@ -157,8 +157,15 @@ struct BlendParams {
     // gsb_set_backward (per-tile lists only): per pixel of the W x H frame, (bits(final transmittance), list position + 1 of the
     // last contributing entry, 0 = none).  Null: a plain frame.  Appended last so the other fields keep their offsets.
     uint2* record;
+    // gsb_set_background: every pixel is stored as c + T_final * background (all zeros: the default kernels, no term).
+    // Appended last so the other fields keep their offsets.
+    float background[3];
 };
 cudaError_t launch_blend(const BlendParams& p, cudaStream_t s);
+
+// A background of zeros (either sign) adds nothing: such frames and backward passes run the default instantiations.
+inline bool has_background(const float bg[3]) { return bg[0] != 0.0f || bg[1] != 0.0f || bg[2] != 0.0f; }
+inline bool has_background(float3 bg) { return bg.x != 0.0f || bg.y != 0.0f || bg.z != 0.0f; }
 
 // gsb_backward.cu: the reverse pass of one whole frame recorded by k_blend<..., RECORD = true>
 struct BackwardParams {
@@ -204,8 +211,17 @@ struct DetBackward {
     uint32_t m_hint;               // sizes the sort's grids only
     uint32_t key_bits;             // bits of the largest compact id
 };
-// antialiased: the frame ran with gsb_set_antialiased on (its opacities carry the compensation, whose chain rule is added)
-cudaError_t launch_backward(const BackwardParams& p, bool antialiased, cudaStream_t s, const DetBackward* det = nullptr);
+// antialiased: the frame ran with gsb_set_antialiased on (its opacities carry the compensation, whose chain rule is added).
+// background: the frame's gsb_set_background, the colour behind every pixel's last contributor.  It is a kernel argument of
+// its own after BackwardParams, not a field of it: a larger BackwardParams would move the arguments that follow it in
+// k_det_reduce.
+cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det = nullptr);
+// gsb_background_gradient: out[c] = sum over the W x H pixels of T_final(p) grad_image(p)[c], from the recorded frame's
+// (bits(T), last) words.  fp64 products and sums in an order fixed by W and H (background_grad_rows(H) per-CTA partials,
+// then one CTA), no atomics.  partials holds 3 doubles per row of background_grad_rows(H).
+uint32_t background_grad_rows(uint32_t height);
+cudaError_t launch_background_grad(const uint2* record, const float* grad_image, size_t row_pitch_bytes, uint32_t width,
+                                   uint32_t height, double* partials, float* out, cudaStream_t s);
 
 // gsb_optim.cu: one Adam step over the scene's rows (gsb_adam_step).  Every per-row array is n x 60 floats = 15 float4 per row.
 struct AdamParams {

@@ -38,12 +38,12 @@ ALL_ROWS = 0xFFFFFFFF
 EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_abi_version", "gsb_device_count", "gsb_create", "gsb_destroy", "gsb_last_error",
     "gsb_scene_upload", "gsb_scene_size", "gsb_set_mode", "gsb_set_debug", "gsb_set_timers", "gsb_set_tile_cull", "gsb_set_sh_storage",
-    "gsb_set_antialiased",
+    "gsb_set_antialiased", "gsb_set_background",
     "gsb_reserve_instances", "gsb_render", "gsb_render_async", "gsb_get_stats", "gsb_debug_size",
     "gsb_debug_download", "gsb_sort_pairs", "gsb_sort_pairs32", "gsb_set_graph", "gsb_host_alloc", "gsb_host_free",
     # reverse mode
     "gsb_set_backward", "gsb_render_backward", "gsb_render_backward_camera", "gsb_render_backward_density",
-    "gsb_set_backward_deterministic",
+    "gsb_set_backward_deterministic", "gsb_background_gradient",
     # training loss, optimizer step and initialisation from a point cloud
     "gsb_image_loss", "gsb_adam_step", "gsb_init_from_points",
     # frame sharding over several GPUs
@@ -151,6 +151,7 @@ lib.gsb_set_debug.argtypes = [_vp, C.c_int]
 lib.gsb_set_timers.argtypes = [_vp, C.c_int]
 lib.gsb_set_tile_cull.argtypes = [_vp, C.c_int]
 lib.gsb_set_antialiased.argtypes = [_vp, C.c_int]
+lib.gsb_set_background.argtypes = [_vp, C.POINTER(C.c_float)]
 lib.gsb_set_sh_storage.argtypes = [_vp, C.c_int]
 lib.gsb_set_graph.argtypes = [_vp, C.c_int]
 lib.gsb_host_alloc.argtypes = [C.POINTER(_vp), C.c_size_t]
@@ -170,6 +171,7 @@ lib.gsb_set_backward_deterministic.argtypes = [_vp, C.c_int]
 lib.gsb_render_backward.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp]
 lib.gsb_render_backward_camera.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp]
 lib.gsb_render_backward_density.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp]
+lib.gsb_background_gradient.argtypes = [_vp, _vp, C.c_size_t, _vp, _vp]
 lib.gsb_image_loss.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_float, _vp,
                                C.c_size_t, _vp, _vp]
 lib.gsb_adam_step.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(AdamConfig), _vp]
@@ -412,6 +414,7 @@ class Context:
         self.h = handle
         self.device = device
         self.frames = 0  # frames rendered through this wrapper (render_torch checks it between forward and backward)
+        self._background = None  # the last set_background colour (render_torch restores it after a frame of its own)
 
     def close(self):
         if self.h and self._own:
@@ -457,6 +460,26 @@ class Context:
         compensation for the 0.3 px dilation (gsplat's antialiased mode).  render_torch, SceneAdam, image_metrics and the
         backward pass follow it (the backward uses the setting of the frame it differentiates)."""
         self._ck(lib.gsb_set_antialiased(self.h, int(on)))
+
+    def set_background(self, rgb=None):
+        """gsb_set_background: from the next frame, every pixel is composited over the colour rgb (3 finite floats; None =
+        black, the default): out = c + T_final * rgb.  The backward pass follows the colour of the frame it differentiates."""
+        self._ck(lib.gsb_set_background(self.h, None if rgb is None else (C.c_float * 3)(*(float(x) for x in rgb))))
+        self._background = None if rgb is None else [float(x) for x in rgb]
+
+    def background_gradient(self, grad_image, stream=None):
+        """gsb_background_gradient of the last (recorded, whole) frame: dL/d(background) = sum_p T_final(p) grad_image(p) as a
+        (3,) float32 CUDA tensor, enqueued on `stream` (a torch stream; default torch's current stream).  grad_image is an
+        (H, W, 4) float32 CUDA tensor (A ignored).  Bitwise reproducible; does not wait on the host."""
+        import torch
+
+        g = grad_image.detach()
+        if g.dtype != torch.float32 or g.dim() != 3 or g.shape[2] != 4 or not g.is_cuda or g.stride(2) != 1 or g.stride(1) != 4:
+            raise ValueError("background_gradient: grad_image must be an (H, W, 4) float32 CUDA tensor with dense pixels")
+        out = torch.empty(3, dtype=torch.float32, device=g.device)
+        s = torch.cuda.current_stream(g.device) if stream is None else stream
+        self._ck(lib.gsb_background_gradient(self.h, g.data_ptr(), g.stride(0) * 4, out.data_ptr(), _torch_stream_arg(s)))
+        return out
 
     def set_sh_storage(self, half=True):
         """gsb_set_sh_storage: fp16 SH coefficients from the next upload on (NOT a parity mode)."""
@@ -674,7 +697,7 @@ def _render_fn():
 
         class RenderFn(torch.autograd.Function):
             @staticmethod
-            def forward(fctx, ctx, vertices, u, ubo, density):
+            def forward(fctx, ctx, vertices, u, ubo, density, background):
                 v = vertices.detach().contiguous()
                 _check_density("render_torch", density, v)
                 fctx.density = density
@@ -684,7 +707,16 @@ def _render_fn():
                 ctx.set_backward(True)
                 torch.cuda.current_stream(v.device).synchronize()  # the upload runs on the context's stream: v must be complete
                 ctx.upload(v)
-                img = ctx._render_whole_frame(u, v.device)
+                if background is None:
+                    img = ctx._render_whole_frame(u, v.device)
+                else:  # this frame over the tensor's colour; the context's own setting is restored after it
+                    fctx.bg_like = (background.dtype, background.device)
+                    previous = ctx._background
+                    ctx.set_background(background.detach().to("cpu", torch.float32).reshape(3).tolist())
+                    try:
+                        img = ctx._render_whole_frame(u, v.device)
+                    finally:
+                        ctx.set_background(previous)
                 fctx.gs_ctx, fctx.frame, fctx.vertices = ctx, ctx.frames, v
                 return img
 
@@ -695,27 +727,31 @@ def _render_fn():
                     raise RuntimeError("render_torch: another frame was rendered on this context between forward and backward")
                 v = fctx.vertices
                 g = grad_img.detach().to(torch.float32).contiguous()
-                need_v, need_ubo = fctx.needs_input_grad[1], fctx.needs_input_grad[3]
+                need_v, need_ubo, need_bg = fctx.needs_input_grad[1], fctx.needs_input_grad[3], fctx.needs_input_grad[5]
                 grad_v = torch.empty_like(v) if need_v else None
-                grad_ubo = None
+                grad_ubo = grad_bg = None
                 # enqueued on torch's current stream (the engine runs backward on the forward's stream), so the gradients
                 # are complete for whatever torch enqueues after them
                 stream = _torch_stream_arg(torch.cuda.current_stream(v.device))
                 gu = torch.empty(40, dtype=torch.float32, device=v.device) if need_ubo else None  # a whole gsb_uniforms
                 ctx.set_backward_deterministic(torch.are_deterministic_algorithms_enabled())
-                ctx._backward(v.data_ptr(), g.data_ptr(), grad_v.data_ptr() if need_v else None, stream,
-                              grad_uniforms_ptr=gu.data_ptr() if need_ubo else None,
-                              density_ptr=None if fctx.density is None else fctx.density.data_ptr())
+                if need_v or need_ubo:
+                    ctx._backward(v.data_ptr(), g.data_ptr(), grad_v.data_ptr() if need_v else None, stream,
+                                  grad_uniforms_ptr=gu.data_ptr() if need_ubo else None,
+                                  density_ptr=None if fctx.density is None else fctx.density.data_ptr())
                 if need_ubo:
                     dtype, device = fctx.ubo_like
                     grad_ubo = gu[UBO_FLOAT_WORDS].to(device=device, dtype=dtype)
-                return None, grad_v, None, grad_ubo, None
+                if need_bg:  # sum_p T_final g, on the same stream
+                    dtype, device = fctx.bg_like
+                    grad_bg = ctx.background_gradient(g, torch.cuda.current_stream(v.device)).to(device=device, dtype=dtype)
+                return None, grad_v, None, grad_ubo, None, grad_bg
 
         _RenderFn = RenderFn
     return _RenderFn
 
 
-def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None):
+def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, background=None):
     """Differentiable frame: vertices is a CUDA float32 tensor (n, 60) of GSScene::Vertex records (activated parameters, as
     gsb_scene_upload takes them).  Uploads it from device memory, renders the whole frame as an (H, W, 4) RGBA32F tensor and,
     on backward, returns dL/dvertices through gsb_render_backward.  Turns gsb_set_backward on for `ctx`.  The frame on the
@@ -728,12 +764,16 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None):
     density (optional): a contiguous (n, 4) float32 tensor on the vertices' device that backward accumulates this frame's
     density-control statistics into (gsb_render_backward_density, on torch's stream): screen-space gradient norm and absolute
     gradient norm in NDC units, the view count and the max pixel radius; see densify_and_prune.  Backward runs only when
-    vertices or ubo requires grad.
+    vertices, ubo or background requires grad.
+
+    background (optional): a (3,) tensor; the frame is rendered over its colour (gsb_set_background) and the context's own
+    setting is restored after the forward.  If it requires grad, backward also returns dL/dbackground = sum_p T_final(p)
+    dL/dimage(p) (gsb_background_gradient, on torch's stream) -- also for frozen vertices, a learned background alone.
 
     Under torch.use_deterministic_algorithms(True), backward turns gsb_set_backward_deterministic on for `ctx` (otherwise
     off): every gradient and density statistic is then bit-identical for the same inputs, at some cost in time.  With
     torch's default settings backward takes the atomic path, whose results may differ in the last bit from run to run."""
-    return _render_fn().apply(ctx, vertices, u, ubo, density)
+    return _render_fn().apply(ctx, vertices, u, ubo, density, background)
 
 
 _LossFn = None
@@ -770,6 +810,23 @@ def image_loss_torch(ctx: "Context", image, target, lambda_dssim=0.2):
     host; backward returns the gradient the forward computed, scaled by the upstream gradient.  The result and the gradient
     are bitwise reproducible for the same inputs.  Bad shapes, dtypes or devices raise ValueError."""
     return _loss_fn().apply(ctx, image, target, float(lambda_dssim))
+
+
+def composite_target(target, background):
+    """An (H, W, 4) RGBA target (float32, or uint8 read as v / 255) composited over `background` (3 values or a (3,) tensor):
+    rgb a + bg (1 - a) as an (H, W, 4) float32 tensor with A = 1 -- what a frame rendered over that background (gsb_set_background)
+    is compared against.  Runs on the target's device."""
+    import torch
+
+    t = target.to(torch.float32) / 255.0 if target.dtype == torch.uint8 else target.to(torch.float32)
+    if t.dim() != 3 or t.shape[2] != 4:
+        raise ValueError("composite_target: target must be (H, W, 4)")
+    bg = torch.as_tensor(background, dtype=torch.float32).to(t.device).reshape(3)
+    a = t[..., 3:4]
+    out = torch.empty_like(t)
+    out[..., :3] = t[..., :3] * a + bg * (1.0 - a)
+    out[..., 3] = 1.0
+    return out
 
 
 def image_metrics(ctx: "Context", image, target):
@@ -873,15 +930,23 @@ class SceneAdam:
     so the caller may change them (a schedule).  selective=True updates only the rows of the Gaussians that survived the
     frame's culls (the "selective Adam" of Mallick et al. 2024); False is torch.optim.Adam's dense update of every row.
     Turns gsb_set_backward on for ctx and uploads `vertices` once; under torch.use_deterministic_algorithms(True) the
-    backward pass runs deterministically, as in render_torch."""
+    backward pass runs deterministically, as in render_torch.
 
-    def __init__(self, ctx: "Context", vertices, lr, betas=(0.9, 0.999), eps=1e-15, selective=True):
+    background: the colour render() composites over (gsb_set_background; None = the context's own setting).
+    random_background=True: every render() draws a fresh uniform [0, 1)^3 colour from a torch.Generator seeded with `seed`
+    (Inria's --random_background: the empty space must stay transparent to match every colour), to be compared against
+    composite_target(rgba_target, opt.background).  `background` holds the colour of the last render() as 3 floats."""
+
+    def __init__(self, ctx: "Context", vertices, lr, betas=(0.9, 0.999), eps=1e-15, selective=True, background=None,
+                 random_background=False, seed=0):
         import torch
 
         if not isinstance(vertices, torch.Tensor) or not vertices.is_cuda or vertices.dim() != 2 or vertices.shape[1] != 60:
             raise ValueError("SceneAdam: vertices must be an (n, 60) CUDA tensor")
         self.ctx, self.lr, self.betas, self.eps, self.selective = ctx, list(lr), tuple(betas), float(eps), bool(selective)
         self.steps = 0
+        self.background = None if background is None else [float(x) for x in background]
+        self._generator = torch.Generator().manual_seed(int(seed)) if random_background else None
         self._adopt(vertices.detach().to(torch.float32).contiguous().clone(), None)
         ctx.set_backward(True)
         self._upload()
@@ -903,7 +968,13 @@ class SceneAdam:
 
     def render(self, u: Uniforms):
         """The resident scene's frame of u as an (H, W, 4) float32 tensor, rendered on torch's current stream with the
-        backward state recorded.  No upload."""
+        backward state recorded, over the optimizer's background (fixed or a fresh random colour).  No upload."""
+        import torch
+
+        if self._generator is not None:
+            self.background = torch.rand(3, generator=self._generator).tolist()
+        if self.background is not None:
+            self.ctx.set_background(self.background)
         return self.ctx._render_whole_frame(u, self.vertices.device)
 
     def step(self, grad_image, density=None):

@@ -183,6 +183,15 @@ int gsb_set_tile_cull(gsb_ctx *ctx, int level);
  * frame; the backward entries and the selective gsb_adam_step follow the setting the last frame was rendered with and
  * differentiate through comp.  NULL ctx or a sharded context (gsb_create_sharded, a gsb_group rank): GSB_ERR_INVALID. */
 int gsb_set_antialiased(gsb_ctx *ctx, int enabled);
+/* Background colour (default black; no reference counterpart).  rgb: 3 host floats, NULL = (0, 0, 0).  render.comp:98 stores
+ * vec4(c, 1), the colour composited over black; with a background every colour channel of every pixel is stored as
+ *     out = c + T_final * bg          (one fp32 multiply, then one add, each rounded; EXACT and FAST alike)
+ * T_final being the transmittance after the pixel's last contributor (at the T' < 1e-4 break, the T before the breaking
+ * Gaussian).  A pixel no Gaussian reaches is bg exactly.  8-bit formats quantise out as before; A stays 1 (255).  All zeros
+ * (either sign) is the default frame, bit for bit.  Any finite values (a learned colour may leave [0, 1]); NaN or +-inf:
+ * GSB_ERR_INVALID.  Takes effect at the next frame; the frame records it and the backward entries follow the frame's value.
+ * Every context accepts it, sharded ones and gsb_group ranks included; changing it drops no captured graph. */
+int gsb_set_background(gsb_ctx *ctx, const float *rgb);
 /* per-stage cudaEvent timers (the QueryManager analogue, Renderer.cpp:85-100). Default on. */
 int gsb_set_timers(gsb_ctx *ctx, int enabled);
 /* Replay the camera-independent middle of the frame (both sorts + key emission) from a captured CUDA graph instead of
@@ -277,6 +286,17 @@ int gsb_render_backward_camera(gsb_ctx *ctx, const float *vertices, const float 
  *                  Culled Gaussians' rows are not touched. */
 int gsb_render_backward_density(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,
                                 float *grad_vertices, gsb_uniforms *grad_uniforms, float *density, void *stream);
+
+/* dL/d(background) of the last frame (gsb_set_background): grad_background (device, 3 floats) is OVERWRITTEN with
+ * sum over the W x H pixels p of T_final(p) g(p), g from grad_image (as for gsb_render_backward: H x W float4,
+ * row_pitch_bytes apart, 0 = tight, A ignored).  It does not depend on the background's value, so it is defined for a frame
+ * rendered over black too.  The products are formed exactly and summed in fp64 in an order that depends only on W and H,
+ * without atomics, then rounded once: the words are a function of the recorded frame and grad_image alone, whatever the
+ * stream, tile-cull level, deterministic switch or arena.  Enqueued on `stream` (NULL = the context's), never synchronises;
+ * runs for an empty scene as well.  The same last-frame preconditions and error codes as gsb_render_backward (fp16 SH storage
+ * excepted: T_final does not depend on it); GSB_ERR_INVALID for a NULL pointer, a bad pitch or a sharded context. */
+int gsb_background_gradient(gsb_ctx *ctx, const float *grad_image, size_t row_pitch_bytes, float *grad_background,
+                            void *stream);
 
 /* Photometric loss of a frame against a target, and its gradient (no reference counterpart): the loss of 3DGS training,
  * loss = (1 - lambda) L1 + lambda (1 - SSIM), with SSIM over an 11 x 11 Gaussian window (sigma 1.5) applied with zero
