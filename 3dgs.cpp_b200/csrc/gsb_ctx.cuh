@@ -191,7 +191,7 @@ struct gsb_ctx {
     bool bw_deterministic = false;  // gsb_set_backward_deterministic
     gsb::DetBuffers bw_det;
     DevArray<double> bg_partials;   // [background_grad_rows(H)][3] per-CTA fp64 partial sums of gsb_background_gradient
-    uint64_t scene_gen = 0;        // bumped by every gsb_scene_upload and gsb_adam_step
+    uint64_t scene_gen = 0;        // bumped by every gsb_scene_upload, gsb_adam_step, gsb_mcmc_noise and gsb_mcmc_relocate
 
     // gsb_image_loss (gsb_loss.cu): allocated on first use, grown with the frame size
     DevArray<float> loss_abc;        // 9 x W x H: the gather terms A, B, C of each RGB channel (only for a gradient)

@@ -46,6 +46,8 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_set_backward_deterministic", "gsb_background_gradient",
     # training loss, optimizer step and initialisation from a point cloud
     "gsb_image_loss", "gsb_adam_step", "gsb_init_from_points",
+    # 3DGS-MCMC: position noise and relocation
+    "gsb_mcmc_noise", "gsb_mcmc_relocate",
     # frame sharding over several GPUs
     "gsb_group_create", "gsb_group_destroy", "gsb_group_size", "gsb_group_context", "gsb_group_last_error",
     "gsb_group_scene_upload", "gsb_group_render", "gsb_group_render_async",
@@ -176,6 +178,8 @@ lib.gsb_image_loss.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp
                                C.c_size_t, _vp, _vp]
 lib.gsb_adam_step.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(AdamConfig), _vp]
 lib.gsb_init_from_points.argtypes = [_vp, _vp, _vp, C.c_uint64, C.c_float, _vp, _vp]
+lib.gsb_mcmc_noise.argtypes = [_vp, _vp, _vp, C.c_float, C.c_uint64, C.c_uint64, _vp]
+lib.gsb_mcmc_relocate.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint64, C.c_float, _vp]
 
 lib.gsb_group_create.argtypes = [C.c_int, C.POINTER(C.c_int), C.POINTER(_vp)]
 lib.gsb_group_destroy.argtypes = [_vp]
@@ -593,19 +597,63 @@ class Context:
         stream, and does not wait for it.  Bad shapes, dtypes, devices or layouts raise ValueError."""
         import torch
 
-        n = self.num_gaussians
-        arrays = {"params": params, "exp_avg": exp_avg, "exp_avg_sq": exp_avg_sq, "grad_vertices": grad_vertices,
-                  "vertices": vertices}
-        for name, t in arrays.items():
-            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
-                raise ValueError(f"adam_step: {name} must be a CUDA tensor on device {self.device}")
-            if t.dtype != torch.float32 or tuple(t.shape) != (n, 60) or not t.is_contiguous():
-                raise ValueError(f"adam_step: {name} must be a contiguous ({n}, 60) float32 tensor, got {tuple(t.shape)} "
-                                 f"{t.dtype}{'' if t.is_contiguous() else ' (not contiguous)'}")
+        self._check_rows("adam_step", {"params": params, "exp_avg": exp_avg, "exp_avg_sq": exp_avg_sq,
+                                       "grad_vertices": grad_vertices, "vertices": vertices})
         s = _torch_stream_arg(torch.cuda.current_stream(params.device) if stream is None else stream)
         self._ck(lib.gsb_adam_step(self.h, params.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(),
                                    grad_vertices.data_ptr(), vertices.data_ptr(), C.byref(cfg), s))
         self.frames += 1  # the scene changed: the last frame can no longer be differentiated
+
+    def _check_rows(self, caller, arrays):
+        """Every tensor of `arrays` (name -> tensor) is a contiguous (n, 60) float32 CUDA tensor on the context's device,
+        n the scene's size; ValueError otherwise."""
+        import torch
+
+        n = self.num_gaussians
+        for name, t in arrays.items():
+            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
+                raise ValueError(f"{caller}: {name} must be a CUDA tensor on device {self.device}")
+            if t.dtype != torch.float32 or tuple(t.shape) != (n, 60) or not t.is_contiguous():
+                raise ValueError(f"{caller}: {name} must be a contiguous ({n}, 60) float32 tensor, got {tuple(t.shape)} "
+                                 f"{t.dtype}{'' if t.is_contiguous() else ' (not contiguous)'}")
+
+    def mcmc_noise(self, params, vertices, scale, seed, step, stream=None):
+        """gsb_mcmc_noise on torch tensors: adds 3DGS-MCMC's position noise Sigma (eps * gate(o) * scale) to every row of
+        params, vertices and the resident scene, eps standard normals drawn by Philox4x32-10 from (seed, step, row), so the
+        same arguments give the same words anywhere.  params and vertices are contiguous (n, 60) float32 CUDA tensors on the
+        context's device; scale is the position learning rate times noise_lr.  Runs on `stream` (a torch stream), by default
+        torch's current stream, and does not wait for it.  Bad shapes, dtypes, devices or layouts raise ValueError."""
+        import torch
+
+        self._check_rows("mcmc_noise", {"params": params, "vertices": vertices})
+        s = _torch_stream_arg(torch.cuda.current_stream(params.device) if stream is None else stream)
+        self._ck(lib.gsb_mcmc_noise(self.h, params.data_ptr(), vertices.data_ptr(), float(scale), int(seed) & (2**64 - 1),
+                                    int(step) & (2**64 - 1), s))
+        self.frames += 1  # the scene changed: the last frame can no longer be differentiated
+
+    def mcmc_relocate(self, params, exp_avg, exp_avg_sq, vertices, dst, src, min_opacity=0.005, stream=None):
+        """gsb_mcmc_relocate on torch tensors: row dst[j] becomes a copy of row src[j], after each source's opacity and scale
+        are corrected for its r = 1 + (times it appears in src) copies; the moments of source and destination rows become
+        zero.  The four arrays are as for adam_step; dst and src are 1-D int32 (or uint32) CUDA tensors of one length k on
+        the context's device.  Runs on `stream` (a torch stream), by default torch's current stream, and returns once the
+        rows are written.  An index >= n, a repeated destination or a destination that is also a source raise GsbError
+        (ERR_INVALID) with nothing written; bad shapes, dtypes, devices or layouts raise ValueError."""
+        import torch
+
+        self._check_rows("mcmc_relocate", {"params": params, "exp_avg": exp_avg, "exp_avg_sq": exp_avg_sq,
+                                           "vertices": vertices})
+        for name, t in (("dst", dst), ("src", src)):
+            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
+                raise ValueError(f"mcmc_relocate: {name} must be a CUDA tensor on device {self.device}")
+            if t.dtype not in (torch.int32, torch.uint32) or t.dim() != 1 or t.shape != dst.shape:
+                raise ValueError(f"mcmc_relocate: {name} must be a 1-D int32 tensor of dst's length, got {tuple(t.shape)} {t.dtype}")
+        k = dst.shape[0]
+        dst, src = dst.contiguous(), src.contiguous()
+        s = _torch_stream_arg(torch.cuda.current_stream(params.device) if stream is None else stream)
+        self._ck(lib.gsb_mcmc_relocate(self.h, params.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(),
+                                       vertices.data_ptr(), dst.data_ptr(), src.data_ptr(), k, float(min_opacity), s))
+        if k:
+            self.frames += 1
 
     def init_from_points(self, xyz, rgb, opacity=0.1):
         """gsb_init_from_points on torch tensors: the (n, 60) float32 activated records of a point cloud, one isotropic
@@ -916,6 +964,28 @@ def adam_state_after_densify(params, exp_avg, exp_avg_sq, vertices, new_vertices
     return p.contiguous(), m.contiguous(), v.contiguous()
 
 
+def mcmc_sample(weights, k, generator=None):
+    """k row indices drawn with replacement in proportion to `weights` (n non-negative finite values, positive sum), by
+    inverse-CDF sampling: the float64 cumulative sum, torch.rand(k, dtype=float64, generator=generator) times the total, and
+    searchsorted(right=True), clamped to the last row of positive weight.  Zero-weight rows are never chosen, any n works
+    (torch.multinomial stops at 2^24 categories), and the work is done on the CPU, so a seeded CPU generator gives the same
+    rows whatever device the weights are on.  Returns an int64 tensor on the weights' device."""
+    import torch
+
+    w = weights.detach().to("cpu", torch.float64).reshape(-1)
+    n = w.shape[0]
+    if k < 0 or n == 0:
+        raise ValueError(f"mcmc_sample: needs k >= 0 and at least one weight, got k = {k}, n = {n}")
+    cdf = torch.cumsum(w, 0)
+    total = float(cdf[-1])
+    if not (total > 0.0 and total < float("inf")) or bool((w < 0).any()):
+        raise ValueError("mcmc_sample: weights must be non-negative and finite with a positive sum")
+    u = torch.rand(int(k), dtype=torch.float64, generator=generator) * total
+    idx = torch.searchsorted(cdf, u, right=True)
+    last = int(torch.searchsorted(cdf, cdf[-1:], right=False))  # u * total may round up to the total itself
+    return idx.clamp_(max=min(n - 1, last)).to(weights.device)
+
+
 class SceneAdam:
     """Trains the scene resident on `ctx` with gsb_adam_step: the fused chain rule through the activations, Adam and the
     scene update in one kernel, so a step needs no upload and waits on nothing.  A training step reads
@@ -935,7 +1005,19 @@ class SceneAdam:
     background: the colour render() composites over (gsb_set_background; None = the context's own setting).
     random_background=True: every render() draws a fresh uniform [0, 1)^3 colour from a torch.Generator seeded with `seed`
     (Inria's --random_background: the empty space must stay transparent to match every colour), to be compared against
-    composite_target(rgba_target, opt.background).  `background` holds the colour of the last render() as 3 floats."""
+    composite_target(rgba_target, opt.background).  `background` holds the colour of the last render() as 3 floats.
+
+    3D Gaussian Splatting as Markov Chain Monte Carlo (Kheradmand et al. 2024, gsplat's MCMCStrategy) instead of
+    densify(): the opacity and scale regularisers in step(), position noise after every step (inject_noise, seeded by
+    `seed` and the step count) and a periodic relocate() that moves dead Gaussians onto live ones and grows the scene up to
+    a budget of cap_max Gaussians:
+
+        img = opt.render(u)
+        ctx.image_loss(img, target, 0.2, grad_image=g)
+        opt.step(g, opacity_reg=0.01, scale_reg=0.01)
+        opt.inject_noise()
+        if 500 < it < 25000 and it % 100 == 0:
+            opt.relocate(cap_max)"""
 
     def __init__(self, ctx: "Context", vertices, lr, betas=(0.9, 0.999), eps=1e-15, selective=True, background=None,
                  random_background=False, seed=0):
@@ -945,6 +1027,7 @@ class SceneAdam:
             raise ValueError("SceneAdam: vertices must be an (n, 60) CUDA tensor")
         self.ctx, self.lr, self.betas, self.eps, self.selective = ctx, list(lr), tuple(betas), float(eps), bool(selective)
         self.steps = 0
+        self.seed = int(seed)
         self.background = None if background is None else [float(x) for x in background]
         self._generator = torch.Generator().manual_seed(int(seed)) if random_background else None
         self._adopt(vertices.detach().to(torch.float32).contiguous().clone(), None)
@@ -977,10 +1060,14 @@ class SceneAdam:
             self.ctx.set_background(self.background)
         return self.ctx._render_whole_frame(u, self.vertices.device)
 
-    def step(self, grad_image, density=None):
+    def step(self, grad_image, density=None, opacity_reg=0.0, scale_reg=0.0):
         """One training step from dL/d(the last render()'s image), an (H, W, 4) float32 tensor: gsb_render_backward into
         `grad` (gsb_render_backward_density, accumulating into `density`, an (n, 4) float32 tensor, when given), then
-        gsb_adam_step.  Everything runs on torch's current stream; nothing waits on the host."""
+        gsb_adam_step.  Everything runs on torch's current stream; nothing waits on the host.
+
+        opacity_reg, scale_reg: 3DGS-MCMC's regularisers opacity_reg * mean(opacity) + scale_reg * mean(scale) (the mean
+        over the n opacities and the 3 n scales), whose gradient opacity_reg / n and scale_reg / (3 n) is added to `grad`'s
+        columns 7 and 4-6 before the Adam step (gsplat uses 0.01 for both).  At 0, nothing is added."""
         import torch
 
         ctx, v = self.ctx, self.vertices
@@ -990,6 +1077,11 @@ class SceneAdam:
         _check_density("SceneAdam.step", density, v)
         ctx._backward(v.data_ptr(), g.data_ptr(), self.grad.data_ptr(), stream,
                       density_ptr=None if density is None else density.data_ptr())
+        n = v.shape[0]
+        if opacity_reg:
+            self.grad[:, 7] += opacity_reg / n
+        if scale_reg:
+            self.grad[:, 4:7] += scale_reg / (3 * n)
         self.steps += 1
         ctx.adam_step(self.params, self.exp_avg, self.exp_avg_sq, self.grad, v,
                       adam_config(self.lr, self.betas, self.eps, self.steps, self.selective))
@@ -1001,6 +1093,51 @@ class SceneAdam:
         self._adopt(new, adam_state_after_densify(self.params, self.exp_avg, self.exp_avg_sq, self.vertices, new, source))
         self._upload()
         return source
+
+    def inject_noise(self, noise_lr=5e5):
+        """3DGS-MCMC's position noise on the resident scene (gsb_mcmc_noise) with scale lr[0] * noise_lr, the optimizer's
+        seed and its step count: every row moves by Sigma eps, gated to zero as its opacity approaches 1.  Runs on torch's
+        current stream without a host wait."""
+        self.ctx.mcmc_noise(self.params, self.vertices, float(self.lr[0]) * float(noise_lr), self.seed, self.steps)
+
+    def relocate(self, cap_max, min_opacity=0.005, growth=0.05, generator=None):
+        """3DGS-MCMC's relocation and growth (gsplat's MCMCStrategy), in two phases; returns (n_relocated, n_added).
+          relocate  the dead rows, vertices[:, 7] <= min_opacity, each become a copy of a live row drawn with mcmc_sample in
+                    proportion to opacity (gsb_mcmc_relocate corrects the sources' opacity and scale for their copies); n
+                    is unchanged and nothing is uploaded.  Skipped when no row is alive.
+          add       k = max(0, min(cap_max, floor((1 + growth) n)) - n) sources drawn over all rows in proportion to
+                    opacity are appended (params and vertices copied, moments zero), the scene is uploaded once, and
+                    gsb_mcmc_relocate makes rows n .. n + k - 1 their copies.
+        generator: a CPU torch.Generator for the draws (None: torch's default)."""
+        import math
+
+        import torch
+
+        v = self.vertices
+        dev = v.device
+        n = v.shape[0]
+        op = v[:, 7]
+        dead = op <= min_opacity
+        n_dead = int(dead.sum())
+        n_relocated = 0
+        if 0 < n_dead < n:
+            src = mcmc_sample(torch.where(dead, torch.zeros_like(op), op), n_dead, generator)
+            dst = torch.nonzero(dead)[:, 0]
+            self.ctx.mcmc_relocate(self.params, self.exp_avg, self.exp_avg_sq, v, dst.to(torch.int32), src.to(torch.int32),
+                                   min_opacity)
+            n_relocated = n_dead
+        k = max(0, min(int(cap_max), int(math.floor((1.0 + growth) * n))) - n)
+        if k > 0:
+            src = mcmc_sample(self.vertices[:, 7], k, generator)
+            zeros = torch.zeros((k, 60), dtype=torch.float32, device=dev)
+            self._adopt(torch.cat([self.vertices, self.vertices[src]]).contiguous(),
+                        (torch.cat([self.params, self.params[src]]).contiguous(),
+                         torch.cat([self.exp_avg, zeros]).contiguous(), torch.cat([self.exp_avg_sq, zeros]).contiguous()))
+            self._upload()
+            dst = torch.arange(n, n + k, dtype=torch.int32, device=dev)
+            self.ctx.mcmc_relocate(self.params, self.exp_avg, self.exp_avg_sq, self.vertices, dst, src.to(torch.int32),
+                                   min_opacity)
+        return n_relocated, k
 
 
 def _uniforms_restated(position, rotation_wxyz, fov_deg, near, far, width, height):

@@ -372,6 +372,43 @@ int gsb_adam_step(gsb_ctx *ctx, float *params, float *exp_avg, float *exp_avg_sq
 int gsb_init_from_points(gsb_ctx *ctx, const float *xyz, const float *rgb, uint64_t n, float opacity, float *vertices,
                          void *stream);
 
+/* ---- training: 3D Gaussian Splatting as Markov Chain Monte Carlo (Kheradmand et al. 2024; no reference counterpart;
+ * DESIGN.md section 16) ----
+ * Both entries update the resident scene in place, as gsb_adam_step does: params, vertices (and for relocation exp_avg,
+ * exp_avg_sq) are device memory of n = gsb_scene_size rows of 60 floats in the column layout of the records, 16-B aligned;
+ * every changed row's scene words become bit-identical to what gsb_scene_upload of its `vertices` row stores; the last frame
+ * no longer describes the scene (gsb_render_backward and a selective gsb_adam_step return GSB_ERR_INVALID until the next
+ * frame) and the captured graphs, the instance arena and the grid hints are kept.  GSB_ERR_NO_SCENE before any upload;
+ * GSB_ERR_INVALID for a NULL ctx or array, a misaligned array, a sharded context or fp16 SH storage.
+ *
+ * SGLD position noise on every row i, enqueued on `stream` (NULL = the context's stream), never synchronises:
+ *   x0..x3  Philox4x32-10 (Random123's philox4x32_10) of counter (i, lo32(step), hi32(step), 0), key (lo32(seed), hi32(seed))
+ *   u_k     ((float)x_k + 0.5f) * 2^-32, in (0, 1]
+ *   eps     eps0 = sqrtf(-2 logf(u0)) cospif(2 u1), eps1 = sqrtf(-2 logf(u0)) sinpif(2 u1), eps2 = sqrtf(-2 logf(u2)) cospif(2 u3)
+ *   gate    1.0f / (1.0f + expf(100.0f * (o - 0.005f))), o the scene's opacity word (0 once expf overflows, o >~ 0.892)
+ *   d       Sigma e with e_k = eps_k * (gate * scale), each row summed ((S_r0 e0 + S_r1 e1) + S_r2 e2), Sigma the scene's words
+ * and p' = params[i, 0:3] + d is written to params columns 0-2, vertices columns 0-2 and the scene's position; nothing else
+ * changes.  The noise is a function of (seed, step, row) alone: bitwise reproducible on any grid or stream.  scale is the
+ * caller's position learning rate times noise_lr (5e5 in the paper); GSB_ERR_INVALID also for a scale below 0 or not finite. */
+int gsb_mcmc_noise(gsb_ctx *ctx, float *params, float *vertices, float scale, uint64_t seed, uint64_t step, void *stream);
+
+/* Relocation: pair j makes row dst[j] (device, k u32) a copy of row src[j] (device, k u32), after the source's opacity and
+ * scale are corrected so that the r = 1 + #{j : src[j] = s} copies of a source s render as it did.  In fp64, alpha =
+ * vertices[s, 7] and the scales vertices[s, 4..6]:
+ *   x      = 1 - (1 - alpha)^(1 / r)
+ *   denom  = sum_{j=1..r} (-1)^(j-1) C(r, j) x^j / sqrt(j), with t_j = C(r, j) x^j as t_j = t_(j-1) (r - j + 1) / j x
+ *   coeff  = alpha / denom                                          (r is not clamped)
+ * each value rounded once to fp32: the source's record gets opacity clamp(x, min_opacity, 1 - 2^-23) and scale s * coeff,
+ * its params the logit log(o / (1 - o)) and log scale log(s), in fp64 of those fp32 values; every dst row of the five arrays
+ * and of the scene becomes the source's new row; exp_avg and exp_avg_sq are zero on source and dst rows; every other row
+ * is untouched.  Each output word is a function of the inputs, whatever the scheduling.  Preconditions, checked on the
+ * device before anything is written: every index < n, the dst rows distinct, no dst row also a src row (src may repeat);
+ * a violation returns GSB_ERR_INVALID with nothing written.  Enqueued on `stream`; returns once the rows are written (the
+ * scratch, n x 8 B, is allocated and freed inside the call).  k == 0 returns GSB_OK and writes nothing (dst and src may then
+ * be NULL).  GSB_ERR_INVALID also for k >= n, a NULL or not 4-B aligned dst or src, and min_opacity outside [0, 1) or NaN. */
+int gsb_mcmc_relocate(gsb_ctx *ctx, float *params, float *exp_avg, float *exp_avg_sq, float *vertices, const uint32_t *dst,
+                      const uint32_t *src, uint64_t k, float min_opacity, void *stream);
+
 /* Size in bytes of a debug buffer for the last frame (0 if unavailable), and its download. */
 size_t gsb_debug_size(gsb_ctx *ctx, gsb_buffer which);
 int gsb_debug_download(gsb_ctx *ctx, gsb_buffer which, void *dst, size_t bytes);
