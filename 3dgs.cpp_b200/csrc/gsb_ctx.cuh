@@ -197,6 +197,9 @@ struct gsb_ctx {
     DevArray<float> loss_abc;        // 9 x W x H: the gather terms A, B, C of each RGB channel (only for a gradient)
     DevArray<double> loss_partials;  // 3 x tiles: per-tile fp64 sums of |x - y|, (x - y)^2 and the SSIM map
 
+    // gsb_bilagrid_backward (gsb_bilagrid.cu): allocated on first use, grown with the frame and grid size
+    DevArray<double> bilagrid_partials;  // [blocks][L][4][12] per-block fp64 sums of the grid gradient
+
     // frame sharding over several GPUs (gsb_shard.cu); null for a plain context
     gsb::ShardState* shard = nullptr;
 };

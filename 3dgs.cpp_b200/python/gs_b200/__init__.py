@@ -46,6 +46,8 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_set_backward_deterministic", "gsb_background_gradient",
     # training loss, optimizer step and initialisation from a point cloud
     "gsb_image_loss", "gsb_adam_step", "gsb_init_from_points",
+    # bilateral-grid appearance correction
+    "gsb_bilagrid_apply", "gsb_bilagrid_backward",
     # 3DGS-MCMC: position noise and relocation
     "gsb_mcmc_noise", "gsb_mcmc_relocate",
     # frame sharding over several GPUs
@@ -176,6 +178,10 @@ lib.gsb_render_backward_density.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp,
 lib.gsb_background_gradient.argtypes = [_vp, _vp, C.c_size_t, _vp, _vp]
 lib.gsb_image_loss.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_float, _vp,
                                C.c_size_t, _vp, _vp]
+lib.gsb_bilagrid_apply.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_uint32, C.c_uint32, C.c_uint32,
+                                   _vp, C.c_size_t, _vp]
+lib.gsb_bilagrid_backward.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_uint32, C.c_uint32, C.c_uint32,
+                                      _vp, C.c_size_t, _vp, C.c_size_t, _vp, _vp]
 lib.gsb_adam_step.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(AdamConfig), _vp]
 lib.gsb_init_from_points.argtypes = [_vp, _vp, _vp, C.c_uint64, C.c_float, _vp, _vp]
 lib.gsb_mcmc_noise.argtypes = [_vp, _vp, _vp, C.c_float, C.c_uint64, C.c_uint64, _vp]
@@ -679,19 +685,74 @@ class Context:
         self._ck(lib.gsb_init_from_points(self.h, xyz.data_ptr(), rgb.data_ptr(), n, float(opacity), out.data_ptr(), s))
         return out
 
-    def _frame_pitch(self, name, t, dtypes, hw):
+    def _frame_pitch(self, name, t, dtypes, hw, caller="image_loss"):
         """Row pitch in bytes of an (H, W, 4) CUDA tensor with dense pixels on this context's device; ValueError otherwise."""
         import torch
 
         if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
-            raise ValueError(f"image_loss: {name} must be a CUDA tensor on device {self.device}")
+            raise ValueError(f"{caller}: {name} must be a CUDA tensor on device {self.device}")
         if t.dim() != 3 or t.shape[2] != 4 or hw is None or tuple(t.shape[:2]) != tuple(hw) or t.numel() == 0:
-            raise ValueError(f"image_loss: {name} must be (H, W, 4) with the image's H and W >= 1, got {tuple(t.shape)}")
+            raise ValueError(f"{caller}: {name} must be (H, W, 4) with the image's H and W >= 1, got {tuple(t.shape)}")
         if t.dtype not in dtypes:
-            raise ValueError(f"image_loss: {name} must be {' or '.join(str(d) for d in dtypes)}, got {t.dtype}")
+            raise ValueError(f"{caller}: {name} must be {' or '.join(str(d) for d in dtypes)}, got {t.dtype}")
         if t.stride(2) != 1 or t.stride(1) != 4 or t.stride(0) < 4 * t.shape[1]:
-            raise ValueError(f"image_loss: {name} must have dense pixels and rows in order, got strides {t.stride()}")
+            raise ValueError(f"{caller}: {name} must have dense pixels and rows in order, got strides {t.stride()}")
         return t.stride(0) * t.element_size()
+
+    def _bilagrid_args(self, caller, image, grid):
+        """(H, W, image pitch, (X, Y, L)) of a bilateral-grid call's image and (12, L, Y, X) grid; ValueError otherwise."""
+        import torch
+
+        pitch = self._frame_pitch("image", image, (torch.float32,), image.shape[:2] if image.dim() == 3 else None, caller)
+        if not isinstance(grid, torch.Tensor) or not grid.is_cuda or grid.device.index != self.device:
+            raise ValueError(f"{caller}: grid must be a CUDA tensor on device {self.device}")
+        if grid.dim() != 4 or grid.shape[0] != 12 or grid.dtype != torch.float32 or not grid.is_contiguous():
+            raise ValueError(f"{caller}: grid must be a contiguous (12, L, Y, X) float32 tensor, got {tuple(grid.shape)} "
+                             f"{grid.dtype}{'' if grid.is_contiguous() else ' (not contiguous)'}")
+        if not all(2 <= d <= 64 for d in grid.shape[1:]):
+            raise ValueError(f"{caller}: grid dimensions must lie in [2, 64], got {tuple(grid.shape)}")
+        return image.shape[0], image.shape[1], pitch, (grid.shape[3], grid.shape[2], grid.shape[1])
+
+    def bilagrid_apply(self, image, grid, out=None, stream=None):
+        """gsb_bilagrid_apply on torch tensors: the frame colour-corrected by the bilateral grid, out = A(p) (r, g, b, 1) with A
+        sliced at the pixel's position and luma (DESIGN.md section 17), A copied.  image and out are (H, W, 4) float32 CUDA
+        tensors on the context's device with dense pixels (rows may be padded); grid is a contiguous (12, L, Y, X) float32
+        tensor, each dimension in [2, 64].  Returns out (a new tensor when None).  Runs on `stream` (a torch stream), by
+        default torch's current stream, without waiting.  Bad shapes, dtypes or devices raise ValueError."""
+        import torch
+
+        H, W, pitch, (X, Y, L) = self._bilagrid_args("bilagrid_apply", image, grid)
+        if out is None:
+            out = torch.empty((H, W, 4), dtype=torch.float32, device=image.device)
+        out_pitch = self._frame_pitch("out", out, (torch.float32,), (H, W), "bilagrid_apply")
+        s = _torch_stream_arg(torch.cuda.current_stream(image.device) if stream is None else stream)
+        self._ck(lib.gsb_bilagrid_apply(self.h, W, H, image.data_ptr(), pitch, grid.data_ptr(), X, Y, L, out.data_ptr(),
+                                        out_pitch, s))
+        return out
+
+    def bilagrid_backward(self, image, grid, grad_out, grad_image=None, grad_grid=None, stream=None):
+        """gsb_bilagrid_backward on torch tensors: d loss / d image (A = 0) into grad_image and d loss / d grid into grad_grid
+        from grad_out = d loss / d out, both overwritten; either may be None, not both.  grad_out and grad_image are (H, W, 4)
+        float32 and grad_grid a contiguous float32 tensor of the grid's shape, all on the context's device.  Bitwise
+        reproducible.  Runs on `stream` (a torch stream), by default torch's current stream, without waiting.  Bad
+        shapes, dtypes or devices raise ValueError."""
+        import torch
+
+        H, W, pitch, (X, Y, L) = self._bilagrid_args("bilagrid_backward", image, grid)
+        go_pitch = self._frame_pitch("grad_out", grad_out, (torch.float32,), (H, W), "bilagrid_backward")
+        gi_pitch = 0 if grad_image is None else self._frame_pitch("grad_image", grad_image, (torch.float32,), (H, W),
+                                                                  "bilagrid_backward")
+        if grad_image is None and grad_grid is None:
+            raise ValueError("bilagrid_backward: grad_image and grad_grid are both None")
+        if grad_grid is not None and (not isinstance(grad_grid, torch.Tensor) or grad_grid.device != grid.device
+                                      or grad_grid.dtype != torch.float32 or grad_grid.shape != grid.shape
+                                      or not grad_grid.is_contiguous()):
+            raise ValueError(f"bilagrid_backward: grad_grid must be a contiguous float32 tensor of shape {tuple(grid.shape)} "
+                             "on the grid's device")
+        s = _torch_stream_arg(torch.cuda.current_stream(image.device) if stream is None else stream)
+        self._ck(lib.gsb_bilagrid_backward(self.h, W, H, image.data_ptr(), pitch, grid.data_ptr(), X, Y, L,
+                                           grad_out.data_ptr(), go_pitch, None if grad_image is None else grad_image.data_ptr(),
+                                           gi_pitch, None if grad_grid is None else grad_grid.data_ptr(), s))
 
     def download(self, which) -> np.ndarray:
         nbytes = lib.gsb_debug_size(self.h, which)
@@ -860,6 +921,71 @@ def image_loss_torch(ctx: "Context", image, target, lambda_dssim=0.2):
     return _loss_fn().apply(ctx, image, target, float(lambda_dssim))
 
 
+_BilagridFn = None
+
+
+def _bilagrid_fn():
+    global _BilagridFn
+    if _BilagridFn is None:
+        import torch
+
+        class BilagridFn(torch.autograd.Function):
+            @staticmethod
+            def forward(fctx, ctx, image, grid):
+                img, grd = image.detach(), grid.detach().contiguous()
+                fctx.ctx = ctx
+                fctx.save_for_backward(img, grd)
+                return ctx.bilagrid_apply(img, grd)  # on torch's current stream
+
+            @staticmethod
+            def backward(fctx, grad_out):
+                img, grd = fctx.saved_tensors
+                want_image, want_grid = fctx.needs_input_grad[1], fctx.needs_input_grad[2]
+                if not (want_image or want_grid):
+                    return None, None, None
+                gi = torch.empty(img.shape, dtype=torch.float32, device=img.device) if want_image else None
+                gg = torch.empty_like(grd) if want_grid else None
+                go = grad_out.to(torch.float32)
+                if go.stride(2) != 1 or go.stride(1) != 4:
+                    go = go.contiguous()
+                fctx.ctx.bilagrid_backward(img, grd, go, gi, gg)
+                if gi is not None:
+                    gi[..., 3] = go[..., 3]  # A is copied
+                return None, gi, gg
+
+        _BilagridFn = BilagridFn
+    return _BilagridFn
+
+
+def bilateral_grid_torch(ctx: "Context", image, grid):
+    """Differentiable bilateral-grid colour correction (Wang et al. 2024; gsplat's BilateralGrid) through gsb_bilagrid_apply:
+    the (H, W, 4) float32 frame (render_torch's or SceneAdam.render's) with each pixel's RGB mapped by the 3 x 4 affine
+    matrix sliced from `grid` at its position and luma, A copied (DESIGN.md section 17).  grid is a (12, L, Y, X) float32
+    tensor, typically grids[i] of an identity_bilateral_grids(n) parameter, so autograd's indexing backward scatters into it.
+    The backward (gsb_bilagrid_backward) returns d/d image and d/d grid for whichever require grad, bitwise reproducibly.
+    Runs on torch's current stream and never waits on the host."""
+    return _bilagrid_fn().apply(ctx, image, grid)
+
+
+def identity_bilateral_grids(n, shape=(16, 16, 8), device=None):
+    """n identity bilateral grids, A = [I | 0] at every node, as an (n, 12, L, Y, X) float32 tensor; shape is (X, Y, L)."""
+    import torch
+
+    X, Y, L = shape
+    g = torch.zeros((n, 12, L, Y, X), dtype=torch.float32, device=device)
+    for c in range(3):
+        g[:, 4 * c + c] = 1.0
+    return g
+
+
+def bilateral_grid_tv(grids):
+    """Total-variation regulariser of bilateral grids (n, 12, L, Y, X) (or one (12, L, Y, X) grid): over the three grid axes,
+    the sum of the mean squared difference of neighbouring nodes, the mean taken over coefficients and node pairs and then
+    over the n grids.  Plain torch: the grids are small."""
+    g = grids if grids.dim() == 5 else grids.unsqueeze(0)
+    return sum(g.diff(dim=d).square().mean() for d in (2, 3, 4))
+
+
 def composite_target(target, background):
     """An (H, W, 4) RGBA target (float32, or uint8 read as v / 255) composited over `background` (3 values or a (3,) tensor):
     rgb a + bg (1 - a) as an (H, W, 4) float32 tensor with A = 1 -- what a frame rendered over that background (gsb_set_background)
@@ -1017,7 +1143,18 @@ class SceneAdam:
         opt.step(g, opacity_reg=0.01, scale_reg=0.01)
         opt.inject_noise()
         if 500 < it < 25000 and it % 100 == 0:
-            opt.relocate(cap_max)"""
+            opt.relocate(cap_max)
+
+    Per-image appearance (exposure, white balance, vignetting) with bilateral grids (Wang et al. 2024, gsplat's
+    BilateralGrid) needs no change here: the frame is corrected by bilateral_grid_torch before the loss, and the image
+    gradient it returns is what step() takes; the grids are an ordinary torch parameter with their own optimizer:
+
+        grids = torch.nn.Parameter(identity_bilateral_grids(n_images, device="cuda"))
+        grid_opt = torch.optim.Adam([grids], lr=2e-3, eps=1e-15)
+        img = opt.render(u).requires_grad_()
+        out = bilateral_grid_torch(ctx, img, grids[i])
+        loss = image_loss_torch(ctx, out, target) + 10.0 * bilateral_grid_tv(grids)
+        loss.backward(); opt.step(img.grad); grid_opt.step(); grid_opt.zero_grad()"""
 
     def __init__(self, ctx: "Context", vertices, lr, betas=(0.9, 0.999), eps=1e-15, selective=True, background=None,
                  random_background=False, seed=0):

@@ -318,6 +318,45 @@ int gsb_image_loss(gsb_ctx *ctx, uint32_t width, uint32_t height, const float *i
                    const void *target, size_t target_pitch, gsb_format target_fmt, float lambda_dssim,
                    float *grad_image, size_t grad_pitch, double *result, void *stream);
 
+/* Bilateral-grid colour correction of a frame (Wang et al. 2024; gsplat's BilateralGrid; DESIGN.md section 17): the per-image
+ * appearance model of training, applied to the rendered frame before the loss.  All pointers are device memory, enqueued on
+ * `stream` (NULL = the context's stream); never synchronises.  Needs no scene and leaves the scene and the last frame's
+ * backward state alone.
+ *   image  H x W float4 (r, g, b, a), RGBA32F layout, image_pitch bytes apart
+ *   grid   12 x L x Y x X floats (grid_l, grid_y, grid_x, each in [2, 64]), contiguous in the order [k][l][y][x]: one row of a
+ *          torch (N, 12, L, Y, X) parameter.  Coefficient k = 4 c + j is row c (output R, G, B), column j of A = [M | t].
+ *          The identity is A = [I | 0] at every node.
+ * Per pixel (px, py), every step an fp32 IEEE operation:
+ *   ix = ((px + 0.5) / W) (X - 1), iy = ((py + 0.5) / H) (Y - 1), gray = (0.299 r + 0.587 g) + 0.114 b,
+ *   iz = clamp(gray, 0, 1) (L - 1) (border padding, align_corners = True in F.grid_sample's terms);
+ *   x0 = min(floor(ix), X - 2), fx = ix - x0, and likewise for y and z;
+ *   A = the trilinear interpolation of each coefficient over the 8 nodes in lerp form, fmaf(f, hi - lo, lo), along x, then
+ *   y, then z (constant nodes give their value exactly);
+ *   out_c = ((A_c0 r + A_c1 g) + A_c2 b) + A_c3, out.a = a.
+ * An identity grid returns the image's RGB bit for bit for finite inputs (a -0 may become +0).
+ * GSB_ERR_INVALID for a NULL ctx, image, grid or out, W or H of 0, a grid dimension outside [2, 64], a pitch below 16 W, a
+ * float4 buffer or pitch not 16-B aligned or a grid not 4-B aligned. */
+int gsb_bilagrid_apply(gsb_ctx *ctx, uint32_t width, uint32_t height, const float *image, size_t image_pitch,
+                       const float *grid, uint32_t grid_x, uint32_t grid_y, uint32_t grid_l,
+                       float *out, size_t out_pitch, void *stream);
+
+/* Gradients of gsb_bilagrid_apply from g = d loss / d out (H x W float4, grad_out_pitch apart; its A channel is ignored):
+ *   grad_image  H x W float4, OVERWRITTEN with d image_j = sum_c A_cj g_c + w_j (L - 1) sum_c g_c sum_k (dA_ck / d iz) in_k,
+ *               in = (r, g, b, 1), w = (0.299, 0.587, 0.114); the luma term is 0 where iz is clamped (gray <= 0 or
+ *               gray >= 1), and at an integer iz it uses the cell z0 above.  A = 0: the grad_image gsb_render_backward takes.
+ *   grad_grid   12 L Y X floats, OVERWRITTEN with d grid[4 c + j][node] = sum_p w_node(p) g_c(p) in_j(p), w_node the pixel's
+ *               trilinear weight of that node.
+ * Either may be NULL, not both; each is the same words whether or not the other is requested.  No atomics: the grid gradient
+ * is summed in fp64 in an order that depends only on W, H and the grid's shape and rounded once, so every output word is a
+ * function of the inputs alone, on any stream and in any context.  With grad_grid the context keeps a scratch of 384 L B per
+ * block of up to 32 x 32 pixels within one grid cell, grown with the frame and grid size and freed with the context; calls on
+ * different streams share it, so the caller orders them.  The error codes of gsb_bilagrid_apply, with grad_out for out, and
+ * GSB_ERR_INVALID also for both gradients NULL or a misaligned grad_image, its pitch or grad_grid. */
+int gsb_bilagrid_backward(gsb_ctx *ctx, uint32_t width, uint32_t height, const float *image, size_t image_pitch,
+                          const float *grid, uint32_t grid_x, uint32_t grid_y, uint32_t grid_l,
+                          const float *grad_out, size_t grad_out_pitch,
+                          float *grad_image, size_t grad_image_pitch, float *grad_grid, void *stream);
+
 /* ---- training: one fused Adam step of the resident scene (no reference counterpart; DESIGN.md section 12) ---- */
 typedef struct gsb_adam_config {
     float lr[6];                  /* position, scale, opacity, rotation, sh dc (columns 12-14), sh rest (15-59); >= 0 */
