@@ -5,12 +5,16 @@
  * tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference
  * legs may load it, and only as the checker (or as the timed CPU baseline).
  *
- * PARITY UNPINNED: the reference (shg8/3DGS.cpp @ f614d66) ships no tests, golden
- * vectors or fixtures for this path (SURVEY.md section 4 / 8c), cannot be built in
- * this image (needs Vulkan SDK, glslang, glm, GLFW, network FetchContent) and its
- * host math comes from glm 1.0.0 (CMakeLists.txt:31-36, not vendored).  This file
- * is therefore a restatement "by formula" of the cited shader / host lines, in
- * fp32 with no FMA contraction (-ffp-contract=off).
+ * PARITY: the reference (shg8/3DGS.cpp @ f614d66) ships no tests, golden vectors or
+ * fixtures for this path (SURVEY.md section 4 / 8c) and needs Vulkan to run.  This file
+ * is a restatement "by formula" of the cited shader / host lines, in fp32 with no FMA
+ * contraction (-ffp-contract=off).
+ *   PINNED: the shader stages (A1, A3-A8) are compared bit for bit with the reference's
+ *   own shader source run on the CPU (ref_driver.cpp, tests/test_ref_shaders.py), except
+ *   the arithmetic GLSL leaves to the implementation (glsl_shim.hpp, DESIGN.md section 2).
+ *   UNPINNED: the host math (A0 gso_load_records / gso_load_ply, A2
+ *   gso_uniforms_from_camera / gso_camera_translate) comes from glm 1.0.0
+ *   (CMakeLists.txt:31-36, not vendored) and stays a restatement of glm's formulas.
  *
  * All matrices are column-major like GLSL/glm: m[col*R + row].
  */

@@ -2,7 +2,8 @@
 
 TEST INFRASTRUCTURE ONLY: may be imported by tests/, __graft_entry__.smoke() and bench.py's
 cpu_baseline / --impl reference legs -- never by the product (3dgs.cpp_b200/).
-PARITY UNPINNED: the reference has no golden vectors for this path (see gs_oracle.h).
+Parity: the shader stages are pinned to the reference's own shaders run on the CPU (ref_shaders.py,
+tests/test_ref_shaders.py); the host camera math and PLY load are not (see gs_oracle.h).
 """
 from __future__ import annotations
 
