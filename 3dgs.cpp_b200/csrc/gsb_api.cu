@@ -2,6 +2,7 @@
 // orchestration.  This is the dispatch glue that replaces Renderer::draw / record*CommandBuffer /
 // create*Pipeline (src/Renderer.cpp:166-364,366-426,468-717): stream ordering instead of
 // pipeline barriers, kernel arguments instead of descriptor sets, and no mid-frame host sync.
+#include <float.h>
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -1055,16 +1056,18 @@ int gsb_background_gradient(gsb_ctx* ctx, const float* grad_image, size_t pitch,
     return GSB_OK;
 }
 
-int gsb_adam_step(gsb_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* grad_vertices, float* vertices,
-                  const gsb_adam_config* cfg, void* stream) {
+// The checks and the launch shared by gsb_adam_step (variance == nullptr) and gsb_adam_step_filter3d (fn names the entry).
+static int adam_step(gsb_ctx* ctx, const char* fn, float* params, float* exp_avg, float* exp_avg_sq, const float* grad_vertices,
+                     float* vertices, const float* variance, bool filter, const gsb_adam_config* cfg, void* stream) {
     if (!ctx) return GSB_ERR_INVALID;
-    auto bad = [&](const char* what) { return fail(ctx, GSB_ERR_INVALID, (std::string("gsb_adam_step: ") + what).c_str()); };
+    auto bad = [&](const char* what) { return fail(ctx, GSB_ERR_INVALID, (std::string(fn) + ": " + what).c_str()); };
     if (ctx->shard) return bad("sharded contexts have no training step");
-    if (!ctx->pos_op) return fail(ctx, GSB_ERR_NO_SCENE, "gsb_adam_step: no scene uploaded");
+    if (!ctx->pos_op) return fail(ctx, GSB_ERR_NO_SCENE, (std::string(fn) + ": no scene uploaded").c_str());
     if (ctx->scene_sh_half) return bad("fp16 SH storage has no training step");
-    if (!params || !exp_avg || !exp_avg_sq || !grad_vertices || !vertices || !cfg) return bad("null argument");
+    if (!params || !exp_avg || !exp_avg_sq || !grad_vertices || !vertices || !cfg || (filter && !variance)) return bad("null argument");
     for (const void* p : {(const void*)params, (const void*)exp_avg, (const void*)exp_avg_sq, (const void*)grad_vertices, (const void*)vertices})
         if (reinterpret_cast<uintptr_t>(p) % 16) return bad("array not aligned to 16 B");
+    if (reinterpret_cast<uintptr_t>(variance) % 4) return bad("variance not aligned to 4 B");
     for (float lr : cfg->lr)
         if (!(lr >= 0.0f)) return bad("learning rate below 0 or NaN");
     if (!(cfg->beta1 >= 0.0f && cfg->beta1 < 1.0f) || !(cfg->beta2 >= 0.0f && cfg->beta2 < 1.0f)) return bad("beta outside [0, 1)");
@@ -1075,7 +1078,7 @@ int gsb_adam_step(gsb_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq
     if (cfg->selective > 1) return bad("selective is neither 0 nor 1");
     CK(cudaSetDevice(ctx->device));
     if (cfg->selective) {  // the survivors of the last frame: what gsb_render_backward differentiates
-        const int rc = check_recorded_frame(ctx, GSB_ERR_INVALID, "gsb_adam_step: selective");
+        const int rc = check_recorded_frame(ctx, GSB_ERR_INVALID, (std::string(fn) + ": selective").c_str());
         if (rc != GSB_OK) return rc;
     }
     AdamParams P{};
@@ -1097,11 +1100,59 @@ int gsb_adam_step(gsb_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq
     P.eps = cfg->eps;
     P.bias_correction1 = cfg->bias_correction1;
     P.bias_correction2_sqrt = cfg->bias_correction2_sqrt;
+    P.variance = variance;
     cudaStream_t s = stream_or_own(ctx, stream);
     // the scene changes in place: the last frame no longer describes it (gsb_render_backward, a second selective step).  The
     // buffers keep their addresses, so the captured graphs, the arena and the grid hints stay.
     ctx->scene_gen++;
     CK(launch_adam(P, ctx->num_sms, s));
+    return GSB_OK;
+}
+
+int gsb_adam_step(gsb_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* grad_vertices, float* vertices,
+                  const gsb_adam_config* cfg, void* stream) {
+    return adam_step(ctx, "gsb_adam_step", params, exp_avg, exp_avg_sq, grad_vertices, vertices, nullptr, false, cfg, stream);
+}
+
+int gsb_adam_step_filter3d(gsb_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* grad_vertices,
+                           float* vertices, const float* variance, const gsb_adam_config* cfg, void* stream) {
+    return adam_step(ctx, "gsb_adam_step_filter3d", params, exp_avg, exp_avg_sq, grad_vertices, vertices, variance, true, cfg,
+                     stream);
+}
+
+int gsb_filter3d_variance(gsb_ctx* ctx, const float* vertices, uint64_t n, const gsb_uniforms* cameras, uint32_t k, float* variance,
+                          void* stream) {
+    if (!ctx) return GSB_ERR_INVALID;
+    auto bad = [&](const char* what) { return fail(ctx, GSB_ERR_INVALID, (std::string("gsb_filter3d_variance: ") + what).c_str()); };
+    if (ctx->shard) return bad("sharded contexts have no training step");
+    if (!cameras || k == 0) return bad("no camera");
+    float focal = 0.0f;  // the largest focal_x, as jacobian() computes it
+    for (uint32_t c = 0; c < k; c++) {
+        const gsb_uniforms& u = cameras[c];
+        if (u.width == 0 || u.height == 0) return bad("a camera of width or height 0");
+        if (!(u.tan_fovx > 0.0f && u.tan_fovx <= FLT_MAX) || !(u.tan_fovy > 0.0f && u.tan_fovy <= FLT_MAX))
+            return bad("a camera's tan_fov is not positive and finite");
+        focal = std::max(focal, (float)u.width / (2.0f * u.tan_fovx));
+    }
+    if (n == 0) return GSB_OK;
+    if (!vertices || !variance) return bad("null argument");
+    if (reinterpret_cast<uintptr_t>(vertices) % 16) return bad("vertices not aligned to 16 B");
+    if (reinterpret_cast<uintptr_t>(variance) % 4) return bad("variance not aligned to 4 B");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = stream_or_own(ctx, stream);
+    // scratch, one allocation freed before returning: the k cameras, then the largest seen depth's bits
+    const size_t cam_bytes = (size_t)k * sizeof(gsb_uniforms);
+    unsigned char* base = nullptr;
+    CK(dev_alloc(&base, cam_bytes + 4));
+    gsb_uniforms* cams = reinterpret_cast<gsb_uniforms*>(base);
+    uint32_t* dmax = reinterpret_cast<uint32_t*>(base + cam_bytes);
+    cudaError_t e = cudaMemcpyAsync(cams, cameras, cam_bytes, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(dmax, 0, 4, s);
+    if (e == cudaSuccess) e = launch_filter3d(reinterpret_cast<const float4*>(vertices), n, cams, k, focal, dmax, variance, ctx->num_sms, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);  // the variances are written and the scratch is free to go
+    else cudaStreamSynchronize(s);
+    cudaFree(base);
+    if (e != cudaSuccess) return fail(ctx, e == cudaErrorMemoryAllocation ? GSB_ERR_OOM : GSB_ERR_CUDA, "gsb_filter3d_variance", e);
     return GSB_OK;
 }
 

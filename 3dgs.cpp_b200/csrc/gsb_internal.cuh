@@ -239,7 +239,15 @@ struct AdamParams {
     const Control* ctl;        // selective: num_visible
     float lr[6];               // position, scale, opacity, rotation, SH DC, SH rest
     float beta1, beta2, eps, bias_correction1, bias_correction2_sqrt;
+    // gsb_adam_step_filter3d: n per-row variances of the 3D smoothing filter (k_adam_step<true>); null: the plain step
+    // (k_adam_step<false>).  Appended last so the other fields keep their offsets.
+    const float* variance;
 };
 cudaError_t launch_adam(const AdamParams& p, int num_sms, cudaStream_t s);
+
+// gsb_filter3d.cu: gsb_filter3d_variance.  cams: k device copies of gsb_uniforms; focal = the largest focal_x of the k;
+// dmax: one zeroed word (the largest seen depth's bits).  variance: n floats, overwritten.
+cudaError_t launch_filter3d(const float4* vertices, uint64_t n, const gsb_uniforms* cams, uint32_t k, float focal,
+                            uint32_t* dmax, float* variance, int num_sms, cudaStream_t s);
 
 }  // namespace gsb

@@ -6,6 +6,8 @@
 // (position, scale + opacity, quaternion, and 12 of SH each stay inside one float4), so every array is read and written
 // with 240 contiguous bytes per row.  Only the scene's Sigma needs position, scale + opacity and quaternion together: those
 // three threads leave their activated float4 in shared memory and one thread per row stores the scene words.  No atomics.
+// FILTER (gsb_adam_step_filter3d, DESIGN.md section 18): the scale and opacity of each row go through Mip-Splatting's 3D
+// smoothing filter of its variance v, in the activation and in the chain rule; only the k == 1 thread reads v.
 // Compiled with -fmad=false: every fp32 operation is one IEEE operation unless spelled fmaf().
 #include <algorithm>
 
@@ -37,6 +39,30 @@ __device__ __forceinline__ float4 normalise(float4 q, float& norm) {
     return make_float4(q.x / norm, q.y / norm, q.z / norm, q.w / norm);
 }
 
+// Mip-Splatting's filtered scale and opacity of log scales (lx, ly, lz), opacity logit lw and filter variance var, each
+// operation one IEEE op in this order: s = exp(l), q = s s, d = q + v, e = sqrt(d), r = q / d; c = sqrt((r0 r1) r2), the
+// opacity factor as a product of per-axis ratios (prod q / prod d underflows once prod s^2 < 1e-38).  With v = 0 every
+// value is the plain activation's: sqrt(fl(s s)) = s, r = 1, c = 1.
+struct Filtered {
+    float s[3], d[3], e[3], o, c, of;
+    __device__ __forceinline__ Filtered(float4 x, float var) {
+        const float l[3] = {x.x, x.y, x.z};
+        float r[3];
+#pragma unroll
+        for (int j = 0; j < 3; j++) {
+            s[j] = expf(l[j]);
+            const float q = s[j] * s[j];
+            d[j] = q + var;
+            e[j] = sqrtf(d[j]);
+            r[j] = q / d[j];
+        }
+        c = sqrtf((r[0] * r[1]) * r[2]);
+        o = sigmoid(x.w);
+        of = o * c;
+    }
+};
+
+template <bool FILTER>
 __global__ void __launch_bounds__(AD_THREADS) k_adam_step(const AdamParams P) {
     __shared__ float4 s_rec[AD_ROWS][3];  // activated position, scale_opacity, rotation of the trip's rows
     __shared__ uint32_t s_row[AD_ROWS];
@@ -67,7 +93,17 @@ __global__ void __launch_bounds__(AD_THREADS) k_adam_step(const AdamParams P) {
                 pv[0] = v.x, pv[1] = v.y, pv[2] = v.z;
                 a = make_float4(x.x, x.y, x.z, 1.0f);
             } else {
-                if (k == 1) {  // log scale, opacity logit: d log s = ds s, d logit = (do o) (1 - o)
+                if (FILTER && k == 1) {  // the record holds e = sqrt(s^2 + v) and o c; v is held constant
+                    // d log s = (de s) (s / e) + (d(oc) oc) (v / d), d logit = ((d(oc) c) o) (1 - o)
+                    const float var = P.variance[row];
+                    const Filtered f(x, var);
+                    adam((g.x * f.s[0]) * (f.s[0] / f.e[0]) + (g.w * f.of) * (var / f.d[0]), x.x, m.x, v.x, step);
+                    adam((g.y * f.s[1]) * (f.s[1] / f.e[1]) + (g.w * f.of) * (var / f.d[1]), x.y, m.y, v.y, step);
+                    adam((g.z * f.s[2]) * (f.s[2] / f.e[2]) + (g.w * f.of) * (var / f.d[2]), x.z, m.z, v.z, step);
+                    adam(((g.w * f.c) * f.o) * (1.0f - f.o), x.w, m.w, v.w, step_w);
+                    const Filtered a1(x, var);
+                    a = make_float4(a1.e[0], a1.e[1], a1.e[2], a1.of);
+                } else if (k == 1) {  // log scale, opacity logit: d log s = ds s, d logit = (do o) (1 - o)
                     const float o = sigmoid(x.w);
                     adam(g.x * expf(x.x), x.x, m.x, v.x, step);
                     adam(g.y * expf(x.y), x.y, m.y, v.y, step);
@@ -106,20 +142,25 @@ __global__ void __launch_bounds__(AD_THREADS) k_adam_step(const AdamParams P) {
     }
 }
 
-}  // namespace
-
-cudaError_t launch_adam(const AdamParams& p, int num_sms, cudaStream_t s) {
-    if (p.n == 0) return cudaSuccess;
+template <bool FILTER>
+cudaError_t launch_adam_t(const AdamParams& p, int num_sms, cudaStream_t s) {
     static int per_sm = 0;  // resident CTAs per SM: the grid is one wave, walking the rows grid-stride
     if (per_sm == 0) {
-        const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_adam_step, AD_THREADS, 0);
+        const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_adam_step<FILTER>, AD_THREADS, 0);
         if (e != cudaSuccess) return e;
         per_sm = per_sm > 0 ? per_sm : 1;
     }
     const uint64_t trips = (p.n + AD_ROWS - 1) / AD_ROWS;  // selective mode: N_v <= n
     const unsigned blocks = (unsigned)std::min<uint64_t>(trips, (uint64_t)num_sms * per_sm);
-    k_adam_step<<<blocks, AD_THREADS, 0, s>>>(p);
+    k_adam_step<FILTER><<<blocks, AD_THREADS, 0, s>>>(p);
     return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_adam(const AdamParams& p, int num_sms, cudaStream_t s) {
+    if (p.n == 0) return cudaSuccess;
+    return p.variance ? launch_adam_t<true>(p, num_sms, s) : launch_adam_t<false>(p, num_sms, s);
 }
 
 }  // namespace gsb

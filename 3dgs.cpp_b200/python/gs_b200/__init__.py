@@ -46,6 +46,8 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_set_backward_deterministic", "gsb_background_gradient",
     # training loss, optimizer step and initialisation from a point cloud
     "gsb_image_loss", "gsb_adam_step", "gsb_init_from_points",
+    # Mip-Splatting's 3D smoothing filter
+    "gsb_filter3d_variance", "gsb_adam_step_filter3d",
     # bilateral-grid appearance correction
     "gsb_bilagrid_apply", "gsb_bilagrid_backward",
     # 3DGS-MCMC: position noise and relocation
@@ -183,6 +185,8 @@ lib.gsb_bilagrid_apply.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t,
 lib.gsb_bilagrid_backward.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_uint32, C.c_uint32, C.c_uint32,
                                       _vp, C.c_size_t, _vp, C.c_size_t, _vp, _vp]
 lib.gsb_adam_step.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(AdamConfig), _vp]
+lib.gsb_filter3d_variance.argtypes = [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, _vp]
+lib.gsb_adam_step_filter3d.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(AdamConfig), _vp]
 lib.gsb_init_from_points.argtypes = [_vp, _vp, _vp, C.c_uint64, C.c_float, _vp, _vp]
 lib.gsb_mcmc_noise.argtypes = [_vp, _vp, _vp, C.c_float, C.c_uint64, C.c_uint64, _vp]
 lib.gsb_mcmc_relocate.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint64, C.c_float, _vp]
@@ -595,20 +599,63 @@ class Context:
                                     None if grad_image is None else grad_image.data_ptr(), grad_pitch, result.data_ptr(), s))
         return result
 
-    def adam_step(self, params, exp_avg, exp_avg_sq, grad_vertices, vertices, cfg: AdamConfig, stream=None):
+    def adam_step(self, params, exp_avg, exp_avg_sq, grad_vertices, vertices, cfg: AdamConfig, stream=None, variance=None):
         """gsb_adam_step on torch tensors: one Adam step of the raw parameters `params` from grad_vertices (dL/d(activated
         record)), updating params, exp_avg and exp_avg_sq in place and writing the activated records into `vertices` and the
         context's scene (no upload needed).  All five are contiguous (n, 60) float32 CUDA tensors on the context's device,
         n the scene's size; cfg is an adam_config(...).  Runs on `stream` (a torch stream), by default torch's current
-        stream, and does not wait for it.  Bad shapes, dtypes, devices or layouts raise ValueError."""
+        stream, and does not wait for it.  Bad shapes, dtypes, devices or layouts raise ValueError.
+
+        variance: an (n,) float32 CUDA tensor of Mip-Splatting's 3D filter (filter3d_variance; finite and >= 0, not checked
+        here): the step is gsb_adam_step_filter3d, whose records carry the filtered scale and opacity (apply_filter_3d)."""
         import torch
 
         self._check_rows("adam_step", {"params": params, "exp_avg": exp_avg, "exp_avg_sq": exp_avg_sq,
                                        "grad_vertices": grad_vertices, "vertices": vertices})
         s = _torch_stream_arg(torch.cuda.current_stream(params.device) if stream is None else stream)
-        self._ck(lib.gsb_adam_step(self.h, params.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(),
-                                   grad_vertices.data_ptr(), vertices.data_ptr(), C.byref(cfg), s))
+        if variance is None:
+            self._ck(lib.gsb_adam_step(self.h, params.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(),
+                                       grad_vertices.data_ptr(), vertices.data_ptr(), C.byref(cfg), s))
+        else:
+            self._check_variance("adam_step", variance, params.shape[0])
+            self._ck(lib.gsb_adam_step_filter3d(self.h, params.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(),
+                                                grad_vertices.data_ptr(), vertices.data_ptr(), variance.data_ptr(),
+                                                C.byref(cfg), s))
         self.frames += 1  # the scene changed: the last frame can no longer be differentiated
+
+    def _check_variance(self, caller, variance, n):
+        """variance is a contiguous (n,) float32 CUDA tensor on the context's device; ValueError otherwise."""
+        import torch
+
+        if not isinstance(variance, torch.Tensor) or not variance.is_cuda or variance.device.index != self.device:
+            raise ValueError(f"{caller}: variance must be a CUDA tensor on device {self.device}")
+        if variance.dtype != torch.float32 or tuple(variance.shape) != (n,) or not variance.is_contiguous():
+            raise ValueError(f"{caller}: variance must be a contiguous ({n},) float32 tensor, got {tuple(variance.shape)} "
+                             f"{variance.dtype}")
+
+    def filter3d_variance(self, vertices, cameras):
+        """gsb_filter3d_variance on torch tensors: the (n,) float32 variance of Mip-Splatting's 3D smoothing filter of the
+        Gaussians at the positions (columns 0-2) of `vertices`, a contiguous (n, 60) float32 CUDA tensor on the context's
+        device (any n: no scene is needed), from `cameras`, a non-empty list of Uniforms (the training views): with d the
+        least view depth over the cameras that see a Gaussian (the largest such d for one no camera sees) and f the largest
+        focal length in pixels, variance = 0.2 (d / f)^2.  Runs on torch's current stream and returns when the variances are
+        written; leaves the context's scene and last frame alone.  Bad arguments raise ValueError or GsbError."""
+        import torch
+
+        if not isinstance(vertices, torch.Tensor) or not vertices.is_cuda or vertices.device.index != self.device:
+            raise ValueError(f"filter3d_variance: vertices must be a CUDA tensor on device {self.device}")
+        if vertices.dtype != torch.float32 or vertices.dim() != 2 or vertices.shape[1] != 60 or not vertices.is_contiguous():
+            raise ValueError(f"filter3d_variance: vertices must be a contiguous (n, 60) float32 tensor, got "
+                             f"{tuple(vertices.shape)} {vertices.dtype}")
+        cams = list(cameras)
+        if not cams:
+            raise ValueError("filter3d_variance: needs at least one camera")
+        arr = (Uniforms * len(cams))(*cams)
+        n = vertices.shape[0]
+        out = torch.empty(n, dtype=torch.float32, device=vertices.device)
+        s = _torch_stream_arg(torch.cuda.current_stream(vertices.device))
+        self._ck(lib.gsb_filter3d_variance(self.h, vertices.data_ptr(), n, arr, len(cams), out.data_ptr(), s))
+        return out
 
     def _check_rows(self, caller, arrays):
         """Every tensor of `arrays` (name -> tensor) is a contiguous (n, 60) float32 CUDA tensor on the context's device,
@@ -1063,6 +1110,33 @@ def densify_and_prune(vertices, density, *, grad_threshold, scene_extent, percen
     return out[keep].contiguous(), source[keep]
 
 
+def apply_filter_3d(vertices, variance):
+    """Mip-Splatting's 3D smoothing filter (get_scaling_with_3D_filter, get_opacity_with_3D_filter) applied to activated
+    (n, 60) records as differentiable torch ops, the variance (n,) held constant: with s the scales and o the opacity,
+    q = s s, d = q + v, e = sqrt(d), r = q / d, c = sqrt((r0 r1) r2); the result's scales are e and its opacity o c, every
+    other column as given.  In float32 on CUDA each op is the one gsb_adam_step_filter3d does, in its order.  For training
+    through render_torch: render_torch(ctx, apply_filter_3d(vertices, variance), u)."""
+    import torch
+
+    v = variance.detach().to(device=vertices.device, dtype=vertices.dtype).reshape(-1, 1)
+    q = vertices[:, 4:7] * vertices[:, 4:7]
+    d = q + v
+    r = q / d
+    c = ((r[:, 0] * r[:, 1]) * r[:, 2]).sqrt()
+    return torch.cat([vertices[:, 0:4], d.sqrt(), (vertices[:, 7] * c)[:, None], vertices[:, 8:60]], 1)
+
+
+def activate_parameters(params):
+    """The activated (n, 60) records of raw parameters, as gsb_adam_step writes them, in torch: (p, 1), exp(log s),
+    sigmoid(logit), q / |q|, SH."""
+    import torch
+
+    p = params.detach()
+    q = p[:, 8:12]
+    return torch.cat([p[:, 0:3], torch.ones_like(p[:, 3:4]), p[:, 4:7].exp(), torch.sigmoid(p[:, 7:8]),
+                      q / q.norm(dim=1, keepdim=True), p[:, 12:60]], 1).contiguous()
+
+
 def raw_parameters(vertices):
     """The raw parameters gsb_adam_step optimises, of activated (n, 60) records: position, column 3 as given, log(scale),
     logit(opacity) (opacity clamped to [1e-6, 1 - 1e-6]), the quaternion and SH as given."""
@@ -1154,10 +1228,23 @@ class SceneAdam:
         img = opt.render(u).requires_grad_()
         out = bilateral_grid_torch(ctx, img, grids[i])
         loss = image_loss_torch(ctx, out, target) + 10.0 * bilateral_grid_tv(grids)
-        loss.backward(); opt.step(img.grad); grid_opt.step(); grid_opt.zero_grad()"""
+        loss.backward(); opt.step(img.grad); grid_opt.step(); grid_opt.zero_grad()
+
+    Mip-Splatting's 3D smoothing filter (Yu et al. 2024), which keeps a scene free of needles and erosion holes when it is
+    rendered closer or larger than its training views: filter_cameras, the list of training Uniforms, turns it on.  Then
+    `params` stay the unfiltered raw parameters, `variance` holds each Gaussian's filter (Context.filter3d_variance) and
+    `vertices` the filtered records (apply_filter_3d of the activated params), which frames render and step() trains
+    through gsb_adam_step_filter3d.  Mip-Splatting recomputes the filter every 100 steps once densification has ended:
+
+        if it >= densify_until and it % 100 == 0:
+            opt.update_filter_3d()
+
+    densify() decides on the unfiltered records and recomputes the filter for the new scene; inject_noise() and relocate()
+    (3DGS-MCMC) raise ValueError with a filter.  The filtered records are an ordinary scene: a plain viewer renders the
+    trained scene, filter included, from write_ply(path, ply_records(raw_parameters(opt.vertices)))."""
 
     def __init__(self, ctx: "Context", vertices, lr, betas=(0.9, 0.999), eps=1e-15, selective=True, background=None,
-                 random_background=False, seed=0):
+                 random_background=False, seed=0, filter_cameras=None):
         import torch
 
         if not isinstance(vertices, torch.Tensor) or not vertices.is_cuda or vertices.dim() != 2 or vertices.shape[1] != 60:
@@ -1167,7 +1254,11 @@ class SceneAdam:
         self.seed = int(seed)
         self.background = None if background is None else [float(x) for x in background]
         self._generator = torch.Generator().manual_seed(int(seed)) if random_background else None
+        self.filter_cameras = None if filter_cameras is None else list(filter_cameras)
+        self.variance = None
         self._adopt(vertices.detach().to(torch.float32).contiguous().clone(), None)
+        if self.filter_cameras is not None:
+            self._set_filter(ctx.filter3d_variance(self.params, self.filter_cameras), self.vertices)
         ctx.set_backward(True)
         self._upload()
 
@@ -1179,6 +1270,25 @@ class SceneAdam:
             state = (raw_parameters(vertices), torch.zeros_like(vertices), torch.zeros_like(vertices))
         self.params, self.exp_avg, self.exp_avg_sq = state
         self.grad = torch.empty_like(vertices)
+
+    def _set_filter(self, variance, unfiltered):
+        """Adopts a filter: `variance` (checked finite and >= 0 here, once) and vertices = the filtered `unfiltered`."""
+        import torch
+
+        if not bool(torch.isfinite(variance).all()) or bool((variance < 0).any()):
+            raise ValueError("SceneAdam: the filter variance must be finite and >= 0")
+        self.variance = variance
+        self.vertices = apply_filter_3d(unfiltered, variance).contiguous()
+
+    def update_filter_3d(self, cameras=None):
+        """Recomputes the 3D filter from the current positions and the training cameras (`cameras`, which then replace
+        filter_cameras; None: filter_cameras), re-activates every row through it and uploads the scene."""
+        if cameras is not None:
+            self.filter_cameras = list(cameras)
+        if self.filter_cameras is None:
+            raise ValueError("SceneAdam.update_filter_3d: no training cameras (filter_cameras)")
+        self._set_filter(self.ctx.filter3d_variance(self.params, self.filter_cameras), activate_parameters(self.params))
+        self._upload()
 
     def _upload(self):
         import torch
@@ -1221,21 +1331,31 @@ class SceneAdam:
             self.grad[:, 4:7] += scale_reg / (3 * n)
         self.steps += 1
         ctx.adam_step(self.params, self.exp_avg, self.exp_avg_sq, self.grad, v,
-                      adam_config(self.lr, self.betas, self.eps, self.steps, self.selective))
+                      adam_config(self.lr, self.betas, self.eps, self.steps, self.selective), variance=self.variance)
 
     def densify(self, density, **kwargs):
         """densify_and_prune(vertices, density, **kwargs) of the resident scene: `vertices` becomes its output, params and
-        the moments follow through adam_state_after_densify, and the new scene is uploaded.  Returns `source`."""
-        new, source = densify_and_prune(self.vertices, density, **kwargs)
-        self._adopt(new, adam_state_after_densify(self.params, self.exp_avg, self.exp_avg_sq, self.vertices, new, source))
+        the moments follow through adam_state_after_densify, and the new scene is uploaded.  Returns `source`.  With the 3D
+        filter the decisions are made on the unfiltered records (activate_parameters(params), as Mip-Splatting's
+        get_scaling and get_opacity), and the filter is recomputed for the new scene before the upload."""
+        unfiltered = self.vertices if self.variance is None else activate_parameters(self.params)
+        new, source = densify_and_prune(unfiltered, density, **kwargs)
+        self._adopt(new, adam_state_after_densify(self.params, self.exp_avg, self.exp_avg_sq, unfiltered, new, source))
+        if self.variance is not None:
+            self._set_filter(self.ctx.filter3d_variance(self.params, self.filter_cameras), new)
         self._upload()
         return source
 
     def inject_noise(self, noise_lr=5e5):
         """3DGS-MCMC's position noise on the resident scene (gsb_mcmc_noise) with scale lr[0] * noise_lr, the optimizer's
         seed and its step count: every row moves by Sigma eps, gated to zero as its opacity approaches 1.  Runs on torch's
-        current stream without a host wait."""
+        current stream without a host wait.  Not defined with the 3D filter: ValueError."""
+        self._no_filter("inject_noise")
         self.ctx.mcmc_noise(self.params, self.vertices, float(self.lr[0]) * float(noise_lr), self.seed, self.steps)
+
+    def _no_filter(self, caller):
+        if self.variance is not None:
+            raise ValueError(f"SceneAdam.{caller}: 3DGS-MCMC is not defined with the 3D filter (filter_cameras)")
 
     def relocate(self, cap_max, min_opacity=0.005, growth=0.05, generator=None):
         """3DGS-MCMC's relocation and growth (gsplat's MCMCStrategy), in two phases; returns (n_relocated, n_added).
@@ -1245,11 +1365,12 @@ class SceneAdam:
           add       k = max(0, min(cap_max, floor((1 + growth) n)) - n) sources drawn over all rows in proportion to
                     opacity are appended (params and vertices copied, moments zero), the scene is uploaded once, and
                     gsb_mcmc_relocate makes rows n .. n + k - 1 their copies.
-        generator: a CPU torch.Generator for the draws (None: torch's default)."""
+        generator: a CPU torch.Generator for the draws (None: torch's default).  Not defined with the 3D filter: ValueError."""
         import math
 
         import torch
 
+        self._no_filter("relocate")
         v = self.vertices
         dev = v.device
         n = v.shape[0]

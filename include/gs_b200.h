@@ -389,6 +389,39 @@ typedef struct gsb_adam_config {
 int gsb_adam_step(gsb_ctx *ctx, float *params, float *exp_avg, float *exp_avg_sq, const float *grad_vertices,
                   float *vertices, const gsb_adam_config *cfg, void *stream);
 
+/* ---- training: Mip-Splatting's 3D smoothing filter (Yu et al. 2024; no reference counterpart; DESIGN.md section 18) ---- */
+/* The per-Gaussian variance of the filter from the k >= 1 training cameras (Mip-Splatting's compute_3D_filter in this
+ * renderer's camera convention).  vertices: n x 60 floats of device memory, 16-B aligned, of which only the positions in
+ * columns 0-2 are read; cameras: k gsb_uniforms in host memory; variance: n floats of device memory, OVERWRITTEN.  Per
+ * Gaussian i and camera c, in fp32 with the frame's own arithmetic (clip_view of preprocess.comp, then ndc2Pix
+ * u = ((ndcx + 1) W - 1) / 2, likewise v, whose half-pixel offset is kept): i is seen by c iff vz > 0.2f,
+ * -0.15f W <= u <= 1.15f W and -0.15f H <= v <= 1.15f H (NaN is never seen).  d_i = the least vz over the cameras that see
+ * i; rows no camera sees take the largest d of the seen rows; f = the largest focal_x = (float)W / (2.0f tan_fovx) over all
+ * k cameras; variance_i = (t t) 0.2f with t = d_i / f.  If no row is seen every variance is 0.  Min and max are exact, so
+ * every output word is a function of the inputs: bitwise reproducible on any stream, in any context, on any grid.
+ * Enqueued on `stream` (NULL = the context's stream); returns when the variances are written.  Needs no scene and leaves
+ * the context's scene and frame state alone, as gsb_init_from_points does; scratch (160 B per camera) is allocated and
+ * freed inside the call.  GSB_ERR_INVALID for a NULL ctx, a sharded context, NULL cameras, k == 0, a camera of width or
+ * height 0 or whose tan_fovx or tan_fovy is not positive and finite; then, for n > 0, a NULL vertices or variance,
+ * vertices not 16-B aligned or variance not 4-B aligned.  n == 0 returns GSB_OK and writes nothing. */
+int gsb_filter3d_variance(gsb_ctx *ctx, const float *vertices, uint64_t n, const gsb_uniforms *cameras, uint32_t k,
+                          float *variance, void *stream);
+
+/* gsb_adam_step with every updated row's scale and opacity passed through the 3D smoothing filter of its variance v
+ * (variance: n floats of device memory, 4-B aligned, finite and >= 0, e.g. from gsb_filter3d_variance; not checked here).
+ * With x the raw parameters, in fp32, each operation one IEEE op in this order, for k = 0, 1, 2:
+ *   s_k = expf(x_k), q_k = s_k s_k, d_k = q_k + v, e_k = sqrtf(d_k), r_k = q_k / d_k
+ *   c = sqrtf((r_0 r_1) r_2), o = sigmoid(x_w), o_f = o c
+ * the record's scale is (e_0, e_1, e_2) and its opacity o_f (Mip-Splatting's get_scaling_with_3D_filter and
+ * get_opacity_with_3D_filter; the product of per-axis ratios does not underflow as prod s^2 / prod (s^2 + v) does); position,
+ * rotation and SH are activated as by gsb_adam_step.  With g the record's gradient and v held constant, the chain rule is
+ *   d logit = ((g_w c) o) (1 - o),   d log s_k = (g_k s_k) (s_k / e_k) + (g_w o_f) (v / d_k)
+ * A zero variance gives gsb_adam_step's words (a -0 may become +0).  Everything else -- preconditions, selective mode, the
+ * scene words (those of gsb_scene_upload of the filtered `vertices`), the error codes, with GSB_ERR_INVALID also for a NULL
+ * or misaligned variance -- is gsb_adam_step's. */
+int gsb_adam_step_filter3d(gsb_ctx *ctx, float *params, float *exp_avg, float *exp_avg_sq, const float *grad_vertices,
+                           float *vertices, const float *variance, const gsb_adam_config *cfg, void *stream);
+
 /* ---- training: a scene initialised from a point cloud (no reference counterpart; DESIGN.md section 13) ---- */
 /* Kerbl et al. 2023's initialisation from SfM points: every point becomes an isotropic Gaussian.  All pointers are device
  * memory: xyz and rgb are n x 3 floats, tightly packed; vertices (n x 60 floats) is OVERWRITTEN with activated
