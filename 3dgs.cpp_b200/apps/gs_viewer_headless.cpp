@@ -1,9 +1,12 @@
 // gs_viewer_headless -- the reference viewer's command line (apps/viewer/main.cpp:12-98) without a window:
 //   gs_viewer_headless [-d DEVICE] [-w WIDTH] [-h HEIGHT] [-v] [--frames N] [--camera x,y,z[,qw,qx,qy,qz]]
 //                      [--fov DEG] [--camera-path poses.txt] [--mode exact|fast] [--cull [LEVEL]] [--antialiased]
-//                      [--background r,g,b] [--out image.ppm] [--float-out image.pfm] scene.ply
+//                      [--background r,g,b] [--fisheye fx,fy,cx,cy[,k1,k2,k3,k4[,max_theta_deg]]] [--out image.ppm]
+//                      [--float-out image.pfm] scene.ply
 // --antialiased: gsb_set_antialiased (opacity compensated for the 0.3 px dilation, as scenes trained that way expect).
 // --background r,g,b: gsb_set_background (e.g. 1,1,1 for an object scene trained over white; default black).
+// --fisheye fx,fy,cx,cy[,k1,k2,k3,k4[,max_theta_deg]]: gsb_set_camera_model with an OpenCV-fisheye lens (pixel (i, j) sampled at
+// (i, j): COLMAP's cx - 0.5); without max_theta_deg, the largest angle up to 175 deg at which theta_d still increases.
 // --camera-path: one pose per line `x y z qw qx qy qz [fov]` (# comments); `--frames` frames are rendered at each pose
 // and one JSON line is printed per pose (SURVEY 8d: record M for every timed camera).
 // Loads the .ply through GSScene, renders N frames through Renderer::draw() (B8G8R8A8 like the swapchain),
@@ -12,6 +15,7 @@
 // unquantised blend render.comp:98 stores: what the 1e-4 parity tolerance is defined on).  The first JSON line also carries
 // the load times (file read + activation, upload + cov3D ingest).  Environment: VKGS_PHYSICAL_DEVICE like the viewer.
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -25,7 +29,8 @@
 static void usage() {
     std::puts("usage: gs_viewer_headless [-d device] [-w width] [-h height] [-v] [--frames n] [--camera x,y,z[,qw,qx,qy,qz]]\n"
               "                          [--fov deg] [--camera-path poses.txt] [--mode exact|fast] [--cull [0|1|2]] [--antialiased]\n"
-              "                          [--background r,g,b] [--out image.ppm] [--float-out image.pfm] scene.ply");
+              "                          [--background r,g,b] [--fisheye fx,fy,cx,cy[,k1,k2,k3,k4[,max_theta_deg]]]\n"
+              "                          [--out image.ppm] [--float-out image.pfm] scene.ply");
 }
 
 int main(int argc, char** argv) {
@@ -35,6 +40,8 @@ int main(int argc, char** argv) {
     uint32_t frames = 1;
     bool verbose = false, cull = false, antialiased = false, background = false;
     float bg[3] = {0, 0, 0};
+    bool fisheye = false;
+    float fish[9] = {0, 0, 0, 0, 0, 0, 0, 0, -1.0f};  // fx fy cx cy k1..k4 max_theta_deg (< 0: the default)
     float cam[7] = {0, 0, 0, 1, 0, 0, 0};
     float fov = 45.0f;
     if (const char* env = std::getenv("VKGS_PHYSICAL_DEVICE")) cfg.physicalDeviceId = static_cast<uint8_t>(std::atoi(env));
@@ -64,6 +71,15 @@ int main(int argc, char** argv) {
             int k = 0;
             for (char* tok = std::strtok(const_cast<char*>(next()), ","); tok && k < 3; tok = std::strtok(nullptr, ",")) bg[k++] = static_cast<float>(std::atof(tok));
         }
+        else if (a == "--fisheye") {
+            fisheye = true;
+            int k = 0;
+            for (char* tok = std::strtok(const_cast<char*>(next()), ","); tok && k < 9; tok = std::strtok(nullptr, ",")) fish[k++] = static_cast<float>(std::atof(tok));
+            if (k < 4) {
+                usage();
+                return 1;
+            }
+        }
         else if (a == "--float-out") float_path = next();
         else if (a == "--out") out_path = next();
         else if (a == "--camera-path") path_file = next();
@@ -88,6 +104,24 @@ int main(int argc, char** argv) {
         if (cull && gsb_set_tile_cull(renderer.context(), cull_level) != GSB_OK) throw std::runtime_error("gsb_set_tile_cull failed");
         if (antialiased && gsb_set_antialiased(renderer.context(), 1) != GSB_OK) throw std::runtime_error("gsb_set_antialiased failed");
         if (background && gsb_set_background(renderer.context(), bg) != GSB_OK) throw std::runtime_error("gsb_set_background failed");
+        if (fisheye) {
+            gsb_camera_model m{};
+            m.kind = GSB_CAMERA_FISHEYE;
+            m.fx = fish[0], m.fy = fish[1], m.cx = fish[2], m.cy = fish[3];
+            for (int k = 0; k < 4; k++) m.k[k] = fish[4 + k];
+            if (fish[8] >= 0.0f) {
+                m.max_theta = fish[8] * static_cast<float>(M_PI / 180.0);
+            } else {  // walk out in 0.1 mrad steps while d theta_d / d theta stays positive
+                const double cap = 175.0 * M_PI / 180.0;
+                double t = 0.0;
+                for (; t + 1e-4 <= cap; t += 1e-4) {
+                    const double u = (t + 1e-4) * (t + 1e-4);
+                    if (!(1.0 + u * (3.0 * m.k[0] + u * (5.0 * m.k[1] + u * (7.0 * m.k[2] + u * 9.0 * m.k[3]))) > 0.0)) break;
+                }
+                m.max_theta = static_cast<float>(t);
+            }
+            if (gsb_set_camera_model(renderer.context(), &m) != GSB_OK) throw std::runtime_error(gsb_last_error(renderer.context()));
+        }
         struct Pose {
             float v[7];
             float fov;

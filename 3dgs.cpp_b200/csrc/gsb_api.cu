@@ -374,7 +374,8 @@ static int enqueue_front(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uin
     if (timers) CK(cudaEventRecord(ctx->ev[0], stream));
 
     // ---- k_project: preprocess.comp + survivor compaction ----
-    CK(launch_project(project_params(ctx, *ubo, rb, re), ctx->debug, ctx->antialiased, stream));
+    const bool fisheye = ctx->camera.kind == GSB_CAMERA_FISHEYE;
+    CK(launch_project(project_params(ctx, *ubo, rb, re), ctx->debug, ctx->antialiased, stream, fisheye ? &ctx->camera : nullptr));
     if (timers) CK(cudaEventRecord(ctx->ev[1], stream));
 
     if (ctx->use_graph && !timers && !ctx->debug) rc = launch_middle_graph(ctx, fp, sv, stream);
@@ -428,6 +429,7 @@ int enqueue_tail(gsb_ctx* ctx, const FramePlan& fp, const gsb_uniforms& ubo, cud
     f.mode = ctx->mode;
     f.antialiased = ctx->antialiased;
     for (int c = 0; c < 3; c++) f.background[c] = ctx->background[c];
+    f.camera = ctx->camera;
     f.scene_gen = ctx->scene_gen;
     f.pending = true;
     f.exists = true;
@@ -894,6 +896,47 @@ int gsb_set_background(gsb_ctx* ctx, const float* rgb) {
     return GSB_OK;
 }
 
+int gsb_set_camera_model(gsb_ctx* ctx, const gsb_camera_model* m) {
+    if (!ctx) return GSB_ERR_INVALID;
+    auto bad = [&](const char* what) { return fail(ctx, GSB_ERR_INVALID, (std::string("gsb_set_camera_model: ") + what).c_str()); };
+    if (ctx->shard) return bad("sharded contexts have only the pinhole camera");
+    if (!m || m->kind == GSB_CAMERA_PINHOLE) {
+        ctx->camera = gsb_camera_model{};
+        return GSB_OK;
+    }
+    if (m->kind != GSB_CAMERA_FISHEYE) return bad("unknown camera kind");
+    if (!(m->fx > 0.0f) || !(m->fy > 0.0f) || !isfinite(m->fx) || !isfinite(m->fy)) return bad("fx and fy must be positive and finite");
+    const float rest[] = {m->cx, m->cy, m->k[0], m->k[1], m->k[2], m->k[3], m->max_theta};
+    for (float x : rest)
+        if (!isfinite(x)) return bad("every field must be finite");
+    const double tmax = m->max_theta, k1 = m->k[0], k2 = m->k[1], k3 = m->k[2], k4 = m->k[3];
+    if (!(tmax > 0.0) || !(tmax < M_PI)) return bad("max_theta must lie in (0, pi)");
+    // theta_d strictly increasing on [0, max_theta]: d theta_d / d theta = 1 + 3 k1 t^2 + 5 k2 t^4 + 7 k3 t^6 + 9 k4 t^8 > 0.  In
+    // u = t^2 that is a quartic q(u) on [0, tmax^2] with q(0) = 1: positive everywhere iff positive at the end and at every
+    // root of q'(u) = 3 k1 + 10 k2 u + 21 k3 u^2 + 36 k4 u^3 inside, which a dense scan brackets and bisection refines.
+    auto q = [&](double u) { return 1.0 + u * (3.0 * k1 + u * (5.0 * k2 + u * (7.0 * k3 + u * 9.0 * k4))); };
+    auto dq = [&](double u) { return 3.0 * k1 + u * (10.0 * k2 + u * (21.0 * k3 + u * 36.0 * k4)); };
+    const double umax = tmax * tmax;
+    double qmin = std::min(q(0.0), q(umax));
+    constexpr int STEPS = 4096;
+    for (int i = 0; i < STEPS; i++) {
+        double a = umax * i / STEPS, b = umax * (i + 1) / STEPS;
+        qmin = std::min(qmin, q(b));
+        if ((dq(a) < 0.0) != (dq(b) < 0.0)) {  // a stationary point of q in [a, b]
+            for (int it = 0; it < 100; it++) {
+                const double mid = 0.5 * (a + b);
+                if ((dq(a) < 0.0) != (dq(mid) < 0.0)) b = mid;
+                else a = mid;
+            }
+            qmin = std::min(qmin, q(0.5 * (a + b)));
+        }
+    }
+    if (!(qmin > 0.0)) return bad("theta_d must be strictly increasing on [0, max_theta]");
+    // k_project is launched outside the captured middle graph: graphs and hints stay
+    ctx->camera = *m;
+    return GSB_OK;
+}
+
 int gsb_set_backward_deterministic(gsb_ctx* ctx, int enabled) {
     if (!ctx) return GSB_ERR_INVALID;
     if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, "gsb_set_backward_deterministic: sharded contexts have no backward pass");
@@ -948,6 +991,8 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     if (ctx->scene_sh_half) return fail(ctx, GSB_ERR_INVALID, msg("fp16 SH storage has no backward pass").c_str());
     if (!args_ok) return fail(ctx, GSB_ERR_INVALID, msg("null argument").c_str());
     const LastFrame& f = ctx->frame;
+    const bool fisheye = f.camera.kind == GSB_CAMERA_FISHEYE;
+    if (fisheye && grad_ubo) return fail(ctx, GSB_ERR_INVALID, msg("a fisheye frame has no camera gradient").c_str());
     const size_t tight = (size_t)f.ubo.width * sizeof(float4);
     if (pitch == 0) pitch = tight;
     if (pitch < tight || pitch % sizeof(float4) != 0) return fail(ctx, GSB_ERR_INVALID, msg("bad row pitch").c_str());
@@ -998,7 +1043,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     bp.density = density;
     const float3 bg = make_float3(f.background[0], f.background[1], f.background[2]);  // the frame's, not the current setting
     if (!det) {
-        CK(launch_backward(bp, f.antialiased, bg, s));
+        CK(launch_backward(bp, f.antialiased, bg, s, nullptr, fisheye ? &f.camera : nullptr));
         return GSB_OK;
     }
     const DetBuffers& d = ctx->bw_det;
@@ -1014,7 +1059,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     db.status_tiles = (uint32_t)(d.status.count / 256);
     db.m_hint = quantise_hint(ctx->m_hint);
     db.key_bits = std::max<uint32_t>(bits_for((uint32_t)n), 1u);  // compact ids < N_v <= n
-    CK(launch_backward(bp, f.antialiased, bg, s, &db));
+    CK(launch_backward(bp, f.antialiased, bg, s, &db, fisheye ? &f.camera : nullptr));
     return GSB_OK;
 }
 

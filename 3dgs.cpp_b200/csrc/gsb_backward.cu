@@ -378,8 +378,18 @@ __host__ __device__ constexpr bool cam_word_live(int j) {
 // warps) into P.cam_partials for k_camera_reduce.  The vertex gradient is written only when P.grad_vertices is set.
 // AA (a frame of gsb_set_antialiased): d[5] is dL/d(o comp), comp = sqrt(det0 / det).  The opacity gets d[5] comp, and
 // g = d[5] o reaches both determinants: dL/d det0 = g comp / (2 det0), dL/d det = -g comp / (2 det), 0 where comp = 0.
-template <bool CAMERA, bool AA>
-__global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ BackwardParams P) {
+// FISHEYE (a frame of gsb_set_camera_model's fisheye, CAMERA = false only): J and uv are the lens's (fisheye_geo,
+// fisheye_jacobian), dL/d(J W) goes to J through the view rotation and on to the view-space position through J's second
+// derivatives (fisheye_grad), and that position to the Gaussian's through the view rotation; the projection matrix takes no
+// part.  Only these instantiations take the larger argument, so the others keep their code.
+struct BackwardFisheyeParams : BackwardParams {
+    gsb_camera_model cam;
+};
+template <bool FISHEYE>
+using PbParams = std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>;
+template <bool CAMERA, bool AA, bool FISHEYE = false>
+__global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ PbParams<FISHEYE> P) {
+    static_assert(!(CAMERA && FISHEYE), "no camera gradient through the fisheye lens");
     const uint32_t nv = P.ctl->num_visible;
     const gsb_uniforms& U = P.ubo;
     const float* pm = U.proj_mat;
@@ -415,7 +425,17 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         const Jacobian J = jacobian(U, cv.vx, cv.vy, vz);
         const float limx = J.limx, limy = J.limy, txtz = J.txtz, tytz = J.tytz, tx = J.tx, ty = J.ty;
         const float focal_x = J.focal_x, focal_y = J.focal_y, ja = J.ja, jb = J.jb, g0 = J.g0, g1 = J.g1;
-        const float(&T0)[3] = J.T0, (&T1)[3] = J.T1;  // rows of J W (W = the view rotation)
+        FisheyeGeo F;
+        FisheyeJ FJ;
+        if constexpr (FISHEYE) {
+            F = fisheye_geo(P.cam, cv.vx, cv.vy, vz);
+            FJ = fisheye_jacobian(P.cam, vm, F, cv.vx, cv.vy);
+        }
+        const auto& JW = [&]() -> const auto& {
+            if constexpr (FISHEYE) return FJ;
+            else return J;
+        }();
+        const float(&T0)[3] = JW.T0, (&T1)[3] = JW.T1;  // rows of J W (W = the view rotation)
         const Cov2d cov = cov2d(T0, T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
         const float(&ST0)[3] = cov.tm0, (&ST1)[3] = cov.tm1;  // Sigma T0, Sigma T1
         const float a = cov.m00, b = cov.m10, c = cov.m11;  // b: the [1][0] entry, rounded like k_project's m10
@@ -478,6 +498,21 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
 #pragma unroll
         for (int k = 0; k < 3; k++)
             dp[k] = ((pm[k * 4 + 0] * dhx + pm[k * 4 + 1] * dhy) + pm[k * 4 + 3] * dhw) + ((vm[k * 4 + 0] * dvx + vm[k * 4 + 1] * dvy) + vm[k * 4 + 2] * dvz);
+        if constexpr (FISHEYE) {  // J W -> J -> view-space position (with uv's own share) -> position
+            float dJ[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+            for (int r = 0; r < 3; r++) {
+#pragma unroll
+                for (int k = 0; k < 3; k++) {
+                    dJ[0][k] += dT0[r] * vm[r * 4 + k];
+                    dJ[1][k] += dT1[r] * vm[r * 4 + k];
+                }
+            }
+            float ftx, fty, ftz;
+            fisheye_grad(P.cam, F, FJ, cv.vx, cv.vy, vz, dJ, d[0], d[1], ftx, fty, ftz);
+#pragma unroll
+            for (int k = 0; k < 3; k++) dp[k] = (vm[k * 4 + 0] * ftx + vm[k * 4 + 1] * fty) + vm[k * 4 + 2] * ftz;
+        }
 
         // ---- colour (preprocess.comp:73-108) -> SH coefficients and the view direction ----
         const float dcr = r2.x > 0.0f ? d[6] : 0.0f;  // :102-104 red clamped at 0 (the record holds the clamped value)
@@ -756,7 +791,9 @@ cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackwar
 
 }  // namespace
 
-cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det) {
+cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det,
+                            const gsb_camera_model* fisheye) {
+    if (fisheye && p.grad_ubo) return cudaErrorInvalidValue;
     const bool density = p.density != nullptr;
     // grid-stride over N_v, which stays on the device: the grid comes from the SM count
     const unsigned grid = (unsigned)p.num_sms * 4u;
@@ -773,6 +810,12 @@ cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 ba
         k_density_accumulate<<<grid, PB_THREADS, 0, s>>>(p);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
+    }
+    if (fisheye) {  // vertex gradients only (checked above)
+        const BackwardFisheyeParams fp{p, *fisheye};
+        if (antialiased) k_preprocess_backward<false, true, true><<<grid, PB_THREADS, 0, s>>>(fp);
+        else k_preprocess_backward<false, false, true><<<grid, PB_THREADS, 0, s>>>(fp);
+        return cudaGetLastError();
     }
     if (!p.grad_ubo) {
         if (antialiased) k_preprocess_backward<false, true><<<grid, PB_THREADS, 0, s>>>(p);

@@ -60,6 +60,97 @@ __device__ __forceinline__ Jacobian jacobian(const gsb_uniforms& U, float vx, fl
     return j;
 }
 
+// The fisheye lens of gsb_set_camera_model (DESIGN.md section 19), for t = (x, y, z) in view space: r = |(x, y)|, d = |t|,
+// theta = atan2(r, z), t2 = theta^2, rho = theta P(t2), rho' = Q(t2), P = 1 + t2 P1, Q = 1 + t2 Q1.  Everything is written in
+// b = theta / r (1 / d on the axis) and S = (sin(2 theta) / 2 - theta) / theta^3, so that nothing divides 0 by 0 on the axis:
+//   s = rho / r = P b,   c = (rho' cos sin - rho) / r^3 = B b^3 with B = S + Q1 sin(2 theta) / (2 theta) - P1,   e = Q / d^2
+//   J = d uv / d t = [fx (s + x^2 c), fx x y c, -fx x e; fy x y c, fy (s + y^2 c), -fy y e]
+// S cancels catastrophically in the direct form for small theta (its numerator is O(theta^3) against O(theta) terms): below
+// FISHEYE_SERIES_THETA it is summed from its Taylor series in t2 (7 terms, truncation < 2e-10 relative at theta = 1), above it
+// the direct form loses at most a few ulps.
+constexpr float FISHEYE_SERIES_THETA = 1.0f;
+__device__ constexpr float FS_A1 = -0.6666666666666666f, FS_A2 = 0.13333333333333333f, FS_A3 = -0.012698412698412698f,
+                           FS_A4 = 0.0007054673721340388f, FS_A5 = -2.565335898669232e-05f, FS_A6 = 6.577784355562133e-07f,
+                           FS_A7 = -1.2529113058213587e-08f;
+struct FisheyeGeo {
+    float r, d, theta, t2, b, P1, Q1, S, scth, s, c, e;  // scth = sin(2 theta) / (2 theta) = 1 + t2 S
+};
+__device__ __forceinline__ FisheyeGeo fisheye_geo(const gsb_camera_model& M, float x, float y, float z) {
+    FisheyeGeo g;
+    const float r2 = x * x + y * y;
+    g.r = sqrtf(r2);
+    g.d = sqrtf(r2 + z * z);
+    g.theta = atan2f(g.r, z);
+    g.t2 = g.theta * g.theta;
+    const float t2 = g.t2;
+    g.b = g.r > 0.0f ? g.theta / g.r : 1.0f / g.d;
+    g.P1 = M.k[0] + t2 * (M.k[1] + t2 * (M.k[2] + t2 * M.k[3]));
+    g.Q1 = 3.0f * M.k[0] + t2 * (5.0f * M.k[1] + t2 * (7.0f * M.k[2] + t2 * (9.0f * M.k[3])));
+    if (g.theta < FISHEYE_SERIES_THETA) {
+        g.S = FS_A1 + t2 * (FS_A2 + t2 * (FS_A3 + t2 * (FS_A4 + t2 * (FS_A5 + t2 * (FS_A6 + t2 * FS_A7)))));
+        g.scth = 1.0f + t2 * g.S;
+    } else {
+        g.scth = ((g.r * z) / (g.d * g.d)) / g.theta;
+        g.S = (g.scth - 1.0f) / t2;
+    }
+    const float B = (g.S + g.Q1 * g.scth) - g.P1;
+    g.s = (1.0f + t2 * g.P1) * g.b;
+    g.c = B * ((g.b * g.b) * g.b);
+    g.e = (1.0f + t2 * g.Q1) / (g.d * g.d);
+    return g;
+}
+// J and the rows of T = J W (T0[r] = V[r][0] J[0][0] + V[r][1] J[0][1] + V[r][2] J[0][2], as jacobian() for its two terms)
+struct FisheyeJ {
+    float J[2][3], T0[3], T1[3];
+};
+__device__ __forceinline__ FisheyeJ fisheye_jacobian(const gsb_camera_model& M, const float* vm, const FisheyeGeo& g, float x, float y) {
+    FisheyeJ j;
+    const float xyc = (x * y) * g.c;
+    j.J[0][0] = M.fx * (g.s + (x * x) * g.c), j.J[0][1] = M.fx * xyc, j.J[0][2] = -M.fx * (x * g.e);
+    j.J[1][0] = M.fy * xyc, j.J[1][1] = M.fy * (g.s + (y * y) * g.c), j.J[1][2] = -M.fy * (y * g.e);
+#pragma unroll
+    for (int r = 0; r < 3; r++) {
+        j.T0[r] = (vm[r * 4 + 0] * j.J[0][0] + vm[r * 4 + 1] * j.J[0][1]) + vm[r * 4 + 2] * j.J[0][2];
+        j.T1[r] = (vm[r * 4 + 0] * j.J[1][0] + vm[r * 4 + 1] * j.J[1][1]) + vm[r * 4 + 2] * j.J[1][2];
+    }
+    return j;
+}
+// The backward's share: dL/dt of Phi = sum_{a,i} dJ[a][i] J[a][i] (dJ = dL/dJ, J's second derivatives) plus J^T duv.  With
+// c_x = dc/dx / x, c_z = dc/dz, e_x = de/dx / x, e_z = de/dz (ds/dx = x c, ds/dz = -e), all stable on the axis:
+//   c_x = 2 B' z b^4 / d^2 + 3 B S b^5,   c_z = -(2 B' theta r b^3 + 3 B b^2) / d^2,   B' = dB / dt2
+//   e_x = (z b R2 - 2 Q) / d^4,           e_z = -(R2 theta r + 2 Q z) / d^4,             R2 = rho'' / theta = 2 dQ / dt2
+__device__ __forceinline__ void fisheye_grad(const gsb_camera_model& M, const FisheyeGeo& g, const FisheyeJ& j, float x, float y,
+                                             float z, const float (&dJ)[2][3], float du, float dv, float& dx, float& dy, float& dz) {
+    const float t2 = g.t2, b = g.b;
+    float dS;
+    if (g.theta < FISHEYE_SERIES_THETA) {
+        dS = FS_A2 + t2 * (2.0f * FS_A3 + t2 * (3.0f * FS_A4 + t2 * (4.0f * FS_A5 + t2 * (5.0f * FS_A6 + t2 * (6.0f * FS_A7)))));
+    } else {  // d scth / d t2 = (cos 2 theta - scth) / (2 t2)
+        const float cos2 = ((z - g.r) * (z + g.r)) / (g.d * g.d);
+        dS = (0.5f * (cos2 - g.scth) - (g.scth - 1.0f)) / (t2 * t2);
+    }
+    const float dP1 = M.k[1] + t2 * (2.0f * M.k[2] + t2 * (3.0f * M.k[3]));
+    const float dQ1 = 5.0f * M.k[1] + t2 * (14.0f * M.k[2] + t2 * (27.0f * M.k[3]));
+    const float B = (g.S + g.Q1 * g.scth) - g.P1;
+    const float dB = ((dS + dQ1 * g.scth) + g.Q1 * (g.S + t2 * dS)) - dP1;
+    const float d2 = g.d * g.d, b2 = b * b, b3 = b2 * b;
+    const float Q = 1.0f + t2 * g.Q1, R2 = 2.0f * (g.Q1 + t2 * dQ1);
+    const float cx = (2.0f * dB * z) * (b3 * b) / d2 + (3.0f * B * g.S) * (b3 * b2);
+    const float cz = -((2.0f * dB * g.theta) * (g.r * b3) + 3.0f * B * b2) / d2;
+    const float ex = ((z * b) * R2 - 2.0f * Q) / (d2 * d2);
+    const float ez = -((R2 * g.theta) * g.r + 2.0f * Q * z) / (d2 * d2);
+    const float A0 = M.fx * dJ[0][0], A1 = M.fx * dJ[0][1], A2 = M.fx * dJ[0][2];
+    const float B0 = M.fy * dJ[1][0], B1 = M.fy * dJ[1][1], B2 = M.fy * dJ[1][2];
+    const float sig = A0 + B1, m = A1 + B0;
+    const float q = ((A0 * x) * x + (m * x) * y) + (B1 * y) * y, l = A2 * x + B2 * y;
+    dx = (((sig * x) * g.c + (q * x) * cx) + g.c * (2.0f * A0 * x + m * y)) - ((l * x) * ex + g.e * A2);
+    dy = (((sig * y) * g.c + (q * y) * cx) + g.c * (2.0f * B1 * y + m * x)) - ((l * y) * ex + g.e * B2);
+    dz = (q * cz - sig * g.e) - l * ez;
+    dx += du * j.J[0][0] + dv * j.J[1][0];
+    dy += du * j.J[0][1] + dv * j.J[1][1];
+    dz += du * j.J[0][2] + dv * j.J[1][2];
+}
+
 // cov2d = transpose(T) Sigma T + 0.3 I (:56-65), Sigma = the cov3d words ca.xyzw, cb.xy; tm0 / tm1 = Sigma T0 / Sigma T1 (S[k] =
 // column k).  m01 and m10 round differently, so each caller states its own determinant.  c00 and c11 are the diagonal before
 // the dilation (the anti-aliased mode's opacity compensation reads them; m01 and m10 are not dilated).

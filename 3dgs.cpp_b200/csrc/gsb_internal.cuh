@@ -103,7 +103,8 @@ struct EmitParams {
 cudaError_t launch_cov3d(const float* vtx_aos, uint64_t count, uint64_t dst_offset, float4* pos_op,
                          float4* cov_a, float2* cov_b, float* sh, float scale_factor, cudaStream_t s, bool sh_half = false);
 // antialiased: gsb_set_antialiased's opacity compensation (not on the routed kernel of a sharded frame)
-cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s);
+// fisheye: gsb_set_camera_model's lens (k_project<..., FISHEYE = true>, plain contexts only); null = the pinhole camera.
+cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* fisheye = nullptr);
 cudaError_t launch_emit(const EmitParams& p, cudaStream_t s);
 
 struct SortParams {  // host-side arguments of launch_sort
@@ -215,7 +216,9 @@ struct DetBackward {
 // background: the frame's gsb_set_background, the colour behind every pixel's last contributor.  It is a kernel argument of
 // its own after BackwardParams, not a field of it: a larger BackwardParams would move the arguments that follow it in
 // k_det_reduce.
-cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det = nullptr);
+// fisheye: the frame's gsb_set_camera_model lens (vertex gradients only: p.grad_ubo must be null), null for a pinhole frame.
+cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det = nullptr,
+                            const gsb_camera_model* fisheye = nullptr);
 // gsb_background_gradient: out[c] = sum over the W x H pixels of T_final(p) grad_image(p)[c], from the recorded frame's
 // (bits(T), last) words.  fp64 products and sums in an order fixed by W and H (background_grad_rows(H) per-CTA partials,
 // then one CTA), no atomics.  partials holds 3 doubles per row of background_grad_rows(H).

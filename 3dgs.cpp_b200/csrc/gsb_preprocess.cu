@@ -16,6 +16,8 @@
 // of the GLSL source, so results are value-identical to the oracle (bit-exact parity).
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "gsb_cull.cuh"
 #include "gsb_geom.cuh"
 #include "gsb_internal.cuh"
@@ -162,6 +164,9 @@ __device__ __forceinline__ void compute_sh(const float4* __restrict__ sh4, float
 #ifndef GSB_PROJECT_MIN_BLOCKS
 #define GSB_PROJECT_MIN_BLOCKS 6  // <= 42 registers: 6 CTAs (48 warps) per SM hide the SH gather latency
 #endif
+#ifndef GSB_PROJECT_FISHEYE_MIN_BLOCKS
+#define GSB_PROJECT_FISHEYE_MIN_BLOCKS 4
+#endif
 // ROUTED (frame sharding, gsb_shard.cu): the single stream compaction becomes one compaction per destination band -- G
 // simultaneous decoupled look-back scans over G-wide status vectors, warp d walking column d -- and the record goes straight
 // from registers into the exchange buffer of every rank whose band the AABB touches (stores into peer-mapped memory over
@@ -169,9 +174,26 @@ __device__ __forceinline__ void compute_sh(const float4* __restrict__ sh4, float
 // ordered exactly like the single-GPU compaction and the band's pixels are bit-identical.
 // AA (gsb_set_antialiased, plain contexts only): the stored opacity is scaled by sqrt(det(cov2d) / det(cov2d + 0.3 I)); the
 // conic, radius, AABB and survivor set are those of AA = false.
-template <bool DEBUG, bool ROUTED, bool SH16, bool AA>
-__global__ void __launch_bounds__(PRE_THREADS, GSB_PROJECT_MIN_BLOCKS) k_project(const __grid_constant__ ProjectParams P) {
+// FISHEYE (gsb_set_camera_model, plain contexts only): the projection, Jacobian and cull of the fisheye lens (gsb_geom.cuh's
+// fisheye_geo / fisheye_jacobian) and the depth key d = |t| instead of z; everything from cov2d on is the pinhole path's.  Only
+// the FISHEYE instantiations take the larger argument, so the others keep their code.
+struct ProjectFisheyeParams : ProjectParams {
+    gsb_camera_model cam;
+};
+template <bool FISHEYE>
+using ProjParams = std::conditional_t<FISHEYE, ProjectFisheyeParams, ProjectParams>;
+template <bool FISHEYE>
+struct ProjectBounds {
+    static constexpr int MIN_BLOCKS = GSB_PROJECT_MIN_BLOCKS;
+};
+template <>
+struct ProjectBounds<true> {
+    static constexpr int MIN_BLOCKS = GSB_PROJECT_FISHEYE_MIN_BLOCKS;
+};
+template <bool DEBUG, bool ROUTED, bool SH16, bool AA, bool FISHEYE = false>
+__global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE>::MIN_BLOCKS) k_project(const __grid_constant__ ProjParams<FISHEYE> P) {
     static_assert(!(ROUTED && AA), "sharded contexts have no anti-aliased mode");
+    static_assert(!(ROUTED && FISHEYE), "sharded contexts have no fisheye camera");
     __shared__ uint32_t s_chunk;
     __shared__ uint32_t s_wsurv[PRE_THREADS / 32];
     __shared__ uint32_t s_base_surv;
@@ -204,9 +226,23 @@ __global__ void __launch_bounds__(PRE_THREADS, GSB_PROJECT_MIN_BLOCKS) k_project
         opac = po.w;
         const ClipView cv = clip_view(U, px, py, pz);
         const float ndcx = cv.ndcx, ndcy = cv.ndcy, vz = cv.vz;
-        if (!(vz <= 0.2f)) {  // :135 (NaN is not culled by the shader's test either)
-            const Jacobian J = jacobian(U, cv.vx, cv.vy, vz);
-            const Cov2d cov = cov2d(J.T0, J.T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
+        FisheyeGeo F;
+        bool front;
+        if constexpr (FISHEYE) {
+            F = fisheye_geo(P.cam, cv.vx, cv.vy, vz);
+            front = F.d > 0.2f && F.theta <= P.cam.max_theta;  // NaN is culled
+        } else {
+            front = !(vz <= 0.2f);  // :135 (NaN is not culled by the shader's test either)
+        }
+        if (front) {
+            Cov2d cov;
+            if constexpr (FISHEYE) {
+                const FisheyeJ J = fisheye_jacobian(P.cam, U.view_mat, F, cv.vx, cv.vy);
+                cov = cov2d(J.T0, J.T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
+            } else {
+                const Jacobian J = jacobian(U, cv.vx, cv.vy, vz);
+                cov = cov2d(J.T0, J.T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
+            }
             const float m00 = cov.m00, m01 = cov.m01, m10 = cov.m10, m11 = cov.m11;
             const float det = m00 * m11 - m10 * m01;  // :138
             if (!(det <= 0.0f)) {                                                  // :139-141
@@ -219,8 +255,13 @@ __global__ void __launch_bounds__(PRE_THREADS, GSB_PROJECT_MIN_BLOCKS) k_project
                 const float sq = sqrtf(fmaxf(0.1f, mid * mid - det));
                 const float lambda = fmaxf(mid + sq, mid - sq);
                 radii = ceilf(3.0f * sqrtf(lambda));                     // :146-151
-                uvx = ((ndcx + 1.0f) * (float)W - 1.0f) * 0.5f;          // :157 ndc2Pix
-                uvy = ((ndcy + 1.0f) * (float)H - 1.0f) * 0.5f;
+                if constexpr (FISHEYE) {
+                    uvx = P.cam.fx * (F.s * cv.vx) + P.cam.cx;
+                    uvy = P.cam.fy * (F.s * cv.vy) + P.cam.cy;
+                } else {
+                    uvx = ((ndcx + 1.0f) * (float)W - 1.0f) * 0.5f;  // :157 ndc2Pix
+                    uvy = ((ndcy + 1.0f) * (float)H - 1.0f) * 0.5f;
+                }
                 // :159-164; cvt.rzi.s32.f32 saturates where GLSL int() is undefined
                 bx0 = clampi(__float2int_rz((uvx - radii) / 16.0f), 0, tiles_x);
                 by0 = clampi(__float2int_rz((uvy - radii) / 16.0f), 0, tiles_y);
@@ -232,7 +273,7 @@ __global__ void __launch_bounds__(PRE_THREADS, GSB_PROJECT_MIN_BLOCKS) k_project
                 if (by1 < by0) by1 = by0;
                 nt = (uint32_t)(bx1 - bx0) * (uint32_t)(by1 - by0);  // :168
                 surv = nt != 0;                                      // :169-171
-                depth = vz;
+                depth = FISHEYE ? F.d : vz;
             }
         }
     }
@@ -342,7 +383,7 @@ __global__ void __launch_bounds__(PRE_THREADS, GSB_PROJECT_MIN_BLOCKS) k_project
                              __uint_as_float((uint32_t)(bx1 - bx0) | ((uint32_t)(by1 - by0) << 16)));
         rec[2] = make_float4(colr, colg, colb, depth);
         rec[3] = make_float4(radii, __uint_as_float(P.index_base + i), 0.f, 0.f);  // global Gaussian index (the sort payload of the reference)
-        P.dkeys[cid] = __float_as_uint(depth);  // depth > 0.2: the IEEE bits are monotone as unsigned
+        P.dkeys[cid] = __float_as_uint(depth);  // depth > 0.2 (z, or d for a fisheye): the IEEE bits are monotone as unsigned
         P.dvals[cid] = cid;
     }
     }
@@ -794,26 +835,32 @@ __global__ void __launch_bounds__(PRE_THREADS) k_emit_coarse(const __grid_consta
 
 }  // namespace
 
-template <bool AA>
-void launch_project_plain(const ProjectParams& p, bool debug, unsigned blocks, cudaStream_t s) {
+template <bool AA, bool FISHEYE>
+void launch_project_plain(const ProjParams<FISHEYE>& p, bool debug, unsigned blocks, cudaStream_t s) {
     if (p.sh_half) {  // fp16 SH storage (non-parity)
-        if (debug) k_project<true, false, true, AA><<<blocks, PRE_THREADS, 0, s>>>(p);
-        else k_project<false, false, true, AA><<<blocks, PRE_THREADS, 0, s>>>(p);
-    } else if (debug) k_project<true, false, false, AA><<<blocks, PRE_THREADS, 0, s>>>(p);
-    else k_project<false, false, false, AA><<<blocks, PRE_THREADS, 0, s>>>(p);
+        if (debug) k_project<true, false, true, AA, FISHEYE><<<blocks, PRE_THREADS, 0, s>>>(p);
+        else k_project<false, false, true, AA, FISHEYE><<<blocks, PRE_THREADS, 0, s>>>(p);
+    } else if (debug) k_project<true, false, false, AA, FISHEYE><<<blocks, PRE_THREADS, 0, s>>>(p);
+    else k_project<false, false, false, AA, FISHEYE><<<blocks, PRE_THREADS, 0, s>>>(p);
 }
 
-cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s) {
+template <bool FISHEYE>
+void launch_project_plain(const ProjParams<FISHEYE>& p, bool debug, bool antialiased, unsigned blocks, cudaStream_t s) {
+    if (antialiased) launch_project_plain<true, FISHEYE>(p, debug, blocks, s);
+    else launch_project_plain<false, FISHEYE>(p, debug, blocks, s);
+}
+
+cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* fisheye) {
     if (p.n == 0) return cudaSuccess;
     const unsigned blocks = (p.n + PRE_THREADS - 1) / PRE_THREADS;
     if (p.route_world > 0) {
-        if (antialiased) return cudaErrorInvalidValue;  // the routed kernel has no AA instantiation
+        if (antialiased || fisheye) return cudaErrorInvalidValue;  // the routed kernel has no AA or fisheye instantiation
         if (p.sh_half) k_project<false, true, true, false><<<blocks, PRE_THREADS, 0, s>>>(p);
         else k_project<false, true, false, false><<<blocks, PRE_THREADS, 0, s>>>(p);
-    } else if (antialiased) {
-        launch_project_plain<true>(p, debug, blocks, s);
+    } else if (fisheye) {
+        launch_project_plain<true>(ProjectFisheyeParams{p, *fisheye}, debug, antialiased, blocks, s);
     } else {
-        launch_project_plain<false>(p, debug, blocks, s);
+        launch_project_plain<false>(p, debug, antialiased, blocks, s);
     }
     return cudaGetLastError();
 }

@@ -31,6 +31,7 @@ ERR_INVALID, ERR_NO_DEVICE, ERR_CUDA, ERR_NO_SCENE, ERR_OOM, ERR_OVERFLOW = -1, 
 FORMAT_RGBA32F, FORMAT_RGBA8, FORMAT_BGRA8 = 0, 1, 2
 MODE_EXACT, MODE_FAST = 0, 1
 MEM_HOST, MEM_DEVICE = 0, 1
+CAMERA_PINHOLE, CAMERA_FISHEYE = 0, 1
 (BUF_COV3D, BUF_ATTR, BUF_TILES_OVERLAP, BUF_PREFIX_SUM, BUF_KEYS_UNSORTED, BUF_VALS_UNSORTED,
  BUF_KEYS_SORTED, BUF_VALS_SORTED, BUF_TILE_BOUNDARY, BUF_DEPTH_ORDER, BUF_EMIT_OFFSETS) = range(11)
 ALL_ROWS = 0xFFFFFFFF
@@ -38,7 +39,7 @@ ALL_ROWS = 0xFFFFFFFF
 EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_abi_version", "gsb_device_count", "gsb_create", "gsb_destroy", "gsb_last_error",
     "gsb_scene_upload", "gsb_scene_size", "gsb_set_mode", "gsb_set_debug", "gsb_set_timers", "gsb_set_tile_cull", "gsb_set_sh_storage",
-    "gsb_set_antialiased", "gsb_set_background",
+    "gsb_set_antialiased", "gsb_set_background", "gsb_set_camera_model",
     "gsb_reserve_instances", "gsb_render", "gsb_render_async", "gsb_get_stats", "gsb_debug_size",
     "gsb_debug_download", "gsb_sort_pairs", "gsb_sort_pairs32", "gsb_set_graph", "gsb_host_alloc", "gsb_host_free",
     # reverse mode
@@ -116,6 +117,38 @@ class SynthParams(C.Structure):
                 ("sh_dc_range", C.c_float), ("sh_rest_sigma", C.c_float)]
 
 
+class CameraModel(C.Structure):
+    """gsb_camera_model: the lens of gsb_set_camera_model (fisheye_camera / fisheye_from_colmap make one)."""
+    _fields_ = [("kind", C.c_uint32), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
+                ("k", C.c_float * 4), ("max_theta", C.c_float)]
+
+
+FISHEYE_MAX_THETA_CAP = 175.0 * np.pi / 180.0  # fisheye_camera's default max_theta never exceeds this (175 deg)
+
+
+def fisheye_camera(fx, fy, cx, cy, k=(0.0, 0.0, 0.0, 0.0), max_theta=None) -> CameraModel:
+    """An OpenCV-fisheye (Kannala-Brandt) lens for Context.set_camera_model: theta_d = theta (1 + k1 theta^2 + k2 theta^4 +
+    k3 theta^6 + k4 theta^8), pixel (i, j) sampled at (i, j) (so cx, cy are COLMAP's plus 0.5; see fisheye_from_colmap).
+    max_theta (radians) culls rays farther off the axis; None = the largest angle up to FISHEYE_MAX_THETA_CAP at which
+    theta_d is still increasing (found on a 0.1 mrad grid, as gs_viewer_headless --fisheye does)."""
+    k = [float(x) for x in k]
+    if len(k) != 4:
+        raise ValueError("fisheye_camera: k must hold 4 coefficients")
+    if max_theta is None:
+        t = np.arange(1, int(FISHEYE_MAX_THETA_CAP / 1e-4) + 1) * 1e-4
+        u = t * t
+        dq = 1.0 + u * (3.0 * k[0] + u * (5.0 * k[1] + u * (7.0 * k[2] + u * 9.0 * k[3])))
+        bad = np.nonzero(~(dq > 0.0))[0]
+        max_theta = float(t[-1] if bad.size == 0 else (t[bad[0] - 1] if bad[0] > 0 else 0.0))
+    return CameraModel(CAMERA_FISHEYE, float(fx), float(fy), float(cx), float(cy), (C.c_float * 4)(*k), float(max_theta))
+
+
+def fisheye_from_colmap(fx, fy, cx, cy, k1, k2, k3, k4) -> CameraModel:
+    """COLMAP's OPENCV_FISHEYE parameters (fx, fy, cx, cy, k1, k2, k3, k4) as a fisheye_camera.  COLMAP puts pixel centres at
+    i + 0.5, this renderer samples pixel (i, j) at (i, j): the principal point moves by half a pixel."""
+    return fisheye_camera(fx, fy, float(cx) - 0.5, float(cy) - 0.5, (k1, k2, k3, k4))
+
+
 class AdamConfig(C.Structure):
     """gsb_adam_config."""
     _fields_ = [("lr", C.c_float * 6), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float),
@@ -158,6 +191,7 @@ lib.gsb_set_timers.argtypes = [_vp, C.c_int]
 lib.gsb_set_tile_cull.argtypes = [_vp, C.c_int]
 lib.gsb_set_antialiased.argtypes = [_vp, C.c_int]
 lib.gsb_set_background.argtypes = [_vp, C.POINTER(C.c_float)]
+lib.gsb_set_camera_model.argtypes = [_vp, C.POINTER(CameraModel)]
 lib.gsb_set_sh_storage.argtypes = [_vp, C.c_int]
 lib.gsb_set_graph.argtypes = [_vp, C.c_int]
 lib.gsb_host_alloc.argtypes = [C.POINTER(_vp), C.c_size_t]
@@ -429,6 +463,7 @@ class Context:
         self.device = device
         self.frames = 0  # frames rendered through this wrapper (render_torch checks it between forward and backward)
         self._background = None  # the last set_background colour (render_torch restores it after a frame of its own)
+        self.camera = None  # the last set_camera_model lens (None: pinhole)
 
     def close(self):
         if self.h and self._own:
@@ -480,6 +515,14 @@ class Context:
         black, the default): out = c + T_final * rgb.  The backward pass follows the colour of the frame it differentiates."""
         self._ck(lib.gsb_set_background(self.h, None if rgb is None else (C.c_float * 3)(*(float(x) for x in rgb))))
         self._background = None if rgb is None else [float(x) for x in rgb]
+
+    def set_camera_model(self, cam=None):
+        """gsb_set_camera_model: from the next frame, project through the lens `cam` (a CameraModel from fisheye_camera or
+        fisheye_from_colmap; None or kind CAMERA_PINHOLE = the UBO's pinhole camera, the default).  A fisheye frame reads only
+        the UBO's view matrix, camera position and size.  Frames, render_torch, SceneAdam and the backward pass follow it
+        (the backward uses the model of the frame it differentiates); there is no camera gradient through a fisheye lens."""
+        self._ck(lib.gsb_set_camera_model(self.h, None if cam is None else C.byref(cam)))
+        self.camera = None if cam is None or cam.kind == CAMERA_PINHOLE else cam
 
     def background_gradient(self, grad_image, stream=None):
         """gsb_background_gradient of the last (recorded, whole) frame: dL/d(background) = sum_p T_final(p) grad_image(p) as a
@@ -858,6 +901,8 @@ def _render_fn():
                 _check_density("render_torch", density, v)
                 fctx.density = density
                 if ubo is not None:  # the camera's float fields come from the tensor, the frame size from u
+                    if ctx.camera is not None:
+                        raise ValueError("render_torch: ubo= (a camera gradient) is not available for a fisheye camera model")
                     u = unpack_uniforms(ubo.detach().to("cpu", torch.float32).numpy(), u.width, u.height)
                     fctx.ubo_like = (ubo.dtype, ubo.device)
                 ctx.set_backward(True)
@@ -928,7 +973,10 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, 
 
     Under torch.use_deterministic_algorithms(True), backward turns gsb_set_backward_deterministic on for `ctx` (otherwise
     off): every gradient and density statistic is then bit-identical for the same inputs, at some cost in time.  With
-    torch's default settings backward takes the atomic path, whose results may differ in the last bit from run to run."""
+    torch's default settings backward takes the atomic path, whose results may differ in the last bit from run to run.
+
+    The frame is projected through the context's camera model (Context.set_camera_model); ubo= on a fisheye context raises
+    ValueError."""
     return _render_fn().apply(ctx, vertices, u, ubo, density, background)
 
 
@@ -1234,7 +1282,9 @@ class SceneAdam:
     rendered closer or larger than its training views: filter_cameras, the list of training Uniforms, turns it on.  Then
     `params` stay the unfiltered raw parameters, `variance` holds each Gaussian's filter (Context.filter3d_variance) and
     `vertices` the filtered records (apply_filter_3d of the activated params), which frames render and step() trains
-    through gsb_adam_step_filter3d.  Mip-Splatting recomputes the filter every 100 steps once densification has ended:
+    through gsb_adam_step_filter3d.  The filter is a pinhole filter: it reads each camera's UBO focal (tan_fov) and
+    ndc2Pix, whatever the context's camera model, so for fisheye training views pass pinhole Uniforms of a matching focal.
+    Mip-Splatting recomputes the filter every 100 steps once densification has ended:
 
         if it >= densify_until and it % 100 == 0:
             opt.update_filter_3d()

@@ -192,6 +192,28 @@ int gsb_set_antialiased(gsb_ctx *ctx, int enabled);
  * GSB_ERR_INVALID.  Takes effect at the next frame; the frame records it and the backward entries follow the frame's value.
  * Every context accepts it, sharded ones and gsb_group ranks included; changing it drops no captured graph. */
 int gsb_set_background(gsb_ctx *ctx, const float *rgb);
+/* Camera model of the frames (default PINHOLE: the UBO's proj_mat / tan_fov, the reference's camera, bit for bit).
+ * FISHEYE is COLMAP's OPENCV_FISHEYE (Kannala-Brandt) lens: k_project reads only view_mat, camera_position, width and height
+ * of the UBO, and with t = (x, y, z) the view-space position (x right, y down, z forward), r = |(x, y)|, d = |t|,
+ * theta = atan2(r, z) and rho = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8):
+ *   culled unless d > 0.2 and theta <= max_theta (NaN culled);  uv = (fx (rho / r) x + cx, fy (rho / r) y + cy), (cx, cy) at r = 0;
+ *   cov2d = J W Sigma W^T J^T + 0.3 I with J = d uv / d t exact (no tan_fov clamp);  depth key d (sorts lenses past 180 deg).
+ * The conic, culls, radius, tile AABB, opacity (and its anti-aliased compensation) and SH colour follow from it as for a
+ * pinhole frame.  Pixel (i, j) is sampled at (i, j): COLMAP's principal point is (cx - 0.5, cy - 0.5) here.
+ * The frame records the model; gsb_render_backward and gsb_render_backward_density follow the frame's, and for a fisheye frame
+ * gsb_render_backward_camera and gsb_render_backward_density with a non-NULL grad_uniforms return GSB_ERR_INVALID (no pose
+ * gradient through the lens).  m NULL or kind PINHOLE: the default.  GSB_ERR_INVALID, the setting unchanged, for a NULL ctx,
+ * a sharded context or gsb_group rank, an unknown kind, fx or fy not positive and finite, any other field not finite,
+ * max_theta outside (0, pi), or d theta_d / d theta <= 0 anywhere on [0, max_theta] (checked on the host in double).
+ * Takes effect at the next frame; changing it drops no captured graph. */
+typedef enum gsb_camera_kind { GSB_CAMERA_PINHOLE = 0, GSB_CAMERA_FISHEYE = 1 } gsb_camera_kind;
+typedef struct gsb_camera_model {
+    uint32_t kind;        /* gsb_camera_kind */
+    float fx, fy, cx, cy; /* pixels; pixel (i, j) is sampled at (i, j), as the blend does (COLMAP's cx - 0.5) */
+    float k[4];           /* Kannala-Brandt / OpenCV fisheye: theta_d = theta (1 + k1 t^2 + k2 t^4 + k3 t^6 + k4 t^8), t = theta */
+    float max_theta;      /* radians, in (0, pi): rays farther off the axis are culled */
+} gsb_camera_model;
+int gsb_set_camera_model(gsb_ctx *ctx, const gsb_camera_model *m);
 /* per-stage cudaEvent timers (the QueryManager analogue, Renderer.cpp:85-100). Default on. */
 int gsb_set_timers(gsb_ctx *ctx, int enabled);
 /* Replay the camera-independent middle of the frame (both sorts + key emission) from a captured CUDA graph instead of
