@@ -387,7 +387,7 @@ static int enqueue_front(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uin
 
 // k_blend over tile rows [b0, b1) of the frame; `band_out` is the first pixel row of the frame's band [fp.rb, fp.re).
 int enqueue_blend(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, uint32_t b0, uint32_t b1, void* band_out, size_t pitch,
-                  int fmt, cudaStream_t stream, void* const* peer_frames, int num_peer_frames) {
+                  int fmt, cudaStream_t stream, void* const* peer_frames, int num_peer_frames, void* depth_out, size_t depth_pitch) {
     BlendParams bp{};
     bp.recs = sv.recs;
     bp.vals = ctx->vals[fp.fin];
@@ -414,6 +414,10 @@ int enqueue_blend(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, uint32
     // gsb_set_backward: the per-pixel state of gsb_render_backward (plain contexts, per-tile lists)
     bp.record = (ctx->backward && fp.cs == 0 && num_peer_frames == 0) ? ctx->bw_record.p : nullptr;
     for (int c = 0; c < 3; c++) bp.background[c] = ctx->background[c];  // gsb_set_background (every context, sharded or not)
+    if (depth_out) {  // gsb_render_depth (plain contexts): the (D, A) band, rows as in `out`
+        bp.depth_alpha = static_cast<unsigned char*>(depth_out) + (size_t)(b0 - fp.rb) * GSB_TILE * depth_pitch;
+        bp.depth_pitch_bytes = depth_pitch;
+    }
     CK(launch_blend(bp, stream));
     return GSB_OK;
 }
@@ -437,12 +441,13 @@ int enqueue_tail(gsb_ctx* ctx, const FramePlan& fp, const gsb_uniforms& ubo, cud
     f.timers = ctx->timers;
     f.recorded = ctx->backward && fp.cs == 0;  // what enqueue_blend records (a sharded context never has the switch on)
     f.band = !(fp.rb == 0 && fp.re == fp.tiles_y);
+    f.depth = false;  // set by gsb_render_depth after this
     return GSB_OK;
 }
 
-// Enqueue one whole frame on `stream`; out_dev is device memory.
+// Enqueue one whole frame on `stream`; out_dev (and depth_dev, gsb_render_depth's (D, A) band or null) is device memory.
 static int enqueue_frame(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, void* out_dev, size_t pitch, int fmt,
-                  cudaStream_t stream) {
+                  cudaStream_t stream, void* depth_dev = nullptr, size_t depth_pitch = 0) {
     ctx->frame.recorded = false;  // the frame overwrites the record and the lists the last one left
     // W x H per-pixel state of the reverse pass, grown on demand while gsb_set_backward is on
     if (ctx->backward) CK(ctx->bw_record.grow((size_t)ubo->width * ubo->height));
@@ -450,9 +455,11 @@ static int enqueue_frame(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uin
     FramePlan fp{};
     int rc = enqueue_front(ctx, ubo, rb, re, sv, stream, &fp);
     if (rc != GSB_OK) return rc;
-    rc = enqueue_blend(ctx, fp, sv, rb, re, out_dev, pitch, fmt, stream);
+    rc = enqueue_blend(ctx, fp, sv, rb, re, out_dev, pitch, fmt, stream, nullptr, 0, depth_dev, depth_pitch);
     if (rc != GSB_OK) return rc;
-    return enqueue_tail(ctx, fp, *ubo, stream);
+    rc = enqueue_tail(ctx, fp, *ubo, stream);
+    ctx->frame.depth = depth_dev != nullptr;
+    return rc;
 }
 
 // the pixel format and image size checks of every render entry point
@@ -752,15 +759,29 @@ int gsb_render_async(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_
     return enqueue_frame(ctx, ubo, rb, re, out_device, pitch, fmt, stream_or_own(ctx, stream));
 }
 
-int gsb_render(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, void* out, size_t pitch, gsb_memory out_mem,
-               gsb_format fmt, void* stream) {
-    int rc = check_render_args(ctx, ubo, rb, re, out, pitch, fmt);
-    if (rc != GSB_OK) return rc;
+}  // extern "C"
+
+namespace gsb {
+
+// A page-locked host pointer's device alias (gsb_render stores straight into it), or null for pageable memory.
+static void* pinned_alias(const gsb_ctx* ctx, void* p) {
+    cudaPointerAttributes pa{};
+    const bool pinned = ctx->host_direct && cudaPointerGetAttributes(&pa, p) == cudaSuccess && pa.type == cudaMemoryTypeHost &&
+                        pa.devicePointer != nullptr;
+    cudaGetLastError();
+    return pinned ? pa.devicePointer : nullptr;
+}
+
+// gsb_render, and with a non-null `depth` (checked by the caller) gsb_render_depth: the (D, A) band goes to `depth`, in the
+// same memory kind as `out`.
+static int render_sync(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, void* out, size_t pitch, gsb_memory out_mem,
+                       gsb_format fmt, void* depth, size_t depth_pitch, void* stream) {
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = stream_or_own(ctx, stream);
     const uint32_t H = ubo->height;
     const uint32_t rows = std::min(H, re * GSB_TILE) - rb * GSB_TILE;
     const size_t tight = (size_t)ubo->width * bytes_per_pixel(fmt);
+    const size_t depth_tight = (size_t)ubo->width * sizeof(float2);
 
     // Host output.  If `out` is page-locked (gsb_host_alloc / cudaHostAlloc / cudaHostRegister) the blend stores the frame
     // straight into it over PCIe: k_blend writes whole 64-B tile rows, the stores are posted and the kernel is issue-bound,
@@ -770,22 +791,32 @@ int gsb_render(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, 
     void* dev_out = out;
     size_t dev_pitch = pitch;
     bool staged = false;
+    void* dev_depth = depth;
+    size_t dev_depth_pitch = depth_pitch;
+    bool depth_staged = false;
     if (out_mem == GSB_MEM_HOST) {
-        cudaPointerAttributes pa{};
-        const bool pinned = ctx->host_direct && cudaPointerGetAttributes(&pa, out) == cudaSuccess &&
-                            pa.type == cudaMemoryTypeHost && pa.devicePointer != nullptr;
-        cudaGetLastError();
-        if (pinned) {
-            dev_out = pa.devicePointer;
+        if (void* alias = pinned_alias(ctx, out)) {
+            dev_out = alias;
         } else {
             CK(ctx->fb.grow(tight * rows));
             dev_out = ctx->fb;
             dev_pitch = tight;
             staged = true;
         }
+        if (depth) {
+            if (void* alias = pinned_alias(ctx, depth)) {
+                dev_depth = alias;
+            } else {
+                CK(ctx->depth_fb.grow(depth_tight * rows));
+                dev_depth = ctx->depth_fb;
+                dev_depth_pitch = depth_tight;
+                depth_staged = true;
+            }
+        }
     }
+    int rc;
     for (int attempt = 0;; attempt++) {
-        rc = enqueue_frame(ctx, ubo, rb, re, dev_out, dev_pitch, fmt, s);
+        rc = enqueue_frame(ctx, ubo, rb, re, dev_out, dev_pitch, fmt, s, dev_depth, dev_depth_pitch);
         if (rc != GSB_OK) return rc;
         rc = wait_frame(ctx);
         if (rc != GSB_OK) return rc;
@@ -794,11 +825,35 @@ int gsb_render(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, 
         rc = regrow_after_overflow(ctx, s);
         if (rc != GSB_OK) return rc;
     }
-    if (staged) {
-        CK(cudaMemcpy2DAsync(out, pitch, dev_out, dev_pitch, tight, rows, cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-    }
+    if (staged) CK(cudaMemcpy2DAsync(out, pitch, dev_out, dev_pitch, tight, rows, cudaMemcpyDeviceToHost, s));
+    if (depth_staged) CK(cudaMemcpy2DAsync(depth, depth_pitch, dev_depth, dev_depth_pitch, depth_tight, rows, cudaMemcpyDeviceToHost, s));
+    if (staged || depth_staged) CK(cudaStreamSynchronize(s));
     return GSB_OK;
+}
+
+}  // namespace gsb
+
+extern "C" {
+
+int gsb_render(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, void* out, size_t pitch, gsb_memory out_mem,
+               gsb_format fmt, void* stream) {
+    int rc = check_render_args(ctx, ubo, rb, re, out, pitch, fmt);
+    if (rc != GSB_OK) return rc;
+    return render_sync(ctx, ubo, rb, re, out, pitch, out_mem, fmt, nullptr, 0, stream);
+}
+
+int gsb_render_depth(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, void* out, size_t pitch, gsb_memory out_mem,
+                     gsb_format fmt, void* depth_alpha, size_t depth_pitch, void* stream) {
+    int rc = check_render_args(ctx, ubo, rb, re, out, pitch, fmt);
+    if (rc != GSB_OK) return rc;
+    auto bad = [&](const char* what) { return fail(ctx, GSB_ERR_INVALID, (std::string("gsb_render_depth: ") + what).c_str()); };
+    if (ctx->shard) return bad("sharded and group contexts have no depth output");
+    if (!depth_alpha) return bad("null depth_alpha");
+    const size_t tight = (size_t)ubo->width * sizeof(float2);
+    if (depth_pitch == 0) depth_pitch = tight;
+    if (depth_pitch < tight || depth_pitch % sizeof(float2) != 0) return bad("bad depth row pitch");
+    if (reinterpret_cast<uintptr_t>(depth_alpha) % sizeof(float2) != 0) return bad("depth_alpha is not 8-byte aligned");
+    return render_sync(ctx, ubo, rb, re, out, pitch, out_mem, fmt, depth_alpha, depth_pitch, stream);
 }
 
 int gsb_get_stats(gsb_ctx* ctx, gsb_stats* out) {
@@ -945,10 +1000,10 @@ int gsb_set_backward_deterministic(gsb_ctx* ctx, int enabled) {
 }
 
 // The buffers of the deterministic reduction for the current arena capacity and scene size (first use, then growth only).
-static int ensure_det_buffers(gsb_ctx* ctx, uint64_t n) {
+static int ensure_det_buffers(gsb_ctx* ctx, uint64_t n, bool depth) {
     DetBuffers& d = ctx->bw_det;
     const uint64_t cap = ctx->capacity;
-    CK(d.slots.grow(cap * 11));
+    CK(d.slots.grow(cap * (depth ? 12 : 11)));  // the depth backward's slots have one more column
     CK(d.keys[0].grow(cap));
     CK(d.keys[1].grow(cap));
     CK(d.pos[0].grow(cap));
@@ -976,11 +1031,14 @@ static int check_recorded_frame(gsb_ctx* ctx, int no_frame, const char* fn) {
     return GSB_OK;
 }
 
-// The checks and the launch shared by gsb_render_backward, gsb_render_backward_camera and gsb_render_backward_density (fn
-// names the entry in messages).  grad_ubo == nullptr: no camera gradient; grad_vertices == nullptr: no scene gradient (each
-// entry's args_ok says which may be null).  density != nullptr: also accumulate the density statistics into it.
+// The checks and the launch shared by gsb_render_backward, gsb_render_backward_camera, gsb_render_backward_density and
+// gsb_render_backward_depth (fn names the entry in messages).  grad_ubo == nullptr: no camera gradient; grad_vertices ==
+// nullptr: no scene gradient (each entry's args_ok says which may be null).  density != nullptr: also accumulate the density
+// statistics into it.  grad_depth != nullptr (gsb_render_backward_depth): the frame must have depth, and grad_image may be
+// null (no colour gradient).
 static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const float* vertices, const float* grad_image, size_t pitch,
-                           float* grad_vertices, gsb_uniforms* grad_ubo, float* density, void* stream) {
+                           float* grad_vertices, gsb_uniforms* grad_ubo, float* density, void* stream, const float* grad_depth = nullptr,
+                           size_t depth_pitch = 0) {
     if (!ctx) return GSB_ERR_INVALID;
     auto msg = [&](const char* what) { return std::string(fn) + ": " + what; };
     if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, msg("sharded contexts have no backward pass").c_str());
@@ -995,7 +1053,14 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     if (fisheye && grad_ubo) return fail(ctx, GSB_ERR_INVALID, msg("a fisheye frame has no camera gradient").c_str());
     const size_t tight = (size_t)f.ubo.width * sizeof(float4);
     if (pitch == 0) pitch = tight;
-    if (pitch < tight || pitch % sizeof(float4) != 0) return fail(ctx, GSB_ERR_INVALID, msg("bad row pitch").c_str());
+    if (grad_image && (pitch < tight || pitch % sizeof(float4) != 0)) return fail(ctx, GSB_ERR_INVALID, msg("bad row pitch").c_str());
+    if (grad_depth) {
+        if (!f.depth) return fail(ctx, GSB_ERR_INVALID, msg("the last frame was not rendered by gsb_render_depth").c_str());
+        const size_t dtight = (size_t)f.ubo.width * sizeof(float2);
+        if (depth_pitch == 0) depth_pitch = dtight;
+        if (depth_pitch < dtight || depth_pitch % sizeof(float2) != 0 || reinterpret_cast<uintptr_t>(grad_depth) % sizeof(float2) != 0)
+            return fail(ctx, GSB_ERR_INVALID, msg("bad depth row pitch or alignment").c_str());
+    }
     const uint64_t n = ctx->n;
     // zeroed once here; k_preprocess_backward returns every entry it reads to zero
     rc = grow_zeroed(ctx, ctx->bw_scratch, n * 9, "ctx->bw_scratch");
@@ -1004,11 +1069,15 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
         rc = grow_zeroed(ctx, ctx->bw_abs, n * 2, "ctx->bw_abs");
         if (rc != GSB_OK) return rc;
     }
+    if (grad_depth) {  // zeroed once here; k_preprocess_backward returns every entry it reads to zero
+        rc = grow_zeroed(ctx, ctx->bw_depth, n, "ctx->bw_depth");
+        if (rc != GSB_OK) return rc;
+    }
     if (grad_ubo)  // one row per CTA of k_preprocess_backward (4 per SM), fully overwritten by each call
         CK(ctx->bw_cam_partials.grow((uint64_t)ctx->num_sms * 4 * GSB_UBO_WORDS));
     const bool det = ctx->bw_deterministic;
     if (det) {
-        rc = ensure_det_buffers(ctx, n);
+        rc = ensure_det_buffers(ctx, n, grad_depth != nullptr);
         if (rc != GSB_OK) return rc;
     }
     cudaStream_t s = stream_or_own(ctx, stream);
@@ -1042,8 +1111,10 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     bp.abs_scratch = density ? ctx->bw_abs.p : nullptr;
     bp.density = density;
     const float3 bg = make_float3(f.background[0], f.background[1], f.background[2]);  // the frame's, not the current setting
+    const DepthBackward depth{reinterpret_cast<const float2*>(grad_depth), depth_pitch, ctx->bw_depth.p};
+    const DepthBackward* dp = grad_depth ? &depth : nullptr;
     if (!det) {
-        CK(launch_backward(bp, f.antialiased, bg, s, nullptr, fisheye ? &f.camera : nullptr));
+        CK(launch_backward(bp, f.antialiased, bg, s, nullptr, fisheye ? &f.camera : nullptr, dp));
         return GSB_OK;
     }
     const DetBuffers& d = ctx->bw_det;
@@ -1059,7 +1130,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     db.status_tiles = (uint32_t)(d.status.count / 256);
     db.m_hint = quantise_hint(ctx->m_hint);
     db.key_bits = std::max<uint32_t>(bits_for((uint32_t)n), 1u);  // compact ids < N_v <= n
-    CK(launch_backward(bp, f.antialiased, bg, s, &db, fisheye ? &f.camera : nullptr));
+    CK(launch_backward(bp, f.antialiased, bg, s, &db, fisheye ? &f.camera : nullptr, dp));
     return GSB_OK;
 }
 
@@ -1078,6 +1149,12 @@ int gsb_render_backward_density(gsb_ctx* ctx, const float* vertices, const float
                                 gsb_uniforms* grad_uniforms, float* density, void* stream) {
     return render_backward(ctx, "gsb_render_backward_density", vertices && grad_image && density && (grad_vertices || grad_uniforms),
                            vertices, grad_image, pitch, grad_vertices, grad_uniforms, density, stream);
+}
+
+int gsb_render_backward_depth(gsb_ctx* ctx, const float* vertices, const float* grad_image, size_t pitch, const float* grad_depth_alpha,
+                              size_t depth_pitch, float* grad_vertices, gsb_uniforms* grad_uniforms, float* density, void* stream) {
+    return render_backward(ctx, "gsb_render_backward_depth", vertices && grad_depth_alpha && (grad_vertices || grad_uniforms), vertices,
+                           grad_image, pitch, grad_vertices, grad_uniforms, density, stream, grad_depth_alpha, depth_pitch);
 }
 
 int gsb_background_gradient(gsb_ctx* ctx, const float* grad_image, size_t pitch, float* grad_background, void* stream) {

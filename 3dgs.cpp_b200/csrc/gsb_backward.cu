@@ -62,7 +62,7 @@ constexpr int PB_THREADS = 256;
 struct __align__(16) BwRec {  // the staged record in k_blend's pre-scaled form (render.comp:66 evaluated identically)
     float4 q0;                // ux uy -A/2 -B
     float4 q1;                // -C/2 opacity r g
-    float4 q2;                // b power_cut bits(compact id) -
+    float4 q2;                // b power_cut bits(compact id) depth (DEPTH; 0 otherwise)
 };
 
 // ABSGRAD (gsb_render_backward_density): each lane's d u and d v -- one pixel's own terms -- also go through the same
@@ -83,17 +83,44 @@ __device__ __forceinline__ float* det_partials() {
 struct BackwardBgParams : BackwardParams {
     float3 bg;
 };
-template <bool BG>
-using BwParams = std::conditional_t<BG, BackwardBgParams, BackwardParams>;
+// DEPTH (gsb_render_backward_depth): the upstream gradient also has dL/dD and dL/dA per pixel (grad_depth, H x W float2,
+// depth_pitch apart), grad_image may be null (no colour gradient), and each survivor's dL/df (f its record's depth) is reduced
+// like the other accumulators into depth_scratch (n x 1 fp64, zero on entry, returned to zero by k_preprocess_backward): one
+// more shared-memory and det-slot column, after the ABSGRAD ones.  Only these instantiations take the larger argument.
+template <typename Base>
+struct BackwardDepthParams : Base {
+    const float2* grad_depth;
+    size_t depth_pitch;
+    double* depth_scratch;
+};
+template <bool BG, bool DEPTH = false>
+using BwParams = std::conditional_t<DEPTH, BackwardDepthParams<std::conditional_t<BG, BackwardBgParams, BackwardParams>>,
+                                    std::conditional_t<BG, BackwardBgParams, BackwardParams>>;
 template <bool BG>
 BwParams<BG> bw_params(const BackwardParams& p, float3 bg) {
     if constexpr (BG) return BackwardBgParams{p, bg};
     else return p;
 }
+template <bool BG, bool DEPTH>
+BwParams<BG, DEPTH> bw_params(const BackwardParams& p, float3 bg, const DepthBackward* dp) {
+    if constexpr (DEPTH) return BwParams<BG, true>{bw_params<BG>(p, bg), dp->grad, dp->pitch, dp->scratch};
+    else return bw_params<BG>(p, bg);
+}
+template <bool ABSGRAD, bool DEPTH>
+constexpr int bw_nacc = BW_NACC + (ABSGRAD ? BW_NABS : 0) + (DEPTH ? 1 : 0);
+// DEPTH: the pixel's dL/dD and dL/dA, the depth and alpha behind the current entry (0 behind the last contributor, also over
+// a background) and the entry's dL/df.  Empty otherwise, for the reason given at det_partials().
+template <bool ON>
+struct DepthWalk {
+    float gd = 0.f, ga = 0.f, acc_d = 0.f, acc_a = 0.f, vd = 0.f;
+};
+template <>
+struct DepthWalk<false> {};
 
-template <int MODE, bool ABSGRAD, bool DET = false, bool BG = false>
-__global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_constant__ BwParams<BG> P) {
-    constexpr int NACC = BW_NACC + (ABSGRAD ? BW_NABS : 0);  // shared-memory columns: the extra two in ABSGRAD only
+template <int MODE, bool ABSGRAD, bool DET = false, bool BG = false, bool DEPTH = false>
+__global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_constant__ BwParams<BG, DEPTH> P) {
+    constexpr int NACC = BW_NACC + (ABSGRAD ? BW_NABS : 0) + (DEPTH ? 1 : 0);  // shared-memory columns: the extras in ABSGRAD / DEPTH only
+    constexpr int DCOL = BW_NACC + (ABSGRAD ? BW_NABS : 0);                       // DEPTH: the column of dL/df
     __shared__ BwRec s_rec[bw_batch<DET>];
     __shared__ double s_acc[DET ? 1 : BW_BATCH][NACC];
     __shared__ uint32_t s_max;
@@ -115,9 +142,24 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
         const uint2 r = P.record[(size_t)py * P.width + px];
         T = __uint_as_float(r.x);
         last = r.y;
-        const float4 g = *reinterpret_cast<const float4*>(reinterpret_cast<const unsigned char*>(P.grad_image) + (size_t)py * P.row_pitch_bytes +
-                                                          (size_t)px * sizeof(float4));
-        gr = g.x, gg = g.y, gb = g.z;  // A is constant 1 in the forward: no gradient
+        const auto load = [&] {
+            const float4 g = *reinterpret_cast<const float4*>(reinterpret_cast<const unsigned char*>(P.grad_image) + (size_t)py * P.row_pitch_bytes +
+                                                              (size_t)px * sizeof(float4));
+            gr = g.x, gg = g.y, gb = g.z;  // A is constant 1 in the forward: no gradient
+        };
+        if constexpr (DEPTH) {
+            if (P.grad_image) load();  // DEPTH: null = no colour gradient
+        } else {
+            load();
+        }
+    }
+    DepthWalk<DEPTH> dw;
+    if constexpr (DEPTH) {
+        if (inside) {
+            const float2 g = *reinterpret_cast<const float2*>(reinterpret_cast<const unsigned char*>(P.grad_depth) + (size_t)py * P.depth_pitch +
+                                                              (size_t)px * sizeof(float2));
+            dw.gd = g.x, dw.ga = g.y;
+        }
     }
     if (tid == 0) s_max = 0;
     __syncthreads();
@@ -144,7 +186,7 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
             const float2 b = __ldg(reinterpret_cast<const float2*>(rec + 1));  // conic.z, opacity
             s_rec[tid].q0 = make_float4(a.x, a.y, -0.5f * a.z, -a.w);
             s_rec[tid].q1 = make_float4(-0.5f * b.x, b.y, col.x, col.y);
-            s_rec[tid].q2 = make_float4(col.z, power_cut(b.y), __uint_as_float(cid), 0.f);
+            s_rec[tid].q2 = make_float4(col.z, power_cut(b.y), __uint_as_float(cid), DEPTH ? col.w : 0.f);
             if constexpr (!DET) {
 #pragma unroll
                 for (int k = 0; k < NACC; k++) s_acc[tid][k] = 0.0;
@@ -178,16 +220,23 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
             float v[BW_NACC];
 #pragma unroll
             for (int j = 0; j < BW_NACC; j++) v[j] = 0.f;
+            if constexpr (DEPTH) dw.vd = 0.f;
             if (contrib) {
                 T = T / (1.0f - al);  // transmittance in front of this entry
                 const float w = al * T;
                 v[6] = gr * w;  // d colour
                 v[7] = gg * w;
                 v[8] = gb * w;
-                const float dal = T * ((gr * (q1.z - acc_r) + gg * (q1.w - acc_g)) + gb * (q2.x - acc_b));
+                float dal = T * ((gr * (q1.z - acc_r) + gg * (q1.w - acc_g)) + gb * (q2.x - acc_b));
                 acc_r = q1.z * al + (1.0f - al) * acc_r;
                 acc_g = q1.w * al + (1.0f - al) * acc_g;
                 acc_b = q2.x * al + (1.0f - al) * acc_b;
+                if constexpr (DEPTH) {  // D: a colour channel of value f over 0; A: one of value 1 over 0
+                    dal += T * (dw.gd * (q2.w - dw.acc_d) + dw.ga * (1.0f - dw.acc_a));
+                    dw.vd = dw.gd * w;  // d f
+                    dw.acc_d = q2.w * al + (1.0f - al) * dw.acc_d;
+                    dw.acc_a = al + (1.0f - al) * dw.acc_a;
+                }
                 if (!(raw > 0.99f)) {           // alpha clamped at 0.99: no gradient through it
                     const float dpw = dal * raw;  // d alpha / d power = opacity * exp(power)
                     v[5] = dal * e;               // d opacity
@@ -216,6 +265,10 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
                     for (int o = 16; o > 0; o >>= 1) va[j] += __shfl_xor_sync(FULL, va[j], o);
                 }
             }
+            if constexpr (DEPTH) {
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) dw.vd += __shfl_xor_sync(FULL, dw.vd, o);
+            }
             if constexpr (DET) {
                 if (lane == 0) {
 #pragma unroll
@@ -224,6 +277,7 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
 #pragma unroll
                         for (int j = 0; j < BW_NABS; j++) det_partials()[(warp * NACC + BW_NACC + j) * bw_batch<true> + k] = va[j];
                     }
+                    if constexpr (DEPTH) det_partials()[(warp * NACC + DCOL) * bw_batch<true> + k] = dw.vd;
                 }
             } else if (lane == 0) {
 #pragma unroll
@@ -233,6 +287,9 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
 #pragma unroll
                     for (int j = 0; j < BW_NABS; j++)
                         if (va[j] != 0.f) atomicAdd(&s_acc[k][BW_NACC + j], (double)va[j]);
+                }
+                if constexpr (DEPTH) {
+                    if (dw.vd != 0.f) atomicAdd(&s_acc[k][DCOL], (double)dw.vd);
                 }
             }
         }
@@ -262,6 +319,10 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
                     const double a = s_acc[tid][BW_NACC + j];
                     if (a != 0.0) atomicAdd(dabs + j, a);
                 }
+            }
+            if constexpr (DEPTH) {
+                const double a = s_acc[tid][DCOL];
+                if (a != 0.0) atomicAdd(P.depth_scratch + __float_as_uint(s_rec[tid].q2.z), a);
             }
         }
         hi = lo;
@@ -320,10 +381,11 @@ __global__ void __launch_bounds__(PB_THREADS) k_det_prepare(const uint32_t* __re
 // P.scratch (and P.abs_scratch), where k_density_accumulate and k_preprocess_backward read them as they read the atomic sums.
 // The sum is sequential so that an entry whose slot is +0 changes nothing: tile-cull level 1's list is level 0's with such
 // entries removed, and both give the same bits.  Loads run UNROLL entries ahead of the adds.
-template <bool ABSGRAD>
+// DEPTH: the slots have one more column, dL/df, stored into depth_scratch.
+template <bool ABSGRAD, bool DEPTH = false>
 __global__ void __launch_bounds__(PB_THREADS) k_det_reduce(const __grid_constant__ BackwardParams P, const uint32_t* __restrict__ pos,
-                                                           const uint2* __restrict__ runs) {
-    constexpr int NACC = BW_NACC + (ABSGRAD ? BW_NABS : 0);
+                                                           const uint2* __restrict__ runs, double* __restrict__ depth_scratch) {
+    constexpr int NACC = bw_nacc<ABSGRAD, DEPTH>;
     constexpr uint32_t UNROLL = 4;
     const uint32_t nv = P.ctl->num_visible;
     const double* __restrict__ slots = P.det_slots;
@@ -362,6 +424,7 @@ __global__ void __launch_bounds__(PB_THREADS) k_det_reduce(const __grid_constant
 #pragma unroll
             for (int k = 0; k < BW_NABS; k++) ab[k] = s[BW_NACC + k];
         }
+        if constexpr (DEPTH) depth_scratch[cid] = s[NACC - 1];
     }
 }
 
@@ -382,13 +445,21 @@ __host__ __device__ constexpr bool cam_word_live(int j) {
 // fisheye_jacobian), dL/d(J W) goes to J through the view rotation and on to the view-space position through J's second
 // derivatives (fisheye_grad), and that position to the Gaussian's through the view rotation; the projection matrix takes no
 // part.  Only these instantiations take the larger argument, so the others keep their code.
+// DEPTH (gsb_render_backward_depth): the survivor's dL/df (depth_scratch, returned to zero here) goes to the position through
+// the forward's own f: the view-space z of clip_view for a pinhole frame (dL/dv.z += dL/df, and with it dL/d(view row 2) in
+// the CAMERA instantiation), the distance d = |t| of fisheye_geo for a fisheye frame (dL/dt += (t / d) dL/df).
 struct BackwardFisheyeParams : BackwardParams {
     gsb_camera_model cam;
 };
-template <bool FISHEYE>
-using PbParams = std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>;
-template <bool CAMERA, bool AA, bool FISHEYE = false>
-__global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ PbParams<FISHEYE> P) {
+template <typename Base>
+struct PbDepthParams : Base {
+    double* depth_scratch;
+};
+template <bool FISHEYE, bool DEPTH = false>
+using PbParams = std::conditional_t<DEPTH, PbDepthParams<std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>,
+                                    std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>;
+template <bool CAMERA, bool AA, bool FISHEYE = false, bool DEPTH = false>
+__global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ PbParams<FISHEYE, DEPTH> P) {
     static_assert(!(CAMERA && FISHEYE), "no camera gradient through the fisheye lens");
     const uint32_t nv = P.ctl->num_visible;
     const gsb_uniforms& U = P.ubo;
@@ -410,9 +481,16 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
             d[k] = (float)a;
             any |= a != 0.0;
         }
+        float df = 0.f;  // DEPTH: dL/df
+        if constexpr (DEPTH) {
+            const double a = P.depth_scratch[cid];
+            df = (float)a;
+            any |= a != 0.0;
+        }
         if (!any) continue;  // in no pixel's contributor set (or every gradient it received was zero)
 #pragma unroll
         for (int k = 0; k < BW_NACC; k++) sc[k] = 0.0;
+        if constexpr (DEPTH) P.depth_scratch[cid] = 0.0;
         const float4 r2 = __ldg(P.recs + (size_t)cid * GSB_REC_F4 + 2), r3 = __ldg(P.recs + (size_t)cid * GSB_REC_F4 + 3);
         const uint32_t i = __float_as_uint(r3.y);
         const float* v = P.vertices + (size_t)i * 60;
@@ -491,6 +569,7 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         else dvx += dtx;
         if (tytz < -limy || tytz > limy) dvz += (tytz > 0.0f ? limy : -limy) * dty;
         else dvy += dty;
+        if constexpr (DEPTH && !FISHEYE) dvz += df;  // f = v.z
         // uv = ((ndc + 1) size - 1) / 2, ndc = h.xy / h.w
         const float dndcx = d[0] * (0.5f * (float)U.width), dndcy = d[1] * (0.5f * (float)U.height);
         const float dhx = dndcx * p_w, dhy = dndcy * p_w, dhw = -(dndcx * ndcx + dndcy * ndcy) * p_w;
@@ -510,6 +589,11 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
             }
             float ftx, fty, ftz;
             fisheye_grad(P.cam, F, FJ, cv.vx, cv.vy, vz, dJ, d[0], d[1], ftx, fty, ftz);
+            if constexpr (DEPTH) {  // f = d = |t|
+                ftx += (cv.vx / F.d) * df;
+                fty += (cv.vy / F.d) * df;
+                ftz += (vz / F.d) * df;
+            }
 #pragma unroll
             for (int k = 0; k < 3; k++) dp[k] = (vm[k * 4 + 0] * ftx + vm[k * 4 + 1] * fty) + vm[k * 4 + 2] * ftz;
         }
@@ -669,30 +753,32 @@ __global__ void __launch_bounds__(CR_THREADS) k_camera_reduce(const double* __re
     }
 }
 
-template <int MODE, bool ABSGRAD, bool BG>
-cudaError_t launch_blend_det(const BackwardParams& p, float3 bg, cudaStream_t s) {
-    constexpr int NACC = BW_NACC + (ABSGRAD ? BW_NABS : 0);
-    const size_t smem = (size_t)BW_WARPS * NACC * BW_DET_BATCH * sizeof(float);  // 36 KB, or 44 KB with ABSGRAD
-    cudaError_t e = cudaFuncSetAttribute(k_blend_backward<MODE, ABSGRAD, true, BG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+template <int MODE, bool ABSGRAD, bool BG, bool DEPTH>
+cudaError_t launch_blend_det(const BackwardParams& p, float3 bg, const DepthBackward* dp, cudaStream_t s) {
+    constexpr int NACC = bw_nacc<ABSGRAD, DEPTH>;
+    const size_t smem = (size_t)BW_WARPS * NACC * BW_DET_BATCH * sizeof(float);  // 36 KB, 44 KB with ABSGRAD, +4 KB with DEPTH
+    cudaError_t e = cudaFuncSetAttribute(k_blend_backward<MODE, ABSGRAD, true, BG, DEPTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    k_blend_backward<MODE, ABSGRAD, true, BG><<<p.num_tiles, BW_THREADS, smem, s>>>(bw_params<BG>(p, bg));
+    k_blend_backward<MODE, ABSGRAD, true, BG, DEPTH><<<p.num_tiles, BW_THREADS, smem, s>>>(bw_params<BG, DEPTH>(p, bg, dp));
     return cudaGetLastError();
 }
 
 template <int MODE, bool ABSGRAD>
-cudaError_t launch_blend_det(const BackwardParams& p, float3 bg, cudaStream_t s) {
-    return has_background(bg) ? launch_blend_det<MODE, ABSGRAD, true>(p, bg, s) : launch_blend_det<MODE, ABSGRAD, false>(p, bg, s);
+cudaError_t launch_blend_det(const BackwardParams& p, float3 bg, const DepthBackward* dp, cudaStream_t s) {
+    if (dp) return has_background(bg) ? launch_blend_det<MODE, ABSGRAD, true, true>(p, bg, dp, s) : launch_blend_det<MODE, ABSGRAD, false, true>(p, bg, dp, s);
+    return has_background(bg) ? launch_blend_det<MODE, ABSGRAD, true, false>(p, bg, dp, s) : launch_blend_det<MODE, ABSGRAD, false, false>(p, bg, dp, s);
 }
 
-template <bool BG>
-void launch_blend_backward(const BackwardParams& p, float3 bg, cudaStream_t s) {
+template <bool BG, bool DEPTH>
+void launch_blend_backward(const BackwardParams& p, float3 bg, const DepthBackward* dp, cudaStream_t s) {
     const bool density = p.density != nullptr;
+    const BwParams<BG, DEPTH> bp = bw_params<BG, DEPTH>(p, bg, dp);
     if (p.mode == GSB_MODE_EXACT) {
-        if (density) k_blend_backward<GSB_MODE_EXACT, true, false, BG><<<p.num_tiles, BW_THREADS, 0, s>>>(bw_params<BG>(p, bg));
-        else k_blend_backward<GSB_MODE_EXACT, false, false, BG><<<p.num_tiles, BW_THREADS, 0, s>>>(bw_params<BG>(p, bg));
+        if (density) k_blend_backward<GSB_MODE_EXACT, true, false, BG, DEPTH><<<p.num_tiles, BW_THREADS, 0, s>>>(bp);
+        else k_blend_backward<GSB_MODE_EXACT, false, false, BG, DEPTH><<<p.num_tiles, BW_THREADS, 0, s>>>(bp);
     } else {
-        if (density) k_blend_backward<GSB_MODE_FAST, true, false, BG><<<p.num_tiles, BW_THREADS, 0, s>>>(bw_params<BG>(p, bg));
-        else k_blend_backward<GSB_MODE_FAST, false, false, BG><<<p.num_tiles, BW_THREADS, 0, s>>>(bw_params<BG>(p, bg));
+        if (density) k_blend_backward<GSB_MODE_FAST, true, false, BG, DEPTH><<<p.num_tiles, BW_THREADS, 0, s>>>(bp);
+        else k_blend_backward<GSB_MODE_FAST, false, false, BG, DEPTH><<<p.num_tiles, BW_THREADS, 0, s>>>(bp);
     }
 }
 
@@ -752,7 +838,7 @@ __global__ void __launch_bounds__(96) k_background_reduce(const double* __restri
 // per (tile, entry); a stable sort of (compact id, list position) over the M entries groups each survivor's slots in tile
 // order, its last pass publishing each survivor's run; k_det_reduce sums every run in order.  Integer atomics remain
 // (the sort's counters and the runs' atomicMin), but their results do not depend on the order they land in.
-cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackward& d, unsigned grid, cudaStream_t s) {
+cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackward& d, const DepthBackward* dp, unsigned grid, cudaStream_t s) {
     const bool density = p.density != nullptr;
     cudaError_t e = cudaMemsetAsync(d.sc, 0, sizeof(SortCtl), s);
     if (e != cudaSuccess) return e;
@@ -779,30 +865,70 @@ cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackwar
     if ((e = launch_sort(sp, &passes, s)) != cudaSuccess) return e;
     if (passes == 0) return cudaErrorInvalidValue;  // key_bits >= 1: the runs come from the last pass
     if (p.num_tiles) {
-        if (p.mode == GSB_MODE_EXACT) e = density ? launch_blend_det<GSB_MODE_EXACT, true>(p, bg, s) : launch_blend_det<GSB_MODE_EXACT, false>(p, bg, s);
-        else e = density ? launch_blend_det<GSB_MODE_FAST, true>(p, bg, s) : launch_blend_det<GSB_MODE_FAST, false>(p, bg, s);
+        if (p.mode == GSB_MODE_EXACT) e = density ? launch_blend_det<GSB_MODE_EXACT, true>(p, bg, dp, s) : launch_blend_det<GSB_MODE_EXACT, false>(p, bg, dp, s);
+        else e = density ? launch_blend_det<GSB_MODE_FAST, true>(p, bg, dp, s) : launch_blend_det<GSB_MODE_FAST, false>(p, bg, dp, s);
         if (e != cudaSuccess) return e;
     }
     const uint32_t* sorted_pos = d.pos[passes & 1];
-    if (density) k_det_reduce<true><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs);
-    else k_det_reduce<false><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs);
+    double* ds = dp ? dp->scratch : nullptr;
+    if (dp) {
+        if (density) k_det_reduce<true, true><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs, ds);
+        else k_det_reduce<false, true><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs, ds);
+    } else {
+        if (density) k_det_reduce<true><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs, ds);
+        else k_det_reduce<false><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs, ds);
+    }
+    return cudaGetLastError();
+}
+
+// The vertex / camera part: k_preprocess_backward over the survivors (after the blend's sums and the density statistics).
+template <bool DEPTH>
+cudaError_t launch_preprocess_backward(const BackwardParams& p, bool antialiased, const gsb_camera_model* fisheye, const DepthBackward* dp,
+                                       unsigned grid, cudaStream_t s) {
+    auto with_depth = [&](const auto& base) {
+        if constexpr (DEPTH) return PbDepthParams<std::decay_t<decltype(base)>>{base, dp->scratch};
+        else return base;
+    };
+    if (fisheye) {  // vertex gradients only (checked above)
+        const auto fp = with_depth(BackwardFisheyeParams{p, *fisheye});
+        if (antialiased) k_preprocess_backward<false, true, true, DEPTH><<<grid, PB_THREADS, 0, s>>>(fp);
+        else k_preprocess_backward<false, false, true, DEPTH><<<grid, PB_THREADS, 0, s>>>(fp);
+        return cudaGetLastError();
+    }
+    const auto pp = with_depth(p);
+    if (!p.grad_ubo) {
+        if (antialiased) k_preprocess_backward<false, true, false, DEPTH><<<grid, PB_THREADS, 0, s>>>(pp);
+        else k_preprocess_backward<false, false, false, DEPTH><<<grid, PB_THREADS, 0, s>>>(pp);
+        return cudaGetLastError();
+    }
+    if (antialiased) k_preprocess_backward<true, true, false, DEPTH><<<grid, PB_THREADS, 0, s>>>(pp);
+    else k_preprocess_backward<true, false, false, DEPTH><<<grid, PB_THREADS, 0, s>>>(pp);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    k_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo);
     return cudaGetLastError();
 }
 
 }  // namespace
 
 cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det,
-                            const gsb_camera_model* fisheye) {
+                            const gsb_camera_model* fisheye, const DepthBackward* depth) {
     if (fisheye && p.grad_ubo) return cudaErrorInvalidValue;
     const bool density = p.density != nullptr;
     // grid-stride over N_v, which stays on the device: the grid comes from the SM count
     const unsigned grid = (unsigned)p.num_sms * 4u;
     if (det) {
-        cudaError_t e = launch_det_sums(p, background, *det, grid, s);
+        cudaError_t e = launch_det_sums(p, background, *det, depth, grid, s);
         if (e != cudaSuccess) return e;
     } else if (p.num_tiles) {
-        if (has_background(background)) launch_blend_backward<true>(p, background, s);  // a frame of gsb_set_background
-        else launch_blend_backward<false>(p, background, s);
+        const bool bg = has_background(background);  // a frame of gsb_set_background
+        if (depth) {
+            if (bg) launch_blend_backward<true, true>(p, background, depth, s);
+            else launch_blend_backward<false, true>(p, background, depth, s);
+        } else {
+            if (bg) launch_blend_backward<true, false>(p, background, depth, s);
+            else launch_blend_backward<false, false>(p, background, depth, s);
+        }
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
@@ -811,23 +937,8 @@ cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 ba
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
-    if (fisheye) {  // vertex gradients only (checked above)
-        const BackwardFisheyeParams fp{p, *fisheye};
-        if (antialiased) k_preprocess_backward<false, true, true><<<grid, PB_THREADS, 0, s>>>(fp);
-        else k_preprocess_backward<false, false, true><<<grid, PB_THREADS, 0, s>>>(fp);
-        return cudaGetLastError();
-    }
-    if (!p.grad_ubo) {
-        if (antialiased) k_preprocess_backward<false, true><<<grid, PB_THREADS, 0, s>>>(p);
-        else k_preprocess_backward<false, false><<<grid, PB_THREADS, 0, s>>>(p);
-        return cudaGetLastError();
-    }
-    if (antialiased) k_preprocess_backward<true, true><<<grid, PB_THREADS, 0, s>>>(p);
-    else k_preprocess_backward<true, false><<<grid, PB_THREADS, 0, s>>>(p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    k_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo);
-    return cudaGetLastError();
+    return depth ? launch_preprocess_backward<true>(p, antialiased, fisheye, depth, grid, s)
+                 : launch_preprocess_backward<false>(p, antialiased, fisheye, depth, grid, s);
 }
 
 uint32_t background_grad_rows(uint32_t height) { return std::min(height, BG_MAX_ROWS); }

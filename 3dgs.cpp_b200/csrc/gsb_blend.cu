@@ -72,7 +72,7 @@ constexpr int BLEND_WARPS = BLEND_THREADS / 32;
 struct __align__(16) StagedRec {  // 48 B: three 16-B slots = three LDS.128 per visited record
     float4 q0;  // ux uy -A/2 -B       (exact power-of-two / sign scalings of the conic: render.comp:66 becomes
     float4 q1;  // -C/2 opacity r g     ((-A/2 dx) dx + (-C/2 dy) dy) + ((-B) dx) dy, bit for bit)
-    float4 q2;  // b power_cut bits(index in batch) -
+    float4 q2;  // b power_cut bits(index in batch) depth (DEPTH; 0 otherwise)
 };
 
 // Bit w set <=> warp w's 8x8 pixel block may receive a contribution from this Gaussian (gsb_cull.cuh).
@@ -89,8 +89,9 @@ __device__ __forceinline__ uint32_t block_mask(float ux, float uy, float A, floa
 }
 
 // Per-pixel state of gsb_set_backward frames (k_blend<..., RECORD = true>): for each of the thread's two pixels, the
-// transmittance after its last contributor and that contributor's list position + 1 (0 = none).  The BG instantiations keep
-// the same state for their background term.  Empty otherwise, so the plain instantiations carry no trace of it.
+// transmittance after its last contributor and that contributor's list position + 1 (0 = none).  The BG and DEPTH
+// instantiations keep the same state for their background term and their alpha.  Empty otherwise, so the plain
+// instantiations carry no trace of it.
 template <bool ON>
 struct BlendRecord {
     float t0 = 1.0f, t1 = 1.0f;
@@ -116,6 +117,15 @@ struct BlendRecord<false> {
     __device__ __forceinline__ void store(const BlendParams&, bool, bool, uint32_t, uint32_t, uint32_t) const {}
 };
 
+// D of the thread's two pixels (k_blend<..., DEPTH = true>).  Empty otherwise: a new local, even unused, changes the
+// scheduling of the other instantiations.
+template <bool ON>
+struct DepthSum {
+    float d0 = 0.f, d1 = 0.f;
+};
+template <>
+struct DepthSum<false> {};
+
 // COARSE (gsb_set_tile_cull level 2): the list is that of a block of 2^cs x 2^cs tiles and every entry's key carries the mask
 // of the block's tiles inside the Gaussian's tile AABB.  Staging becomes a stream compaction: the CTA scans the list 128
 // entries at a time (keys + payloads only, coalesced), keeps the entries whose mask has this tile's bit -- in list order, so
@@ -127,7 +137,11 @@ struct BlendRecord<false> {
 // BG (gsb_set_background, a non-zero P.background): the pixels keep the same final transmittance (BlendRecord's note, stored
 // only when RECORD) and every colour channel is stored as c + T_final * bg (one multiply, one add, both rounded), in both
 // store paths.  A pixel no entry reaches keeps T_final = 1 and is stored as bg exactly.
-template <int MODE, bool STATS, bool COARSE, bool RECORD = false, bool BG = false>
+// DEPTH (gsb_render_depth, a non-null P.depth_alpha): the record's depth f (q2.w of the survivor record: view-space z, or the
+// distance d for a fisheye frame) is staged too, each pixel accumulates D = sum f alpha T like a colour channel (EXACT:
+// (f * alpha) * T and __fadd_rn, predicated like the colours; FAST: f * (alpha * T)) and keeps T_final (BlendRecord), and
+// (D, 1 - T_final) is stored as a float2 into P.depth_alpha with the band offset of the RGBA32F path.  The image is unchanged.
+template <int MODE, bool STATS, bool COARSE, bool RECORD = false, bool BG = false, bool DEPTH = false>
 __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(const __grid_constant__ BlendParams P) {
     static_assert(!(RECORD && COARSE), "the backward state is recorded on per-tile lists only");
     __shared__ StagedRec s_rec[BLEND_BATCH];
@@ -172,7 +186,8 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
     float T0 = in0 ? 1.0f : 0.0f, T1 = in1 ? 1.0f : 0.0f, ca0 = 0.f, ca1 = 0.f, cb0 = 0.f, cb1 = 0.f, cc0 = 0.f, cc1 = 0.f;
 #define BLEND_DONE (T0 == 0.0f && T1 == 0.0f)
     uint32_t used = 0, walked = 0, hits = 0, staged = 0;
-    BlendRecord<RECORD || BG> brec;
+    BlendRecord<RECORD || BG || DEPTH> brec;
+    DepthSum<DEPTH> dsum;
     const uint32_t rec_sh = (uint32_t)__cvta_generic_to_shared(&s_rec[0]);
     const uint32_t list_sh = (uint32_t)__cvta_generic_to_shared(&s_list[warp][0]);
 
@@ -271,7 +286,7 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
                     s_rec[li].q0 = make_float4(a.x, a.y, -0.5f * a.z, -a.w);
                     s_rec[li].q1 = make_float4(-0.5f * b.x, b.y, col.x, col.y);
                     // q2.z: position in the list relative to the batch's base offset (the consumed-entries statistic)
-                    s_rec[li].q2 = make_float4(col.z, cut, __uint_as_float(COARSE ? s_eidx[li] : li), 0.f);
+                    s_rec[li].q2 = make_float4(col.z, cut, __uint_as_float(COARSE ? s_eidx[li] : li), DEPTH ? col.w : 0.f);
                 }
                 s_mask[li] = (uint8_t)m;
             }
@@ -351,7 +366,13 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
                         cb1 = __fadd_rn(cb1, w1b);
                         cc1 = __fadd_rn(cc1, w1c);
                     }
-                    if constexpr (RECORD || BG) brec.note(ok0, ok1, tt0, tt1, base_off + __float_as_uint(q2.z) + 1u);
+                    if constexpr (DEPTH) {  // one more colour channel: the depth
+                        const float w0d = MODE == GSB_MODE_EXACT ? (q2.w * al0) * T0 : q2.w * (al0 * T0);
+                        const float w1d = MODE == GSB_MODE_EXACT ? (q2.w * al1) * T1 : q2.w * (al1 * T1);
+                        if (ok0) dsum.d0 = __fadd_rn(dsum.d0, w0d);
+                        if (ok1) dsum.d1 = __fadd_rn(dsum.d1, w1d);
+                    }
+                    if constexpr (RECORD || BG || DEPTH) brec.note(ok0, ok1, tt0, tt1, base_off + __float_as_uint(q2.z) + 1u);
                     if (in0k) T0 = ok0 ? tt0 : 0.0f;  // :88, or the break
                     if (in1k) T1 = ok1 ? tt1 : 0.0f;
                 }
@@ -366,6 +387,12 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
 #undef BLEND_DONE
     if (COARSE && seg_pending) mbar_wait(&s_bar, seg_parity);  // never leave with a bulk copy still writing this CTA's shared memory
     if constexpr (RECORD) brec.store(P, in0, in1, px, py0, py1);
+    if constexpr (DEPTH) {  // (D, A = 1 - T_final) into the band's depth buffer, rows as in the RGBA32F path below
+        unsigned char* band = static_cast<unsigned char*>(P.depth_alpha);
+        const uint32_t row = py0 - P.out_first_row;
+        if (in0) reinterpret_cast<float2*>(band + (size_t)row * P.depth_pitch_bytes)[px] = make_float2(dsum.d0, 1.0f - brec.t0);
+        if (in1) reinterpret_cast<float2*>(band + (size_t)(row + 4) * P.depth_pitch_bytes)[px] = make_float2(dsum.d1, 1.0f - brec.t1);
+    }
     if constexpr (BG) {  // what both store paths below write: c + T_final * bg
         ca0 = __fadd_rn(ca0, __fmul_rn(brec.t0, P.background[0]));
         cb0 = __fadd_rn(cb0, __fmul_rn(brec.t0, P.background[1]));
@@ -434,30 +461,30 @@ __global__ void __launch_bounds__(BLEND_THREADS, GSB_BLEND_MIN_BLOCKS) k_blend(c
     }
 }
 
-template <bool BG>
+template <bool BG, bool DEPTH>
 void launch_blend_as(const BlendParams& p, uint32_t blocks, cudaStream_t s) {
     if (p.coarse_shift) {
         if (p.stats) {
-            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, true, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
-            else k_blend<GSB_MODE_FAST, true, true, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, true, false, BG, DEPTH><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            else k_blend<GSB_MODE_FAST, true, true, false, BG, DEPTH><<<blocks, BLEND_THREADS, 0, s>>>(p);
         } else {
-            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, true, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
-            else k_blend<GSB_MODE_FAST, false, true, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, true, false, BG, DEPTH><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            else k_blend<GSB_MODE_FAST, false, true, false, BG, DEPTH><<<blocks, BLEND_THREADS, 0, s>>>(p);
         }
     } else if (p.record) {  // gsb_set_backward
         if (p.stats) {
-            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, false, true, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
-            else k_blend<GSB_MODE_FAST, true, false, true, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, false, true, BG, DEPTH><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            else k_blend<GSB_MODE_FAST, true, false, true, BG, DEPTH><<<blocks, BLEND_THREADS, 0, s>>>(p);
         } else {
-            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, false, true, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
-            else k_blend<GSB_MODE_FAST, false, false, true, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, false, true, BG, DEPTH><<<blocks, BLEND_THREADS, 0, s>>>(p);
+            else k_blend<GSB_MODE_FAST, false, false, true, BG, DEPTH><<<blocks, BLEND_THREADS, 0, s>>>(p);
         }
     } else if (p.stats) {
-        if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, false, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
-        else k_blend<GSB_MODE_FAST, true, false, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, true, false, false, BG, DEPTH><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        else k_blend<GSB_MODE_FAST, true, false, false, BG, DEPTH><<<blocks, BLEND_THREADS, 0, s>>>(p);
     } else {
-        if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, false, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
-        else k_blend<GSB_MODE_FAST, false, false, false, BG><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        if (p.mode == GSB_MODE_EXACT) k_blend<GSB_MODE_EXACT, false, false, false, BG, DEPTH><<<blocks, BLEND_THREADS, 0, s>>>(p);
+        else k_blend<GSB_MODE_FAST, false, false, false, BG, DEPTH><<<blocks, BLEND_THREADS, 0, s>>>(p);
     }
 }
 
@@ -467,8 +494,14 @@ cudaError_t launch_blend(const BlendParams& p, cudaStream_t s) {
     const uint32_t rows = p.tile_row_end - p.tile_row_begin;
     const uint32_t blocks = rows * p.tiles_x;
     if (blocks == 0) return cudaSuccess;
-    if (has_background(p.background)) launch_blend_as<true>(p, blocks, s);  // gsb_set_background
-    else launch_blend_as<false>(p, blocks, s);
+    const bool bg = has_background(p.background);  // gsb_set_background
+    if (p.depth_alpha) {  // gsb_render_depth
+        if (bg) launch_blend_as<true, true>(p, blocks, s);
+        else launch_blend_as<false, true>(p, blocks, s);
+    } else {
+        if (bg) launch_blend_as<true, false>(p, blocks, s);
+        else launch_blend_as<false, false>(p, blocks, s);
+    }
     return cudaGetLastError();
 }
 

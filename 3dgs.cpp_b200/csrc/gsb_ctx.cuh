@@ -70,7 +70,7 @@ struct Survivors {
 // gsb_set_backward_deterministic: the buffers behind DetBackward, allocated on first deterministic use, grown with the arena
 // and the scene, and freed with bw_record.
 struct DetBuffers {
-    DevArray<double> slots;  // 11 fp64 per arena entry (the blend's per-(tile, entry) partials)
+    DevArray<double> slots;  // 11 fp64 per arena entry (the blend's per-(tile, entry) partials), 12 once a depth backward ran
     DevArray<uint32_t> keys[2];
     DevArray<uint32_t> pos[2];
     DevArray<unsigned long long> status;
@@ -102,6 +102,7 @@ struct LastFrame {
     bool timers = false;     // recorded the stage events (gsb_get_stats may read them)
     bool recorded = false;   // its backward state is stored: per-pixel record and per-tile lists (gsb_set_backward, cs == 0)
     bool band = false;       // a band of tile rows, not the whole frame
+    bool depth = false;      // rendered by gsb_render_depth (gsb_render_backward_depth needs such a frame)
 };
 }  // namespace gsb
 using gsb::Control;
@@ -154,6 +155,7 @@ struct gsb_ctx {
     DevArray<unsigned long long> sort_status;  // [tiles][256] look-back words of the frame's sorts
     DevArray<uint2> ranges;
     DevArray<unsigned char> fb;   // staging frame of gsb_render to pageable host memory
+    DevArray<unsigned char> depth_fb;  // staging (D, A) band of gsb_render_depth to pageable host memory
 
     int mode = GSB_MODE_EXACT;
     bool debug = false;
@@ -190,6 +192,7 @@ struct gsb_ctx {
     DevArray<double> bw_scratch;    // n x 9 per-survivor fp64 accumulators of the blend backward (kept zero between calls)
     DevArray<double> bw_cam_partials;  // [4 * num_sms][GSB_UBO_WORDS] per-CTA fp64 partial sums of gsb_render_backward_camera
     DevArray<double> bw_abs;        // n x 2 per-survivor fp64 sums of |d u|, |d v| of gsb_render_backward_density (kept zero)
+    DevArray<double> bw_depth;      // n x 1 per-survivor fp64 dL/d depth of gsb_render_backward_depth (kept zero)
     bool bw_deterministic = false;  // gsb_set_backward_deterministic
     gsb::DetBuffers bw_det;
     DevArray<double> bg_partials;   // [background_grad_rows(H)][3] per-CTA fp64 partial sums of gsb_background_gradient
@@ -235,8 +238,10 @@ int plan_frame(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, 
 ProjectParams project_params(const gsb_ctx* ctx, const gsb_uniforms& ubo, uint32_t rb, uint32_t re);
 int enqueue_middle(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, cudaStream_t stream, bool events);
 int launch_middle_graph(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, cudaStream_t stream);
+// depth_out (gsb_render_depth): the band's (D, A) buffer, depth_pitch bytes per row, laid out like band_out; null for none
 int enqueue_blend(gsb_ctx* ctx, const FramePlan& fp, const Survivors& sv, uint32_t b0, uint32_t b1, void* band_out, size_t pitch,
-                  int fmt, cudaStream_t stream, void* const* peer_frames = nullptr, int num_peer_frames = 0);
+                  int fmt, cudaStream_t stream, void* const* peer_frames = nullptr, int num_peer_frames = 0, void* depth_out = nullptr,
+                  size_t depth_pitch = 0);
 int enqueue_tail(gsb_ctx* ctx, const FramePlan& fp, const gsb_uniforms& ubo, cudaStream_t stream);
 int check_image(gsb_ctx* ctx, const gsb_uniforms* ubo, int fmt);
 int check_render_args(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t& rb, uint32_t& re, const void* out, size_t& pitch, int fmt);

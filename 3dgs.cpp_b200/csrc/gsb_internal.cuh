@@ -161,6 +161,11 @@ struct BlendParams {
     // gsb_set_background: every pixel is stored as c + T_final * background (all zeros: the default kernels, no term).
     // Appended last so the other fields keep their offsets.
     float background[3];
+    // gsb_render_depth: per pixel of the band, (D, A) as a float2, depth_pitch_bytes apart, pixel row `out_first_row` at
+    // depth_alpha + 0 (never with num_peers).  Null: no depth output (the default kernels).  Appended last so the other fields
+    // keep their offsets.
+    void* depth_alpha;
+    size_t depth_pitch_bytes;
 };
 cudaError_t launch_blend(const BlendParams& p, cudaStream_t s);
 
@@ -217,8 +222,15 @@ struct DetBackward {
 // its own after BackwardParams, not a field of it: a larger BackwardParams would move the arguments that follow it in
 // k_det_reduce.
 // fisheye: the frame's gsb_set_camera_model lens (vertex gradients only: p.grad_ubo must be null), null for a pinhole frame.
+// depth: gsb_render_backward_depth's upstream dL/d(D, A) and its per-survivor scratch (p.grad_image may then be null); null for
+// the colour-only entries.
+struct DepthBackward {
+    const float2* grad;  // H x W (dL/dD, dL/dA), pitch bytes apart
+    size_t pitch;
+    double* scratch;     // n x 1 fp64 dL/df per survivor: zero on entry, zero again on exit
+};
 cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det = nullptr,
-                            const gsb_camera_model* fisheye = nullptr);
+                            const gsb_camera_model* fisheye = nullptr, const DepthBackward* depth = nullptr);
 // gsb_background_gradient: out[c] = sum over the W x H pixels of T_final(p) grad_image(p)[c], from the recorded frame's
 // (bits(T), last) words.  fp64 products and sums in an order fixed by W and H (background_grad_rows(H) per-CTA partials,
 // then one CTA), no atomics.  partials holds 3 doubles per row of background_grad_rows(H).

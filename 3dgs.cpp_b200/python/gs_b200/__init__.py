@@ -45,6 +45,8 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     # reverse mode
     "gsb_set_backward", "gsb_render_backward", "gsb_render_backward_camera", "gsb_render_backward_density",
     "gsb_set_backward_deterministic", "gsb_background_gradient",
+    # rendered depth and alpha with their gradients
+    "gsb_render_depth", "gsb_render_backward_depth",
     # training loss, optimizer step and initialisation from a point cloud
     "gsb_image_loss", "gsb_adam_step", "gsb_init_from_points",
     # Mip-Splatting's 3D smoothing filter
@@ -212,6 +214,9 @@ lib.gsb_render_backward.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp]
 lib.gsb_render_backward_camera.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp]
 lib.gsb_render_backward_density.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp]
 lib.gsb_background_gradient.argtypes = [_vp, _vp, C.c_size_t, _vp, _vp]
+lib.gsb_render_depth.argtypes = [_vp, C.POINTER(Uniforms), C.c_uint32, C.c_uint32, _vp, C.c_size_t, C.c_int, C.c_int, _vp,
+                                 C.c_size_t, _vp]
+lib.gsb_render_backward_depth.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, C.c_size_t, _vp, _vp, _vp, _vp]
 lib.gsb_image_loss.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_float, _vp,
                                C.c_size_t, _vp, _vp]
 lib.gsb_bilagrid_apply.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_uint32, C.c_uint32, C.c_uint32,
@@ -462,6 +467,7 @@ class Context:
         self.h = handle
         self.device = device
         self.frames = 0  # frames rendered through this wrapper (render_torch checks it between forward and backward)
+        self._depth_frame_id = -1  # the value of `frames` after the last gsb_render_depth frame
         self._background = None  # the last set_background colour (render_torch restores it after a frame of its own)
         self.camera = None  # the last set_camera_model lens (None: pinhole)
 
@@ -566,6 +572,23 @@ class Context:
         self._ck(lib.gsb_render(self.h, C.byref(u), rb, re, out.ctypes.data, 0, MEM_HOST, fmt, None))
         return out
 
+    def render_depth(self, u: Uniforms, fmt=FORMAT_RGBA32F, rows=None):
+        """gsb_render_depth to HOST numpy arrays: (image, depth_alpha), the image as render() gives it and depth_alpha an
+        (rows, W, 2) float32 array of (D, A) per pixel: D = sum f alpha T (f the view-space z, or the distance for a fisheye
+        camera) and A = 1 - T_final.  Expected depth is D / A."""
+        rb, re, nrows = self.band_rows(u, rows)
+        out = np.empty((nrows, u.width, 4), np.float32 if fmt == FORMAT_RGBA32F else np.uint8)
+        da = np.empty((nrows, u.width, 2), np.float32)
+        self.frames += 1
+        self._ck(lib.gsb_render_depth(self.h, C.byref(u), rb, re, out.ctypes.data, 0, MEM_HOST, fmt, da.ctypes.data, 0, None))
+        self._depth_frame_id = self.frames
+        return out, da
+
+    @property
+    def _depth_frame(self):
+        """The last frame rendered through this wrapper came from gsb_render_depth, and nothing changed since."""
+        return self._depth_frame_id == self.frames
+
     def render_into(self, u: Uniforms, out_ptr: int, fmt=FORMAT_RGBA32F, rows=None, stream=None, sync=True):
         """Render into DEVICE memory at out_ptr (e.g. tensor.data_ptr())."""
         rb, re, _ = self.band_rows(u, rows)
@@ -600,9 +623,13 @@ class Context:
                        grad_uniforms_ptr, density_ptr)
 
     def _backward(self, vertices_ptr, grad_image_ptr, grad_vertices_ptr, stream, row_pitch_bytes=0, grad_uniforms_ptr=None,
-                  density_ptr=None):
-        """render_backward with `stream` already the C ABI's cudaStream_t argument."""
-        if density_ptr is not None:
+                  density_ptr=None, grad_depth_alpha_ptr=None):
+        """render_backward with `stream` already the C ABI's cudaStream_t argument.  With grad_depth_alpha_ptr (H x W float2
+        of device memory, dL/d(D, A) of a render_depth frame), gsb_render_backward_depth; grad_image_ptr may then be None."""
+        if grad_depth_alpha_ptr is not None:
+            self._ck(lib.gsb_render_backward_depth(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_depth_alpha_ptr, 0,
+                                                   grad_vertices_ptr, grad_uniforms_ptr, density_ptr, stream))
+        elif density_ptr is not None:
             self._ck(lib.gsb_render_backward_density(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
                                                      grad_uniforms_ptr, density_ptr, stream))
         elif grad_uniforms_ptr is None:
@@ -611,15 +638,22 @@ class Context:
             self._ck(lib.gsb_render_backward_camera(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
                                                     grad_uniforms_ptr, stream))
 
-    def _render_whole_frame(self, u: Uniforms, device):
-        """The whole frame of u, recorded while gsb_set_backward is on, as a new tensor on torch's current stream."""
+    def _render_whole_frame(self, u: Uniforms, device, depth=False):
+        """The whole frame of u, recorded while gsb_set_backward is on, as a new tensor on torch's current stream; with
+        depth, (image, depth_alpha) from gsb_render_depth, depth_alpha an (H, W, 2) tensor."""
         import torch
 
         img = torch.empty((u.height, u.width, 4), dtype=torch.float32, device=device)
         self.frames += 1
-        self._ck(lib.gsb_render(self.h, C.byref(u), 0, ALL_ROWS, img.data_ptr(), 0, MEM_DEVICE, FORMAT_RGBA32F,
-                                _torch_stream_arg(torch.cuda.current_stream(device))))
-        return img
+        stream = _torch_stream_arg(torch.cuda.current_stream(device))
+        if not depth:
+            self._ck(lib.gsb_render(self.h, C.byref(u), 0, ALL_ROWS, img.data_ptr(), 0, MEM_DEVICE, FORMAT_RGBA32F, stream))
+            return img
+        da = torch.empty((u.height, u.width, 2), dtype=torch.float32, device=device)
+        self._ck(lib.gsb_render_depth(self.h, C.byref(u), 0, ALL_ROWS, img.data_ptr(), 0, MEM_DEVICE, FORMAT_RGBA32F,
+                                      da.data_ptr(), 0, stream))
+        self._depth_frame_id = self.frames
+        return img, da
 
     def image_loss(self, image, target, lambda_dssim=0.2, grad_image=None, stream=None):
         """gsb_image_loss on torch tensors: the photometric loss (1 - lambda) L1 + lambda (1 - SSIM) of `image` against
@@ -896,8 +930,9 @@ def _render_fn():
 
         class RenderFn(torch.autograd.Function):
             @staticmethod
-            def forward(fctx, ctx, vertices, u, ubo, density, background):
+            def forward(fctx, ctx, vertices, u, ubo, density, background, depth):
                 v = vertices.detach().contiguous()
+                fctx.depth = bool(depth)
                 _check_density("render_torch", density, v)
                 fctx.density = density
                 if ubo is not None:  # the camera's float fields come from the tensor, the frame size from u
@@ -909,25 +944,29 @@ def _render_fn():
                 torch.cuda.current_stream(v.device).synchronize()  # the upload runs on the context's stream: v must be complete
                 ctx.upload(v)
                 if background is None:
-                    img = ctx._render_whole_frame(u, v.device)
+                    out = ctx._render_whole_frame(u, v.device, fctx.depth)
                 else:  # this frame over the tensor's colour; the context's own setting is restored after it
                     fctx.bg_like = (background.dtype, background.device)
                     previous = ctx._background
                     ctx.set_background(background.detach().to("cpu", torch.float32).reshape(3).tolist())
                     try:
-                        img = ctx._render_whole_frame(u, v.device)
+                        out = ctx._render_whole_frame(u, v.device, fctx.depth)
                     finally:
                         ctx.set_background(previous)
                 fctx.gs_ctx, fctx.frame, fctx.vertices = ctx, ctx.frames, v
-                return img
+                return out
 
             @staticmethod
-            def backward(fctx, grad_img):
+            def backward(fctx, grad_img, grad_da=None):
                 ctx = fctx.gs_ctx
                 if ctx.frames != fctx.frame:
                     raise RuntimeError("render_torch: another frame was rendered on this context between forward and backward")
                 v = fctx.vertices
                 g = grad_img.detach().to(torch.float32).contiguous()
+                gda = None  # depth frames: dL/d(D, A), zeros where torch gave none
+                if fctx.depth:
+                    gda = (torch.zeros(tuple(g.shape[:2]) + (2,), dtype=torch.float32, device=v.device) if grad_da is None
+                           else grad_da.detach().to(torch.float32).contiguous())
                 need_v, need_ubo, need_bg = fctx.needs_input_grad[1], fctx.needs_input_grad[3], fctx.needs_input_grad[5]
                 grad_v = torch.empty_like(v) if need_v else None
                 grad_ubo = grad_bg = None
@@ -939,20 +978,21 @@ def _render_fn():
                 if need_v or need_ubo:
                     ctx._backward(v.data_ptr(), g.data_ptr(), grad_v.data_ptr() if need_v else None, stream,
                                   grad_uniforms_ptr=gu.data_ptr() if need_ubo else None,
-                                  density_ptr=None if fctx.density is None else fctx.density.data_ptr())
+                                  density_ptr=None if fctx.density is None else fctx.density.data_ptr(),
+                                  grad_depth_alpha_ptr=None if gda is None else gda.data_ptr())
                 if need_ubo:
                     dtype, device = fctx.ubo_like
                     grad_ubo = gu[UBO_FLOAT_WORDS].to(device=device, dtype=dtype)
                 if need_bg:  # sum_p T_final g, on the same stream
                     dtype, device = fctx.bg_like
                     grad_bg = ctx.background_gradient(g, torch.cuda.current_stream(v.device)).to(device=device, dtype=dtype)
-                return None, grad_v, None, grad_ubo, None, grad_bg
+                return None, grad_v, None, grad_ubo, None, grad_bg, None
 
         _RenderFn = RenderFn
     return _RenderFn
 
 
-def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, background=None):
+def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, background=None, depth=False):
     """Differentiable frame: vertices is a CUDA float32 tensor (n, 60) of GSScene::Vertex records (activated parameters, as
     gsb_scene_upload takes them).  Uploads it from device memory, renders the whole frame as an (H, W, 4) RGBA32F tensor and,
     on backward, returns dL/dvertices through gsb_render_backward.  Turns gsb_set_backward on for `ctx`.  The frame on the
@@ -976,8 +1016,14 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, 
     torch's default settings backward takes the atomic path, whose results may differ in the last bit from run to run.
 
     The frame is projected through the context's camera model (Context.set_camera_model); ubo= on a fisheye context raises
-    ValueError."""
-    return _render_fn().apply(ctx, vertices, u, ubo, density, background)
+    ValueError.
+
+    depth=True renders with gsb_render_depth and returns (img, depth_alpha), depth_alpha an (H, W, 2) tensor of (D, A):
+    D = sum f alpha T, f the view-space z (the distance from the camera for a fisheye model), and A = 1 - T_final, the
+    accumulated opacity.  Backward then takes dL/dimg and dL/d(depth_alpha), either of them unused (zero), through
+    gsb_render_backward_depth; it composes with ubo=, density=, background= and the deterministic mode.  Expected depth is
+    D / A.clamp_min(1e-10), inverse depth its reciprocal, and a mask loss reads A directly."""
+    return _render_fn().apply(ctx, vertices, u, ubo, density, background, depth)
 
 
 _LossFn = None
@@ -1346,34 +1392,44 @@ class SceneAdam:
         torch.cuda.current_stream(self.vertices.device).synchronize()  # the upload runs on the context's own stream
         self.ctx.upload(self.vertices)
 
-    def render(self, u: Uniforms):
+    def render(self, u: Uniforms, depth=False):
         """The resident scene's frame of u as an (H, W, 4) float32 tensor, rendered on torch's current stream with the
-        backward state recorded, over the optimizer's background (fixed or a fresh random colour).  No upload."""
+        backward state recorded, over the optimizer's background (fixed or a fresh random colour).  No upload.  depth=True:
+        (image, depth_alpha) from gsb_render_depth (see render_torch), for step(..., grad_depth_alpha=)."""
         import torch
 
         if self._generator is not None:
             self.background = torch.rand(3, generator=self._generator).tolist()
         if self.background is not None:
             self.ctx.set_background(self.background)
-        return self.ctx._render_whole_frame(u, self.vertices.device)
+        return self.ctx._render_whole_frame(u, self.vertices.device, depth)
 
-    def step(self, grad_image, density=None, opacity_reg=0.0, scale_reg=0.0):
+    def step(self, grad_image, density=None, opacity_reg=0.0, scale_reg=0.0, grad_depth_alpha=None):
         """One training step from dL/d(the last render()'s image), an (H, W, 4) float32 tensor: gsb_render_backward into
         `grad` (gsb_render_backward_density, accumulating into `density`, an (n, 4) float32 tensor, when given), then
         gsb_adam_step.  Everything runs on torch's current stream; nothing waits on the host.
 
         opacity_reg, scale_reg: 3DGS-MCMC's regularisers opacity_reg * mean(opacity) + scale_reg * mean(scale) (the mean
         over the n opacities and the 3 n scales), whose gradient opacity_reg / n and scale_reg / (3 n) is added to `grad`'s
-        columns 7 and 4-6 before the Adam step (gsplat uses 0.01 for both).  At 0, nothing is added."""
+        columns 7 and 4-6 before the Adam step (gsplat uses 0.01 for both).  At 0, nothing is added.
+
+        grad_depth_alpha: dL/d(depth_alpha) of the last render(u, depth=True), an (H, W, 2) float32 tensor, trained through
+        gsb_render_backward_depth; grad_image may then be None (no colour loss).  ValueError if the last render had no depth."""
         import torch
 
         ctx, v = self.ctx, self.vertices
-        g = grad_image.detach().to(torch.float32).contiguous()
+        if grad_depth_alpha is not None and not ctx._depth_frame:
+            raise ValueError("SceneAdam.step: grad_depth_alpha needs a frame of render(u, depth=True)")
+        if grad_image is None and grad_depth_alpha is None:
+            raise ValueError("SceneAdam.step: no gradient (grad_image and grad_depth_alpha are both None)")
+        g = None if grad_image is None else grad_image.detach().to(torch.float32).contiguous()
+        gda = None if grad_depth_alpha is None else grad_depth_alpha.detach().to(torch.float32).contiguous()
         stream = _torch_stream_arg(torch.cuda.current_stream(v.device))
         ctx.set_backward_deterministic(torch.are_deterministic_algorithms_enabled())
         _check_density("SceneAdam.step", density, v)
-        ctx._backward(v.data_ptr(), g.data_ptr(), self.grad.data_ptr(), stream,
-                      density_ptr=None if density is None else density.data_ptr())
+        ctx._backward(v.data_ptr(), None if g is None else g.data_ptr(), self.grad.data_ptr(), stream,
+                      density_ptr=None if density is None else density.data_ptr(),
+                      grad_depth_alpha_ptr=None if gda is None else gda.data_ptr())
         n = v.shape[0]
         if opacity_reg:
             self.grad[:, 7] += opacity_reg / n

@@ -242,6 +242,27 @@ int gsb_reserve_instances(gsb_ctx *ctx, uint64_t capacity);
 int gsb_render(gsb_ctx *ctx, const gsb_uniforms *ubo, uint32_t tile_row_begin, uint32_t tile_row_end,
                void *out, size_t row_pitch_bytes, gsb_memory out_mem, gsb_format fmt, void *stream);
 
+/* gsb_render plus two per-pixel outputs for depth and mask supervision: depth_alpha receives the same rows as `out`
+ * (the band of tile rows [tile_row_begin, tile_row_end)), W float2 (D, A) per row, depth_pitch_bytes apart (0 = tight,
+ * 8 W), in the same memory kind as `out` (out_mem).  For a pixel whose contributors, in list order, are i = 1..k -- the
+ * frame's own set: alpha_i = min(0.99, .), the alpha < 1/255 and power tests and the T' < 1e-4 break -- with T_i the
+ * transmittance in front of i:
+ *   D = sum_i f_i alpha_i T_i   f_i the Gaussian's depth key: view-space z for a pinhole frame, the distance |t| from the
+ *                               camera for a fisheye frame (the only depth that stays monotone past 180 degrees, where
+ *                               visible Gaussians have z < 0).  GSB_MODE_EXACT accumulates D like a colour channel, op for op:
+ *                               D = D + (f * alpha) * T, each op rounded; GSB_MODE_FAST forms f * (alpha * T).
+ *   A = 1 - T_final             one fp32 subtraction; T_final is the transmittance the frame records, the T that
+ *                               gsb_background_gradient uses.
+ * A pixel no entry reaches has D = 0 and A = 0.  Expected depth is D / A and inverse depth A / D, formed by the caller.
+ * The image is bit for bit gsb_render's (its A channel stays 1), and with gsb_set_backward on the frame is recorded as
+ * gsb_render records it (and noted as a depth frame for gsb_render_backward_depth).  Every tile-cull level, graph replay,
+ * gsb_set_antialiased, gsb_set_background and both camera models apply.  The same error codes as gsb_render, and also
+ * GSB_ERR_INVALID for a NULL depth_alpha, a depth_pitch_bytes below 8 W or not a multiple of 8, a depth_alpha not 8-byte
+ * aligned, or a sharded or group context. */
+int gsb_render_depth(gsb_ctx *ctx, const gsb_uniforms *ubo, uint32_t tile_row_begin, uint32_t tile_row_end, void *out,
+                     size_t row_pitch_bytes, gsb_memory out_mem, gsb_format fmt, void *depth_alpha, size_t depth_pitch_bytes,
+                     void *stream);
+
 /* Enqueue-only variant for pipelined callers (bench e2e): never synchronises, never regrows;
  * overflow is reported by the next gsb_get_stats()/gsb_render().  out must be device memory. */
 int gsb_render_async(gsb_ctx *ctx, const gsb_uniforms *ubo, uint32_t tile_row_begin,
@@ -308,6 +329,24 @@ int gsb_render_backward_camera(gsb_ctx *ctx, const float *vertices, const float 
  *                  Culled Gaussians' rows are not touched. */
 int gsb_render_backward_density(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,
                                 float *grad_vertices, gsb_uniforms *grad_uniforms, float *density, void *stream);
+
+/* The backward pass of a gsb_render_depth frame, with gradients of its depth D and alpha A besides the image's: the
+ * arguments, preconditions and error codes of gsb_render_backward_density, except that
+ *   grad_image        may be NULL: no colour gradient (zero)
+ *   grad_depth_alpha  device memory, H x W float2 (dL/dD, dL/dA), depth_pitch_bytes apart (0 = tight, 8 W); required
+ *   density           may be NULL (no statistics)
+ * and GSB_ERR_INVALID also when the last frame was not rendered by gsb_render_depth, or for a depth_pitch_bytes below 8 W
+ * or not a multiple of 8 or a grad_depth_alpha not 8-byte aligned.  A fisheye frame has no camera gradient here either.
+ * The chain rule is exact for the frame's D and A: through every contributor's alpha (A is a colour channel of value 1 over
+ * a background of 0, D one of value f over 0) and through f to the position: f = z of the view matrix's row 2 for a pinhole
+ * frame (grad_uniforms' view_mat row 2 then includes dL/df (p, 1)), f = |t| for a fisheye frame.  density column 0 and 1
+ * include the depth and alpha terms of dL/duv.  Zero depth and alpha gradients give gsb_render_backward_density's words
+ * (a -0 may become +0); gsb_set_backward_deterministic applies, and its first depth call grows the per-entry slots by 8 B.
+ * gsb_render_backward and gsb_background_gradient of a depth frame give the words they give for the same frame rendered by
+ * gsb_render. */
+int gsb_render_backward_depth(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,
+                              const float *grad_depth_alpha, size_t depth_pitch_bytes, float *grad_vertices,
+                              gsb_uniforms *grad_uniforms, float *density, void *stream);
 
 /* dL/d(background) of the last frame (gsb_set_background): grad_background (device, 3 floats) is OVERWRITTEN with
  * sum over the W x H pixels p of T_final(p) g(p), g from grad_image (as for gsb_render_backward: H x W float4,
