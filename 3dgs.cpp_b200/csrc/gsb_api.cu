@@ -1000,10 +1000,10 @@ int gsb_set_backward_deterministic(gsb_ctx* ctx, int enabled) {
 }
 
 // The buffers of the deterministic reduction for the current arena capacity and scene size (first use, then growth only).
-static int ensure_det_buffers(gsb_ctx* ctx, uint64_t n, bool depth) {
+static int ensure_det_buffers(gsb_ctx* ctx, uint64_t n, uint64_t slot_columns) {
     DetBuffers& d = ctx->bw_det;
     const uint64_t cap = ctx->capacity;
-    CK(d.slots.grow(cap * (depth ? 12 : 11)));  // the depth backward's slots have one more column
+    CK(d.slots.grow(cap * slot_columns));
     CK(d.keys[0].grow(cap));
     CK(d.keys[1].grow(cap));
     CK(d.pos[0].grow(cap));
@@ -1031,14 +1031,69 @@ static int check_recorded_frame(gsb_ctx* ctx, int no_frame, const char* fn) {
     return GSB_OK;
 }
 
-// The checks and the launch shared by gsb_render_backward, gsb_render_backward_camera, gsb_render_backward_density and
-// gsb_render_backward_depth (fn names the entry in messages).  grad_ubo == nullptr: no camera gradient; grad_vertices ==
+// The last recorded frame's state as gsb_features.cu reads it.
+static FeatureParams feature_frame_params(gsb_ctx* ctx, const float* features, uint32_t channels) {
+    const LastFrame& f = ctx->frame;
+    FeatureParams p{};
+    p.recs = ctx->recs;
+    p.vals = ctx->vals[f.plan.fin];
+    p.ranges = ctx->ranges;
+    p.record = ctx->bw_record;
+    p.ctl = ctx->ctl;
+    p.width = f.ubo.width;
+    p.height = f.ubo.height;
+    p.tiles_x = f.plan.tiles_x;
+    p.num_tiles = f.plan.T;
+    p.mode = f.mode;
+    p.num_sms = ctx->num_sms;
+    p.features = features;
+    p.channels = channels;
+    return p;
+}
+
+// The map's row pitch: 0 = tight (4 C W); GSB_ERR_INVALID below that or not a multiple of 4.
+static bool feature_pitch(const LastFrame& f, uint32_t channels, size_t& pitch) {
+    const size_t tight = (size_t)f.ubo.width * channels * sizeof(float);
+    if (pitch == 0) pitch = tight;
+    return pitch >= tight && pitch % sizeof(float) == 0;
+}
+
+int gsb_render_features(gsb_ctx* ctx, const float* features, uint32_t channels, float* feature_map, size_t pitch, void* stream) {
+    if (!ctx) return GSB_ERR_INVALID;
+    const char* fn = "gsb_render_features";
+    auto bad = [&](const char* what) { return fail(ctx, GSB_ERR_INVALID, (std::string(fn) + ": " + what).c_str()); };
+    if (ctx->shard) return bad("sharded and group contexts have no feature maps");
+    if (!ctx->pos_op) return fail(ctx, GSB_ERR_NO_SCENE, (std::string(fn) + ": no scene uploaded").c_str());
+    CK(cudaSetDevice(ctx->device));
+    const int rc = check_recorded_frame(ctx, GSB_ERR_NO_SCENE, fn);
+    if (rc != GSB_OK) return rc;
+    if (!features || !feature_map) return bad("null argument");
+    if (channels < 1 || channels > GSB_MAX_FEATURE_CHANNELS) return bad("channels outside [1, 128]");
+    if (!feature_pitch(ctx->frame, channels, pitch)) return bad("bad feature row pitch");
+    if (reinterpret_cast<uintptr_t>(features) % 4 || reinterpret_cast<uintptr_t>(feature_map) % 4) return bad("array not aligned to 4 B");
+    FeatureParams p = feature_frame_params(ctx, features, channels);
+    p.map = feature_map;
+    p.map_pitch = pitch;
+    CK(launch_render_features(p, stream_or_own(ctx, stream)));
+    return GSB_OK;
+}
+
+// gsb_render_backward_features' feature arguments for render_backward, checked by the entry.
+struct FeatureArgs {
+    const float* features;
+    uint32_t channels;
+    const float* grad_map;
+    size_t pitch;
+    float* grad_features;
+};
+// The checks and the launch shared by gsb_render_backward, gsb_render_backward_camera, gsb_render_backward_density,
+// gsb_render_backward_depth and gsb_render_backward_features (fn names the entry in messages).  grad_ubo == nullptr: no camera gradient; grad_vertices ==
 // nullptr: no scene gradient (each entry's args_ok says which may be null).  density != nullptr: also accumulate the density
 // statistics into it.  grad_depth != nullptr (gsb_render_backward_depth): the frame must have depth, and grad_image may be
-// null (no colour gradient).
+// null (no colour gradient).  feat != nullptr (gsb_render_backward_features): also the feature map's gradient.
 static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const float* vertices, const float* grad_image, size_t pitch,
                            float* grad_vertices, gsb_uniforms* grad_ubo, float* density, void* stream, const float* grad_depth = nullptr,
-                           size_t depth_pitch = 0) {
+                           size_t depth_pitch = 0, const FeatureArgs* feat = nullptr) {
     if (!ctx) return GSB_ERR_INVALID;
     auto msg = [&](const char* what) { return std::string(fn) + ": " + what; };
     if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, msg("sharded contexts have no backward pass").c_str());
@@ -1051,6 +1106,8 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     const LastFrame& f = ctx->frame;
     const bool fisheye = f.camera.kind == GSB_CAMERA_FISHEYE;
     if (fisheye && grad_ubo) return fail(ctx, GSB_ERR_INVALID, msg("a fisheye frame has no camera gradient").c_str());
+    if (feat && density && !grad_vertices && !grad_ubo)
+        return fail(ctx, GSB_ERR_INVALID, msg("density needs grad_vertices or grad_uniforms").c_str());
     const size_t tight = (size_t)f.ubo.width * sizeof(float4);
     if (pitch == 0) pitch = tight;
     if (grad_image && (pitch < tight || pitch % sizeof(float4) != 0)) return fail(ctx, GSB_ERR_INVALID, msg("bad row pitch").c_str());
@@ -1073,15 +1130,21 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
         rc = grow_zeroed(ctx, ctx->bw_depth, n, "ctx->bw_depth");
         if (rc != GSB_OK) return rc;
     }
+    const bool det = ctx->bw_deterministic;
+    if (feat && feat->grad_features && !det) {  // zeroed once here; k_feature_flush returns every entry it reads to zero
+        rc = grow_zeroed(ctx, ctx->bw_feat, n * 16, "ctx->bw_feat");
+        if (rc != GSB_OK) return rc;
+    }
     if (grad_ubo)  // one row per CTA of k_preprocess_backward (4 per SM), fully overwritten by each call
         CK(ctx->bw_cam_partials.grow((uint64_t)ctx->num_sms * 4 * GSB_UBO_WORDS));
-    const bool det = ctx->bw_deterministic;
-    if (det) {
-        rc = ensure_det_buffers(ctx, n, grad_depth != nullptr);
+    if (det) {  // the depth backward's slots have one more column; the feature pass's 8 + its chunk width
+        const uint64_t cols = std::max<uint64_t>(grad_depth ? 12 : 11, feat ? 8 + feature_chunk(feat->channels) : 0);
+        rc = ensure_det_buffers(ctx, n, cols);
         if (rc != GSB_OK) return rc;
     }
     cudaStream_t s = stream_or_own(ctx, stream);
     if (grad_vertices) CK(cudaMemsetAsync(grad_vertices, 0, (size_t)n * 60 * sizeof(float), s));
+    if (feat && feat->grad_features) CK(cudaMemsetAsync(feat->grad_features, 0, (size_t)n * feat->channels * sizeof(float), s));
     if (n == 0) {
         if (grad_ubo) CK(cudaMemsetAsync(grad_ubo, 0, sizeof(gsb_uniforms), s));
         return GSB_OK;
@@ -1113,8 +1176,17 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     const float3 bg = make_float3(f.background[0], f.background[1], f.background[2]);  // the frame's, not the current setting
     const DepthBackward depth{reinterpret_cast<const float2*>(grad_depth), depth_pitch, ctx->bw_depth.p};
     const DepthBackward* dp = grad_depth ? &depth : nullptr;
+    FeatureParams fp{};
+    if (feat) {
+        fp = feature_frame_params(ctx, feat->features, feat->channels);
+        fp.grad_map = feat->grad_map;
+        fp.grad_pitch = feat->pitch;
+        fp.grad_features = feat->grad_features;
+        fp.feat_scratch = feat->grad_features && !det ? ctx->bw_feat.p : nullptr;
+    }
+    const FeatureParams* fpp = feat ? &fp : nullptr;
     if (!det) {
-        CK(launch_backward(bp, f.antialiased, bg, s, nullptr, fisheye ? &f.camera : nullptr, dp));
+        CK(launch_backward(bp, f.antialiased, bg, s, nullptr, fisheye ? &f.camera : nullptr, dp, fpp));
         return GSB_OK;
     }
     const DetBuffers& d = ctx->bw_det;
@@ -1130,7 +1202,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     db.status_tiles = (uint32_t)(d.status.count / 256);
     db.m_hint = quantise_hint(ctx->m_hint);
     db.key_bits = std::max<uint32_t>(bits_for((uint32_t)n), 1u);  // compact ids < N_v <= n
-    CK(launch_backward(bp, f.antialiased, bg, s, &db, fisheye ? &f.camera : nullptr, dp));
+    CK(launch_backward(bp, f.antialiased, bg, s, &db, fisheye ? &f.camera : nullptr, dp, fpp));
     return GSB_OK;
 }
 
@@ -1155,6 +1227,24 @@ int gsb_render_backward_depth(gsb_ctx* ctx, const float* vertices, const float* 
                               size_t depth_pitch, float* grad_vertices, gsb_uniforms* grad_uniforms, float* density, void* stream) {
     return render_backward(ctx, "gsb_render_backward_depth", vertices && grad_depth_alpha && (grad_vertices || grad_uniforms), vertices,
                            grad_image, pitch, grad_vertices, grad_uniforms, density, stream, grad_depth_alpha, depth_pitch);
+}
+
+int gsb_render_backward_features(gsb_ctx* ctx, const float* vertices, const float* grad_image, size_t pitch, const float* grad_depth_alpha,
+                                 size_t depth_pitch, const float* features, uint32_t channels, const float* grad_feature_map,
+                                 size_t feature_pitch_bytes, float* grad_vertices, gsb_uniforms* grad_uniforms, float* grad_features,
+                                 float* density, void* stream) {
+    const char* fn = "gsb_render_backward_features";
+    if (ctx && !ctx->shard && ctx->pos_op) {  // the feature arguments; render_backward checks the rest
+        auto bad = [&](const char* what) { return fail(ctx, GSB_ERR_INVALID, (std::string(fn) + ": " + what).c_str()); };
+        if (!vertices || !features || !grad_feature_map || (!grad_vertices && !grad_uniforms && !grad_features)) return bad("null argument");
+        if (channels < 1 || channels > GSB_MAX_FEATURE_CHANNELS) return bad("channels outside [1, 128]");
+        if (ctx->frame.scene_gen != 0 && !feature_pitch(ctx->frame, channels, feature_pitch_bytes)) return bad("bad feature row pitch");
+        for (const void* p : {(const void*)features, (const void*)grad_feature_map, (const void*)grad_features})
+            if (reinterpret_cast<uintptr_t>(p) % 4) return bad("array not aligned to 4 B");
+    }
+    const FeatureArgs fa{features, channels, grad_feature_map, feature_pitch_bytes, grad_features};
+    return render_backward(ctx, fn, true, vertices, grad_image, pitch, grad_vertices, grad_uniforms, density, stream, grad_depth_alpha,
+                           depth_pitch, &fa);
 }
 
 int gsb_background_gradient(gsb_ctx* ctx, const float* grad_image, size_t pitch, float* grad_background, void* stream) {
@@ -1240,6 +1330,48 @@ int gsb_adam_step_filter3d(gsb_ctx* ctx, float* params, float* exp_avg, float* e
                            float* vertices, const float* variance, const gsb_adam_config* cfg, void* stream) {
     return adam_step(ctx, "gsb_adam_step_filter3d", params, exp_avg, exp_avg_sq, grad_vertices, vertices, variance, true, cfg,
                      stream);
+}
+
+int gsb_adam_step_features(gsb_ctx* ctx, float* features, float* exp_avg, float* exp_avg_sq, const float* grad_features, uint32_t channels,
+                           float lr, const gsb_adam_config* cfg, void* stream) {
+    if (!ctx) return GSB_ERR_INVALID;
+    const char* fn = "gsb_adam_step_features";
+    auto bad = [&](const char* what) { return fail(ctx, GSB_ERR_INVALID, (std::string(fn) + ": " + what).c_str()); };
+    if (ctx->shard) return bad("sharded contexts have no training step");
+    if (!ctx->pos_op) return fail(ctx, GSB_ERR_NO_SCENE, (std::string(fn) + ": no scene uploaded").c_str());
+    if (!features || !exp_avg || !exp_avg_sq || !grad_features || !cfg) return bad("null argument");
+    for (const void* p : {(const void*)features, (const void*)exp_avg, (const void*)exp_avg_sq, (const void*)grad_features})
+        if (reinterpret_cast<uintptr_t>(p) % 4) return bad("array not aligned to 4 B");
+    if (channels < 1 || channels > GSB_MAX_FEATURE_CHANNELS) return bad("channels outside [1, 128]");
+    if (!(lr >= 0.0f)) return bad("learning rate below 0 or NaN");
+    if (!(cfg->beta1 >= 0.0f && cfg->beta1 < 1.0f) || !(cfg->beta2 >= 0.0f && cfg->beta2 < 1.0f)) return bad("beta outside [0, 1)");
+    if (!(cfg->eps >= 0.0f)) return bad("eps below 0 or NaN");
+    if (!(cfg->bias_correction1 > 0.0f && cfg->bias_correction1 <= 1.0f) ||
+        !(cfg->bias_correction2_sqrt > 0.0f && cfg->bias_correction2_sqrt <= 1.0f))
+        return bad("bias correction outside (0, 1]");
+    if (cfg->selective > 1) return bad("selective is neither 0 nor 1");
+    CK(cudaSetDevice(ctx->device));
+    if (cfg->selective) {  // the survivors of the last frame; the scene is not changed, so the frame stays valid
+        const int rc = check_recorded_frame(ctx, GSB_ERR_INVALID, (std::string(fn) + ": selective").c_str());
+        if (rc != GSB_OK) return rc;
+    }
+    FeatureAdamParams P{};
+    P.features = features;
+    P.exp_avg = exp_avg;
+    P.exp_avg_sq = exp_avg_sq;
+    P.grad = grad_features;
+    P.n = ctx->n;
+    P.channels = channels;
+    P.recs = cfg->selective ? ctx->recs.p : nullptr;
+    P.ctl = ctx->ctl;
+    P.lr = lr;
+    P.beta1 = cfg->beta1;
+    P.beta2 = cfg->beta2;
+    P.eps = cfg->eps;
+    P.bias_correction1 = cfg->bias_correction1;
+    P.bias_correction2_sqrt = cfg->bias_correction2_sqrt;
+    CK(launch_adam_features(P, ctx->num_sms, stream_or_own(ctx, stream)));
+    return GSB_OK;
 }
 
 int gsb_filter3d_variance(gsb_ctx* ctx, const float* vertices, uint64_t n, const gsb_uniforms* cameras, uint32_t k, float* variance,

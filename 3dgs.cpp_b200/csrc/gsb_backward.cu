@@ -838,7 +838,10 @@ __global__ void __launch_bounds__(96) k_background_reduce(const double* __restri
 // per (tile, entry); a stable sort of (compact id, list position) over the M entries groups each survivor's slots in tile
 // order, its last pass publishing each survivor's run; k_det_reduce sums every run in order.  Integer atomics remain
 // (the sort's counters and the runs' atomicMin), but their results do not depend on the order they land in.
-cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackward& d, const DepthBackward* dp, unsigned grid, cudaStream_t s) {
+// colour = false (gsb_render_backward_features without an image or depth gradient): the sort only, for the feature pass's
+// reduction; the scratch keeps its zeros.  *sorted_pos receives the sorted list positions.
+cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackward& d, const DepthBackward* dp, unsigned grid, cudaStream_t s,
+                            bool colour, const uint32_t** sorted_pos_out) {
     const bool density = p.density != nullptr;
     cudaError_t e = cudaMemsetAsync(d.sc, 0, sizeof(SortCtl), s);
     if (e != cudaSuccess) return e;
@@ -864,12 +867,14 @@ cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackwar
     uint32_t passes = 0;
     if ((e = launch_sort(sp, &passes, s)) != cudaSuccess) return e;
     if (passes == 0) return cudaErrorInvalidValue;  // key_bits >= 1: the runs come from the last pass
+    const uint32_t* sorted_pos = d.pos[passes & 1];
+    *sorted_pos_out = sorted_pos;
+    if (!colour) return cudaSuccess;
     if (p.num_tiles) {
         if (p.mode == GSB_MODE_EXACT) e = density ? launch_blend_det<GSB_MODE_EXACT, true>(p, bg, dp, s) : launch_blend_det<GSB_MODE_EXACT, false>(p, bg, dp, s);
         else e = density ? launch_blend_det<GSB_MODE_FAST, true>(p, bg, dp, s) : launch_blend_det<GSB_MODE_FAST, false>(p, bg, dp, s);
         if (e != cudaSuccess) return e;
     }
-    const uint32_t* sorted_pos = d.pos[passes & 1];
     double* ds = dp ? dp->scratch : nullptr;
     if (dp) {
         if (density) k_det_reduce<true, true><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs, ds);
@@ -912,15 +917,18 @@ cudaError_t launch_preprocess_backward(const BackwardParams& p, bool antialiased
 }  // namespace
 
 cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det,
-                            const gsb_camera_model* fisheye, const DepthBackward* depth) {
+                            const gsb_camera_model* fisheye, const DepthBackward* depth, const FeatureParams* features) {
     if (fisheye && p.grad_ubo) return cudaErrorInvalidValue;
     const bool density = p.density != nullptr;
+    const bool geometry = p.grad_vertices || p.grad_ubo;  // false only for a feature gradient alone
+    const bool colour = geometry && (p.grad_image || depth);
     // grid-stride over N_v, which stays on the device: the grid comes from the SM count
     const unsigned grid = (unsigned)p.num_sms * 4u;
+    const uint32_t* sorted_pos = nullptr;
     if (det) {
-        cudaError_t e = launch_det_sums(p, background, *det, depth, grid, s);
+        cudaError_t e = launch_det_sums(p, background, *det, depth, grid, s, colour, &sorted_pos);
         if (e != cudaSuccess) return e;
-    } else if (p.num_tiles) {
+    } else if (p.num_tiles && colour) {
         const bool bg = has_background(background);  // a frame of gsb_set_background
         if (depth) {
             if (bg) launch_blend_backward<true, true>(p, background, depth, s);
@@ -931,6 +939,19 @@ cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 ba
         }
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
+    }
+    if (features) {  // adds its share to the scratch the colour pass filled
+        FeatureParams fp = *features;
+        fp.scratch = geometry ? p.scratch : nullptr;
+        fp.abs_scratch = p.abs_scratch;
+        if (det) {
+            fp.det_slots = p.det_slots;
+            fp.pos = sorted_pos;
+            fp.runs = det->runs;
+        }
+        cudaError_t e = launch_feature_backward(fp, det != nullptr, s);
+        if (e != cudaSuccess) return e;
+        if (!geometry) return cudaSuccess;
     }
     if (density) {  // reads d uv before k_preprocess_backward clears it
         k_density_accumulate<<<grid, PB_THREADS, 0, s>>>(p);

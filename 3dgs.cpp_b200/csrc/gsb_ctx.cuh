@@ -70,7 +70,8 @@ struct Survivors {
 // gsb_set_backward_deterministic: the buffers behind DetBackward, allocated on first deterministic use, grown with the arena
 // and the scene, and freed with bw_record.
 struct DetBuffers {
-    DevArray<double> slots;  // 11 fp64 per arena entry (the blend's per-(tile, entry) partials), 12 once a depth backward ran
+    DevArray<double> slots;  // 11 fp64 per arena entry (the blend's per-(tile, entry) partials), 12 once a depth backward ran,
+                             // 24 once a feature backward of more than 4 channels ran
     DevArray<uint32_t> keys[2];
     DevArray<uint32_t> pos[2];
     DevArray<unsigned long long> status;
@@ -193,6 +194,7 @@ struct gsb_ctx {
     DevArray<double> bw_cam_partials;  // [4 * num_sms][GSB_UBO_WORDS] per-CTA fp64 partial sums of gsb_render_backward_camera
     DevArray<double> bw_abs;        // n x 2 per-survivor fp64 sums of |d u|, |d v| of gsb_render_backward_density (kept zero)
     DevArray<double> bw_depth;      // n x 1 per-survivor fp64 dL/d depth of gsb_render_backward_depth (kept zero)
+    DevArray<double> bw_feat;       // n x 16 per-survivor fp64 dL/d features of gsb_render_backward_features' atomic path (kept zero)
     bool bw_deterministic = false;  // gsb_set_backward_deterministic
     gsb::DetBuffers bw_det;
     DevArray<double> bg_partials;   // [background_grad_rows(H)][3] per-CTA fp64 partial sums of gsb_background_gradient

@@ -229,8 +229,42 @@ struct DepthBackward {
     size_t pitch;
     double* scratch;     // n x 1 fp64 dL/df per survivor: zero on entry, zero again on exit
 };
+// gsb_features.cu: feature maps of the last recorded frame (gsb_render_features) and their backward pass.  The frame's fields
+// and the caller's arrays are filled in by gsb_api.cu; launch_backward fills the scratch and deterministic ones.
+struct FeatureParams {
+    const float4* recs;
+    const uint32_t* vals;
+    const uint2* ranges;
+    const uint2* record;
+    const Control* ctl;
+    uint32_t width, height, tiles_x, num_tiles;
+    int mode;
+    int num_sms;
+    const float* features;  // n x channels, tight
+    uint32_t channels;
+    uint32_t c0;            // first channel of the chunk being launched
+    float* map;             // gsb_render_features: H x W x channels, map_pitch bytes per row
+    size_t map_pitch;
+    const float* grad_map;  // backward: dL/d map, H x W x channels, grad_pitch bytes per row
+    size_t grad_pitch;
+    float* grad_features;   // n x channels, written for the survivors (zeroed by the caller); null: none
+    double* scratch;        // the colour pass's n x 9 per-survivor sums: columns 0-5 gain the feature terms; null: no geometry
+    double* abs_scratch;    // n x 2 |d u|, |d v| sums of gsb_render_backward_density; null: no density statistics
+    double* feat_scratch;   // atomic path: n x 16 fp64 per-survivor feature sums, zero on entry and on exit
+    double* det_slots;      // deterministic path: (8 + chunk width) fp64 per arena entry
+    const uint32_t* pos;    // deterministic path: the colour pass's sorted list positions and per-survivor runs
+    const uint2* runs;
+};
+uint32_t feature_chunk(uint32_t channels);  // channels per pass: 4 or 16
+cudaError_t launch_render_features(FeatureParams p, cudaStream_t s);
+cudaError_t launch_feature_backward(FeatureParams p, bool det, cudaStream_t s);
+
+// features: gsb_render_backward_features' feature arguments (null for the other entries).  Its pass runs after the colour
+// pass's sums (which are skipped when there is neither an image nor a depth gradient) and before k_density_accumulate and
+// k_preprocess_backward; with neither grad_vertices nor grad_ubo only the feature gradient is formed.
 cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det = nullptr,
-                            const gsb_camera_model* fisheye = nullptr, const DepthBackward* depth = nullptr);
+                            const gsb_camera_model* fisheye = nullptr, const DepthBackward* depth = nullptr,
+                            const FeatureParams* features = nullptr);
 // gsb_background_gradient: out[c] = sum over the W x H pixels of T_final(p) grad_image(p)[c], from the recorded frame's
 // (bits(T), last) words.  fp64 products and sums in an order fixed by W and H (background_grad_rows(H) per-CTA partials,
 // then one CTA), no atomics.  partials holds 3 doubles per row of background_grad_rows(H).
@@ -259,6 +293,21 @@ struct AdamParams {
     const float* variance;
 };
 cudaError_t launch_adam(const AdamParams& p, int num_sms, cudaStream_t s);
+
+// gsb_features.cu: gsb_adam_step_features, n x channels raw features and their moments (rows of the last frame's survivors
+// when recs is set).
+struct FeatureAdamParams {
+    float* features;
+    float* exp_avg;
+    float* exp_avg_sq;
+    const float* grad;
+    uint64_t n;
+    uint32_t channels;
+    const float4* recs;  // selective: the last frame's survivor records (index in q3.y); null: every row
+    const Control* ctl;  // selective: num_visible
+    float lr, beta1, beta2, eps, bias_correction1, bias_correction2_sqrt;
+};
+cudaError_t launch_adam_features(const FeatureAdamParams& p, int num_sms, cudaStream_t s);
 
 // gsb_filter3d.cu: gsb_filter3d_variance.  cams: k device copies of gsb_uniforms; focal = the largest focal_x of the k;
 // dmax: one zeroed word (the largest seen depth's bits).  variance: n floats, overwritten.

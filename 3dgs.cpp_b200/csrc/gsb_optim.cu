@@ -20,17 +20,7 @@ namespace {
 constexpr int AD_ROWS = 16;                // rows per CTA and loop trip
 constexpr int AD_THREADS = AD_ROWS * 15;   // one thread per float4 of a row
 
-struct Adam {
-    float w1, w2, beta2, eps, bc2_sqrt;
-    // torch's exp_avg.lerp_(g, 1 - beta1); exp_avg_sq.mul_(beta2).addcmul_(g, g, value=1 - beta2);
-    // denom = sqrt(exp_avg_sq) / bc2_sqrt + eps; param.addcdiv_(exp_avg, denom, value=-step_size)
-    __device__ __forceinline__ void operator()(float g, float& x, float& m, float& v, float step_size) const {
-        m = w1 < 0.5f ? fmaf(w1, g - m, m) : fmaf(w1 - 1.0f, g - m, g);
-        v = fmaf(w2 * g, g, v * beta2);
-        const float denom = sqrtf(v) / bc2_sqrt + eps;
-        x = fmaf(-step_size, m / denom, x);
-    }
-};
+using Adam = AdamUpdate;
 
 __device__ __forceinline__ float sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
 

@@ -47,6 +47,8 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_set_backward_deterministic", "gsb_background_gradient",
     # rendered depth and alpha with their gradients
     "gsb_render_depth", "gsb_render_backward_depth",
+    # rendered feature maps with their gradients
+    "gsb_render_features", "gsb_render_backward_features", "gsb_adam_step_features",
     # training loss, optimizer step and initialisation from a point cloud
     "gsb_image_loss", "gsb_adam_step", "gsb_init_from_points",
     # Mip-Splatting's 3D smoothing filter
@@ -217,6 +219,10 @@ lib.gsb_background_gradient.argtypes = [_vp, _vp, C.c_size_t, _vp, _vp]
 lib.gsb_render_depth.argtypes = [_vp, C.POINTER(Uniforms), C.c_uint32, C.c_uint32, _vp, C.c_size_t, C.c_int, C.c_int, _vp,
                                  C.c_size_t, _vp]
 lib.gsb_render_backward_depth.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, C.c_size_t, _vp, _vp, _vp, _vp]
+lib.gsb_render_features.argtypes = [_vp, _vp, C.c_uint32, _vp, C.c_size_t, _vp]
+lib.gsb_render_backward_features.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, C.c_size_t, _vp, C.c_uint32, _vp, C.c_size_t, _vp, _vp,
+                                             _vp, _vp, _vp]
+lib.gsb_adam_step_features.argtypes = [_vp, _vp, _vp, _vp, _vp, C.c_uint32, C.c_float, C.POINTER(AdamConfig), _vp]
 lib.gsb_image_loss.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_float, _vp,
                                C.c_size_t, _vp, _vp]
 lib.gsb_bilagrid_apply.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_uint32, C.c_uint32, C.c_uint32,
@@ -467,6 +473,7 @@ class Context:
         self.h = handle
         self.device = device
         self.frames = 0  # frames rendered through this wrapper (render_torch checks it between forward and backward)
+        self._frame_hw = (0, 0, -1)  # (H, W, frames) of the last frame rendered through this wrapper
         self._depth_frame_id = -1  # the value of `frames` after the last gsb_render_depth frame
         self._background = None  # the last set_background colour (render_torch restores it after a frame of its own)
         self.camera = None  # the last set_camera_model lens (None: pinhole)
@@ -569,6 +576,7 @@ class Context:
         rb, re, nrows = self.band_rows(u, rows)
         out = np.empty((nrows, u.width, 4), np.float32 if fmt == FORMAT_RGBA32F else np.uint8)
         self.frames += 1
+        self._frame_hw = (u.height, u.width, self.frames)
         self._ck(lib.gsb_render(self.h, C.byref(u), rb, re, out.ctypes.data, 0, MEM_HOST, fmt, None))
         return out
 
@@ -580,6 +588,7 @@ class Context:
         out = np.empty((nrows, u.width, 4), np.float32 if fmt == FORMAT_RGBA32F else np.uint8)
         da = np.empty((nrows, u.width, 2), np.float32)
         self.frames += 1
+        self._frame_hw = (u.height, u.width, self.frames)
         self._ck(lib.gsb_render_depth(self.h, C.byref(u), rb, re, out.ctypes.data, 0, MEM_HOST, fmt, da.ctypes.data, 0, None))
         self._depth_frame_id = self.frames
         return out, da
@@ -589,10 +598,66 @@ class Context:
         """The last frame rendered through this wrapper came from gsb_render_depth, and nothing changed since."""
         return self._depth_frame_id == self.frames
 
+    def render_features(self, features, out=None, stream=None):
+        """gsb_render_features: the (H, W, C) float32 feature map of the last frame (recorded with set_backward, whole) from
+        features, an (n, C) float32 CUDA tensor in the upload's row order, C <= 128.  F_c = sum f_ic alpha_i T_i over the frame's
+        contributors, 0 where none.  Into `out` (a new tensor if None; rows may be padded) on `stream` (a torch stream; None =
+        torch's current stream)."""
+        import torch
+
+        f = _check_features("Context.render_features", features, features.device)
+        h, w = self._frame_size("Context.render_features")
+        if out is None:
+            out = torch.empty((h, w, f.shape[1]), dtype=torch.float32, device=f.device)
+        if out.dtype != torch.float32 or tuple(out.shape) != (h, w, f.shape[1]) or out.stride()[1:] != (f.shape[1], 1):
+            raise ValueError(f"Context.render_features: out must be an ({h}, {w}, {f.shape[1]}) float32 tensor with dense pixels")
+        s = _torch_stream_arg(torch.cuda.current_stream(f.device) if stream is None else stream)
+        self._ck(lib.gsb_render_features(self.h, f.data_ptr(), f.shape[1], out.data_ptr(), out.stride()[0] * 4, s))
+        return out
+
+    def render_backward_features(self, vertices_ptr, features, grad_feature_map, grad_vertices_ptr=None, grad_features_ptr=None,
+                                 grad_image_ptr=None, grad_depth_alpha_ptr=None, grad_uniforms_ptr=None, density_ptr=None,
+                                 stream=None):
+        """gsb_render_backward_features: one backward pass of the image (grad_image_ptr, may be None), depth / alpha
+        (grad_depth_alpha_ptr, a render_depth frame only) and the feature map (grad_feature_map, an (H, W, C) float32 CUDA
+        tensor, dense pixels) of the last frame.  features: the (n, C) tensor the map was rendered from.  grad_features_ptr
+        (n x C floats) is overwritten; grad_vertices_ptr, grad_uniforms_ptr and grad_features_ptr may each be None, not all."""
+        import torch
+
+        f = _check_features("Context.render_backward_features", features, features.device)
+        _check_feature_map("Context.render_backward_features", grad_feature_map, self._frame_size("Context.render_backward_features"),
+                           f)
+        s = _torch_stream_arg(torch.cuda.current_stream(features.device) if stream is None else stream)
+        self._backward(vertices_ptr, grad_image_ptr, grad_vertices_ptr, s, grad_uniforms_ptr=grad_uniforms_ptr, density_ptr=density_ptr,
+                       grad_depth_alpha_ptr=grad_depth_alpha_ptr, features=features, grad_feature_map=grad_feature_map,
+                       grad_features_ptr=grad_features_ptr)
+
+    def _frame_size(self, caller):
+        """(H, W) of the last frame, which must have been rendered through this wrapper with nothing rendered, uploaded or
+        stepped after it: the C entries see only the feature map's row pitch, so its height is checked here."""
+        h, w, frame = self._frame_hw
+        if frame != self.frames:
+            raise ValueError(f"{caller}: the last frame was not rendered through this Context, or the scene changed after it")
+        return h, w
+
+    def adam_step_features(self, features, exp_avg, exp_avg_sq, grad_features, lr, cfg: AdamConfig, stream=None):
+        """gsb_adam_step_features: torch.optim.Adam (no weight decay) of the (n, C) float32 CUDA tensor `features` in place,
+        with its moments, at learning rate lr and cfg's betas, eps, bias corrections and selective (cfg.lr is not read).
+        It does not change the scene: the last frame stays valid (a selective step must precede adam_step)."""
+        import torch
+
+        f = _check_features("Context.adam_step_features", features, features.device)
+        for t in (exp_avg, exp_avg_sq, grad_features):
+            _check_features("Context.adam_step_features", t, f.device, f.shape[1])
+        s = _torch_stream_arg(torch.cuda.current_stream(f.device) if stream is None else stream)
+        self._ck(lib.gsb_adam_step_features(self.h, f.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(), grad_features.data_ptr(),
+                                            f.shape[1], float(lr), C.byref(cfg), s))
+
     def render_into(self, u: Uniforms, out_ptr: int, fmt=FORMAT_RGBA32F, rows=None, stream=None, sync=True):
         """Render into DEVICE memory at out_ptr (e.g. tensor.data_ptr())."""
         rb, re, _ = self.band_rows(u, rows)
         self.frames += 1
+        self._frame_hw = (u.height, u.width, self.frames)
         if sync:
             self._ck(lib.gsb_render(self.h, C.byref(u), rb, re, out_ptr, 0, MEM_DEVICE, fmt, stream_ptr(stream)))
         else:
@@ -623,10 +688,16 @@ class Context:
                        grad_uniforms_ptr, density_ptr)
 
     def _backward(self, vertices_ptr, grad_image_ptr, grad_vertices_ptr, stream, row_pitch_bytes=0, grad_uniforms_ptr=None,
-                  density_ptr=None, grad_depth_alpha_ptr=None):
+                  density_ptr=None, grad_depth_alpha_ptr=None, features=None, grad_feature_map=None, grad_features_ptr=None):
         """render_backward with `stream` already the C ABI's cudaStream_t argument.  With grad_depth_alpha_ptr (H x W float2
-        of device memory, dL/d(D, A) of a render_depth frame), gsb_render_backward_depth; grad_image_ptr may then be None."""
-        if grad_depth_alpha_ptr is not None:
+        of device memory, dL/d(D, A) of a render_depth frame), gsb_render_backward_depth; grad_image_ptr may then be None.
+        With features ((n, C) tensor) and grad_feature_map ((H, W, C) tensor, dense pixels), gsb_render_backward_features."""
+        if features is not None:
+            self._ck(lib.gsb_render_backward_features(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_depth_alpha_ptr, 0,
+                                                      features.data_ptr(), features.shape[1], grad_feature_map.data_ptr(),
+                                                      grad_feature_map.stride()[0] * 4, grad_vertices_ptr, grad_uniforms_ptr,
+                                                      grad_features_ptr, density_ptr, stream))
+        elif grad_depth_alpha_ptr is not None:
             self._ck(lib.gsb_render_backward_depth(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_depth_alpha_ptr, 0,
                                                    grad_vertices_ptr, grad_uniforms_ptr, density_ptr, stream))
         elif density_ptr is not None:
@@ -645,6 +716,7 @@ class Context:
 
         img = torch.empty((u.height, u.width, 4), dtype=torch.float32, device=device)
         self.frames += 1
+        self._frame_hw = (u.height, u.width, self.frames)
         stream = _torch_stream_arg(torch.cuda.current_stream(device))
         if not depth:
             self._ck(lib.gsb_render(self.h, C.byref(u), 0, ALL_ROWS, img.data_ptr(), 0, MEM_DEVICE, FORMAT_RGBA32F, stream))
@@ -904,6 +976,7 @@ class Context:
 
 # ---------------------------------------------------------------- differentiable rendering (torch imported lazily)
 _RenderFn = None
+MAX_FEATURE_CHANNELS = 128  # GSB_MAX_FEATURE_CHANNELS
 CUDA_STREAM_LEGACY = 1  # cudaStreamLegacy: the C ABI reads a NULL stream as "the context's own stream"
 
 
@@ -923,6 +996,27 @@ def _check_density(caller, density, vertices):
         raise ValueError(f"{caller}: density must be a contiguous ({n}, 4) float32 tensor on the vertices' device")
 
 
+def _check_features(caller, features, device, channels=None):
+    """features as an (n, C) contiguous float32 tensor on `device`, 1 <= C <= 128 (C == channels when given); else ValueError."""
+    import torch
+
+    if (not isinstance(features, torch.Tensor) or features.dtype != torch.float32 or features.dim() != 2 or features.device != device
+            or not features.is_contiguous() or not 1 <= features.shape[1] <= MAX_FEATURE_CHANNELS
+            or (channels is not None and features.shape[1] != channels)):
+        raise ValueError(f"{caller}: features must be a contiguous (n, C) float32 tensor on {device}, 1 <= C <= {MAX_FEATURE_CHANNELS}")
+    return features
+
+
+def _check_feature_map(caller, fmap, hw, features):
+    """ValueError unless fmap is an (H, W, C) float32 tensor on the features' device with dense pixels, C = features' width."""
+    import torch
+
+    shape = (hw[0], hw[1], features.shape[1])
+    if (not isinstance(fmap, torch.Tensor) or fmap.dtype != torch.float32 or tuple(fmap.shape) != shape
+            or fmap.device != features.device or fmap.stride()[1:] != (features.shape[1], 1)):
+        raise ValueError(f"{caller}: the feature map must be a {shape} float32 tensor on {features.device} with dense pixels")
+
+
 def _render_fn():
     global _RenderFn
     if _RenderFn is None:
@@ -930,9 +1024,14 @@ def _render_fn():
 
         class RenderFn(torch.autograd.Function):
             @staticmethod
-            def forward(fctx, ctx, vertices, u, ubo, density, background, depth):
+            def forward(fctx, ctx, vertices, u, ubo, density, background, depth, features):
                 v = vertices.detach().contiguous()
                 fctx.depth = bool(depth)
+                fctx.features = None
+                if features is not None:
+                    if features.shape[0] != v.shape[0]:
+                        raise ValueError("render_torch: features must have one row per vertex")
+                    fctx.features = _check_features("render_torch", features.detach().contiguous(), v.device)
                 _check_density("render_torch", density, v)
                 fctx.density = density
                 if ubo is not None:  # the camera's float fields come from the tensor, the frame size from u
@@ -954,10 +1053,15 @@ def _render_fn():
                     finally:
                         ctx.set_background(previous)
                 fctx.gs_ctx, fctx.frame, fctx.vertices = ctx, ctx.frames, v
-                return out
+                if fctx.features is None:
+                    return out
+                fmap = ctx.render_features(fctx.features)
+                return (*out, fmap) if fctx.depth else (out, fmap)
 
             @staticmethod
-            def backward(fctx, grad_img, grad_da=None):
+            def backward(fctx, grad_img, *grads):
+                grad_da = grads[0] if fctx.depth else None
+                grad_fm = grads[-1] if fctx.features is not None else None
                 ctx = fctx.gs_ctx
                 if ctx.frames != fctx.frame:
                     raise RuntimeError("render_torch: another frame was rendered on this context between forward and backward")
@@ -968,14 +1072,25 @@ def _render_fn():
                     gda = (torch.zeros(tuple(g.shape[:2]) + (2,), dtype=torch.float32, device=v.device) if grad_da is None
                            else grad_da.detach().to(torch.float32).contiguous())
                 need_v, need_ubo, need_bg = fctx.needs_input_grad[1], fctx.needs_input_grad[3], fctx.needs_input_grad[5]
+                need_f = fctx.features is not None and fctx.needs_input_grad[7]
                 grad_v = torch.empty_like(v) if need_v else None
-                grad_ubo = grad_bg = None
+                grad_ubo = grad_bg = grad_f = None
                 # enqueued on torch's current stream (the engine runs backward on the forward's stream), so the gradients
                 # are complete for whatever torch enqueues after them
                 stream = _torch_stream_arg(torch.cuda.current_stream(v.device))
                 gu = torch.empty(40, dtype=torch.float32, device=v.device) if need_ubo else None  # a whole gsb_uniforms
                 ctx.set_backward_deterministic(torch.are_deterministic_algorithms_enabled())
-                if need_v or need_ubo:
+                if fctx.features is not None and (need_f or (grad_fm is not None and (need_v or need_ubo))):  # one pass for all
+                    f = fctx.features
+                    gfm = (torch.zeros((g.shape[0], g.shape[1], f.shape[1]), dtype=torch.float32, device=v.device) if grad_fm is None
+                           else grad_fm.detach().to(torch.float32).contiguous())
+                    grad_f = torch.empty_like(f) if need_f else None
+                    ctx._backward(v.data_ptr(), g.data_ptr(), grad_v.data_ptr() if need_v else None, stream,
+                                  grad_uniforms_ptr=gu.data_ptr() if need_ubo else None,
+                                  density_ptr=None if fctx.density is None or not (need_v or need_ubo) else fctx.density.data_ptr(),
+                                  grad_depth_alpha_ptr=None if gda is None else gda.data_ptr(), features=f, grad_feature_map=gfm,
+                                  grad_features_ptr=grad_f.data_ptr() if need_f else None)
+                elif need_v or need_ubo:
                     ctx._backward(v.data_ptr(), g.data_ptr(), grad_v.data_ptr() if need_v else None, stream,
                                   grad_uniforms_ptr=gu.data_ptr() if need_ubo else None,
                                   density_ptr=None if fctx.density is None else fctx.density.data_ptr(),
@@ -986,13 +1101,13 @@ def _render_fn():
                 if need_bg:  # sum_p T_final g, on the same stream
                     dtype, device = fctx.bg_like
                     grad_bg = ctx.background_gradient(g, torch.cuda.current_stream(v.device)).to(device=device, dtype=dtype)
-                return None, grad_v, None, grad_ubo, None, grad_bg, None
+                return None, grad_v, None, grad_ubo, None, grad_bg, None, grad_f
 
         _RenderFn = RenderFn
     return _RenderFn
 
 
-def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, background=None, depth=False):
+def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, background=None, depth=False, features=None):
     """Differentiable frame: vertices is a CUDA float32 tensor (n, 60) of GSScene::Vertex records (activated parameters, as
     gsb_scene_upload takes them).  Uploads it from device memory, renders the whole frame as an (H, W, 4) RGBA32F tensor and,
     on backward, returns dL/dvertices through gsb_render_backward.  Turns gsb_set_backward on for `ctx`.  The frame on the
@@ -1022,8 +1137,13 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, 
     D = sum f alpha T, f the view-space z (the distance from the camera for a fisheye model), and A = 1 - T_final, the
     accumulated opacity.  Backward then takes dL/dimg and dL/d(depth_alpha), either of them unused (zero), through
     gsb_render_backward_depth; it composes with ubo=, density=, background= and the deterministic mode.  Expected depth is
-    D / A.clamp_min(1e-10), inverse depth its reciprocal, and a mask loss reads A directly."""
-    return _render_fn().apply(ctx, vertices, u, ubo, density, background, depth)
+    D / A.clamp_min(1e-10), inverse depth its reciprocal, and a mask loss reads A directly.
+
+    features (optional): an (n, C) float32 CUDA tensor of per-Gaussian features, C <= 128.  The frame then also returns its
+    (H, W, C) feature map F_c = sum f_ic alpha_i T_i over 0 (gsb_render_features): (img, fmap), or (img, depth_alpha, fmap)
+    with depth=True.  Backward differentiates the image, depth / alpha and map in one gsb_render_backward_features pass, into
+    vertices, ubo, density and -- when it requires grad -- features."""
+    return _render_fn().apply(ctx, vertices, u, ubo, density, background, depth, features)
 
 
 _LossFn = None
@@ -1337,10 +1457,18 @@ class SceneAdam:
 
     densify() decides on the unfiltered records and recomputes the filter for the new scene; inject_noise() and relocate()
     (3DGS-MCMC) raise ValueError with a filter.  The filtered records are an ordinary scene: a plain viewer renders the
-    trained scene, filter included, from write_ply(path, ply_records(raw_parameters(opt.vertices)))."""
+    trained scene, filter included, from write_ply(path, ply_records(raw_parameters(opt.vertices))).
+
+    Feature fields (Gaussian Grouping, LangSplat, Feature 3DGS): features, an (n, C) float32 tensor (C <= 128), makes the
+    optimizer own `features` (a copy), its moments `feature_exp_avg` / `feature_exp_avg_sq` and `grad_features`, trained with
+    Adam at feature_lr (identity activation; `selective` applies).  render(u, features=True) also returns the feature map
+    (gsb_render_features), and step(..., grad_feature_map=) runs one gsb_render_backward_features pass, then the feature step
+    (gsb_adam_step_features), then the scene step.  densify() gathers the feature rows by `source` (split children copy their
+    parent's row and start with zero moments, as adam_state_after_densify does for the scene), and relocate() copies the
+    source rows onto the relocated ones with zero moments and appends features[src] when it grows."""
 
     def __init__(self, ctx: "Context", vertices, lr, betas=(0.9, 0.999), eps=1e-15, selective=True, background=None,
-                 random_background=False, seed=0, filter_cameras=None):
+                 random_background=False, seed=0, filter_cameras=None, features=None, feature_lr=0.0):
         import torch
 
         if not isinstance(vertices, torch.Tensor) or not vertices.is_cuda or vertices.dim() != 2 or vertices.shape[1] != 60:
@@ -1353,6 +1481,14 @@ class SceneAdam:
         self.filter_cameras = None if filter_cameras is None else list(filter_cameras)
         self.variance = None
         self._adopt(vertices.detach().to(torch.float32).contiguous().clone(), None)
+        self.features = self.feature_lr = None
+        if features is not None:
+            f = features.detach().to(torch.float32).contiguous().clone()
+            _check_features("SceneAdam", f, vertices.device)
+            if f.shape[0] != vertices.shape[0]:
+                raise ValueError("SceneAdam: features must have one row per vertex")
+            self.feature_lr = float(feature_lr)
+            self._adopt_features(f, torch.zeros_like(f), torch.zeros_like(f))
         if self.filter_cameras is not None:
             self._set_filter(ctx.filter3d_variance(self.params, self.filter_cameras), self.vertices)
         ctx.set_backward(True)
@@ -1366,6 +1502,12 @@ class SceneAdam:
             state = (raw_parameters(vertices), torch.zeros_like(vertices), torch.zeros_like(vertices))
         self.params, self.exp_avg, self.exp_avg_sq = state
         self.grad = torch.empty_like(vertices)
+
+    def _adopt_features(self, features, exp_avg, exp_avg_sq):
+        import torch
+
+        self.features, self.feature_exp_avg, self.feature_exp_avg_sq = features, exp_avg, exp_avg_sq
+        self.grad_features = torch.empty_like(features)
 
     def _set_filter(self, variance, unfiltered):
         """Adopts a filter: `variance` (checked finite and >= 0 here, once) and vertices = the filtered `unfiltered`."""
@@ -1392,19 +1534,26 @@ class SceneAdam:
         torch.cuda.current_stream(self.vertices.device).synchronize()  # the upload runs on the context's own stream
         self.ctx.upload(self.vertices)
 
-    def render(self, u: Uniforms, depth=False):
+    def render(self, u: Uniforms, depth=False, features=False):
         """The resident scene's frame of u as an (H, W, 4) float32 tensor, rendered on torch's current stream with the
         backward state recorded, over the optimizer's background (fixed or a fresh random colour).  No upload.  depth=True:
-        (image, depth_alpha) from gsb_render_depth (see render_torch), for step(..., grad_depth_alpha=)."""
+        (image, depth_alpha) from gsb_render_depth (see render_torch), for step(..., grad_depth_alpha=).  features=True (an
+        optimizer with features): the (H, W, C) feature map is appended to what is returned, for step(..., grad_feature_map=)."""
         import torch
 
+        if features and self.features is None:
+            raise ValueError("SceneAdam.render: features=True needs an optimizer made with features=")
         if self._generator is not None:
             self.background = torch.rand(3, generator=self._generator).tolist()
         if self.background is not None:
             self.ctx.set_background(self.background)
-        return self.ctx._render_whole_frame(u, self.vertices.device, depth)
+        out = self.ctx._render_whole_frame(u, self.vertices.device, depth)
+        if not features:
+            return out
+        fmap = self.ctx.render_features(self.features)
+        return (*out, fmap) if depth else (out, fmap)
 
-    def step(self, grad_image, density=None, opacity_reg=0.0, scale_reg=0.0, grad_depth_alpha=None):
+    def step(self, grad_image, density=None, opacity_reg=0.0, scale_reg=0.0, grad_depth_alpha=None, grad_feature_map=None):
         """One training step from dL/d(the last render()'s image), an (H, W, 4) float32 tensor: gsb_render_backward into
         `grad` (gsb_render_backward_density, accumulating into `density`, an (n, 4) float32 tensor, when given), then
         gsb_adam_step.  Everything runs on torch's current stream; nothing waits on the host.
@@ -1414,14 +1563,23 @@ class SceneAdam:
         columns 7 and 4-6 before the Adam step (gsplat uses 0.01 for both).  At 0, nothing is added.
 
         grad_depth_alpha: dL/d(depth_alpha) of the last render(u, depth=True), an (H, W, 2) float32 tensor, trained through
-        gsb_render_backward_depth; grad_image may then be None (no colour loss).  ValueError if the last render had no depth."""
+        gsb_render_backward_depth; grad_image may then be None (no colour loss).  ValueError if the last render had no depth.
+
+        grad_feature_map: dL/d(the last render's feature map), an (H, W, C) float32 tensor (an optimizer with features): the
+        backward is then gsb_render_backward_features, and `features` take their Adam step before the scene does."""
         import torch
 
         ctx, v = self.ctx, self.vertices
         if grad_depth_alpha is not None and not ctx._depth_frame:
             raise ValueError("SceneAdam.step: grad_depth_alpha needs a frame of render(u, depth=True)")
-        if grad_image is None and grad_depth_alpha is None:
-            raise ValueError("SceneAdam.step: no gradient (grad_image and grad_depth_alpha are both None)")
+        if grad_feature_map is not None and self.features is None:
+            raise ValueError("SceneAdam.step: grad_feature_map needs an optimizer made with features=")
+        if grad_image is None and grad_depth_alpha is None and grad_feature_map is None:
+            raise ValueError("SceneAdam.step: no gradient (grad_image, grad_depth_alpha and grad_feature_map are all None)")
+        gfm = None
+        if grad_feature_map is not None:
+            gfm = grad_feature_map.detach().to(torch.float32).contiguous()
+            _check_feature_map("SceneAdam.step", gfm, ctx._frame_size("SceneAdam.step"), self.features)
         g = None if grad_image is None else grad_image.detach().to(torch.float32).contiguous()
         gda = None if grad_depth_alpha is None else grad_depth_alpha.detach().to(torch.float32).contiguous()
         stream = _torch_stream_arg(torch.cuda.current_stream(v.device))
@@ -1429,13 +1587,19 @@ class SceneAdam:
         _check_density("SceneAdam.step", density, v)
         ctx._backward(v.data_ptr(), None if g is None else g.data_ptr(), self.grad.data_ptr(), stream,
                       density_ptr=None if density is None else density.data_ptr(),
-                      grad_depth_alpha_ptr=None if gda is None else gda.data_ptr())
+                      grad_depth_alpha_ptr=None if gda is None else gda.data_ptr(),
+                      features=None if gfm is None else self.features, grad_feature_map=gfm,
+                      grad_features_ptr=None if gfm is None else self.grad_features.data_ptr())
         n = v.shape[0]
         if opacity_reg:
             self.grad[:, 7] += opacity_reg / n
         if scale_reg:
             self.grad[:, 4:7] += scale_reg / (3 * n)
         self.steps += 1
+        cfg = adam_config(self.lr, self.betas, self.eps, self.steps, self.selective)
+        if gfm is not None:  # before the scene step, while the frame (its survivors, for selective) is still valid
+            ctx.adam_step_features(self.features, self.feature_exp_avg, self.feature_exp_avg_sq, self.grad_features,
+                                   self.feature_lr, cfg)
         ctx.adam_step(self.params, self.exp_avg, self.exp_avg_sq, self.grad, v,
                       adam_config(self.lr, self.betas, self.eps, self.steps, self.selective), variance=self.variance)
 
@@ -1446,6 +1610,12 @@ class SceneAdam:
         get_scaling and get_opacity), and the filter is recomputed for the new scene before the upload."""
         unfiltered = self.vertices if self.variance is None else activate_parameters(self.params)
         new, source = densify_and_prune(unfiltered, density, **kwargs)
+        if self.features is not None:  # split children (scale changed, as adam_state_after_densify finds them): zero moments
+            child = (new[:, 4:7] != unfiltered[source, 4:7]).any(1)
+            m, s = self.feature_exp_avg[source], self.feature_exp_avg_sq[source]
+            m[child] = 0.0
+            s[child] = 0.0
+            self._adopt_features(self.features[source].contiguous(), m.contiguous(), s.contiguous())
         self._adopt(new, adam_state_after_densify(self.params, self.exp_avg, self.exp_avg_sq, unfiltered, new, source))
         if self.variance is not None:
             self._set_filter(self.ctx.filter3d_variance(self.params, self.filter_cameras), new)
@@ -1489,6 +1659,10 @@ class SceneAdam:
             dst = torch.nonzero(dead)[:, 0]
             self.ctx.mcmc_relocate(self.params, self.exp_avg, self.exp_avg_sq, v, dst.to(torch.int32), src.to(torch.int32),
                                    min_opacity)
+            if self.features is not None:
+                self.features[dst] = self.features[src]
+                self.feature_exp_avg[dst] = 0.0
+                self.feature_exp_avg_sq[dst] = 0.0
             n_relocated = n_dead
         k = max(0, min(int(cap_max), int(math.floor((1.0 + growth) * n))) - n)
         if k > 0:
@@ -1497,6 +1671,10 @@ class SceneAdam:
             self._adopt(torch.cat([self.vertices, self.vertices[src]]).contiguous(),
                         (torch.cat([self.params, self.params[src]]).contiguous(),
                          torch.cat([self.exp_avg, zeros]).contiguous(), torch.cat([self.exp_avg_sq, zeros]).contiguous()))
+            if self.features is not None:
+                fz = torch.zeros((k, self.features.shape[1]), dtype=torch.float32, device=dev)
+                self._adopt_features(torch.cat([self.features, self.features[src]]).contiguous(),
+                                     torch.cat([self.feature_exp_avg, fz]).contiguous(), torch.cat([self.feature_exp_avg_sq, fz]).contiguous())
             self._upload()
             dst = torch.arange(n, n + k, dtype=torch.int32, device=dev)
             self.ctx.mcmc_relocate(self.params, self.exp_avg, self.exp_avg_sq, self.vertices, dst, src.to(torch.int32),

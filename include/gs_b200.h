@@ -348,6 +348,47 @@ int gsb_render_backward_depth(gsb_ctx *ctx, const float *vertices, const float *
                               const float *grad_depth_alpha, size_t depth_pitch_bytes, float *grad_vertices,
                               gsb_uniforms *grad_uniforms, float *density, void *stream);
 
+/* ---- rendered feature maps: C per-Gaussian channels composited like a colour (DESIGN.md section 21) ----
+ * A feature map of the last frame, which must be recorded (gsb_set_backward) and whole, F_c = sum_i f_ic alpha_i T_i over the
+ * frame's own contributors i (the alpha clamp, the power and 1/255 tests and the T' < 1e-4 break, as for gsb_render_depth's
+ * D), from +0; a pixel no Gaussian reaches gets 0 (there is no background term).  GSB_MODE_EXACT adds (f * alpha) * T,
+ * GSB_MODE_FAST f * (alpha * T), each sum rounded: with f the frame's colours F is the RGB gsb_render stores over black, and
+ * with f the depth keys it is gsb_render_depth's D, bit for bit.  It reads nothing of the camera model, so AA, background,
+ * fisheye and depth frames all apply, and it leaves the frame's recorded state as it was.
+ *   features      device memory, n x channels fp32 in the upload's row order, rows tight
+ *   channels      C, 1 to GSB_MAX_FEATURE_CHANNELS
+ *   feature_map   device memory, H x W x C fp32, channel-last (a torch (H, W, C) tensor), rows feature_pitch_bytes apart
+ *                 (0 = tight, 4 C W)
+ * Enqueued on `stream` (NULL = the context's stream).  The preconditions and error codes of gsb_render_backward (it waits for
+ * the last frame, as the backward does, to know that it did not overflow), and GSB_ERR_INVALID for a NULL pointer, C outside
+ * [1, 128], a pitch below 4 C W or not a multiple of 4, an array not 4-byte aligned, or a sharded or group context.
+ * fp16 SH storage does not matter here. */
+#define GSB_MAX_FEATURE_CHANNELS 128
+int gsb_render_features(gsb_ctx *ctx, const float *features, uint32_t channels, float *feature_map, size_t feature_pitch_bytes,
+                        void *stream);
+
+/* One backward pass of the last frame's image, depth / alpha and feature map together: the arguments, preconditions and error
+ * codes of gsb_render_backward_depth, except that
+ *   grad_image         may be NULL (no colour gradient)
+ *   grad_depth_alpha   may be NULL (no depth or alpha gradient); non-NULL only for a gsb_render_depth frame
+ *   features, channels the values and width the map was rendered from (documented, not checked)
+ *   grad_feature_map   device memory, dL/dF, H x W x C pitched like the map (feature_pitch_bytes, 0 = tight); required
+ *   grad_features      n x C fp32, OVERWRITTEN: dL/df_ic = sum_p g_c alpha_i T_i; zero for rows that contribute nowhere
+ *   grad_vertices, grad_uniforms, grad_features  each may be NULL, but not all three; density may be NULL, and needs
+ *                      grad_vertices or grad_uniforms
+ * Every contributor's alpha also gains T_i sum_c g_c (f_ic - acc_c), acc composited back to front from 0 (no gradient through
+ * a clamped alpha), which reaches positions, scales, rotations, opacities and the pinhole camera through the same chain rule as
+ * the colour.  A zero feature gradient gives gsb_render_backward_density's / _depth's words (a -0 may become +0).  density
+ * column 0 includes the feature terms exactly; column 1 adds the feature pass's own per-pixel |d u|, |d v|, summed per chunk
+ * of 4 or 16 channels apart from the colour pass's, so it is an upper bound of the per-pixel |total| the colour-only entries
+ * use.  Channels are processed 16 at a time (4 when C <= 4), each chunk walking the lists again.  The atomic path keeps
+ * 128 B per Gaussian of fp64 feature sums; under gsb_set_backward_deterministic every output word is reproducible as for the
+ * other entries, and the per-entry slots grow to 24 fp64 (192 B per arena entry; 12 at C <= 4). */
+int gsb_render_backward_features(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,
+                                 const float *grad_depth_alpha, size_t depth_pitch_bytes, const float *features, uint32_t channels,
+                                 const float *grad_feature_map, size_t feature_pitch_bytes, float *grad_vertices,
+                                 gsb_uniforms *grad_uniforms, float *grad_features, float *density, void *stream);
+
 /* dL/d(background) of the last frame (gsb_set_background): grad_background (device, 3 floats) is OVERWRITTEN with
  * sum over the W x H pixels p of T_final(p) g(p), g from grad_image (as for gsb_render_backward: H x W float4,
  * row_pitch_bytes apart, 0 = tight, A ignored).  It does not depend on the background's value, so it is defined for a frame
@@ -482,6 +523,15 @@ int gsb_filter3d_variance(gsb_ctx *ctx, const float *vertices, uint64_t n, const
  * or misaligned variance -- is gsb_adam_step's. */
 int gsb_adam_step_filter3d(gsb_ctx *ctx, float *params, float *exp_avg, float *exp_avg_sq, const float *grad_vertices,
                            float *vertices, const float *variance, const gsb_adam_config *cfg, void *stream);
+
+/* torch.optim.Adam (no weight decay) of n x C raw per-Gaussian features (gsb_render_features' rows) with their moments, all
+ * device memory, n the scene's size: lr is the features' learning rate, and cfg's betas, eps, bias corrections and selective
+ * apply as in gsb_adam_step (cfg->lr is not read).  selective = 1 updates only the rows of the last frame's survivors (the
+ * frame must still be valid, so call it before gsb_adam_step) and leaves the others' bits untouched.  It does not change the
+ * scene: the last frame stays valid.  No atomics.  GSB_ERR_INVALID for NULL or misaligned (4 B) arrays, C outside [1, 128],
+ * a bad configuration, selective without a valid recorded frame, or a sharded context; GSB_ERR_NO_SCENE before any upload. */
+int gsb_adam_step_features(gsb_ctx *ctx, float *features, float *exp_avg, float *exp_avg_sq, const float *grad_features,
+                           uint32_t channels, float lr, const gsb_adam_config *cfg, void *stream);
 
 /* ---- training: a scene initialised from a point cloud (no reference counterpart; DESIGN.md section 13) ---- */
 /* Kerbl et al. 2023's initialisation from SfM points: every point becomes an isotropic Gaussian.  All pointers are device
