@@ -1091,9 +1091,12 @@ struct FeatureArgs {
 // nullptr: no scene gradient (each entry's args_ok says which may be null).  density != nullptr: also accumulate the density
 // statistics into it.  grad_depth != nullptr (gsb_render_backward_depth): the frame must have depth, and grad_image may be
 // null (no colour gradient).  feat != nullptr (gsb_render_backward_features): also the feature map's gradient.
+// lens (gsb_render_backward_fisheye): the frame must be a fisheye frame, whose camera gradient goes to grad_ubo and grad_lens
+// (each may be null); grad_lens is set only then.
 static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const float* vertices, const float* grad_image, size_t pitch,
                            float* grad_vertices, gsb_uniforms* grad_ubo, float* density, void* stream, const float* grad_depth = nullptr,
-                           size_t depth_pitch = 0, const FeatureArgs* feat = nullptr) {
+                           size_t depth_pitch = 0, const FeatureArgs* feat = nullptr, bool lens = false,
+                           gsb_camera_model* grad_lens = nullptr) {
     if (!ctx) return GSB_ERR_INVALID;
     auto msg = [&](const char* what) { return std::string(fn) + ": " + what; };
     if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, msg("sharded contexts have no backward pass").c_str());
@@ -1105,8 +1108,12 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     if (!args_ok) return fail(ctx, GSB_ERR_INVALID, msg("null argument").c_str());
     const LastFrame& f = ctx->frame;
     const bool fisheye = f.camera.kind == GSB_CAMERA_FISHEYE;
-    if (fisheye && grad_ubo) return fail(ctx, GSB_ERR_INVALID, msg("a fisheye frame has no camera gradient").c_str());
-    if (feat && density && !grad_vertices && !grad_ubo)
+    if (lens && !fisheye)
+        return fail(ctx, GSB_ERR_INVALID, msg("the last frame is a pinhole frame (its camera gradient is gsb_render_backward_camera's)").c_str());
+    if (!lens && fisheye && grad_ubo) return fail(ctx, GSB_ERR_INVALID, msg("a fisheye frame has no camera gradient").c_str());
+    if (lens && density && !grad_vertices && !grad_ubo && !grad_lens)
+        return fail(ctx, GSB_ERR_INVALID, msg("density needs grad_vertices, grad_uniforms or grad_lens").c_str());
+    if (!lens && feat && density && !grad_vertices && !grad_ubo)
         return fail(ctx, GSB_ERR_INVALID, msg("density needs grad_vertices or grad_uniforms").c_str());
     const size_t tight = (size_t)f.ubo.width * sizeof(float4);
     if (pitch == 0) pitch = tight;
@@ -1135,7 +1142,8 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
         rc = grow_zeroed(ctx, ctx->bw_feat, n * 16, "ctx->bw_feat");
         if (rc != GSB_OK) return rc;
     }
-    if (grad_ubo)  // one row per CTA of k_preprocess_backward (4 per SM), fully overwritten by each call
+    const bool camera = grad_ubo || grad_lens;
+    if (camera)  // one row per CTA of k_preprocess_backward (4 per SM), fully overwritten by each call
         CK(ctx->bw_cam_partials.grow((uint64_t)ctx->num_sms * 4 * GSB_UBO_WORDS));
     if (det) {  // the depth backward's slots have one more column; the feature pass's 8 + its chunk width
         const uint64_t cols = std::max<uint64_t>(grad_depth ? 12 : 11, feat ? 8 + feature_chunk(feat->channels) : 0);
@@ -1147,6 +1155,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     if (feat && feat->grad_features) CK(cudaMemsetAsync(feat->grad_features, 0, (size_t)n * feat->channels * sizeof(float), s));
     if (n == 0) {
         if (grad_ubo) CK(cudaMemsetAsync(grad_ubo, 0, sizeof(gsb_uniforms), s));
+        if (grad_lens) CK(cudaMemsetAsync(grad_lens, 0, sizeof(gsb_camera_model), s));
         return GSB_OK;
     }
     BackwardParams bp{};
@@ -1169,7 +1178,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     bp.scratch = ctx->bw_scratch;
     bp.grad_vertices = grad_vertices;
     bp.num_sms = ctx->num_sms;
-    bp.cam_partials = grad_ubo ? ctx->bw_cam_partials.p : nullptr;
+    bp.cam_partials = camera ? ctx->bw_cam_partials.p : nullptr;
     bp.grad_ubo = grad_ubo;
     bp.abs_scratch = density ? ctx->bw_abs.p : nullptr;
     bp.density = density;
@@ -1186,7 +1195,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     }
     const FeatureParams* fpp = feat ? &fp : nullptr;
     if (!det) {
-        CK(launch_backward(bp, f.antialiased, bg, s, nullptr, fisheye ? &f.camera : nullptr, dp, fpp));
+        CK(launch_backward(bp, f.antialiased, bg, s, nullptr, fisheye ? &f.camera : nullptr, dp, fpp, grad_lens));
         return GSB_OK;
     }
     const DetBuffers& d = ctx->bw_det;
@@ -1202,7 +1211,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     db.status_tiles = (uint32_t)(d.status.count / 256);
     db.m_hint = quantise_hint(ctx->m_hint);
     db.key_bits = std::max<uint32_t>(bits_for((uint32_t)n), 1u);  // compact ids < N_v <= n
-    CK(launch_backward(bp, f.antialiased, bg, s, &db, fisheye ? &f.camera : nullptr, dp, fpp));
+    CK(launch_backward(bp, f.antialiased, bg, s, &db, fisheye ? &f.camera : nullptr, dp, fpp, grad_lens));
     return GSB_OK;
 }
 
@@ -1245,6 +1254,28 @@ int gsb_render_backward_features(gsb_ctx* ctx, const float* vertices, const floa
     const FeatureArgs fa{features, channels, grad_feature_map, feature_pitch_bytes, grad_features};
     return render_backward(ctx, fn, true, vertices, grad_image, pitch, grad_vertices, grad_uniforms, density, stream, grad_depth_alpha,
                            depth_pitch, &fa);
+}
+
+int gsb_render_backward_fisheye(gsb_ctx* ctx, const float* vertices, const float* grad_image, size_t pitch, const float* grad_depth_alpha,
+                                size_t depth_pitch, const float* features, uint32_t channels, const float* grad_feature_map,
+                                size_t feature_pitch_bytes, float* grad_vertices, gsb_uniforms* grad_uniforms, gsb_camera_model* grad_lens,
+                                float* grad_features, float* density, void* stream) {
+    const char* fn = "gsb_render_backward_fisheye";
+    const bool has_features = features || channels || grad_feature_map || grad_features;
+    if (ctx && !ctx->shard && ctx->pos_op) {  // the feature arguments; render_backward checks the rest
+        auto bad = [&](const char* what) { return fail(ctx, GSB_ERR_INVALID, (std::string(fn) + ": " + what).c_str()); };
+        if (!vertices || (!grad_vertices && !grad_uniforms && !grad_lens && !grad_features)) return bad("null argument");
+        if (has_features) {
+            if (!features || !grad_feature_map) return bad("features and grad_feature_map go together (or channels = 0 and all NULL)");
+            if (channels < 1 || channels > GSB_MAX_FEATURE_CHANNELS) return bad("channels outside [1, 128]");
+            if (ctx->frame.scene_gen != 0 && !feature_pitch(ctx->frame, channels, feature_pitch_bytes)) return bad("bad feature row pitch");
+            for (const void* p : {(const void*)features, (const void*)grad_feature_map, (const void*)grad_features})
+                if (reinterpret_cast<uintptr_t>(p) % 4) return bad("array not aligned to 4 B");
+        }
+    }
+    const FeatureArgs fa{features, channels, grad_feature_map, feature_pitch_bytes, grad_features};
+    return render_backward(ctx, fn, true, vertices, grad_image, pitch, grad_vertices, grad_uniforms, density, stream, grad_depth_alpha,
+                           depth_pitch, has_features ? &fa : nullptr, true, grad_lens);
 }
 
 int gsb_background_gradient(gsb_ctx* ctx, const float* grad_image, size_t pitch, float* grad_background, void* stream) {

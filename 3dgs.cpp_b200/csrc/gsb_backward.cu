@@ -24,7 +24,10 @@
 //                         record and returns its scratch accumulators to zero for the next call.  The CAMERA instantiation
 //                         (gsb_render_backward_camera) also keeps the camera's share of that chain rule -- view matrix,
 //                         projection matrix, camera position, tan_fov -- summed per thread, then per CTA into one fp64 row.
-//   k_camera_reduce       one CTA: sums those rows in a fixed order into the fp32 gsb_uniforms of gradients.
+//                         For a fisheye frame (gsb_render_backward_fisheye) the row holds the view matrix, the camera position
+//                         and the lens's fx, fy, cx, cy, k1..k4 instead.
+//   k_camera_reduce       one CTA: sums those rows in a fixed order into the fp32 gsb_uniforms of gradients
+//                         (k_fisheye_camera_reduce: into gsb_uniforms and gsb_camera_model).
 //
 // The atomics make the sums depend on the order in which warps and CTAs add their partial sums: by default gradients are NOT
 // guaranteed to be bitwise reproducible from run to run (fp64 accumulation makes a difference in the final fp32 value rare).
@@ -441,10 +444,12 @@ __host__ __device__ constexpr bool cam_word_live(int j) {
 // warps) into P.cam_partials for k_camera_reduce.  The vertex gradient is written only when P.grad_vertices is set.
 // AA (a frame of gsb_set_antialiased): d[5] is dL/d(o comp), comp = sqrt(det0 / det).  The opacity gets d[5] comp, and
 // g = d[5] o reaches both determinants: dL/d det0 = g comp / (2 det0), dL/d det = -g comp / (2 det), 0 where comp = 0.
-// FISHEYE (a frame of gsb_set_camera_model's fisheye, CAMERA = false only): J and uv are the lens's (fisheye_geo,
+// FISHEYE (a frame of gsb_set_camera_model's fisheye): J and uv are the lens's (fisheye_geo,
 // fisheye_jacobian), dL/d(J W) goes to J through the view rotation and on to the view-space position through J's second
 // derivatives (fisheye_grad), and that position to the Gaussian's through the view rotation; the projection matrix takes no
-// part.  Only these instantiations take the larger argument, so the others keep their code.
+// part.  Only these instantiations take the larger argument, so the others keep their code.  With CAMERA as well
+// (gsb_render_backward_fisheye) the camera's share is dL/dt through t = V (p, 1), dL/d(J W) through W, the view direction and
+// the lens (fisheye_lens_grad), reduced by k_fisheye_camera_reduce.
 // DEPTH (gsb_render_backward_depth): the survivor's dL/df (depth_scratch, returned to zero here) goes to the position through
 // the forward's own f: the view-space z of clip_view for a pinhole frame (dL/dv.z += dL/df, and with it dL/d(view row 2) in
 // the CAMERA instantiation), the distance d = |t| of fisheye_geo for a fisheye frame (dL/dt += (t / d) dL/df).
@@ -458,18 +463,32 @@ struct PbDepthParams : Base {
 template <bool FISHEYE, bool DEPTH = false>
 using PbParams = std::conditional_t<DEPTH, PbDepthParams<std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>,
                                     std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>;
+// CAMERA && FISHEYE (gsb_render_backward_fisheye): only the live words are accumulated -- camera_position.xyz, view_mat rows
+// 0-2 and the lens's fx, fy, cx, cy, k1..k4 -- and each CTA writes one fp64 row of FC_WORDS in this compact order for
+// k_fisheye_camera_reduce: [FC_POS + k] camera_position[k], [FC_VIEW + c * 3 + k] V[k][c] (word U_VIEW + c * 4 + k), [FC_LENS + j].
+constexpr int FC_POS = 0, FC_VIEW = 3, FC_LENS = 15, FC_WORDS = 23;
+template <bool ON>
+struct FisheyeCamAcc {
+    float w[FC_WORDS];
+};
+template <>
+struct FisheyeCamAcc<false> {};  // empty outside the new instantiations, for the reason given at det_partials()
 template <bool CAMERA, bool AA, bool FISHEYE = false, bool DEPTH = false>
 __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ PbParams<FISHEYE, DEPTH> P) {
-    static_assert(!(CAMERA && FISHEYE), "no camera gradient through the fisheye lens");
     const uint32_t nv = P.ctl->num_visible;
     const gsb_uniforms& U = P.ubo;
     const float* pm = U.proj_mat;
     const float* vm = U.view_mat;
     const bool store_v = !CAMERA || P.grad_vertices != nullptr;  // frozen scene: camera only
     float cam[GSB_UBO_WORDS];
-    if constexpr (CAMERA) {
+    if constexpr (CAMERA && !FISHEYE) {
 #pragma unroll
         for (int j = 0; j < GSB_UBO_WORDS; j++) cam[j] = 0.f;
+    }
+    FisheyeCamAcc<CAMERA && FISHEYE> fc;
+    if constexpr (CAMERA && FISHEYE) {
+#pragma unroll
+        for (int j = 0; j < FC_WORDS; j++) fc.w[j] = 0.f;
     }
     for (uint32_t cid = blockIdx.x * blockDim.x + threadIdx.x; cid < nv; cid += gridDim.x * blockDim.x) {
         double* sc = P.scratch + (size_t)cid * BW_NACC;
@@ -596,6 +615,18 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
             }
 #pragma unroll
             for (int k = 0; k < 3; k++) dp[k] = (vm[k * 4 + 0] * ftx + vm[k * 4 + 1] * fty) + vm[k * 4 + 2] * ftz;
+            if constexpr (CAMERA) {  // t = V (p, 1) rows 0-2, the view rotation W inside T = J W, and the lens
+                const float p3[3] = {px, py, pz}, dt[3] = {ftx, fty, ftz};
+#pragma unroll
+                for (int k = 0; k < 3; k++) {
+#pragma unroll
+                    for (int c = 0; c < 3; c++) fc.w[FC_VIEW + c * 3 + k] += dt[k] * p3[c];
+                    fc.w[FC_VIEW + 9 + k] += dt[k];
+#pragma unroll
+                    for (int r = 0; r < 3; r++) fc.w[FC_VIEW + r * 3 + k] += dT0[r] * FJ.J[0][k] + dT1[r] * FJ.J[1][k];
+                }
+                fisheye_lens_grad(P.cam, F, cv.vx, cv.vy, dJ, d[0], d[1], fc.w + FC_LENS);
+            }
         }
 
         // ---- colour (preprocess.comp:73-108) -> SH coefficients and the view direction ----
@@ -647,7 +678,12 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         dp[1] += (ddy - y * dot) / len;
         dp[2] += (ddz - z * dot) / len;
 
-        if constexpr (CAMERA) {  // ---- this survivor's share of dL/d(UBO), the UBO's fields taken as independent inputs ----
+        if constexpr (CAMERA && FISHEYE) {  // the view direction p - camera_position (the view and lens words are above)
+            fc.w[FC_POS + 0] -= (ddx - x * dot) / len;
+            fc.w[FC_POS + 1] -= (ddy - y * dot) / len;
+            fc.w[FC_POS + 2] -= (ddz - z * dot) / len;
+        }
+        if constexpr (CAMERA && !FISHEYE) {  // ---- this survivor's share of dL/d(UBO), the UBO's fields taken as independent inputs ----
             const float p3[3] = {px, py, pz}, dv[3] = {dvx, dvy, dvz}, dh[4] = {dhx, dhy, 0.f, dhw};
 #pragma unroll
             for (int r = 0; r < 3; r++) {
@@ -716,7 +752,25 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         gv[10] = dqy;
         gv[11] = dqz;
     }
-    if constexpr (CAMERA) {  // one row of fp64 partial sums per CTA
+    if constexpr (CAMERA && FISHEYE) {  // one row of FC_WORDS fp64 partial sums per CTA, as below
+        __shared__ double s_fc[PB_THREADS / 32][FC_WORDS];
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+        for (int j = 0; j < FC_WORDS; j++) {
+            double a = (double)fc.w[j];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(FULL, a, o);
+            if (lane == 0) s_fc[warp][j] = a;
+        }
+        __syncthreads();
+        if (threadIdx.x < FC_WORDS) {
+            double a = 0.0;
+#pragma unroll
+            for (int w = 0; w < PB_THREADS / 32; w++) a += s_fc[w][threadIdx.x];
+            P.cam_partials[(size_t)blockIdx.x * FC_WORDS + threadIdx.x] = a;
+        }
+    }
+    if constexpr (CAMERA && !FISHEYE) {  // one row of fp64 partial sums per CTA
         __shared__ double s_cam[PB_THREADS / 32][GSB_UBO_WORDS];
         const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
@@ -750,6 +804,37 @@ __global__ void __launch_bounds__(CR_THREADS) k_camera_reduce(const double* __re
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(FULL, a, o);
         if (lane == 0) reinterpret_cast<float*>(out)[j] = (float)a;  // 0.0f is also the bit pattern of width = height = 0
+    }
+}
+
+// The fisheye form of k_camera_reduce: sums the `rows` FC_WORDS-wide rows of k_preprocess_backward<true, AA, true> in the same
+// fixed order and writes the whole gsb_uniforms (zero outside camera_position.xyz and view rows 0-2) and the whole
+// gsb_camera_model of gradients (kind and max_theta 0); either output may be null.
+__global__ void __launch_bounds__(CR_THREADS) k_fisheye_camera_reduce(const double* __restrict__ partials, uint32_t rows, gsb_uniforms* out,
+                                                                      gsb_camera_model* lens) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (out) {  // the words no fisheye frame reads
+        for (int j = threadIdx.x; j < GSB_UBO_WORDS; j += CR_THREADS) {
+            const bool live = j < 3 || (j >= U_VIEW && j < U_VIEW + 16 && (j & 3) != 3);
+            if (!live) reinterpret_cast<float*>(out)[j] = 0.0f;
+        }
+    }
+    if (lens && threadIdx.x == 0) {
+        lens->kind = 0;
+        lens->max_theta = 0.0f;
+    }
+    for (int j = warp; j < FC_WORDS; j += CR_THREADS / 32) {
+        double a = 0.0;
+        for (uint32_t r = lane; r < rows; r += 32) a += partials[(size_t)r * FC_WORDS + j];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(FULL, a, o);
+        if (lane != 0) continue;
+        if (j >= FC_LENS) {
+            if (lens) reinterpret_cast<float*>(lens)[1 + j - FC_LENS] = (float)a;  // fx, fy, cx, cy, k[0..3]: words 1-8
+        } else if (out) {
+            const int w = j < FC_VIEW ? U_CAMPOS + j : U_VIEW + ((j - FC_VIEW) / 3) * 4 + (j - FC_VIEW) % 3;
+            reinterpret_cast<float*>(out)[w] = (float)a;
+        }
     }
 }
 
@@ -889,15 +974,23 @@ cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackwar
 // The vertex / camera part: k_preprocess_backward over the survivors (after the blend's sums and the density statistics).
 template <bool DEPTH>
 cudaError_t launch_preprocess_backward(const BackwardParams& p, bool antialiased, const gsb_camera_model* fisheye, const DepthBackward* dp,
-                                       unsigned grid, cudaStream_t s) {
+                                       unsigned grid, cudaStream_t s, gsb_camera_model* grad_lens) {
     auto with_depth = [&](const auto& base) {
         if constexpr (DEPTH) return PbDepthParams<std::decay_t<decltype(base)>>{base, dp->scratch};
         else return base;
     };
-    if (fisheye) {  // vertex gradients only (checked above)
+    if (fisheye) {
         const auto fp = with_depth(BackwardFisheyeParams{p, *fisheye});
-        if (antialiased) k_preprocess_backward<false, true, true, DEPTH><<<grid, PB_THREADS, 0, s>>>(fp);
-        else k_preprocess_backward<false, false, true, DEPTH><<<grid, PB_THREADS, 0, s>>>(fp);
+        if (!p.cam_partials) {  // vertex gradients only
+            if (antialiased) k_preprocess_backward<false, true, true, DEPTH><<<grid, PB_THREADS, 0, s>>>(fp);
+            else k_preprocess_backward<false, false, true, DEPTH><<<grid, PB_THREADS, 0, s>>>(fp);
+            return cudaGetLastError();
+        }
+        if (antialiased) k_preprocess_backward<true, true, true, DEPTH><<<grid, PB_THREADS, 0, s>>>(fp);
+        else k_preprocess_backward<true, false, true, DEPTH><<<grid, PB_THREADS, 0, s>>>(fp);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+        k_fisheye_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo, grad_lens);
         return cudaGetLastError();
     }
     const auto pp = with_depth(p);
@@ -917,10 +1010,11 @@ cudaError_t launch_preprocess_backward(const BackwardParams& p, bool antialiased
 }  // namespace
 
 cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det,
-                            const gsb_camera_model* fisheye, const DepthBackward* depth, const FeatureParams* features) {
-    if (fisheye && p.grad_ubo) return cudaErrorInvalidValue;
+                            const gsb_camera_model* fisheye, const DepthBackward* depth, const FeatureParams* features,
+                            gsb_camera_model* grad_lens) {
+    if (grad_lens && !fisheye) return cudaErrorInvalidValue;
     const bool density = p.density != nullptr;
-    const bool geometry = p.grad_vertices || p.grad_ubo;  // false only for a feature gradient alone
+    const bool geometry = p.grad_vertices || p.cam_partials;  // false only for a feature gradient alone
     const bool colour = geometry && (p.grad_image || depth);
     // grid-stride over N_v, which stays on the device: the grid comes from the SM count
     const unsigned grid = (unsigned)p.num_sms * 4u;
@@ -958,8 +1052,8 @@ cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 ba
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
-    return depth ? launch_preprocess_backward<true>(p, antialiased, fisheye, depth, grid, s)
-                 : launch_preprocess_backward<false>(p, antialiased, fisheye, depth, grid, s);
+    return depth ? launch_preprocess_backward<true>(p, antialiased, fisheye, depth, grid, s, grad_lens)
+                 : launch_preprocess_backward<false>(p, antialiased, fisheye, depth, grid, s, grad_lens);
 }
 
 uint32_t background_grad_rows(uint32_t height) { return std::min(height, BG_MAX_ROWS); }

@@ -150,6 +150,35 @@ __device__ __forceinline__ void fisheye_grad(const gsb_camera_model& M, const Fi
     dy += du * j.J[0][1] + dv * j.J[1][1];
     dz += du * j.J[0][2] + dv * j.J[1][2];
 }
+// The lens's share (gsb_render_backward_fisheye): adds dL/d(fx, fy, cx, cy, k1..k4) of uv and J to dl.  With P = 1 + t2 P1 and
+// Q = 1 + t2 Q1, s = P b, c = B b^3, e = Q / d^2 as in fisheye_geo:
+//   d uv / d(fx, fy) = (s x, 0), (0, s y);  d uv / d(cx, cy) = (1, 0), (0, 1);  d J / d fx = J's row 0 / fx (row 1 for fy)
+//   d s / d k_j = b t2^j,  d c / d k_j = t2^(j-1) ((2j + 1) scth - 1) b^3,  d e / d k_j = (2j + 1) t2^j / d^2
+// so that, with fisheye_grad's sig, q, l (dJ weighted by fx, fy) and Ls = fx du x + fy dv y + sig,
+//   dL/dk_j = t2^(j-1) ((t2 b Ls - b^3 q) + (2j + 1) (scth b^3 q - t2 l / d^2)).
+// Every factor is finite on the axis (b = 1 / d, x = y = 0 there).
+__device__ __forceinline__ void fisheye_lens_grad(const gsb_camera_model& M, const FisheyeGeo& g, float x, float y,
+                                                  const float (&dJ)[2][3], float du, float dv, float* dl) {
+    const float xyc = (x * y) * g.c, j00 = g.s + (x * x) * g.c, j11 = g.s + (y * y) * g.c;
+    dl[0] += du * (g.s * x) + ((dJ[0][0] * j00 + dJ[0][1] * xyc) - dJ[0][2] * (x * g.e));
+    dl[1] += dv * (g.s * y) + ((dJ[1][0] * xyc + dJ[1][1] * j11) - dJ[1][2] * (y * g.e));
+    dl[2] += du;
+    dl[3] += dv;
+    const float A0 = M.fx * dJ[0][0], A1 = M.fx * dJ[0][1], A2 = M.fx * dJ[0][2];
+    const float B0 = M.fy * dJ[1][0], B1 = M.fy * dJ[1][1], B2 = M.fy * dJ[1][2];
+    const float sig = A0 + B1, m = A1 + B0;
+    const float q = ((A0 * x) * x + (m * x) * y) + (B1 * y) * y, l = A2 * x + B2 * y;
+    const float Ls = ((M.fx * du) * x + (M.fy * dv) * y) + sig;
+    const float b3 = (g.b * g.b) * g.b;
+    const float al = (g.t2 * g.b) * Ls, be = b3 * q, ga = (g.t2 * l) / (g.d * g.d);
+    const float base = al - be, odd = g.scth * be - ga;
+    float pw = 1.0f;  // t2^(j-1)
+#pragma unroll
+    for (int j = 1; j <= 4; j++) {
+        dl[3 + j] += pw * (base + (float)(2 * j + 1) * odd);
+        pw *= g.t2;
+    }
+}
 
 // cov2d = transpose(T) Sigma T + 0.3 I (:56-65), Sigma = the cov3d words ca.xyzw, cb.xy; tm0 / tm1 = Sigma T0 / Sigma T1 (S[k] =
 // column k).  m01 and m10 round differently, so each caller states its own determinant.  c00 and c11 are the diagonal before

@@ -221,7 +221,8 @@ struct DetBackward {
 // background: the frame's gsb_set_background, the colour behind every pixel's last contributor.  It is a kernel argument of
 // its own after BackwardParams, not a field of it: a larger BackwardParams would move the arguments that follow it in
 // k_det_reduce.
-// fisheye: the frame's gsb_set_camera_model lens (vertex gradients only: p.grad_ubo must be null), null for a pinhole frame.
+// fisheye: the frame's gsb_set_camera_model lens, null for a pinhole frame.  With p.cam_partials set, a fisheye frame's camera
+// gradient (gsb_render_backward_fisheye): p.grad_ubo and grad_lens, either may be null; grad_lens needs a fisheye frame.
 // depth: gsb_render_backward_depth's upstream dL/d(D, A) and its per-survivor scratch (p.grad_image may then be null); null for
 // the colour-only entries.
 struct DepthBackward {
@@ -264,7 +265,7 @@ cudaError_t launch_feature_backward(FeatureParams p, bool det, cudaStream_t s);
 // k_preprocess_backward; with neither grad_vertices nor grad_ubo only the feature gradient is formed.
 cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det = nullptr,
                             const gsb_camera_model* fisheye = nullptr, const DepthBackward* depth = nullptr,
-                            const FeatureParams* features = nullptr);
+                            const FeatureParams* features = nullptr, gsb_camera_model* grad_lens = nullptr);
 // gsb_background_gradient: out[c] = sum over the W x H pixels of T_final(p) grad_image(p)[c], from the recorded frame's
 // (bits(T), last) words.  fp64 products and sums in an order fixed by W and H (background_grad_rows(H) per-CTA partials,
 // then one CTA), no atomics.  partials holds 3 doubles per row of background_grad_rows(H).

@@ -49,6 +49,8 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_render_depth", "gsb_render_backward_depth",
     # rendered feature maps with their gradients
     "gsb_render_features", "gsb_render_backward_features", "gsb_adam_step_features",
+    # camera and lens gradients through the fisheye
+    "gsb_render_backward_fisheye",
     # training loss, optimizer step and initialisation from a point cloud
     "gsb_image_loss", "gsb_adam_step", "gsb_init_from_points",
     # Mip-Splatting's 3D smoothing filter
@@ -147,6 +149,27 @@ def fisheye_camera(fx, fy, cx, cy, k=(0.0, 0.0, 0.0, 0.0), max_theta=None) -> Ca
     return CameraModel(CAMERA_FISHEYE, float(fx), float(fy), float(cx), float(cy), (C.c_float * 4)(*k), float(max_theta))
 
 
+LENS_WORDS = 8  # (fx, fy, cx, cy, k1, k2, k3, k4): lens_tensor's layout and gsb_render_backward_fisheye's grad_lens words 1-8
+
+
+def lens_tensor(cam: CameraModel, device=None):
+    """The (8,) float32 tensor (fx, fy, cx, cy, k1..k4) of a fisheye CameraModel, for render_torch(..., lens=): a lens a
+    torch optimizer can refine.  lens_camera turns it back into the same CameraModel, bit for bit."""
+    import torch
+
+    return torch.tensor(np.array([cam.fx, cam.fy, cam.cx, cam.cy, *cam.k], np.float32), device=device)
+
+
+def lens_camera(lens, max_theta) -> CameraModel:
+    """The fisheye CameraModel of an (8,) lens tensor (lens_tensor's layout) culled at max_theta (radians), bit for bit."""
+    import torch
+
+    w = lens.detach().to("cpu", torch.float32).reshape(-1).numpy() if isinstance(lens, torch.Tensor) else np.asarray(lens, np.float32)
+    if w.shape != (LENS_WORDS,):
+        raise ValueError(f"lens_camera: the lens must hold {LENS_WORDS} values (fx, fy, cx, cy, k1..k4)")
+    return CameraModel(CAMERA_FISHEYE, *(float(x) for x in w[:4]), (C.c_float * 4)(*(float(x) for x in w[4:])), float(max_theta))
+
+
 def fisheye_from_colmap(fx, fy, cx, cy, k1, k2, k3, k4) -> CameraModel:
     """COLMAP's OPENCV_FISHEYE parameters (fx, fy, cx, cy, k1, k2, k3, k4) as a fisheye_camera.  COLMAP puts pixel centres at
     i + 0.5, this renderer samples pixel (i, j) at (i, j): the principal point moves by half a pixel."""
@@ -222,6 +245,8 @@ lib.gsb_render_backward_depth.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, C.c_si
 lib.gsb_render_features.argtypes = [_vp, _vp, C.c_uint32, _vp, C.c_size_t, _vp]
 lib.gsb_render_backward_features.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, C.c_size_t, _vp, C.c_uint32, _vp, C.c_size_t, _vp, _vp,
                                              _vp, _vp, _vp]
+lib.gsb_render_backward_fisheye.argtypes = [_vp, _vp, _vp, C.c_size_t, _vp, C.c_size_t, _vp, C.c_uint32, _vp, C.c_size_t, _vp, _vp,
+                                            _vp, _vp, _vp, _vp]
 lib.gsb_adam_step_features.argtypes = [_vp, _vp, _vp, _vp, _vp, C.c_uint32, C.c_float, C.POINTER(AdamConfig), _vp]
 lib.gsb_image_loss.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_float, _vp,
                                C.c_size_t, _vp, _vp]
@@ -533,7 +558,8 @@ class Context:
         """gsb_set_camera_model: from the next frame, project through the lens `cam` (a CameraModel from fisheye_camera or
         fisheye_from_colmap; None or kind CAMERA_PINHOLE = the UBO's pinhole camera, the default).  A fisheye frame reads only
         the UBO's view matrix, camera position and size.  Frames, render_torch, SceneAdam and the backward pass follow it
-        (the backward uses the model of the frame it differentiates); there is no camera gradient through a fisheye lens."""
+        (the backward uses the model of the frame it differentiates).  The camera and lens gradients of a fisheye frame come
+        from gsb_render_backward_fisheye (Context._backward_fisheye, render_torch(..., lens=), SceneAdam.step)."""
         self._ck(lib.gsb_set_camera_model(self.h, None if cam is None else C.byref(cam)))
         self.camera = None if cam is None or cam.kind == CAMERA_PINHOLE else cam
 
@@ -708,6 +734,18 @@ class Context:
         else:
             self._ck(lib.gsb_render_backward_camera(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_vertices_ptr,
                                                     grad_uniforms_ptr, stream))
+
+    def _backward_fisheye(self, vertices_ptr, grad_image_ptr, grad_vertices_ptr, stream, grad_uniforms_ptr=None, grad_lens_ptr=None,
+                          density_ptr=None, grad_depth_alpha_ptr=None, features=None, grad_feature_map=None, grad_features_ptr=None,
+                          row_pitch_bytes=0):
+        """gsb_render_backward_fisheye on device pointers, `stream` the C ABI's cudaStream_t: _backward's arguments plus the
+        camera gradient of the last (fisheye) frame, grad_uniforms_ptr (160 B, dL/d gsb_uniforms, pose words only) and
+        grad_lens_ptr (40 B, a gsb_camera_model of dL/d(fx, fy, cx, cy, k)), each overwritten and each may be None."""
+        fptr, fch, gfm, fpitch = (None, 0, None, 0) if features is None else (
+            features.data_ptr(), features.shape[1], grad_feature_map.data_ptr(), grad_feature_map.stride()[0] * 4)
+        self._ck(lib.gsb_render_backward_fisheye(self.h, vertices_ptr, grad_image_ptr, row_pitch_bytes, grad_depth_alpha_ptr, 0, fptr,
+                                                 fch, gfm, fpitch, grad_vertices_ptr, grad_uniforms_ptr, grad_lens_ptr,
+                                                 grad_features_ptr, density_ptr, stream))
 
     def _render_whole_frame(self, u: Uniforms, device, depth=False):
         """The whole frame of u, recorded while gsb_set_backward is on, as a new tensor on torch's current stream; with
@@ -1024,7 +1062,7 @@ def _render_fn():
 
         class RenderFn(torch.autograd.Function):
             @staticmethod
-            def forward(fctx, ctx, vertices, u, ubo, density, background, depth, features):
+            def forward(fctx, ctx, vertices, u, ubo, density, background, depth, features, lens):
                 v = vertices.detach().contiguous()
                 fctx.depth = bool(depth)
                 fctx.features = None
@@ -1034,24 +1072,45 @@ def _render_fn():
                     fctx.features = _check_features("render_torch", features.detach().contiguous(), v.device)
                 _check_density("render_torch", density, v)
                 fctx.density = density
+                fctx.lens_like = None
+                cam = None
+                if lens is not None:  # this frame through the tensor's lens, culled at the context's max_theta or the default
+                    w = lens.detach().to("cpu", torch.float32).reshape(-1)
+                    max_theta = (ctx.camera.max_theta if ctx.camera is not None
+                                 else fisheye_camera(*w[:4].tolist(), w[4:].tolist()).max_theta)
+                    cam = lens_camera(w, max_theta)
+                    fctx.lens_like = (lens.dtype, lens.device)
                 if ubo is not None:  # the camera's float fields come from the tensor, the frame size from u
-                    if ctx.camera is not None:
-                        raise ValueError("render_torch: ubo= (a camera gradient) is not available for a fisheye camera model")
+                    if ctx.camera is not None and cam is None:
+                        raise ValueError("render_torch: ubo= on a fisheye camera model needs lens= (its camera gradient is "
+                                         "gsb_render_backward_fisheye's)")
                     u = unpack_uniforms(ubo.detach().to("cpu", torch.float32).numpy(), u.width, u.height)
                     fctx.ubo_like = (ubo.dtype, ubo.device)
                 ctx.set_backward(True)
                 torch.cuda.current_stream(v.device).synchronize()  # the upload runs on the context's stream: v must be complete
                 ctx.upload(v)
-                if background is None:
-                    out = ctx._render_whole_frame(u, v.device, fctx.depth)
-                else:  # this frame over the tensor's colour; the context's own setting is restored after it
+
+                def frame():
+                    if background is None:
+                        return ctx._render_whole_frame(u, v.device, fctx.depth)
+                    # this frame over the tensor's colour; the context's own setting is restored after it
                     fctx.bg_like = (background.dtype, background.device)
                     previous = ctx._background
                     ctx.set_background(background.detach().to("cpu", torch.float32).reshape(3).tolist())
                     try:
-                        out = ctx._render_whole_frame(u, v.device, fctx.depth)
+                        return ctx._render_whole_frame(u, v.device, fctx.depth)
                     finally:
                         ctx.set_background(previous)
+
+                if cam is None:
+                    out = frame()
+                else:  # the context's own model is restored after the frame (a lens it refuses raises and changes nothing)
+                    previous_cam = ctx.camera
+                    ctx.set_camera_model(cam)
+                    try:
+                        out = frame()
+                    finally:
+                        ctx.set_camera_model(previous_cam)
                 fctx.gs_ctx, fctx.frame, fctx.vertices = ctx, ctx.frames, v
                 if fctx.features is None:
                     return out
@@ -1073,14 +1132,34 @@ def _render_fn():
                            else grad_da.detach().to(torch.float32).contiguous())
                 need_v, need_ubo, need_bg = fctx.needs_input_grad[1], fctx.needs_input_grad[3], fctx.needs_input_grad[5]
                 need_f = fctx.features is not None and fctx.needs_input_grad[7]
+                need_lens = fctx.lens_like is not None and fctx.needs_input_grad[8]
                 grad_v = torch.empty_like(v) if need_v else None
-                grad_ubo = grad_bg = grad_f = None
+                grad_ubo = grad_bg = grad_f = grad_lens = None
                 # enqueued on torch's current stream (the engine runs backward on the forward's stream), so the gradients
                 # are complete for whatever torch enqueues after them
                 stream = _torch_stream_arg(torch.cuda.current_stream(v.device))
                 gu = torch.empty(40, dtype=torch.float32, device=v.device) if need_ubo else None  # a whole gsb_uniforms
                 ctx.set_backward_deterministic(torch.are_deterministic_algorithms_enabled())
-                if fctx.features is not None and (need_f or (grad_fm is not None and (need_v or need_ubo))):  # one pass for all
+                if fctx.lens_like is not None:  # a frame through lens=: every output in one gsb_render_backward_fisheye pass
+                    f = fctx.features if fctx.features is not None and (need_f or grad_fm is not None) else None
+                    gfm = None
+                    if f is not None:
+                        gfm = (torch.zeros((g.shape[0], g.shape[1], f.shape[1]), dtype=torch.float32, device=v.device)
+                               if grad_fm is None else grad_fm.detach().to(torch.float32).contiguous())
+                    grad_f = torch.empty_like(f) if need_f else None
+                    gl = torch.empty(10, dtype=torch.float32, device=v.device) if need_lens else None  # a gsb_camera_model
+                    if need_v or need_ubo or need_lens or need_f:
+                        geometry = need_v or need_ubo or need_lens
+                        ctx._backward_fisheye(v.data_ptr(), g.data_ptr(), grad_v.data_ptr() if need_v else None, stream,
+                                              grad_uniforms_ptr=gu.data_ptr() if need_ubo else None,
+                                              grad_lens_ptr=gl.data_ptr() if need_lens else None,
+                                              density_ptr=None if fctx.density is None or not geometry else fctx.density.data_ptr(),
+                                              grad_depth_alpha_ptr=None if gda is None else gda.data_ptr(), features=f,
+                                              grad_feature_map=gfm, grad_features_ptr=grad_f.data_ptr() if need_f else None)
+                    if need_lens:
+                        dtype, device = fctx.lens_like
+                        grad_lens = gl[1:1 + LENS_WORDS].to(device=device, dtype=dtype)
+                elif fctx.features is not None and (need_f or (grad_fm is not None and (need_v or need_ubo))):  # one pass for all
                     f = fctx.features
                     gfm = (torch.zeros((g.shape[0], g.shape[1], f.shape[1]), dtype=torch.float32, device=v.device) if grad_fm is None
                            else grad_fm.detach().to(torch.float32).contiguous())
@@ -1101,13 +1180,14 @@ def _render_fn():
                 if need_bg:  # sum_p T_final g, on the same stream
                     dtype, device = fctx.bg_like
                     grad_bg = ctx.background_gradient(g, torch.cuda.current_stream(v.device)).to(device=device, dtype=dtype)
-                return None, grad_v, None, grad_ubo, None, grad_bg, None, grad_f
+                return None, grad_v, None, grad_ubo, None, grad_bg, None, grad_f, grad_lens
 
         _RenderFn = RenderFn
     return _RenderFn
 
 
-def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, background=None, depth=False, features=None):
+def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, background=None, depth=False, features=None,
+                 lens=None):
     """Differentiable frame: vertices is a CUDA float32 tensor (n, 60) of GSScene::Vertex records (activated parameters, as
     gsb_scene_upload takes them).  Uploads it from device memory, renders the whole frame as an (H, W, 4) RGBA32F tensor and,
     on backward, returns dL/dvertices through gsb_render_backward.  Turns gsb_set_backward on for `ctx`.  The frame on the
@@ -1131,7 +1211,14 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, 
     torch's default settings backward takes the atomic path, whose results may differ in the last bit from run to run.
 
     The frame is projected through the context's camera model (Context.set_camera_model); ubo= on a fisheye context raises
-    ValueError.
+    ValueError unless lens= is given.
+
+    lens (optional): an (8,) tensor (fx, fy, cx, cy, k1..k4) (lens_tensor makes one).  The frame is rendered through
+    lens_camera(lens, max_theta), max_theta that of the context's fisheye model if one is set, else fisheye_camera's default
+    for these k, and the context's own model is restored after the forward (a lens gsb_set_camera_model refuses raises
+    GsbError and changes nothing).  Backward runs gsb_render_backward_fisheye: dL/dlens when lens requires grad, dL/dubo
+    (camera_position and view rows 0-2 only; the rest is 0) when ubo requires grad, and the other inputs' gradients as
+    without lens=.  It composes with depth=, features=, density=, background= and the deterministic mode.
 
     depth=True renders with gsb_render_depth and returns (img, depth_alpha), depth_alpha an (H, W, 2) tensor of (D, A):
     D = sum f alpha T, f the view-space z (the distance from the camera for a fisheye model), and A = 1 - T_final, the
@@ -1143,7 +1230,7 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, 
     (H, W, C) feature map F_c = sum f_ic alpha_i T_i over 0 (gsb_render_features): (img, fmap), or (img, depth_alpha, fmap)
     with depth=True.  Backward differentiates the image, depth / alpha and map in one gsb_render_backward_features pass, into
     vertices, ubo, density and -- when it requires grad -- features."""
-    return _render_fn().apply(ctx, vertices, u, ubo, density, background, depth, features)
+    return _render_fn().apply(ctx, vertices, u, ubo, density, background, depth, features, lens)
 
 
 _LossFn = None
@@ -1553,7 +1640,8 @@ class SceneAdam:
         fmap = self.ctx.render_features(self.features)
         return (*out, fmap) if depth else (out, fmap)
 
-    def step(self, grad_image, density=None, opacity_reg=0.0, scale_reg=0.0, grad_depth_alpha=None, grad_feature_map=None):
+    def step(self, grad_image, density=None, opacity_reg=0.0, scale_reg=0.0, grad_depth_alpha=None, grad_feature_map=None,
+             grad_uniforms=None, grad_lens=None):
         """One training step from dL/d(the last render()'s image), an (H, W, 4) float32 tensor: gsb_render_backward into
         `grad` (gsb_render_backward_density, accumulating into `density`, an (n, 4) float32 tensor, when given), then
         gsb_adam_step.  Everything runs on torch's current stream; nothing waits on the host.
@@ -1566,7 +1654,22 @@ class SceneAdam:
         gsb_render_backward_depth; grad_image may then be None (no colour loss).  ValueError if the last render had no depth.
 
         grad_feature_map: dL/d(the last render's feature map), an (H, W, C) float32 tensor (an optimizer with features): the
-        backward is then gsb_render_backward_features, and `features` take their Adam step before the scene does."""
+        backward is then gsb_render_backward_features, and `features` take their Adam step before the scene does.
+
+        grad_uniforms, grad_lens: optional (40,) and (8,) float32 CUDA tensors, overwritten by the same backward pass with
+        dL/d(the frame's gsb_uniforms, all 40 words) and dL/d(fx, fy, cx, cy, k1..k4) of the frame's lens.  A pinhole frame
+        fills grad_uniforms through gsb_render_backward_camera's words (grad_lens: ValueError); a fisheye frame fills both
+        through gsb_render_backward_fisheye (pose words only).  `grad`, the features and the step are the same as without them.
+        Joint pose refinement, with per-view poses (and a lens tensor) in a torch optimizer:
+
+            gu = torch.empty(40, device="cuda")
+            ubo = uniforms_torch(pos[i], rot[i], fov, near, far, W, H)  # pos[i], rot[i] require grad
+            img = opt.render(unpack_uniforms(ubo.detach().cpu().numpy(), W, H))
+            ctx.image_loss(img, target[i], 0.2, grad_image=g)
+            opt.step(g, grad_uniforms=gu)
+            ubo.backward(gu[UBO_FLOAT_WORDS]); pose_opt.step(); pose_opt.zero_grad()
+
+        For a lens, render through ctx.set_camera_model(lens_camera(lens, max_theta)) and add lens.grad += the grad_lens."""
         import torch
 
         ctx, v = self.ctx, self.vertices
@@ -1585,11 +1688,28 @@ class SceneAdam:
         stream = _torch_stream_arg(torch.cuda.current_stream(v.device))
         ctx.set_backward_deterministic(torch.are_deterministic_algorithms_enabled())
         _check_density("SceneAdam.step", density, v)
-        ctx._backward(v.data_ptr(), None if g is None else g.data_ptr(), self.grad.data_ptr(), stream,
-                      density_ptr=None if density is None else density.data_ptr(),
+        for name, t, size in (("grad_uniforms", grad_uniforms, 40), ("grad_lens", grad_lens, LENS_WORDS)):
+            if t is not None and (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or tuple(t.shape) != (size,)
+                                  or t.device != v.device or not t.is_contiguous()):
+                raise ValueError(f"SceneAdam.step: {name} must be a contiguous ({size},) float32 tensor on {v.device}")
+        common = dict(density_ptr=None if density is None else density.data_ptr(),
                       grad_depth_alpha_ptr=None if gda is None else gda.data_ptr(),
                       features=None if gfm is None else self.features, grad_feature_map=gfm,
                       grad_features_ptr=None if gfm is None else self.grad_features.data_ptr())
+        gu = None if grad_uniforms is None else grad_uniforms.data_ptr()
+        if ctx.camera is None:
+            if grad_lens is not None:
+                raise ValueError("SceneAdam.step: grad_lens needs a fisheye frame (Context.set_camera_model)")
+            ctx._backward(v.data_ptr(), None if g is None else g.data_ptr(), self.grad.data_ptr(), stream, grad_uniforms_ptr=gu,
+                          **common)
+        elif grad_uniforms is None and grad_lens is None:
+            ctx._backward(v.data_ptr(), None if g is None else g.data_ptr(), self.grad.data_ptr(), stream, **common)
+        else:
+            gl = None if grad_lens is None else torch.empty(10, dtype=torch.float32, device=v.device)  # a gsb_camera_model
+            ctx._backward_fisheye(v.data_ptr(), None if g is None else g.data_ptr(), self.grad.data_ptr(), stream,
+                                  grad_uniforms_ptr=gu, grad_lens_ptr=None if gl is None else gl.data_ptr(), **common)
+            if gl is not None:
+                grad_lens.copy_(gl[1:1 + LENS_WORDS])
         n = v.shape[0]
         if opacity_reg:
             self.grad[:, 7] += opacity_reg / n

@@ -389,6 +389,34 @@ int gsb_render_backward_features(gsb_ctx *ctx, const float *vertices, const floa
                                  const float *grad_feature_map, size_t feature_pitch_bytes, float *grad_vertices,
                                  gsb_uniforms *grad_uniforms, float *grad_features, float *density, void *stream);
 
+/* The camera gradient of a fisheye frame (gsb_set_camera_model): pose refinement and lens self-calibration through the lens.
+ * The arguments, preconditions and error codes of gsb_render_backward_features, except that
+ *   features, channels, grad_feature_map, grad_features
+ *                      features == NULL with channels == 0 means no feature map; grad_feature_map and grad_features must then
+ *                      be NULL too.  Otherwise as for gsb_render_backward_features.
+ *   grad_uniforms      device memory or NULL, OVERWRITTEN with dL/d(the frame's gsb_uniforms) in fp32.  Non-zero only in
+ *                      camera_position[0..2] (the SH view direction) and view_mat rows 0-2 ([c*4 + r], r != 3): through the
+ *                      view-space position t = V (p, 1) and through the view rotation W inside the EWA term J W.  Every other
+ *                      word -- proj_mat, tan_fovx, tan_fovy, view_mat row 3, camera_position[3], width, height -- is 0: a
+ *                      fisheye frame does not read them.
+ *   grad_lens          device memory or NULL, OVERWRITTEN with dL/d(fx, fy, cx, cy, k[0..3]) of the frame's lens, through uv
+ *                      and through the Jacobian J of the EWA term; kind and max_theta are written 0 (max_theta, the culls,
+ *                      radii and tile AABBs are step functions of the lens).
+ *   grad_vertices, grad_uniforms, grad_lens, grad_features
+ *                      each may be NULL, but not all four; density may be NULL, and needs grad_vertices, grad_uniforms or
+ *                      grad_lens
+ * and GSB_ERR_INVALID also when the last frame is a pinhole frame (its camera gradient is gsb_render_backward_camera's).
+ * grad_vertices, grad_features and density receive the words the other backward entries give for the same frame and upstream
+ * gradients.  The depth term (f = |t|) and the feature map's alpha terms reach the camera and lens words in the same pass.
+ * The camera words are reduced without global atomics, per CTA in fp64 then in one fixed-order pass; under
+ * gsb_set_backward_deterministic they are reproducible bit for bit, as the other outputs.  gsb_render_backward_camera,
+ * _density, _depth and _features keep returning GSB_ERR_INVALID for a non-NULL grad_uniforms on a fisheye frame. */
+int gsb_render_backward_fisheye(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,
+                                const float *grad_depth_alpha, size_t depth_pitch_bytes, const float *features, uint32_t channels,
+                                const float *grad_feature_map, size_t feature_pitch_bytes, float *grad_vertices,
+                                gsb_uniforms *grad_uniforms, gsb_camera_model *grad_lens, float *grad_features, float *density,
+                                void *stream);
+
 /* dL/d(background) of the last frame (gsb_set_background): grad_background (device, 3 floats) is OVERWRITTEN with
  * sum over the W x H pixels p of T_final(p) g(p), g from grad_image (as for gsb_render_backward: H x W float4,
  * row_pitch_bytes apart, 0 = tight, A ignored).  It does not depend on the background's value, so it is defined for a frame
