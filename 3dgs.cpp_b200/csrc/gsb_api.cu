@@ -374,8 +374,8 @@ static int enqueue_front(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uin
     if (timers) CK(cudaEventRecord(ctx->ev[0], stream));
 
     // ---- k_project: preprocess.comp + survivor compaction ----
-    const bool fisheye = ctx->camera.kind == GSB_CAMERA_FISHEYE;
-    CK(launch_project(project_params(ctx, *ubo, rb, re), ctx->debug, ctx->antialiased, stream, fisheye ? &ctx->camera : nullptr));
+    const bool lens = ctx->camera.kind != GSB_CAMERA_PINHOLE;
+    CK(launch_project(project_params(ctx, *ubo, rb, re), ctx->debug, ctx->antialiased, stream, lens ? &ctx->camera : nullptr));
     if (timers) CK(cudaEventRecord(ctx->ev[1], stream));
 
     if (ctx->use_graph && !timers && !ctx->debug) rc = launch_middle_graph(ctx, fp, sv, stream);
@@ -959,12 +959,28 @@ int gsb_set_camera_model(gsb_ctx* ctx, const gsb_camera_model* m) {
         ctx->camera = gsb_camera_model{};
         return GSB_OK;
     }
-    if (m->kind != GSB_CAMERA_FISHEYE) return bad("unknown camera kind");
+    if (m->kind != GSB_CAMERA_FISHEYE && m->kind != GSB_CAMERA_OPENCV) return bad("unknown camera kind");
     if (!(m->fx > 0.0f) || !(m->fy > 0.0f) || !isfinite(m->fx) || !isfinite(m->fy)) return bad("fx and fy must be positive and finite");
     const float rest[] = {m->cx, m->cy, m->k[0], m->k[1], m->k[2], m->k[3], m->max_theta};
     for (float x : rest)
         if (!isfinite(x)) return bad("every field must be finite");
     const double tmax = m->max_theta, k1 = m->k[0], k2 = m->k[1], k3 = m->k[2], k4 = m->k[3];
+    if (m->kind == GSB_CAMERA_OPENCV) {
+        if (!(tmax > 0.0) || !(tmax < M_PI / 2)) return bad("max_theta must lie in (0, pi / 2)");
+        // r R(r^2) strictly increasing on [0, tan max_theta]: d(r R) / dr = 1 + 3 k1 u + 5 k2 u^2 > 0 on u = r^2 in [0, umax].  A
+        // quadratic with value 1 at 0: positive everywhere iff positive at umax and at its vertex when that lies inside.  With
+        // p1 = p2 = 0 this also makes det D = R (1 + 3 k1 u + 5 k2 u^2) positive on the whole disc (R > 0 follows from r R > 0).
+        const double tt = std::tan(tmax), umax = tt * tt;
+        auto q = [&](double u) { return 1.0 + u * (3.0 * k1 + u * (5.0 * k2)); };
+        double qmin = q(umax);
+        if (k2 != 0.0) {
+            const double vertex = -3.0 * k1 / (10.0 * k2);
+            if (vertex > 0.0 && vertex < umax) qmin = std::min(qmin, q(vertex));
+        }
+        if (!(qmin > 0.0)) return bad("the radial map r R(r^2) must be strictly increasing on [0, tan max_theta]");
+        ctx->camera = *m;
+        return GSB_OK;
+    }
     if (!(tmax > 0.0) || !(tmax < M_PI)) return bad("max_theta must lie in (0, pi)");
     // theta_d strictly increasing on [0, max_theta]: d theta_d / d theta = 1 + 3 k1 t^2 + 5 k2 t^4 + 7 k3 t^6 + 9 k4 t^8 > 0.  In
     // u = t^2 that is a quartic q(u) on [0, tmax^2] with q(0) = 1: positive everywhere iff positive at the end and at every
@@ -1091,8 +1107,8 @@ struct FeatureArgs {
 // nullptr: no scene gradient (each entry's args_ok says which may be null).  density != nullptr: also accumulate the density
 // statistics into it.  grad_depth != nullptr (gsb_render_backward_depth): the frame must have depth, and grad_image may be
 // null (no colour gradient).  feat != nullptr (gsb_render_backward_features): also the feature map's gradient.
-// lens (gsb_render_backward_fisheye): the frame must be a fisheye frame, whose camera gradient goes to grad_ubo and grad_lens
-// (each may be null); grad_lens is set only then.
+// lens (gsb_render_backward_fisheye): the frame must be a lens frame (fisheye or OpenCV), whose camera gradient goes to
+// grad_ubo and grad_lens (each may be null); grad_lens is set only then.
 static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const float* vertices, const float* grad_image, size_t pitch,
                            float* grad_vertices, gsb_uniforms* grad_ubo, float* density, void* stream, const float* grad_depth = nullptr,
                            size_t depth_pitch = 0, const FeatureArgs* feat = nullptr, bool lens = false,
@@ -1107,10 +1123,13 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     if (ctx->scene_sh_half) return fail(ctx, GSB_ERR_INVALID, msg("fp16 SH storage has no backward pass").c_str());
     if (!args_ok) return fail(ctx, GSB_ERR_INVALID, msg("null argument").c_str());
     const LastFrame& f = ctx->frame;
-    const bool fisheye = f.camera.kind == GSB_CAMERA_FISHEYE;
-    if (lens && !fisheye)
+    const bool lens_frame = f.camera.kind != GSB_CAMERA_PINHOLE;  // fisheye or OpenCV
+    if (lens && !lens_frame)
         return fail(ctx, GSB_ERR_INVALID, msg("the last frame is a pinhole frame (its camera gradient is gsb_render_backward_camera's)").c_str());
-    if (!lens && fisheye && grad_ubo) return fail(ctx, GSB_ERR_INVALID, msg("a fisheye frame has no camera gradient").c_str());
+    if (!lens && lens_frame && grad_ubo)
+        return fail(ctx, GSB_ERR_INVALID,
+                    msg(f.camera.kind == GSB_CAMERA_FISHEYE ? "a fisheye frame has no camera gradient" : "an OpenCV frame has no camera gradient")
+                        .c_str());
     if (lens && density && !grad_vertices && !grad_ubo && !grad_lens)
         return fail(ctx, GSB_ERR_INVALID, msg("density needs grad_vertices, grad_uniforms or grad_lens").c_str());
     if (!lens && feat && density && !grad_vertices && !grad_ubo)
@@ -1195,7 +1214,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     }
     const FeatureParams* fpp = feat ? &fp : nullptr;
     if (!det) {
-        CK(launch_backward(bp, f.antialiased, bg, s, nullptr, fisheye ? &f.camera : nullptr, dp, fpp, grad_lens));
+        CK(launch_backward(bp, f.antialiased, bg, s, nullptr, lens_frame ? &f.camera : nullptr, dp, fpp, grad_lens));
         return GSB_OK;
     }
     const DetBuffers& d = ctx->bw_det;
@@ -1211,7 +1230,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     db.status_tiles = (uint32_t)(d.status.count / 256);
     db.m_hint = quantise_hint(ctx->m_hint);
     db.key_bits = std::max<uint32_t>(bits_for((uint32_t)n), 1u);  // compact ids < N_v <= n
-    CK(launch_backward(bp, f.antialiased, bg, s, &db, fisheye ? &f.camera : nullptr, dp, fpp, grad_lens));
+    CK(launch_backward(bp, f.antialiased, bg, s, &db, lens_frame ? &f.camera : nullptr, dp, fpp, grad_lens));
     return GSB_OK;
 }
 

@@ -24,8 +24,8 @@
 //                         record and returns its scratch accumulators to zero for the next call.  The CAMERA instantiation
 //                         (gsb_render_backward_camera) also keeps the camera's share of that chain rule -- view matrix,
 //                         projection matrix, camera position, tan_fov -- summed per thread, then per CTA into one fp64 row.
-//                         For a fisheye frame (gsb_render_backward_fisheye) the row holds the view matrix, the camera position
-//                         and the lens's fx, fy, cx, cy, k1..k4 instead.
+//                         For a lens frame, fisheye or OpenCV (gsb_render_backward_fisheye), the row holds the view matrix, the
+//                         camera position and the lens's fx, fy, cx, cy, k[0..3] instead.
 //   k_camera_reduce       one CTA: sums those rows in a fixed order into the fp32 gsb_uniforms of gradients
 //                         (k_fisheye_camera_reduce: into gsb_uniforms and gsb_camera_model).
 //
@@ -453,6 +453,9 @@ __host__ __device__ constexpr bool cam_word_live(int j) {
 // DEPTH (gsb_render_backward_depth): the survivor's dL/df (depth_scratch, returned to zero here) goes to the position through
 // the forward's own f: the view-space z of clip_view for a pinhole frame (dL/dv.z += dL/df, and with it dL/d(view row 2) in
 // the CAMERA instantiation), the distance d = |t| of fisheye_geo for a fisheye frame (dL/dt += (t / d) dL/df).
+// OPENCV (a frame of gsb_set_camera_model's OpenCV lens): as FISHEYE, through opencv_geo / opencv_jacobian / opencv_grad and,
+// with CAMERA, opencv_lens_grad.  It takes the fisheye's argument struct (the lens alone; the cull bound is not needed here).
+// Its depth key is z, so DEPTH adds dL/df to dL/dt.z.
 struct BackwardFisheyeParams : BackwardParams {
     gsb_camera_model cam;
 };
@@ -463,30 +466,33 @@ struct PbDepthParams : Base {
 template <bool FISHEYE, bool DEPTH = false>
 using PbParams = std::conditional_t<DEPTH, PbDepthParams<std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>,
                                     std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>;
-// CAMERA && FISHEYE (gsb_render_backward_fisheye): only the live words are accumulated -- camera_position.xyz, view_mat rows
-// 0-2 and the lens's fx, fy, cx, cy, k1..k4 -- and each CTA writes one fp64 row of FC_WORDS in this compact order for
-// k_fisheye_camera_reduce: [FC_POS + k] camera_position[k], [FC_VIEW + c * 3 + k] V[k][c] (word U_VIEW + c * 4 + k), [FC_LENS + j].
+// CAMERA on a lens frame (gsb_render_backward_fisheye, fisheye or OpenCV): only the live words are accumulated --
+// camera_position.xyz, view_mat rows 0-2 and the lens's fx, fy, cx, cy, k[0..3] -- and each CTA writes one fp64 row of FC_WORDS
+// in this compact order for k_fisheye_camera_reduce: [FC_POS + k] camera_position[k], [FC_VIEW + c * 3 + k] V[k][c] (word
+// U_VIEW + c * 4 + k), [FC_LENS + j].
 constexpr int FC_POS = 0, FC_VIEW = 3, FC_LENS = 15, FC_WORDS = 23;
 template <bool ON>
-struct FisheyeCamAcc {
+struct LensCamAcc {
     float w[FC_WORDS];
 };
 template <>
-struct FisheyeCamAcc<false> {};  // empty outside the new instantiations, for the reason given at det_partials()
-template <bool CAMERA, bool AA, bool FISHEYE = false, bool DEPTH = false>
-__global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ PbParams<FISHEYE, DEPTH> P) {
+struct LensCamAcc<false> {};  // empty outside the lens camera instantiations, for the reason given at det_partials()
+template <bool CAMERA, bool AA, bool FISHEYE = false, bool DEPTH = false, bool OPENCV = false>
+__global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ PbParams<FISHEYE || OPENCV, DEPTH> P) {
+    static_assert(!(FISHEYE && OPENCV), "one lens per frame");
+    constexpr bool LENS = FISHEYE || OPENCV;
     const uint32_t nv = P.ctl->num_visible;
     const gsb_uniforms& U = P.ubo;
     const float* pm = U.proj_mat;
     const float* vm = U.view_mat;
     const bool store_v = !CAMERA || P.grad_vertices != nullptr;  // frozen scene: camera only
     float cam[GSB_UBO_WORDS];
-    if constexpr (CAMERA && !FISHEYE) {
+    if constexpr (CAMERA && !LENS) {
 #pragma unroll
         for (int j = 0; j < GSB_UBO_WORDS; j++) cam[j] = 0.f;
     }
-    FisheyeCamAcc<CAMERA && FISHEYE> fc;
-    if constexpr (CAMERA && FISHEYE) {
+    LensCamAcc<CAMERA && LENS> fc;
+    if constexpr (CAMERA && LENS) {
 #pragma unroll
         for (int j = 0; j < FC_WORDS; j++) fc.w[j] = 0.f;
     }
@@ -523,13 +529,17 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         const float limx = J.limx, limy = J.limy, txtz = J.txtz, tytz = J.tytz, tx = J.tx, ty = J.ty;
         const float focal_x = J.focal_x, focal_y = J.focal_y, ja = J.ja, jb = J.jb, g0 = J.g0, g1 = J.g1;
         FisheyeGeo F;
-        FisheyeJ FJ;
+        OpencvGeo O;
+        LensJ FJ;
         if constexpr (FISHEYE) {
             F = fisheye_geo(P.cam, cv.vx, cv.vy, vz);
             FJ = fisheye_jacobian(P.cam, vm, F, cv.vx, cv.vy);
+        } else if constexpr (OPENCV) {
+            O = opencv_geo(P.cam, cv.vx, cv.vy, vz);
+            FJ = opencv_jacobian(P.cam, vm, O, vz);
         }
         const auto& JW = [&]() -> const auto& {
-            if constexpr (FISHEYE) return FJ;
+            if constexpr (LENS) return FJ;
             else return J;
         }();
         const float(&T0)[3] = JW.T0, (&T1)[3] = JW.T1;  // rows of J W (W = the view rotation)
@@ -588,7 +598,7 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         else dvx += dtx;
         if (tytz < -limy || tytz > limy) dvz += (tytz > 0.0f ? limy : -limy) * dty;
         else dvy += dty;
-        if constexpr (DEPTH && !FISHEYE) dvz += df;  // f = v.z
+        if constexpr (DEPTH && !LENS) dvz += df;  // f = v.z
         // uv = ((ndc + 1) size - 1) / 2, ndc = h.xy / h.w
         const float dndcx = d[0] * (0.5f * (float)U.width), dndcy = d[1] * (0.5f * (float)U.height);
         const float dhx = dndcx * p_w, dhy = dndcy * p_w, dhw = -(dndcx * ndcx + dndcy * ndcy) * p_w;
@@ -596,7 +606,7 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
 #pragma unroll
         for (int k = 0; k < 3; k++)
             dp[k] = ((pm[k * 4 + 0] * dhx + pm[k * 4 + 1] * dhy) + pm[k * 4 + 3] * dhw) + ((vm[k * 4 + 0] * dvx + vm[k * 4 + 1] * dvy) + vm[k * 4 + 2] * dvz);
-        if constexpr (FISHEYE) {  // J W -> J -> view-space position (with uv's own share) -> position
+        if constexpr (LENS) {  // J W -> J -> view-space position (with uv's own share) -> position
             float dJ[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
 #pragma unroll
             for (int r = 0; r < 3; r++) {
@@ -607,11 +617,16 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
                 }
             }
             float ftx, fty, ftz;
-            fisheye_grad(P.cam, F, FJ, cv.vx, cv.vy, vz, dJ, d[0], d[1], ftx, fty, ftz);
-            if constexpr (DEPTH) {  // f = d = |t|
-                ftx += (cv.vx / F.d) * df;
-                fty += (cv.vy / F.d) * df;
-                ftz += (vz / F.d) * df;
+            if constexpr (FISHEYE) {
+                fisheye_grad(P.cam, F, FJ, cv.vx, cv.vy, vz, dJ, d[0], d[1], ftx, fty, ftz);
+                if constexpr (DEPTH) {  // f = d = |t|
+                    ftx += (cv.vx / F.d) * df;
+                    fty += (cv.vy / F.d) * df;
+                    ftz += (vz / F.d) * df;
+                }
+            } else {
+                opencv_grad(P.cam, O, vz, dJ, d[0], d[1], ftx, fty, ftz);
+                if constexpr (DEPTH) ftz += df;  // f = z
             }
 #pragma unroll
             for (int k = 0; k < 3; k++) dp[k] = (vm[k * 4 + 0] * ftx + vm[k * 4 + 1] * fty) + vm[k * 4 + 2] * ftz;
@@ -625,7 +640,8 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
 #pragma unroll
                     for (int r = 0; r < 3; r++) fc.w[FC_VIEW + r * 3 + k] += dT0[r] * FJ.J[0][k] + dT1[r] * FJ.J[1][k];
                 }
-                fisheye_lens_grad(P.cam, F, cv.vx, cv.vy, dJ, d[0], d[1], fc.w + FC_LENS);
+                if constexpr (FISHEYE) fisheye_lens_grad(P.cam, F, cv.vx, cv.vy, dJ, d[0], d[1], fc.w + FC_LENS);
+                else opencv_lens_grad(P.cam, O, vz, dJ, d[0], d[1], fc.w + FC_LENS);
             }
         }
 
@@ -678,12 +694,12 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         dp[1] += (ddy - y * dot) / len;
         dp[2] += (ddz - z * dot) / len;
 
-        if constexpr (CAMERA && FISHEYE) {  // the view direction p - camera_position (the view and lens words are above)
+        if constexpr (CAMERA && LENS) {  // the view direction p - camera_position (the view and lens words are above)
             fc.w[FC_POS + 0] -= (ddx - x * dot) / len;
             fc.w[FC_POS + 1] -= (ddy - y * dot) / len;
             fc.w[FC_POS + 2] -= (ddz - z * dot) / len;
         }
-        if constexpr (CAMERA && !FISHEYE) {  // ---- this survivor's share of dL/d(UBO), the UBO's fields taken as independent inputs ----
+        if constexpr (CAMERA && !LENS) {  // ---- this survivor's share of dL/d(UBO), the UBO's fields taken as independent inputs ----
             const float p3[3] = {px, py, pz}, dv[3] = {dvx, dvy, dvz}, dh[4] = {dhx, dhy, 0.f, dhw};
 #pragma unroll
             for (int r = 0; r < 3; r++) {
@@ -752,7 +768,7 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         gv[10] = dqy;
         gv[11] = dqz;
     }
-    if constexpr (CAMERA && FISHEYE) {  // one row of FC_WORDS fp64 partial sums per CTA, as below
+    if constexpr (CAMERA && LENS) {  // one row of FC_WORDS fp64 partial sums per CTA, as below
         __shared__ double s_fc[PB_THREADS / 32][FC_WORDS];
         const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
@@ -770,7 +786,7 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
             P.cam_partials[(size_t)blockIdx.x * FC_WORDS + threadIdx.x] = a;
         }
     }
-    if constexpr (CAMERA && !FISHEYE) {  // one row of fp64 partial sums per CTA
+    if constexpr (CAMERA && !LENS) {  // one row of fp64 partial sums per CTA
         __shared__ double s_cam[PB_THREADS / 32][GSB_UBO_WORDS];
         const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
@@ -807,13 +823,13 @@ __global__ void __launch_bounds__(CR_THREADS) k_camera_reduce(const double* __re
     }
 }
 
-// The fisheye form of k_camera_reduce: sums the `rows` FC_WORDS-wide rows of k_preprocess_backward<true, AA, true> in the same
-// fixed order and writes the whole gsb_uniforms (zero outside camera_position.xyz and view rows 0-2) and the whole
-// gsb_camera_model of gradients (kind and max_theta 0); either output may be null.
+// The lens form of k_camera_reduce: sums the `rows` FC_WORDS-wide rows of k_preprocess_backward<true, AA, ...> on a fisheye or
+// OpenCV frame in the same fixed order and writes the whole gsb_uniforms (zero outside camera_position.xyz and view rows 0-2)
+// and the whole gsb_camera_model of gradients (kind and max_theta 0); either output may be null.
 __global__ void __launch_bounds__(CR_THREADS) k_fisheye_camera_reduce(const double* __restrict__ partials, uint32_t rows, gsb_uniforms* out,
                                                                       gsb_camera_model* lens) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (out) {  // the words no fisheye frame reads
+    if (out) {  // the words no lens frame reads
         for (int j = threadIdx.x; j < GSB_UBO_WORDS; j += CR_THREADS) {
             const bool live = j < 3 || (j >= U_VIEW && j < U_VIEW + 16 && (j & 3) != 3);
             if (!live) reinterpret_cast<float*>(out)[j] = 0.0f;
@@ -973,25 +989,29 @@ cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackwar
 
 // The vertex / camera part: k_preprocess_backward over the survivors (after the blend's sums and the density statistics).
 template <bool DEPTH>
-cudaError_t launch_preprocess_backward(const BackwardParams& p, bool antialiased, const gsb_camera_model* fisheye, const DepthBackward* dp,
+cudaError_t launch_preprocess_backward(const BackwardParams& p, bool antialiased, const gsb_camera_model* lens, const DepthBackward* dp,
                                        unsigned grid, cudaStream_t s, gsb_camera_model* grad_lens) {
     auto with_depth = [&](const auto& base) {
         if constexpr (DEPTH) return PbDepthParams<std::decay_t<decltype(base)>>{base, dp->scratch};
         else return base;
     };
-    if (fisheye) {
-        const auto fp = with_depth(BackwardFisheyeParams{p, *fisheye});
-        if (!p.cam_partials) {  // vertex gradients only
-            if (antialiased) k_preprocess_backward<false, true, true, DEPTH><<<grid, PB_THREADS, 0, s>>>(fp);
-            else k_preprocess_backward<false, false, true, DEPTH><<<grid, PB_THREADS, 0, s>>>(fp);
+    if (lens) {  // fisheye or OpenCV: the same launches, one lens instantiation each
+        const auto fp = with_depth(BackwardFisheyeParams{p, *lens});
+        auto launch = [&](auto opencv) {
+            constexpr bool OC = decltype(opencv)::value, FE = !OC;
+            if (!p.cam_partials) {  // vertex gradients only
+                if (antialiased) k_preprocess_backward<false, true, FE, DEPTH, OC><<<grid, PB_THREADS, 0, s>>>(fp);
+                else k_preprocess_backward<false, false, FE, DEPTH, OC><<<grid, PB_THREADS, 0, s>>>(fp);
+                return cudaGetLastError();
+            }
+            if (antialiased) k_preprocess_backward<true, true, FE, DEPTH, OC><<<grid, PB_THREADS, 0, s>>>(fp);
+            else k_preprocess_backward<true, false, FE, DEPTH, OC><<<grid, PB_THREADS, 0, s>>>(fp);
+            cudaError_t e = cudaGetLastError();
+            if (e != cudaSuccess) return e;
+            k_fisheye_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo, grad_lens);
             return cudaGetLastError();
-        }
-        if (antialiased) k_preprocess_backward<true, true, true, DEPTH><<<grid, PB_THREADS, 0, s>>>(fp);
-        else k_preprocess_backward<true, false, true, DEPTH><<<grid, PB_THREADS, 0, s>>>(fp);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return e;
-        k_fisheye_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo, grad_lens);
-        return cudaGetLastError();
+        };
+        return lens->kind == GSB_CAMERA_OPENCV ? launch(std::true_type{}) : launch(std::false_type{});
     }
     const auto pp = with_depth(p);
     if (!p.grad_ubo) {
@@ -1010,9 +1030,9 @@ cudaError_t launch_preprocess_backward(const BackwardParams& p, bool antialiased
 }  // namespace
 
 cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det,
-                            const gsb_camera_model* fisheye, const DepthBackward* depth, const FeatureParams* features,
+                            const gsb_camera_model* lens, const DepthBackward* depth, const FeatureParams* features,
                             gsb_camera_model* grad_lens) {
-    if (grad_lens && !fisheye) return cudaErrorInvalidValue;
+    if (grad_lens && !lens) return cudaErrorInvalidValue;
     const bool density = p.density != nullptr;
     const bool geometry = p.grad_vertices || p.cam_partials;  // false only for a feature gradient alone
     const bool colour = geometry && (p.grad_image || depth);
@@ -1052,8 +1072,8 @@ cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 ba
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
-    return depth ? launch_preprocess_backward<true>(p, antialiased, fisheye, depth, grid, s, grad_lens)
-                 : launch_preprocess_backward<false>(p, antialiased, fisheye, depth, grid, s, grad_lens);
+    return depth ? launch_preprocess_backward<true>(p, antialiased, lens, depth, grid, s, grad_lens)
+                 : launch_preprocess_backward<false>(p, antialiased, lens, depth, grid, s, grad_lens);
 }
 
 uint32_t background_grad_rows(uint32_t height) { return std::min(height, BG_MAX_ROWS); }

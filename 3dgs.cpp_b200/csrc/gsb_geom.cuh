@@ -99,12 +99,13 @@ __device__ __forceinline__ FisheyeGeo fisheye_geo(const gsb_camera_model& M, flo
     g.e = (1.0f + t2 * g.Q1) / (g.d * g.d);
     return g;
 }
-// J and the rows of T = J W (T0[r] = V[r][0] J[0][0] + V[r][1] J[0][1] + V[r][2] J[0][2], as jacobian() for its two terms)
-struct FisheyeJ {
+// J of a lens frame (fisheye or OpenCV) and the rows of T = J W (T0[r] = V[r][0] J[0][0] + V[r][1] J[0][1] + V[r][2] J[0][2],
+// as jacobian() for its two terms)
+struct LensJ {
     float J[2][3], T0[3], T1[3];
 };
-__device__ __forceinline__ FisheyeJ fisheye_jacobian(const gsb_camera_model& M, const float* vm, const FisheyeGeo& g, float x, float y) {
-    FisheyeJ j;
+__device__ __forceinline__ LensJ fisheye_jacobian(const gsb_camera_model& M, const float* vm, const FisheyeGeo& g, float x, float y) {
+    LensJ j;
     const float xyc = (x * y) * g.c;
     j.J[0][0] = M.fx * (g.s + (x * x) * g.c), j.J[0][1] = M.fx * xyc, j.J[0][2] = -M.fx * (x * g.e);
     j.J[1][0] = M.fy * xyc, j.J[1][1] = M.fy * (g.s + (y * y) * g.c), j.J[1][2] = -M.fy * (y * g.e);
@@ -119,7 +120,7 @@ __device__ __forceinline__ FisheyeJ fisheye_jacobian(const gsb_camera_model& M, 
 // c_x = dc/dx / x, c_z = dc/dz, e_x = de/dx / x, e_z = de/dz (ds/dx = x c, ds/dz = -e), all stable on the axis:
 //   c_x = 2 B' z b^4 / d^2 + 3 B S b^5,   c_z = -(2 B' theta r b^3 + 3 B b^2) / d^2,   B' = dB / dt2
 //   e_x = (z b R2 - 2 Q) / d^4,           e_z = -(R2 theta r + 2 Q z) / d^4,             R2 = rho'' / theta = 2 dQ / dt2
-__device__ __forceinline__ void fisheye_grad(const gsb_camera_model& M, const FisheyeGeo& g, const FisheyeJ& j, float x, float y,
+__device__ __forceinline__ void fisheye_grad(const gsb_camera_model& M, const FisheyeGeo& g, const LensJ& j, float x, float y,
                                              float z, const float (&dJ)[2][3], float du, float dv, float& dx, float& dy, float& dz) {
     const float t2 = g.t2, b = g.b;
     float dS;
@@ -178,6 +179,103 @@ __device__ __forceinline__ void fisheye_lens_grad(const gsb_camera_model& M, con
         dl[3 + j] += pw * (base + (float)(2 * j + 1) * odd);
         pw *= g.t2;
     }
+}
+
+// The OpenCV (Brown-Conrady radial-tangential) lens of gsb_set_camera_model (DESIGN.md section 23), for t = (x, y, z) in view
+// space with z > 0.2 and k = (k1, k2, p1, p2):
+//   xn = x / z, yn = y / z, r2 = xn^2 + yn^2, R = 1 + k1 r2 + k2 r2^2, R' = dR / dr2 = k1 + 2 k2 r2
+//   xd = xn R + 2 p1 xn yn + p2 (r2 + 2 xn^2),   yd = yn R + p1 (r2 + 2 yn^2) + 2 p2 xn yn,   uv = (fx xd + cx, fy yd + cy)
+//   D = d(xd, yd) / d(xn, yn), symmetric:  D00 = R + 2 xn^2 R' + 2 p1 yn + 6 p2 xn,  D11 = R + 2 yn^2 R' + 6 p1 yn + 2 p2 xn,
+//                                          D01 = D10 = 2 xn yn R' + 2 p1 xn + 2 p2 yn
+//   J = d uv / d t = diag(fx, fy) D N,  N = d(xn, yn) / dt = [1, 0, -xn; 0, 1, -yn] / z,  so with (e0, e1) = D (xn, yn):
+//   J = [fx D00, fx D01, -fx e0; fy D01, fy D11, -fy e1] / z
+// Polynomial in (xn, yn): no series and no singularity inside the cull (z > 0.2, r2 <= tan^2 max_theta, det D > 0).
+struct OpencvGeo {
+    float xn, yn, r2, R, Rp, xd, yd, D00, D01, D11, e0, e1, det;
+};
+__device__ __forceinline__ OpencvGeo opencv_geo(const gsb_camera_model& M, float x, float y, float z) {
+    const float k1 = M.k[0], k2 = M.k[1], p1 = M.k[2], p2 = M.k[3];
+    OpencvGeo g;
+    g.xn = x / z, g.yn = y / z;
+    const float xn = g.xn, yn = g.yn, xx = xn * xn, yy = yn * yn, xy = xn * yn;
+    g.r2 = xx + yy;
+    g.R = 1.0f + g.r2 * (k1 + g.r2 * k2);
+    g.Rp = k1 + (2.0f * k2) * g.r2;
+    g.xd = xn * g.R + ((2.0f * p1) * xy + p2 * (g.r2 + 2.0f * xx));
+    g.yd = yn * g.R + (p1 * (g.r2 + 2.0f * yy) + (2.0f * p2) * xy);
+    g.D00 = ((g.R + (2.0f * xx) * g.Rp) + (2.0f * p1) * yn) + (6.0f * p2) * xn;
+    g.D11 = ((g.R + (2.0f * yy) * g.Rp) + (6.0f * p1) * yn) + (2.0f * p2) * xn;
+    g.D01 = ((2.0f * xy) * g.Rp + (2.0f * p1) * xn) + (2.0f * p2) * yn;
+    g.e0 = g.D00 * xn + g.D01 * yn;
+    g.e1 = g.D01 * xn + g.D11 * yn;
+    g.det = g.D00 * g.D11 - g.D01 * g.D01;
+    return g;
+}
+__device__ __forceinline__ LensJ opencv_jacobian(const gsb_camera_model& M, const float* vm, const OpencvGeo& g, float z) {
+    LensJ j;
+    j.J[0][0] = (M.fx * g.D00) / z, j.J[0][1] = (M.fx * g.D01) / z, j.J[0][2] = -(M.fx * g.e0) / z;
+    j.J[1][0] = (M.fy * g.D01) / z, j.J[1][1] = (M.fy * g.D11) / z, j.J[1][2] = -(M.fy * g.e1) / z;
+#pragma unroll
+    for (int r = 0; r < 3; r++) {
+        j.T0[r] = (vm[r * 4 + 0] * j.J[0][0] + vm[r * 4 + 1] * j.J[0][1]) + vm[r * 4 + 2] * j.J[0][2];
+        j.T1[r] = (vm[r * 4 + 0] * j.J[1][0] + vm[r * 4 + 1] * j.J[1][1]) + vm[r * 4 + 2] * j.J[1][2];
+    }
+    return j;
+}
+// dL/dJ weighted by the focal lengths, (A, B) = (fx dJ[0], fy dJ[1]), folded through N: the J term of the loss is
+// Psi / z with Psi = a D00 + m D01 + c D11, a = A0 - A2 xn, m = A1 + B0 - A2 yn - B2 xn, c = B1 - B2 yn.
+struct OpencvDJ {
+    float A2, B2, a, m, c;
+};
+__device__ __forceinline__ OpencvDJ opencv_dj(const gsb_camera_model& M, const OpencvGeo& g, const float (&dJ)[2][3]) {
+    const float A0 = M.fx * dJ[0][0], A1 = M.fx * dJ[0][1], A2 = M.fx * dJ[0][2];
+    const float B0 = M.fy * dJ[1][0], B1 = M.fy * dJ[1][1], B2 = M.fy * dJ[1][2];
+    return OpencvDJ{A2, B2, A0 - A2 * g.xn, (A1 + B0) - (A2 * g.yn + B2 * g.xn), B1 - B2 * g.yn};
+}
+// The backward's share: dL/dt of Phi = Psi / z + du u + dv v.  D's derivatives are the third derivatives of one potential, so
+// four numbers hold them (R'' = 2 k2):
+//   H000 = dD00/dxn = 6 xn R' + 8 k2 xn^3 + 6 p2,        H001 = dD00/dyn = dD01/dxn = 2 yn R' + 8 k2 xn^2 yn + 2 p1
+//   H011 = dD11/dxn = dD01/dyn = 2 xn R' + 8 k2 xn yn^2 + 2 p2,   H111 = dD11/dyn = 6 yn R' + 8 k2 yn^3 + 6 p1
+// Then G = dPhi/d(xn, yn) = (dPsi/d(xn, yn)) / z + D (fx du, fy dv), and through (xn, yn, 1 / z) = (x, y, 1) / z:
+//   dx = Gx / z,  dy = Gy / z,  dz = -(Gx xn + Gy yn + Psi / z) / z.
+__device__ __forceinline__ void opencv_grad(const gsb_camera_model& M, const OpencvGeo& g, float z, const float (&dJ)[2][3], float du,
+                                            float dv, float& dx, float& dy, float& dz) {
+    const float k8 = 8.0f * M.k[1], p1 = M.k[2], p2 = M.k[3], xn = g.xn, yn = g.yn;
+    const OpencvDJ w = opencv_dj(M, g, dJ);
+    const float psi = (w.a * g.D00 + w.m * g.D01) + w.c * g.D11;
+    const float H000 = ((6.0f * xn) * g.Rp + ((k8 * xn) * xn) * xn) + 6.0f * p2;
+    const float H001 = ((2.0f * yn) * g.Rp + ((k8 * xn) * xn) * yn) + 2.0f * p1;
+    const float H011 = ((2.0f * xn) * g.Rp + ((k8 * yn) * yn) * xn) + 2.0f * p2;
+    const float H111 = ((6.0f * yn) * g.Rp + ((k8 * yn) * yn) * yn) + 6.0f * p1;
+    const float psx = ((w.a * H000 + w.m * H001) + w.c * H011) - (w.A2 * g.D00 + w.B2 * g.D01);
+    const float psy = ((w.a * H001 + w.m * H011) + w.c * H111) - (w.A2 * g.D01 + w.B2 * g.D11);
+    const float Lu = M.fx * du, Lv = M.fy * dv;
+    const float gx = psx / z + (Lu * g.D00 + Lv * g.D01);
+    const float gy = psy / z + (Lu * g.D01 + Lv * g.D11);
+    dx = gx / z;
+    dy = gy / z;
+    dz = -((gx * xn + gy * yn) + psi / z) / z;
+}
+// The lens's share (gsb_render_backward_fisheye on an OpenCV frame): adds dL/d(fx, fy, cx, cy, k1, k2, p1, p2) of uv and J to
+// dl.  d J / d fx = J's row 0 / fx (row 1 for fy), d uv / d(fx, fy) = (xd, 0), (0, yd), and with s = a + c,
+// q = a xn^2 + m xn yn + c yn^2, Ld = fx du xn + fy dv yn (opencv_dj's a, m, c):
+//   dL/dk1 = (r2 s + 2 q) / z + r2 Ld,   dL/dk2 = r2 ((r2 s + 4 q) / z + r2 Ld)
+//   dL/dp1 = (2 a yn + 2 m xn + 6 c yn) / z + fx du 2 xn yn + fy dv (r2 + 2 yn^2)
+//   dL/dp2 = (6 a xn + 2 m yn + 2 c xn) / z + fx du (r2 + 2 xn^2) + fy dv 2 xn yn
+__device__ __forceinline__ void opencv_lens_grad(const gsb_camera_model& M, const OpencvGeo& g, float z, const float (&dJ)[2][3],
+                                                 float du, float dv, float* dl) {
+    const float xn = g.xn, yn = g.yn, xx = xn * xn, yy = yn * yn, xy = xn * yn, r2 = g.r2;
+    dl[0] += du * g.xd + ((dJ[0][0] * g.D00 + dJ[0][1] * g.D01) - dJ[0][2] * g.e0) / z;
+    dl[1] += dv * g.yd + ((dJ[1][0] * g.D01 + dJ[1][1] * g.D11) - dJ[1][2] * g.e1) / z;
+    dl[2] += du;
+    dl[3] += dv;
+    const OpencvDJ w = opencv_dj(M, g, dJ);
+    const float Lu = M.fx * du, Lv = M.fy * dv;
+    const float s = w.a + w.c, q = ((w.a * xx + w.m * xy) + w.c * yy), Ld = Lu * xn + Lv * yn;
+    dl[4] += (r2 * s + 2.0f * q) / z + r2 * Ld;
+    dl[5] += r2 * ((r2 * s + 4.0f * q) / z + r2 * Ld);
+    dl[6] += (((2.0f * w.a) * yn + (2.0f * w.m) * xn) + (6.0f * w.c) * yn) / z + (Lu * (2.0f * xy) + Lv * (r2 + 2.0f * yy));
+    dl[7] += (((6.0f * w.a) * xn + (2.0f * w.m) * yn) + (2.0f * w.c) * xn) / z + (Lu * (r2 + 2.0f * xx) + Lv * (2.0f * xy));
 }
 
 // cov2d = transpose(T) Sigma T + 0.3 I (:56-65), Sigma = the cov3d words ca.xyzw, cb.xy; tm0 / tm1 = Sigma T0 / Sigma T1 (S[k] =

@@ -103,8 +103,9 @@ struct EmitParams {
 cudaError_t launch_cov3d(const float* vtx_aos, uint64_t count, uint64_t dst_offset, float4* pos_op,
                          float4* cov_a, float2* cov_b, float* sh, float scale_factor, cudaStream_t s, bool sh_half = false);
 // antialiased: gsb_set_antialiased's opacity compensation (not on the routed kernel of a sharded frame)
-// fisheye: gsb_set_camera_model's lens (k_project<..., FISHEYE = true>, plain contexts only); null = the pinhole camera.
-cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* fisheye = nullptr);
+// lens: gsb_set_camera_model's fisheye or OpenCV lens (k_project<..., FISHEYE> or <..., OPENCV>, plain contexts only); null =
+// the pinhole camera.
+cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* lens = nullptr);
 cudaError_t launch_emit(const EmitParams& p, cudaStream_t s);
 
 struct SortParams {  // host-side arguments of launch_sort
@@ -221,8 +222,8 @@ struct DetBackward {
 // background: the frame's gsb_set_background, the colour behind every pixel's last contributor.  It is a kernel argument of
 // its own after BackwardParams, not a field of it: a larger BackwardParams would move the arguments that follow it in
 // k_det_reduce.
-// fisheye: the frame's gsb_set_camera_model lens, null for a pinhole frame.  With p.cam_partials set, a fisheye frame's camera
-// gradient (gsb_render_backward_fisheye): p.grad_ubo and grad_lens, either may be null; grad_lens needs a fisheye frame.
+// lens: the frame's gsb_set_camera_model lens (fisheye or OpenCV), null for a pinhole frame.  With p.cam_partials set, a lens
+// frame's camera gradient (gsb_render_backward_fisheye): p.grad_ubo and grad_lens, either may be null; grad_lens needs a lens.
 // depth: gsb_render_backward_depth's upstream dL/d(D, A) and its per-survivor scratch (p.grad_image may then be null); null for
 // the colour-only entries.
 struct DepthBackward {
@@ -264,7 +265,7 @@ cudaError_t launch_feature_backward(FeatureParams p, bool det, cudaStream_t s);
 // pass's sums (which are skipped when there is neither an image nor a depth gradient) and before k_density_accumulate and
 // k_preprocess_backward; with neither grad_vertices nor grad_ubo only the feature gradient is formed.
 cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det = nullptr,
-                            const gsb_camera_model* fisheye = nullptr, const DepthBackward* depth = nullptr,
+                            const gsb_camera_model* lens = nullptr, const DepthBackward* depth = nullptr,
                             const FeatureParams* features = nullptr, gsb_camera_model* grad_lens = nullptr);
 // gsb_background_gradient: out[c] = sum over the W x H pixels of T_final(p) grad_image(p)[c], from the recorded frame's
 // (bits(T), last) words.  fp64 products and sums in an order fixed by W and H (background_grad_rows(H) per-CTA partials,

@@ -16,6 +16,7 @@
 // of the GLSL source, so results are value-identical to the oracle (bit-exact parity).
 #include <cuda_fp16.h>
 
+#include <cmath>
 #include <type_traits>
 
 #include "gsb_cull.cuh"
@@ -167,6 +168,9 @@ __device__ __forceinline__ void compute_sh(const float4* __restrict__ sh4, float
 #ifndef GSB_PROJECT_FISHEYE_MIN_BLOCKS
 #define GSB_PROJECT_FISHEYE_MIN_BLOCKS 4
 #endif
+#ifndef GSB_PROJECT_OPENCV_MIN_BLOCKS
+#define GSB_PROJECT_OPENCV_MIN_BLOCKS 4
+#endif
 // ROUTED (frame sharding, gsb_shard.cu): the single stream compaction becomes one compaction per destination band -- G
 // simultaneous decoupled look-back scans over G-wide status vectors, warp d walking column d -- and the record goes straight
 // from registers into the exchange buffer of every rank whose band the AABB touches (stores into peer-mapped memory over
@@ -177,12 +181,18 @@ __device__ __forceinline__ void compute_sh(const float4* __restrict__ sh4, float
 // FISHEYE (gsb_set_camera_model, plain contexts only): the projection, Jacobian and cull of the fisheye lens (gsb_geom.cuh's
 // fisheye_geo / fisheye_jacobian) and the depth key d = |t| instead of z; everything from cov2d on is the pinhole path's.  Only
 // the FISHEYE instantiations take the larger argument, so the others keep their code.
+// OPENCV (gsb_set_camera_model, plain contexts only): the projection, Jacobian and cull of the OpenCV lens (opencv_geo /
+// opencv_jacobian); the depth key stays z.  tan2_max is tan^2(max_theta), rounded to fp32 once on the host.
 struct ProjectFisheyeParams : ProjectParams {
     gsb_camera_model cam;
 };
-template <bool FISHEYE>
-using ProjParams = std::conditional_t<FISHEYE, ProjectFisheyeParams, ProjectParams>;
-template <bool FISHEYE>
+struct ProjectOpencvParams : ProjectParams {
+    gsb_camera_model cam;
+    float tan2_max;
+};
+template <bool FISHEYE, bool OPENCV = false>
+using ProjParams = std::conditional_t<FISHEYE, ProjectFisheyeParams, std::conditional_t<OPENCV, ProjectOpencvParams, ProjectParams>>;
+template <bool FISHEYE, bool OPENCV = false>
 struct ProjectBounds {
     static constexpr int MIN_BLOCKS = GSB_PROJECT_MIN_BLOCKS;
 };
@@ -190,10 +200,16 @@ template <>
 struct ProjectBounds<true> {
     static constexpr int MIN_BLOCKS = GSB_PROJECT_FISHEYE_MIN_BLOCKS;
 };
-template <bool DEBUG, bool ROUTED, bool SH16, bool AA, bool FISHEYE = false>
-__global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE>::MIN_BLOCKS) k_project(const __grid_constant__ ProjParams<FISHEYE> P) {
+template <>
+struct ProjectBounds<false, true> {
+    static constexpr int MIN_BLOCKS = GSB_PROJECT_OPENCV_MIN_BLOCKS;
+};
+template <bool DEBUG, bool ROUTED, bool SH16, bool AA, bool FISHEYE = false, bool OPENCV = false>
+__global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE, OPENCV>::MIN_BLOCKS)
+    k_project(const __grid_constant__ ProjParams<FISHEYE, OPENCV> P) {
     static_assert(!(ROUTED && AA), "sharded contexts have no anti-aliased mode");
     static_assert(!(ROUTED && FISHEYE), "sharded contexts have no fisheye camera");
+    static_assert(!(ROUTED && OPENCV) && !(FISHEYE && OPENCV), "sharded contexts have no OpenCV camera; one lens per frame");
     __shared__ uint32_t s_chunk;
     __shared__ uint32_t s_wsurv[PRE_THREADS / 32];
     __shared__ uint32_t s_base_surv;
@@ -227,17 +243,24 @@ __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE>::MIN_BLOCK
         const ClipView cv = clip_view(U, px, py, pz);
         const float ndcx = cv.ndcx, ndcy = cv.ndcy, vz = cv.vz;
         FisheyeGeo F;
+        OpencvGeo O;
         bool front;
         if constexpr (FISHEYE) {
             F = fisheye_geo(P.cam, cv.vx, cv.vy, vz);
             front = F.d > 0.2f && F.theta <= P.cam.max_theta;  // NaN is culled
+        } else if constexpr (OPENCV) {
+            O = opencv_geo(P.cam, cv.vx, cv.vy, vz);
+            front = vz > 0.2f && O.r2 <= P.tan2_max && O.det > 0.0f;  // NaN is culled; so is a tangential fold
         } else {
             front = !(vz <= 0.2f);  // :135 (NaN is not culled by the shader's test either)
         }
         if (front) {
             Cov2d cov;
             if constexpr (FISHEYE) {
-                const FisheyeJ J = fisheye_jacobian(P.cam, U.view_mat, F, cv.vx, cv.vy);
+                const LensJ J = fisheye_jacobian(P.cam, U.view_mat, F, cv.vx, cv.vy);
+                cov = cov2d(J.T0, J.T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
+            } else if constexpr (OPENCV) {
+                const LensJ J = opencv_jacobian(P.cam, U.view_mat, O, vz);
                 cov = cov2d(J.T0, J.T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
             } else {
                 const Jacobian J = jacobian(U, cv.vx, cv.vy, vz);
@@ -258,6 +281,9 @@ __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE>::MIN_BLOCK
                 if constexpr (FISHEYE) {
                     uvx = P.cam.fx * (F.s * cv.vx) + P.cam.cx;
                     uvy = P.cam.fy * (F.s * cv.vy) + P.cam.cy;
+                } else if constexpr (OPENCV) {
+                    uvx = P.cam.fx * O.xd + P.cam.cx;
+                    uvy = P.cam.fy * O.yd + P.cam.cy;
                 } else {
                     uvx = ((ndcx + 1.0f) * (float)W - 1.0f) * 0.5f;  // :157 ndc2Pix
                     uvy = ((ndcy + 1.0f) * (float)H - 1.0f) * 0.5f;
@@ -835,30 +861,35 @@ __global__ void __launch_bounds__(PRE_THREADS) k_emit_coarse(const __grid_consta
 
 }  // namespace
 
-template <bool AA, bool FISHEYE>
-void launch_project_plain(const ProjParams<FISHEYE>& p, bool debug, unsigned blocks, cudaStream_t s) {
+template <bool AA, bool FISHEYE, bool OPENCV>
+void launch_project_plain(const ProjParams<FISHEYE, OPENCV>& p, bool debug, unsigned blocks, cudaStream_t s) {
     if (p.sh_half) {  // fp16 SH storage (non-parity)
-        if (debug) k_project<true, false, true, AA, FISHEYE><<<blocks, PRE_THREADS, 0, s>>>(p);
-        else k_project<false, false, true, AA, FISHEYE><<<blocks, PRE_THREADS, 0, s>>>(p);
-    } else if (debug) k_project<true, false, false, AA, FISHEYE><<<blocks, PRE_THREADS, 0, s>>>(p);
-    else k_project<false, false, false, AA, FISHEYE><<<blocks, PRE_THREADS, 0, s>>>(p);
+        if (debug) k_project<true, false, true, AA, FISHEYE, OPENCV><<<blocks, PRE_THREADS, 0, s>>>(p);
+        else k_project<false, false, true, AA, FISHEYE, OPENCV><<<blocks, PRE_THREADS, 0, s>>>(p);
+    } else if (debug) k_project<true, false, false, AA, FISHEYE, OPENCV><<<blocks, PRE_THREADS, 0, s>>>(p);
+    else k_project<false, false, false, AA, FISHEYE, OPENCV><<<blocks, PRE_THREADS, 0, s>>>(p);
 }
 
-template <bool FISHEYE>
-void launch_project_plain(const ProjParams<FISHEYE>& p, bool debug, bool antialiased, unsigned blocks, cudaStream_t s) {
-    if (antialiased) launch_project_plain<true, FISHEYE>(p, debug, blocks, s);
-    else launch_project_plain<false, FISHEYE>(p, debug, blocks, s);
+template <bool FISHEYE, bool OPENCV = false>
+void launch_project_plain(const ProjParams<FISHEYE, OPENCV>& p, bool debug, bool antialiased, unsigned blocks, cudaStream_t s) {
+    if (antialiased) launch_project_plain<true, FISHEYE, OPENCV>(p, debug, blocks, s);
+    else launch_project_plain<false, FISHEYE, OPENCV>(p, debug, blocks, s);
 }
 
-cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* fisheye) {
+cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* lens) {
+    const gsb_camera_model* fisheye = lens && lens->kind == GSB_CAMERA_FISHEYE ? lens : nullptr;
+    const gsb_camera_model* opencv = lens && lens->kind == GSB_CAMERA_OPENCV ? lens : nullptr;
     if (p.n == 0) return cudaSuccess;
     const unsigned blocks = (p.n + PRE_THREADS - 1) / PRE_THREADS;
     if (p.route_world > 0) {
-        if (antialiased || fisheye) return cudaErrorInvalidValue;  // the routed kernel has no AA or fisheye instantiation
+        if (antialiased || lens) return cudaErrorInvalidValue;  // the routed kernel has no AA or lens instantiation
         if (p.sh_half) k_project<false, true, true, false><<<blocks, PRE_THREADS, 0, s>>>(p);
         else k_project<false, true, false, false><<<blocks, PRE_THREADS, 0, s>>>(p);
     } else if (fisheye) {
         launch_project_plain<true>(ProjectFisheyeParams{p, *fisheye}, debug, antialiased, blocks, s);
+    } else if (opencv) {
+        const double t = std::tan((double)opencv->max_theta);
+        launch_project_plain<false, true>(ProjectOpencvParams{p, *opencv, (float)(t * t)}, debug, antialiased, blocks, s);
     } else {
         launch_project_plain<false>(p, debug, antialiased, blocks, s);
     }

@@ -31,7 +31,7 @@ ERR_INVALID, ERR_NO_DEVICE, ERR_CUDA, ERR_NO_SCENE, ERR_OOM, ERR_OVERFLOW = -1, 
 FORMAT_RGBA32F, FORMAT_RGBA8, FORMAT_BGRA8 = 0, 1, 2
 MODE_EXACT, MODE_FAST = 0, 1
 MEM_HOST, MEM_DEVICE = 0, 1
-CAMERA_PINHOLE, CAMERA_FISHEYE = 0, 1
+CAMERA_PINHOLE, CAMERA_FISHEYE, CAMERA_OPENCV = 0, 1, 2
 (BUF_COV3D, BUF_ATTR, BUF_TILES_OVERLAP, BUF_PREFIX_SUM, BUF_KEYS_UNSORTED, BUF_VALS_UNSORTED,
  BUF_KEYS_SORTED, BUF_VALS_SORTED, BUF_TILE_BOUNDARY, BUF_DEPTH_ORDER, BUF_EMIT_OFFSETS) = range(11)
 ALL_ROWS = 0xFFFFFFFF
@@ -49,7 +49,7 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_render_depth", "gsb_render_backward_depth",
     # rendered feature maps with their gradients
     "gsb_render_features", "gsb_render_backward_features", "gsb_adam_step_features",
-    # camera and lens gradients through the fisheye
+    # camera and lens gradients through a lens (fisheye or OpenCV)
     "gsb_render_backward_fisheye",
     # training loss, optimizer step and initialisation from a point cloud
     "gsb_image_loss", "gsb_adam_step", "gsb_init_from_points",
@@ -124,7 +124,8 @@ class SynthParams(C.Structure):
 
 
 class CameraModel(C.Structure):
-    """gsb_camera_model: the lens of gsb_set_camera_model (fisheye_camera / fisheye_from_colmap make one)."""
+    """gsb_camera_model: the lens of gsb_set_camera_model (fisheye_camera, fisheye_from_colmap, opencv_camera,
+    opencv_from_colmap and camera_from_colmap make one)."""
     _fields_ = [("kind", C.c_uint32), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
                 ("k", C.c_float * 4), ("max_theta", C.c_float)]
 
@@ -149,25 +150,94 @@ def fisheye_camera(fx, fy, cx, cy, k=(0.0, 0.0, 0.0, 0.0), max_theta=None) -> Ca
     return CameraModel(CAMERA_FISHEYE, float(fx), float(fy), float(cx), float(cy), (C.c_float * 4)(*k), float(max_theta))
 
 
-LENS_WORDS = 8  # (fx, fy, cx, cy, k1, k2, k3, k4): lens_tensor's layout and gsb_render_backward_fisheye's grad_lens words 1-8
+# opencv_camera's default max_theta never exceeds this (80 deg).  A choice, not a measured optimum: a phone or DSLR lens
+# calibrated as OPENCV rarely sees farther off the axis, and past it the polynomial is an extrapolation of the calibration.
+OPENCV_MAX_THETA_CAP = 80.0 * np.pi / 180.0
+
+
+def opencv_monotone_limit(k1, k2) -> float:
+    """The largest r^2 up to which the radial map r R(r^2), R = 1 + k1 r^2 + k2 r^4, is strictly increasing: the smallest
+    positive root of 1 + 3 k1 u + 5 k2 u^2 (inf if there is none), in closed form."""
+    k1, k2 = float(k1), float(k2)
+    if k2 == 0.0:
+        return -1.0 / (3.0 * k1) if k1 < 0.0 else np.inf
+    disc = 9.0 * k1 * k1 - 20.0 * k2
+    if disc < 0.0:
+        return np.inf
+    sq = np.sqrt(disc)
+    # the two roots as -2 / (3 k1 +- sq) (the stable form of (-3 k1 -+ sq) / (10 k2)); only a positive one bounds the map
+    roots = [-2.0 / d for d in (3.0 * k1 + sq, 3.0 * k1 - sq) if d != 0.0]
+    positive = [r for r in roots if r > 0.0]
+    return min(positive) if positive else np.inf
+
+
+def opencv_camera(fx, fy, cx, cy, k=(0.0, 0.0, 0.0, 0.0), max_theta=None) -> CameraModel:
+    """An OpenCV (Brown-Conrady radial-tangential) lens for Context.set_camera_model, k = (k1, k2, p1, p2) in COLMAP's OPENCV
+    order: xn = x / z, yn = y / z, r^2 = xn^2 + yn^2, R = 1 + k1 r^2 + k2 r^4, xd = xn R + 2 p1 xn yn + p2 (r^2 + 2 xn^2),
+    yd = yn R + p1 (r^2 + 2 yn^2) + 2 p2 xn yn, uv = (fx xd + cx, fy yd + cy), pixel (i, j) sampled at (i, j) (so cx, cy are
+    COLMAP's minus 0.5; see opencv_from_colmap).  max_theta (radians, in (0, pi/2)) culls rays farther off the axis; None =
+    the largest angle up to OPENCV_MAX_THETA_CAP at which r R(r^2) is still increasing (opencv_monotone_limit, less 1e-4 of
+    it in r^2 so that gsb_set_camera_model's strict test passes)."""
+    k = [float(x) for x in k]
+    if len(k) != 4:
+        raise ValueError("opencv_camera: k must hold 4 coefficients (k1, k2, p1, p2)")
+    if max_theta is None:
+        u0 = opencv_monotone_limit(k[0], k[1])
+        max_theta = OPENCV_MAX_THETA_CAP if not np.isfinite(u0) else min(OPENCV_MAX_THETA_CAP, float(np.arctan(np.sqrt(u0 * (1.0 - 1e-4)))))
+    return CameraModel(CAMERA_OPENCV, float(fx), float(fy), float(cx), float(cy), (C.c_float * 4)(*k), float(max_theta))
+
+
+def opencv_from_colmap(fx, fy, cx, cy, k1, k2, p1, p2) -> CameraModel:
+    """COLMAP's OPENCV parameters (fx, fy, cx, cy, k1, k2, p1, p2) as an opencv_camera.  COLMAP puts pixel centres at i + 0.5,
+    this renderer samples pixel (i, j) at (i, j): the principal point moves by half a pixel."""
+    return opencv_camera(fx, fy, float(cx) - 0.5, float(cy) - 0.5, (k1, k2, p1, p2))
+
+
+def camera_from_colmap(model: str, params) -> CameraModel:
+    """The CameraModel of a COLMAP camera (its model name and params, as cameras.txt lists them).  SIMPLE_PINHOLE (f, cx, cy),
+    PINHOLE (fx, fy, cx, cy), SIMPLE_RADIAL (f, cx, cy, k), RADIAL (f, cx, cy, k1, k2) and OPENCV (fx, fy, cx, cy, k1, k2, p1,
+    p2) become opencv_from_colmap with 0 for the coefficients a model lacks; OPENCV_FISHEYE (fx, fy, cx, cy, k1..k4) becomes
+    fisheye_from_colmap.  Any other model (FULL_OPENCV, THIN_PRISM_FISHEYE, ...) raises ValueError."""
+    p = [float(x) for x in params]
+    counts = {"SIMPLE_PINHOLE": 3, "PINHOLE": 4, "SIMPLE_RADIAL": 4, "RADIAL": 5, "OPENCV": 8, "OPENCV_FISHEYE": 8}
+    if model not in counts:
+        raise ValueError(f"camera_from_colmap: unsupported COLMAP camera model {model!r}")
+    if len(p) != counts[model]:
+        raise ValueError(f"camera_from_colmap: {model} takes {counts[model]} parameters, got {len(p)}")
+    if model == "OPENCV_FISHEYE":
+        return fisheye_from_colmap(*p)
+    if model == "OPENCV":
+        return opencv_from_colmap(*p)
+    if model == "PINHOLE":
+        return opencv_from_colmap(*p, 0.0, 0.0, 0.0, 0.0)
+    f, cx, cy, ks = p[0], p[1], p[2], p[3:]
+    k1, k2 = (ks + [0.0, 0.0])[:2]
+    return opencv_from_colmap(f, f, cx, cy, k1, k2, 0.0, 0.0)
+
+
+LENS_WORDS = 8  # (fx, fy, cx, cy, k[0..3]): lens_tensor's layout and gsb_render_backward_fisheye's grad_lens words 1-8
 
 
 def lens_tensor(cam: CameraModel, device=None):
-    """The (8,) float32 tensor (fx, fy, cx, cy, k1..k4) of a fisheye CameraModel, for render_torch(..., lens=): a lens a
-    torch optimizer can refine.  lens_camera turns it back into the same CameraModel, bit for bit."""
+    """The (8,) float32 tensor (fx, fy, cx, cy, k[0..3]) of a fisheye or OpenCV CameraModel (k1..k4 for a fisheye, k1, k2, p1,
+    p2 for OpenCV), for render_torch(..., lens=): a lens a torch optimizer can refine.  lens_camera turns it back into the
+    same CameraModel, bit for bit."""
     import torch
 
     return torch.tensor(np.array([cam.fx, cam.fy, cam.cx, cam.cy, *cam.k], np.float32), device=device)
 
 
-def lens_camera(lens, max_theta) -> CameraModel:
-    """The fisheye CameraModel of an (8,) lens tensor (lens_tensor's layout) culled at max_theta (radians), bit for bit."""
+def lens_camera(lens, max_theta, kind=CAMERA_FISHEYE) -> CameraModel:
+    """The CameraModel of kind `kind` (CAMERA_FISHEYE, the default, or CAMERA_OPENCV) of an (8,) lens tensor (lens_tensor's
+    layout) culled at max_theta (radians), bit for bit."""
     import torch
 
     w = lens.detach().to("cpu", torch.float32).reshape(-1).numpy() if isinstance(lens, torch.Tensor) else np.asarray(lens, np.float32)
     if w.shape != (LENS_WORDS,):
-        raise ValueError(f"lens_camera: the lens must hold {LENS_WORDS} values (fx, fy, cx, cy, k1..k4)")
-    return CameraModel(CAMERA_FISHEYE, *(float(x) for x in w[:4]), (C.c_float * 4)(*(float(x) for x in w[4:])), float(max_theta))
+        raise ValueError(f"lens_camera: the lens must hold {LENS_WORDS} values (fx, fy, cx, cy, k[0..3])")
+    if kind not in (CAMERA_FISHEYE, CAMERA_OPENCV):
+        raise ValueError("lens_camera: kind must be CAMERA_FISHEYE or CAMERA_OPENCV")
+    return CameraModel(kind, *(float(x) for x in w[:4]), (C.c_float * 4)(*(float(x) for x in w[4:])), float(max_theta))
 
 
 def fisheye_from_colmap(fx, fy, cx, cy, k1, k2, k3, k4) -> CameraModel:
@@ -555,11 +625,12 @@ class Context:
         self._background = None if rgb is None else [float(x) for x in rgb]
 
     def set_camera_model(self, cam=None):
-        """gsb_set_camera_model: from the next frame, project through the lens `cam` (a CameraModel from fisheye_camera or
-        fisheye_from_colmap; None or kind CAMERA_PINHOLE = the UBO's pinhole camera, the default).  A fisheye frame reads only
-        the UBO's view matrix, camera position and size.  Frames, render_torch, SceneAdam and the backward pass follow it
-        (the backward uses the model of the frame it differentiates).  The camera and lens gradients of a fisheye frame come
-        from gsb_render_backward_fisheye (Context._backward_fisheye, render_torch(..., lens=), SceneAdam.step)."""
+        """gsb_set_camera_model: from the next frame, project through the lens `cam` (a CameraModel from fisheye_camera,
+        fisheye_from_colmap, opencv_camera, opencv_from_colmap or camera_from_colmap; None or kind CAMERA_PINHOLE = the UBO's
+        pinhole camera, the default).  A lens frame (fisheye or OpenCV) reads only the UBO's view matrix, camera position and
+        size.  Frames, render_torch, SceneAdam and the backward pass follow it (the backward uses the model of the frame it
+        differentiates).  The camera and lens gradients of a lens frame come from gsb_render_backward_fisheye
+        (Context._backward_fisheye, render_torch(..., lens=), SceneAdam.step)."""
         self._ck(lib.gsb_set_camera_model(self.h, None if cam is None else C.byref(cam)))
         self.camera = None if cam is None or cam.kind == CAMERA_PINHOLE else cam
 
@@ -609,7 +680,7 @@ class Context:
     def render_depth(self, u: Uniforms, fmt=FORMAT_RGBA32F, rows=None):
         """gsb_render_depth to HOST numpy arrays: (image, depth_alpha), the image as render() gives it and depth_alpha an
         (rows, W, 2) float32 array of (D, A) per pixel: D = sum f alpha T (f the view-space z, or the distance for a fisheye
-        camera) and A = 1 - T_final.  Expected depth is D / A."""
+        camera; z for an OpenCV camera) and A = 1 - T_final.  Expected depth is D / A."""
         rb, re, nrows = self.band_rows(u, rows)
         out = np.empty((nrows, u.width, 4), np.float32 if fmt == FORMAT_RGBA32F else np.uint8)
         da = np.empty((nrows, u.width, 2), np.float32)
@@ -739,7 +810,7 @@ class Context:
                           density_ptr=None, grad_depth_alpha_ptr=None, features=None, grad_feature_map=None, grad_features_ptr=None,
                           row_pitch_bytes=0):
         """gsb_render_backward_fisheye on device pointers, `stream` the C ABI's cudaStream_t: _backward's arguments plus the
-        camera gradient of the last (fisheye) frame, grad_uniforms_ptr (160 B, dL/d gsb_uniforms, pose words only) and
+        camera gradient of the last (fisheye or OpenCV) frame, grad_uniforms_ptr (160 B, dL/d gsb_uniforms, pose words only) and
         grad_lens_ptr (40 B, a gsb_camera_model of dL/d(fx, fy, cx, cy, k)), each overwritten and each may be None."""
         fptr, fch, gfm, fpitch = (None, 0, None, 0) if features is None else (
             features.data_ptr(), features.shape[1], grad_feature_map.data_ptr(), grad_feature_map.stride()[0] * 4)
@@ -1074,15 +1145,16 @@ def _render_fn():
                 fctx.density = density
                 fctx.lens_like = None
                 cam = None
-                if lens is not None:  # this frame through the tensor's lens, culled at the context's max_theta or the default
-                    w = lens.detach().to("cpu", torch.float32).reshape(-1)
-                    max_theta = (ctx.camera.max_theta if ctx.camera is not None
-                                 else fisheye_camera(*w[:4].tolist(), w[4:].tolist()).max_theta)
-                    cam = lens_camera(w, max_theta)
+                if lens is not None:  # this frame through the tensor's lens, of the context's kind and max_theta, or the
+                    w = lens.detach().to("cpu", torch.float32).reshape(-1)  # fisheye's default on a pinhole context
+                    if ctx.camera is not None:
+                        cam = lens_camera(w, ctx.camera.max_theta, ctx.camera.kind)
+                    else:
+                        cam = lens_camera(w, fisheye_camera(*w[:4].tolist(), w[4:].tolist()).max_theta)
                     fctx.lens_like = (lens.dtype, lens.device)
                 if ubo is not None:  # the camera's float fields come from the tensor, the frame size from u
                     if ctx.camera is not None and cam is None:
-                        raise ValueError("render_torch: ubo= on a fisheye camera model needs lens= (its camera gradient is "
+                        raise ValueError("render_torch: ubo= on a lens camera model needs lens= (its camera gradient is "
                                          "gsb_render_backward_fisheye's)")
                     u = unpack_uniforms(ubo.detach().to("cpu", torch.float32).numpy(), u.width, u.height)
                     fctx.ubo_like = (ubo.dtype, ubo.device)
@@ -1210,18 +1282,19 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, 
     off): every gradient and density statistic is then bit-identical for the same inputs, at some cost in time.  With
     torch's default settings backward takes the atomic path, whose results may differ in the last bit from run to run.
 
-    The frame is projected through the context's camera model (Context.set_camera_model); ubo= on a fisheye context raises
-    ValueError unless lens= is given.
+    The frame is projected through the context's camera model (Context.set_camera_model); ubo= on a fisheye or OpenCV
+    context raises ValueError unless lens= is given.
 
-    lens (optional): an (8,) tensor (fx, fy, cx, cy, k1..k4) (lens_tensor makes one).  The frame is rendered through
-    lens_camera(lens, max_theta), max_theta that of the context's fisheye model if one is set, else fisheye_camera's default
-    for these k, and the context's own model is restored after the forward (a lens gsb_set_camera_model refuses raises
+    lens (optional): an (8,) tensor (fx, fy, cx, cy, k[0..3]) (lens_tensor makes one).  The frame is rendered through
+    lens_camera(lens, max_theta, kind), kind and max_theta those of the context's lens model if one is set (k1, k2, p1, p2
+    for an OpenCV model), else a fisheye at fisheye_camera's default max_theta for these k, and the context's own model is
+    restored after the forward (a lens gsb_set_camera_model refuses raises
     GsbError and changes nothing).  Backward runs gsb_render_backward_fisheye: dL/dlens when lens requires grad, dL/dubo
     (camera_position and view rows 0-2 only; the rest is 0) when ubo requires grad, and the other inputs' gradients as
     without lens=.  It composes with depth=, features=, density=, background= and the deterministic mode.
 
     depth=True renders with gsb_render_depth and returns (img, depth_alpha), depth_alpha an (H, W, 2) tensor of (D, A):
-    D = sum f alpha T, f the view-space z (the distance from the camera for a fisheye model), and A = 1 - T_final, the
+    D = sum f alpha T, f the view-space z (the distance from the camera for a fisheye model, z for OpenCV), and A = 1 - T_final, the
     accumulated opacity.  Backward then takes dL/dimg and dL/d(depth_alpha), either of them unused (zero), through
     gsb_render_backward_depth; it composes with ubo=, density=, background= and the deterministic mode.  Expected depth is
     D / A.clamp_min(1e-10), inverse depth its reciprocal, and a mask loss reads A directly.
@@ -1536,7 +1609,8 @@ class SceneAdam:
     `params` stay the unfiltered raw parameters, `variance` holds each Gaussian's filter (Context.filter3d_variance) and
     `vertices` the filtered records (apply_filter_3d of the activated params), which frames render and step() trains
     through gsb_adam_step_filter3d.  The filter is a pinhole filter: it reads each camera's UBO focal (tan_fov) and
-    ndc2Pix, whatever the context's camera model, so for fisheye training views pass pinhole Uniforms of a matching focal.
+    ndc2Pix, whatever the context's camera model, so for fisheye or OpenCV training views pass pinhole Uniforms of a matching
+    focal.
     Mip-Splatting recomputes the filter every 100 steps once densification has ended:
 
         if it >= densify_until and it % 100 == 0:
@@ -1657,9 +1731,9 @@ class SceneAdam:
         backward is then gsb_render_backward_features, and `features` take their Adam step before the scene does.
 
         grad_uniforms, grad_lens: optional (40,) and (8,) float32 CUDA tensors, overwritten by the same backward pass with
-        dL/d(the frame's gsb_uniforms, all 40 words) and dL/d(fx, fy, cx, cy, k1..k4) of the frame's lens.  A pinhole frame
-        fills grad_uniforms through gsb_render_backward_camera's words (grad_lens: ValueError); a fisheye frame fills both
-        through gsb_render_backward_fisheye (pose words only).  `grad`, the features and the step are the same as without them.
+        dL/d(the frame's gsb_uniforms, all 40 words) and dL/d(fx, fy, cx, cy, k[0..3]) of the frame's lens (k1..k4 for a
+        fisheye, k1, k2, p1, p2 for OpenCV).  A pinhole frame fills grad_uniforms through gsb_render_backward_camera's words
+        (grad_lens: ValueError); a fisheye or OpenCV frame fills both through gsb_render_backward_fisheye (pose words only).  `grad`, the features and the step are the same as without them.
         Joint pose refinement, with per-view poses (and a lens tensor) in a torch optimizer:
 
             gu = torch.empty(40, device="cuda")
@@ -1669,7 +1743,7 @@ class SceneAdam:
             opt.step(g, grad_uniforms=gu)
             ubo.backward(gu[UBO_FLOAT_WORDS]); pose_opt.step(); pose_opt.zero_grad()
 
-        For a lens, render through ctx.set_camera_model(lens_camera(lens, max_theta)) and add lens.grad += the grad_lens."""
+        For a lens, render through ctx.set_camera_model(lens_camera(lens, max_theta, kind)) and add lens.grad += the grad_lens."""
         import torch
 
         ctx, v = self.ctx, self.vertices
@@ -1699,7 +1773,7 @@ class SceneAdam:
         gu = None if grad_uniforms is None else grad_uniforms.data_ptr()
         if ctx.camera is None:
             if grad_lens is not None:
-                raise ValueError("SceneAdam.step: grad_lens needs a fisheye frame (Context.set_camera_model)")
+                raise ValueError("SceneAdam.step: grad_lens needs a fisheye or OpenCV frame (Context.set_camera_model)")
             ctx._backward(v.data_ptr(), None if g is None else g.data_ptr(), self.grad.data_ptr(), stream, grad_uniforms_ptr=gu,
                           **common)
         elif grad_uniforms is None and grad_lens is None:

@@ -200,18 +200,28 @@ int gsb_set_background(gsb_ctx *ctx, const float *rgb);
  *   cov2d = J W Sigma W^T J^T + 0.3 I with J = d uv / d t exact (no tan_fov clamp);  depth key d (sorts lenses past 180 deg).
  * The conic, culls, radius, tile AABB, opacity (and its anti-aliased compensation) and SH colour follow from it as for a
  * pinhole frame.  Pixel (i, j) is sampled at (i, j): COLMAP's principal point is (cx - 0.5, cy - 0.5) here.
- * The frame records the model; gsb_render_backward and gsb_render_backward_density follow the frame's, and for a fisheye frame
- * gsb_render_backward_camera and gsb_render_backward_density with a non-NULL grad_uniforms return GSB_ERR_INVALID (no pose
- * gradient through the lens).  m NULL or kind PINHOLE: the default.  GSB_ERR_INVALID, the setting unchanged, for a NULL ctx,
- * a sharded context or gsb_group rank, an unknown kind, fx or fy not positive and finite, any other field not finite,
- * max_theta outside (0, pi), or d theta_d / d theta <= 0 anywhere on [0, max_theta] (checked on the host in double).
+ * OPENCV is COLMAP's OPENCV (Brown-Conrady radial-tangential) lens, which also states SIMPLE_PINHOLE, PINHOLE, SIMPLE_RADIAL
+ * and RADIAL with the missing coefficients 0.  It reads the same UBO words, and with xn = x / z, yn = y / z,
+ * r^2 = xn^2 + yn^2, R = 1 + k1 r^2 + k2 r^4 (k = (k1, k2, p1, p2)):
+ *   xd = xn R + 2 p1 xn yn + p2 (r^2 + 2 xn^2),  yd = yn R + p1 (r^2 + 2 yn^2) + 2 p2 xn yn,  uv = (fx xd + cx, fy yd + cy);
+ *   culled unless z > 0.2, r^2 <= tan^2(max_theta) (rounded to fp32 once) and det d(xd, yd) / d(xn, yn) > 0 (NaN culled);
+ *   cov2d = J W Sigma W^T J^T + 0.3 I with J = d uv / d t exact (no tan_fov clamp);  depth key z, as for a pinhole frame.
+ * The frame records the model; every backward entry follows the frame's.  For a fisheye or OpenCV frame (a lens frame)
+ * gsb_render_backward_camera, _density, _depth and _features with a non-NULL grad_uniforms return GSB_ERR_INVALID: the
+ * camera gradient of a lens frame is gsb_render_backward_fisheye's.  m NULL or kind PINHOLE: the default.  GSB_ERR_INVALID,
+ * the setting unchanged, for a NULL ctx, a sharded context or gsb_group rank, an unknown kind, fx or fy not positive and
+ * finite, any other field not finite, and (checked on the host in double)
+ *   FISHEYE: max_theta outside (0, pi), or d theta_d / d theta <= 0 anywhere on [0, max_theta];
+ *   OPENCV:  max_theta outside (0, pi / 2), or r R(r^2) not strictly increasing on [0, tan max_theta], i.e.
+ *            1 + 3 k1 u + 5 k2 u^2 <= 0 somewhere on u in [0, tan^2 max_theta].
  * Takes effect at the next frame; changing it drops no captured graph. */
-typedef enum gsb_camera_kind { GSB_CAMERA_PINHOLE = 0, GSB_CAMERA_FISHEYE = 1 } gsb_camera_kind;
+typedef enum gsb_camera_kind { GSB_CAMERA_PINHOLE = 0, GSB_CAMERA_FISHEYE = 1, GSB_CAMERA_OPENCV = 2 } gsb_camera_kind;
 typedef struct gsb_camera_model {
     uint32_t kind;        /* gsb_camera_kind */
     float fx, fy, cx, cy; /* pixels; pixel (i, j) is sampled at (i, j), as the blend does (COLMAP's cx - 0.5) */
-    float k[4];           /* Kannala-Brandt / OpenCV fisheye: theta_d = theta (1 + k1 t^2 + k2 t^4 + k3 t^6 + k4 t^8), t = theta */
-    float max_theta;      /* radians, in (0, pi): rays farther off the axis are culled */
+    float k[4];           /* FISHEYE, Kannala-Brandt: theta_d = theta (1 + k1 t^2 + k2 t^4 + k3 t^6 + k4 t^8), t = theta;
+                             OPENCV: (k1, k2, p1, p2) in COLMAP's OPENCV order */
+    float max_theta;      /* radians, in (0, pi) (FISHEYE) or (0, pi / 2) (OPENCV): rays farther off the axis are culled */
 } gsb_camera_model;
 int gsb_set_camera_model(gsb_ctx *ctx, const gsb_camera_model *m);
 /* per-stage cudaEvent timers (the QueryManager analogue, Renderer.cpp:85-100). Default on. */
@@ -389,7 +399,8 @@ int gsb_render_backward_features(gsb_ctx *ctx, const float *vertices, const floa
                                  const float *grad_feature_map, size_t feature_pitch_bytes, float *grad_vertices,
                                  gsb_uniforms *grad_uniforms, float *grad_features, float *density, void *stream);
 
-/* The camera gradient of a fisheye frame (gsb_set_camera_model): pose refinement and lens self-calibration through the lens.
+/* The camera gradient of a lens frame (fisheye or OpenCV, gsb_set_camera_model): pose refinement and lens self-calibration
+ * through the lens.
  * The arguments, preconditions and error codes of gsb_render_backward_features, except that
  *   features, channels, grad_feature_map, grad_features
  *                      features == NULL with channels == 0 means no feature map; grad_feature_map and grad_features must then
@@ -398,19 +409,21 @@ int gsb_render_backward_features(gsb_ctx *ctx, const float *vertices, const floa
  *                      camera_position[0..2] (the SH view direction) and view_mat rows 0-2 ([c*4 + r], r != 3): through the
  *                      view-space position t = V (p, 1) and through the view rotation W inside the EWA term J W.  Every other
  *                      word -- proj_mat, tan_fovx, tan_fovy, view_mat row 3, camera_position[3], width, height -- is 0: a
- *                      fisheye frame does not read them.
- *   grad_lens          device memory or NULL, OVERWRITTEN with dL/d(fx, fy, cx, cy, k[0..3]) of the frame's lens, through uv
- *                      and through the Jacobian J of the EWA term; kind and max_theta are written 0 (max_theta, the culls,
+ *                      lens frame does not read them.
+ *   grad_lens          device memory or NULL, OVERWRITTEN with dL/d(fx, fy, cx, cy, k[0..3]) of the frame's lens (k in the
+ *                      model's own order: k1..k4 for a fisheye, k1, k2, p1, p2 for OpenCV), through uv and through the
+ *                      Jacobian J of the EWA term; kind and max_theta are written 0 (max_theta, the culls,
  *                      radii and tile AABBs are step functions of the lens).
  *   grad_vertices, grad_uniforms, grad_lens, grad_features
  *                      each may be NULL, but not all four; density may be NULL, and needs grad_vertices, grad_uniforms or
  *                      grad_lens
  * and GSB_ERR_INVALID also when the last frame is a pinhole frame (its camera gradient is gsb_render_backward_camera's).
  * grad_vertices, grad_features and density receive the words the other backward entries give for the same frame and upstream
- * gradients.  The depth term (f = |t|) and the feature map's alpha terms reach the camera and lens words in the same pass.
+ * gradients.  The depth term (f = |t| for a fisheye, z for OpenCV) and the feature map's alpha terms reach the camera and lens
+ * words in the same pass.
  * The camera words are reduced without global atomics, per CTA in fp64 then in one fixed-order pass; under
  * gsb_set_backward_deterministic they are reproducible bit for bit, as the other outputs.  gsb_render_backward_camera,
- * _density, _depth and _features keep returning GSB_ERR_INVALID for a non-NULL grad_uniforms on a fisheye frame. */
+ * _density, _depth and _features keep returning GSB_ERR_INVALID for a non-NULL grad_uniforms on a lens frame. */
 int gsb_render_backward_fisheye(gsb_ctx *ctx, const float *vertices, const float *grad_image, size_t row_pitch_bytes,
                                 const float *grad_depth_alpha, size_t depth_pitch_bytes, const float *features, uint32_t channels,
                                 const float *grad_feature_map, size_t feature_pitch_bytes, float *grad_vertices,
