@@ -10,6 +10,7 @@
 
 #include <algorithm>
 #include <new>
+#include <string>
 #include <thread>
 #include <vector>
 
@@ -951,22 +952,17 @@ int gsb_set_background(gsb_ctx* ctx, const float* rgb) {
     return GSB_OK;
 }
 
-int gsb_set_camera_model(gsb_ctx* ctx, const gsb_camera_model* m) {
-    if (!ctx) return GSB_ERR_INVALID;
-    auto bad = [&](const char* what) { return fail(ctx, GSB_ERR_INVALID, (std::string("gsb_set_camera_model: ") + what).c_str()); };
-    if (ctx->shard) return bad("sharded contexts have only the pinhole camera");
-    if (!m || m->kind == GSB_CAMERA_PINHOLE) {
-        ctx->camera = gsb_camera_model{};
-        return GSB_OK;
-    }
-    if (m->kind != GSB_CAMERA_FISHEYE && m->kind != GSB_CAMERA_OPENCV) return bad("unknown camera kind");
-    if (!(m->fx > 0.0f) || !(m->fy > 0.0f) || !isfinite(m->fx) || !isfinite(m->fy)) return bad("fx and fy must be positive and finite");
-    const float rest[] = {m->cx, m->cy, m->k[0], m->k[1], m->k[2], m->k[3], m->max_theta};
+// The checks gsb_set_camera_model makes of a FISHEYE or OPENCV model, and gsb_filter3d_variance_lens of each of its lenses:
+// nullptr if m is a lens the frames can project through, else why not.
+static const char* camera_model_error(const gsb_camera_model& m) {
+    if (m.kind != GSB_CAMERA_FISHEYE && m.kind != GSB_CAMERA_OPENCV) return "unknown camera kind";
+    if (!(m.fx > 0.0f) || !(m.fy > 0.0f) || !isfinite(m.fx) || !isfinite(m.fy)) return "fx and fy must be positive and finite";
+    const float rest[] = {m.cx, m.cy, m.k[0], m.k[1], m.k[2], m.k[3], m.max_theta};
     for (float x : rest)
-        if (!isfinite(x)) return bad("every field must be finite");
-    const double tmax = m->max_theta, k1 = m->k[0], k2 = m->k[1], k3 = m->k[2], k4 = m->k[3];
-    if (m->kind == GSB_CAMERA_OPENCV) {
-        if (!(tmax > 0.0) || !(tmax < M_PI / 2)) return bad("max_theta must lie in (0, pi / 2)");
+        if (!isfinite(x)) return "every field must be finite";
+    const double tmax = m.max_theta, k1 = m.k[0], k2 = m.k[1], k3 = m.k[2], k4 = m.k[3];
+    if (m.kind == GSB_CAMERA_OPENCV) {
+        if (!(tmax > 0.0) || !(tmax < M_PI / 2)) return "max_theta must lie in (0, pi / 2)";
         // r R(r^2) strictly increasing on [0, tan max_theta]: d(r R) / dr = 1 + 3 k1 u + 5 k2 u^2 > 0 on u = r^2 in [0, umax].  A
         // quadratic with value 1 at 0: positive everywhere iff positive at umax and at its vertex when that lies inside.  With
         // p1 = p2 = 0 this also makes det D = R (1 + 3 k1 u + 5 k2 u^2) positive on the whole disc (R > 0 follows from r R > 0).
@@ -977,11 +973,10 @@ int gsb_set_camera_model(gsb_ctx* ctx, const gsb_camera_model* m) {
             const double vertex = -3.0 * k1 / (10.0 * k2);
             if (vertex > 0.0 && vertex < umax) qmin = std::min(qmin, q(vertex));
         }
-        if (!(qmin > 0.0)) return bad("the radial map r R(r^2) must be strictly increasing on [0, tan max_theta]");
-        ctx->camera = *m;
-        return GSB_OK;
+        if (!(qmin > 0.0)) return "the radial map r R(r^2) must be strictly increasing on [0, tan max_theta]";
+        return nullptr;
     }
-    if (!(tmax > 0.0) || !(tmax < M_PI)) return bad("max_theta must lie in (0, pi)");
+    if (!(tmax > 0.0) || !(tmax < M_PI)) return "max_theta must lie in (0, pi)";
     // theta_d strictly increasing on [0, max_theta]: d theta_d / d theta = 1 + 3 k1 t^2 + 5 k2 t^4 + 7 k3 t^6 + 9 k4 t^8 > 0.  In
     // u = t^2 that is a quartic q(u) on [0, tmax^2] with q(0) = 1: positive everywhere iff positive at the end and at every
     // root of q'(u) = 3 k1 + 10 k2 u + 21 k3 u^2 + 36 k4 u^3 inside, which a dense scan brackets and bisection refines.
@@ -1002,7 +997,19 @@ int gsb_set_camera_model(gsb_ctx* ctx, const gsb_camera_model* m) {
             qmin = std::min(qmin, q(0.5 * (a + b)));
         }
     }
-    if (!(qmin > 0.0)) return bad("theta_d must be strictly increasing on [0, max_theta]");
+    if (!(qmin > 0.0)) return "theta_d must be strictly increasing on [0, max_theta]";
+    return nullptr;
+}
+
+int gsb_set_camera_model(gsb_ctx* ctx, const gsb_camera_model* m) {
+    if (!ctx) return GSB_ERR_INVALID;
+    auto bad = [&](const char* what) { return fail(ctx, GSB_ERR_INVALID, (std::string("gsb_set_camera_model: ") + what).c_str()); };
+    if (ctx->shard) return bad("sharded contexts have only the pinhole camera");
+    if (!m || m->kind == GSB_CAMERA_PINHOLE) {
+        ctx->camera = gsb_camera_model{};
+        return GSB_OK;
+    }
+    if (const char* why = camera_model_error(*m)) return bad(why);
     // k_project is launched outside the captured middle graph: graphs and hints stay
     ctx->camera = *m;
     return GSB_OK;
@@ -1457,6 +1464,56 @@ int gsb_filter3d_variance(gsb_ctx* ctx, const float* vertices, uint64_t n, const
     else cudaStreamSynchronize(s);
     cudaFree(base);
     if (e != cudaSuccess) return fail(ctx, e == cudaErrorMemoryAllocation ? GSB_ERR_OOM : GSB_ERR_CUDA, "gsb_filter3d_variance", e);
+    return GSB_OK;
+}
+
+int gsb_filter3d_variance_lens(gsb_ctx* ctx, const float* vertices, uint64_t n, const gsb_uniforms* cameras,
+                               const gsb_camera_model* models, uint32_t k, float* variance, void* stream) {
+    if (!ctx) return GSB_ERR_INVALID;
+    auto bad = [&](const std::string& what) { return fail(ctx, GSB_ERR_INVALID, ("gsb_filter3d_variance_lens: " + what).c_str()); };
+    if (ctx->shard) return bad("sharded contexts have no training step");
+    if (!cameras || k == 0) return bad("no camera");
+    if (!models) return bad("no lens models");
+    std::vector<gsb_camera_model> staged(k);  // the kernel's copies: an OpenCV max_theta becomes k_project's tan^2 bound
+    for (uint32_t c = 0; c < k; c++) {
+        const gsb_uniforms& u = cameras[c];
+        const gsb_camera_model& m = models[c];
+        if (u.width == 0 || u.height == 0) return bad("a camera of width or height 0");
+        if (m.kind == GSB_CAMERA_PINHOLE) {
+            if (!(u.tan_fovx > 0.0f && u.tan_fovx <= FLT_MAX) || !(u.tan_fovy > 0.0f && u.tan_fovy <= FLT_MAX))
+                return bad("a camera's tan_fov is not positive and finite");
+            staged[c] = gsb_camera_model{};
+            continue;
+        }
+        if (const char* why = camera_model_error(m)) return bad("camera " + std::to_string(c) + ": " + why);
+        staged[c] = m;
+        if (m.kind == GSB_CAMERA_OPENCV) {
+            const double t = std::tan((double)m.max_theta);
+            staged[c].max_theta = (float)(t * t);
+        }
+    }
+    if (n == 0) return GSB_OK;
+    if (!vertices || !variance) return bad("null argument");
+    if (reinterpret_cast<uintptr_t>(vertices) % 16) return bad("vertices not aligned to 16 B");
+    if (reinterpret_cast<uintptr_t>(variance) % 4) return bad("variance not aligned to 4 B");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = stream_or_own(ctx, stream);
+    // scratch, one allocation freed before returning: the k cameras, their k models, then the largest seen scale's bits
+    const size_t cam_bytes = (size_t)k * sizeof(gsb_uniforms), model_bytes = (size_t)k * sizeof(gsb_camera_model);
+    unsigned char* base = nullptr;
+    CK(dev_alloc(&base, cam_bytes + model_bytes + 4));
+    gsb_uniforms* cams = reinterpret_cast<gsb_uniforms*>(base);
+    gsb_camera_model* lens = reinterpret_cast<gsb_camera_model*>(base + cam_bytes);
+    uint32_t* smax = reinterpret_cast<uint32_t*>(base + cam_bytes + model_bytes);
+    cudaError_t e = cudaMemcpyAsync(cams, cameras, cam_bytes, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(lens, staged.data(), model_bytes, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(smax, 0, 4, s);
+    if (e == cudaSuccess)
+        e = launch_filter3d_lens(reinterpret_cast<const float4*>(vertices), n, cams, lens, k, smax, variance, ctx->num_sms, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);  // the variances are written and the scratch (and `staged`) may go
+    else cudaStreamSynchronize(s);
+    cudaFree(base);
+    if (e != cudaSuccess) return fail(ctx, e == cudaErrorMemoryAllocation ? GSB_ERR_OOM : GSB_ERR_CUDA, "gsb_filter3d_variance_lens", e);
     return GSB_OK;
 }
 

@@ -315,5 +315,10 @@ cudaError_t launch_adam_features(const FeatureAdamParams& p, int num_sms, cudaSt
 // dmax: one zeroed word (the largest seen depth's bits).  variance: n floats, overwritten.
 cudaError_t launch_filter3d(const float4* vertices, uint64_t n, const gsb_uniforms* cams, uint32_t k, float focal,
                             uint32_t* dmax, float* variance, int num_sms, cudaStream_t s);
+// gsb_filter3d_variance_lens.  models: k device copies of the cameras' lens models, an OPENCV one with max_theta replaced by
+// tan^2(max_theta) rounded to fp32 once (as ProjectOpencvParams carries it); smax: one zeroed word (the largest seen
+// scale's bits).  variance: n floats, overwritten.
+cudaError_t launch_filter3d_lens(const float4* vertices, uint64_t n, const gsb_uniforms* cams, const gsb_camera_model* models,
+                                 uint32_t k, uint32_t* smax, float* variance, int num_sms, cudaStream_t s);
 
 }  // namespace gsb

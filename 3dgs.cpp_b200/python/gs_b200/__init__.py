@@ -54,7 +54,7 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     # training loss, optimizer step and initialisation from a point cloud
     "gsb_image_loss", "gsb_adam_step", "gsb_init_from_points",
     # Mip-Splatting's 3D smoothing filter
-    "gsb_filter3d_variance", "gsb_adam_step_filter3d",
+    "gsb_filter3d_variance", "gsb_adam_step_filter3d", "gsb_filter3d_variance_lens",
     # bilateral-grid appearance correction
     "gsb_bilagrid_apply", "gsb_bilagrid_backward",
     # 3DGS-MCMC: position noise and relocation
@@ -326,6 +326,7 @@ lib.gsb_bilagrid_backward.argtypes = [_vp, C.c_uint32, C.c_uint32, _vp, C.c_size
                                       _vp, C.c_size_t, _vp, C.c_size_t, _vp, _vp]
 lib.gsb_adam_step.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(AdamConfig), _vp]
 lib.gsb_filter3d_variance.argtypes = [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, _vp]
+lib.gsb_filter3d_variance_lens.argtypes = [_vp, _vp, C.c_uint64, _vp, _vp, C.c_uint32, _vp, _vp]
 lib.gsb_adam_step_filter3d.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(AdamConfig), _vp]
 lib.gsb_init_from_points.argtypes = [_vp, _vp, _vp, C.c_uint64, C.c_float, _vp, _vp]
 lib.gsb_mcmc_noise.argtypes = [_vp, _vp, _vp, C.c_float, C.c_uint64, C.c_uint64, _vp]
@@ -891,13 +892,19 @@ class Context:
             raise ValueError(f"{caller}: variance must be a contiguous ({n},) float32 tensor, got {tuple(variance.shape)} "
                              f"{variance.dtype}")
 
-    def filter3d_variance(self, vertices, cameras):
+    def filter3d_variance(self, vertices, cameras, lenses=None):
         """gsb_filter3d_variance on torch tensors: the (n,) float32 variance of Mip-Splatting's 3D smoothing filter of the
         Gaussians at the positions (columns 0-2) of `vertices`, a contiguous (n, 60) float32 CUDA tensor on the context's
         device (any n: no scene is needed), from `cameras`, a non-empty list of Uniforms (the training views): with d the
         least view depth over the cameras that see a Gaussian (the largest such d for one no camera sees) and f the largest
         focal length in pixels, variance = 0.2 (d / f)^2.  Runs on torch's current stream and returns when the variances are
-        written; leaves the context's scene and last frame alone.  Bad arguments raise ValueError or GsbError."""
+        written; leaves the context's scene and last frame alone.  Bad arguments raise ValueError or GsbError.
+
+        lenses: the cameras' lens models (gsb_filter3d_variance_lens), one CameraModel for every camera or a list of one per
+        camera (a CameraModel of kind CAMERA_PINHOLE, e.g. CameraModel(), is that camera's UBO pinhole).  Each camera then
+        sees a Gaussian as a frame through its lens does, and d / f becomes the least over those cameras of the footprint
+        scale 1 / sigma_min(d uv / d t), the world size of one pixel at the camera's finest image axis.  None: the pinhole
+        filter above."""
         import torch
 
         if not isinstance(vertices, torch.Tensor) or not vertices.is_cuda or vertices.device.index != self.device:
@@ -912,7 +919,14 @@ class Context:
         n = vertices.shape[0]
         out = torch.empty(n, dtype=torch.float32, device=vertices.device)
         s = _torch_stream_arg(torch.cuda.current_stream(vertices.device))
-        self._ck(lib.gsb_filter3d_variance(self.h, vertices.data_ptr(), n, arr, len(cams), out.data_ptr(), s))
+        if lenses is None:
+            self._ck(lib.gsb_filter3d_variance(self.h, vertices.data_ptr(), n, arr, len(cams), out.data_ptr(), s))
+            return out
+        models = [lenses] * len(cams) if isinstance(lenses, CameraModel) else list(lenses)
+        if len(models) != len(cams) or not all(isinstance(m, CameraModel) for m in models):
+            raise ValueError(f"filter3d_variance: lenses must be one CameraModel or a list of {len(cams)}")
+        marr = (CameraModel * len(models))(*models)
+        self._ck(lib.gsb_filter3d_variance_lens(self.h, vertices.data_ptr(), n, arr, marr, len(cams), out.data_ptr(), s))
         return out
 
     def _check_rows(self, caller, arrays):
@@ -1608,9 +1622,10 @@ class SceneAdam:
     rendered closer or larger than its training views: filter_cameras, the list of training Uniforms, turns it on.  Then
     `params` stay the unfiltered raw parameters, `variance` holds each Gaussian's filter (Context.filter3d_variance) and
     `vertices` the filtered records (apply_filter_3d of the activated params), which frames render and step() trains
-    through gsb_adam_step_filter3d.  The filter is a pinhole filter: it reads each camera's UBO focal (tan_fov) and
-    ndc2Pix, whatever the context's camera model, so for fisheye or OpenCV training views pass pinhole Uniforms of a matching
-    focal.
+    through gsb_adam_step_filter3d.  filter_lenses gives the training views' lens models (Context.filter3d_variance's
+    `lenses`: one CameraModel for all views or a list of one per view), so that fisheye and OpenCV views, mixed lenses
+    included, see each Gaussian and resolve it as their frames do; without it the filter reads each view's UBO pinhole
+    (tan_fov and ndc2Pix), whatever the context's camera model.
     Mip-Splatting recomputes the filter every 100 steps once densification has ended:
 
         if it >= densify_until and it % 100 == 0:
@@ -1629,7 +1644,7 @@ class SceneAdam:
     source rows onto the relocated ones with zero moments and appends features[src] when it grows."""
 
     def __init__(self, ctx: "Context", vertices, lr, betas=(0.9, 0.999), eps=1e-15, selective=True, background=None,
-                 random_background=False, seed=0, filter_cameras=None, features=None, feature_lr=0.0):
+                 random_background=False, seed=0, filter_cameras=None, features=None, feature_lr=0.0, filter_lenses=None):
         import torch
 
         if not isinstance(vertices, torch.Tensor) or not vertices.is_cuda or vertices.dim() != 2 or vertices.shape[1] != 60:
@@ -1640,6 +1655,7 @@ class SceneAdam:
         self.background = None if background is None else [float(x) for x in background]
         self._generator = torch.Generator().manual_seed(int(seed)) if random_background else None
         self.filter_cameras = None if filter_cameras is None else list(filter_cameras)
+        self.filter_lenses = filter_lenses
         self.variance = None
         self._adopt(vertices.detach().to(torch.float32).contiguous().clone(), None)
         self.features = self.feature_lr = None
@@ -1651,7 +1667,7 @@ class SceneAdam:
             self.feature_lr = float(feature_lr)
             self._adopt_features(f, torch.zeros_like(f), torch.zeros_like(f))
         if self.filter_cameras is not None:
-            self._set_filter(ctx.filter3d_variance(self.params, self.filter_cameras), self.vertices)
+            self._set_filter(self._filter_variance(), self.vertices)
         ctx.set_backward(True)
         self._upload()
 
@@ -1679,14 +1695,20 @@ class SceneAdam:
         self.variance = variance
         self.vertices = apply_filter_3d(unfiltered, variance).contiguous()
 
-    def update_filter_3d(self, cameras=None):
+    def _filter_variance(self):
+        return self.ctx.filter3d_variance(self.params, self.filter_cameras, self.filter_lenses)
+
+    def update_filter_3d(self, cameras=None, lenses=None):
         """Recomputes the 3D filter from the current positions and the training cameras (`cameras`, which then replace
-        filter_cameras; None: filter_cameras), re-activates every row through it and uploads the scene."""
+        filter_cameras; None: filter_cameras) through their lenses (`lenses`, which then replace filter_lenses; None:
+        filter_lenses), re-activates every row through it and uploads the scene."""
         if cameras is not None:
             self.filter_cameras = list(cameras)
+        if lenses is not None:
+            self.filter_lenses = lenses
         if self.filter_cameras is None:
             raise ValueError("SceneAdam.update_filter_3d: no training cameras (filter_cameras)")
-        self._set_filter(self.ctx.filter3d_variance(self.params, self.filter_cameras), activate_parameters(self.params))
+        self._set_filter(self._filter_variance(), activate_parameters(self.params))
         self._upload()
 
     def _upload(self):
@@ -1812,7 +1834,7 @@ class SceneAdam:
             self._adopt_features(self.features[source].contiguous(), m.contiguous(), s.contiguous())
         self._adopt(new, adam_state_after_densify(self.params, self.exp_avg, self.exp_avg_sq, unfiltered, new, source))
         if self.variance is not None:
-            self._set_filter(self.ctx.filter3d_variance(self.params, self.filter_cameras), new)
+            self._set_filter(self._filter_variance(), new)
         self._upload()
         return source
 

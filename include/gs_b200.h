@@ -550,6 +550,23 @@ int gsb_adam_step(gsb_ctx *ctx, float *params, float *exp_avg, float *exp_avg_sq
 int gsb_filter3d_variance(gsb_ctx *ctx, const float *vertices, uint64_t n, const gsb_uniforms *cameras, uint32_t k,
                           float *variance, void *stream);
 
+/* The filter's variance from k >= 1 training cameras that each have their own lens (DESIGN.md section 24): camera c is the
+ * UBO cameras[c] seen through models[c] (k host entries; kind PINHOLE: the UBO's own camera), as a frame of that model
+ * projects it.  Per Gaussian i and camera c, in fp32 with t = (x, y, z) from clip_view's view rows:
+ *   seen iff the frame's cull for the kind keeps i and its uv lies in -0.15f W <= u <= 1.15f W, -0.15f H <= v <= 1.15f H
+ *   (PINHOLE: gsb_filter3d_variance's test; FISHEYE: d > 0.2, theta <= max_theta; OPENCV: z > 0.2,
+ *   r^2 <= tan^2(max_theta) rounded to fp32 once, det D > 0; NaN is never seen);
+ *   s_ic = 1 / sigma_min(J), J = d uv / d t of the frame's Jacobian (lens kinds), or vz / min(focal_x, focal_y) with the
+ *   UBO's focals (PINHOLE); a camera whose s_ic is not positive and finite does not count as seeing i.
+ * s_i = the least s_ic over the cameras that see i; rows no camera sees take the largest s_i of the seen rows; variance_i =
+ * (s_i s_i) 0.2f; all zero if no row is seen.  Bitwise reproducible, on any stream, context or grid and in any camera order.
+ * All-PINHOLE cameras sharing one focal_x == focal_y give gsb_filter3d_variance's words.  A lens camera's proj_mat and
+ * tan_fov are not read.  Otherwise as gsb_filter3d_variance, scratch 200 B per camera + 4 B: GSB_ERR_INVALID for everything
+ * it refuses (a PINHOLE camera keeps its tan_fov checks), and also for NULL models and for any lens model
+ * gsb_set_camera_model would refuse. */
+int gsb_filter3d_variance_lens(gsb_ctx *ctx, const float *vertices, uint64_t n, const gsb_uniforms *cameras,
+                               const gsb_camera_model *models, uint32_t k, float *variance, void *stream);
+
 /* gsb_adam_step with every updated row's scale and opacity passed through the 3D smoothing filter of its variance v
  * (variance: n floats of device memory, 4-B aligned, finite and >= 0, e.g. from gsb_filter3d_variance; not checked here).
  * With x the raw parameters, in fp32, each operation one IEEE op in this order, for k = 0, 1, 2:
