@@ -1,9 +1,10 @@
 // gs_viewer_headless -- the reference viewer's command line (apps/viewer/main.cpp:12-98) without a window:
 //   gs_viewer_headless [-d DEVICE] [-w WIDTH] [-h HEIGHT] [-v] [--frames N] [--camera x,y,z[,qw,qx,qy,qz]]
 //                      [--fov DEG] [--camera-path poses.txt] [--mode exact|fast] [--cull [LEVEL]] [--antialiased]
-//                      [--background r,g,b] [--fisheye fx,fy,cx,cy[,k1,k2,k3,k4[,max_theta_deg]]]
+//                      [--sh-degree N] [--background r,g,b] [--fisheye fx,fy,cx,cy[,k1,k2,k3,k4[,max_theta_deg]]]
 //                      [--opencv fx,fy,cx,cy[,k1,k2,p1,p2[,max_theta_deg]]] [--out image.ppm] [--float-out image.pfm] scene.ply
 // --antialiased: gsb_set_antialiased (opacity compensated for the 0.3 px dilation, as scenes trained that way expect).
+// --sh-degree N: gsb_set_sh_degree (0..3; the colour sums the SH bands <= N only, e.g. for a scene trained at a lower degree).
 // --background r,g,b: gsb_set_background (e.g. 1,1,1 for an object scene trained over white; default black).
 // --fisheye fx,fy,cx,cy[,k1,k2,k3,k4[,max_theta_deg]]: gsb_set_camera_model with an OpenCV-fisheye lens (pixel (i, j) sampled at
 // (i, j): COLMAP's cx - 0.5); without max_theta_deg, the largest angle up to 175 deg at which theta_d still increases.
@@ -31,7 +32,7 @@
 static void usage() {
     std::puts("usage: gs_viewer_headless [-d device] [-w width] [-h height] [-v] [--frames n] [--camera x,y,z[,qw,qx,qy,qz]]\n"
               "                          [--fov deg] [--camera-path poses.txt] [--mode exact|fast] [--cull [0|1|2]] [--antialiased]\n"
-              "                          [--background r,g,b] [--fisheye fx,fy,cx,cy[,k1,k2,k3,k4[,max_theta_deg]]]\n"
+              "                          [--sh-degree 0|1|2|3] [--background r,g,b] [--fisheye fx,fy,cx,cy[,k1,k2,k3,k4[,max_theta_deg]]]\n"
               "                          [--opencv fx,fy,cx,cy[,k1,k2,p1,p2[,max_theta_deg]]]\n"
               "                          [--out image.ppm] [--float-out image.pfm] scene.ply");
 }
@@ -39,7 +40,7 @@ static void usage() {
 int main(int argc, char** argv) {
     Renderer::Configuration cfg;
     std::string out_path, float_path, scene, path_file;
-    int cull_level = 0;
+    int cull_level = 0, sh_degree = 3;
     uint32_t frames = 1;
     bool verbose = false, cull = false, antialiased = false, background = false;
     float bg[3] = {0, 0, 0};
@@ -69,6 +70,14 @@ int main(int argc, char** argv) {
             cull_level = 1;
             if (i + 1 < argc && std::strlen(argv[i + 1]) == 1 && argv[i + 1][0] >= '0' && argv[i + 1][0] <= '2') cull_level = argv[++i][0] - '0';
         } else if (a == "--antialiased") antialiased = true;
+        else if (a == "--sh-degree") {
+            const std::string d = next();
+            if (d.size() != 1 || d[0] < '0' || d[0] > '3') {
+                usage();
+                return 1;
+            }
+            sh_degree = d[0] - '0';
+        }
         else if (a == "--background") {
             background = true;
             int k = 0;
@@ -106,6 +115,7 @@ int main(int argc, char** argv) {
         const double load_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
         if (cull && gsb_set_tile_cull(renderer.context(), cull_level) != GSB_OK) throw std::runtime_error("gsb_set_tile_cull failed");
         if (antialiased && gsb_set_antialiased(renderer.context(), 1) != GSB_OK) throw std::runtime_error("gsb_set_antialiased failed");
+        if (sh_degree != 3 && gsb_set_sh_degree(renderer.context(), sh_degree) != GSB_OK) throw std::runtime_error("gsb_set_sh_degree failed");
         if (background && gsb_set_background(renderer.context(), bg) != GSB_OK) throw std::runtime_error("gsb_set_background failed");
         if (lens_kind != GSB_CAMERA_PINHOLE) {
             gsb_camera_model m{};

@@ -376,7 +376,7 @@ static int enqueue_front(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uin
 
     // ---- k_project: preprocess.comp + survivor compaction ----
     const bool lens = ctx->camera.kind != GSB_CAMERA_PINHOLE;
-    CK(launch_project(project_params(ctx, *ubo, rb, re), ctx->debug, ctx->antialiased, stream, lens ? &ctx->camera : nullptr));
+    CK(launch_project(project_params(ctx, *ubo, rb, re), ctx->debug, ctx->antialiased, stream, lens ? &ctx->camera : nullptr, ctx->sh_degree));
     if (timers) CK(cudaEventRecord(ctx->ev[1], stream));
 
     if (ctx->use_graph && !timers && !ctx->debug) rc = launch_middle_graph(ctx, fp, sv, stream);
@@ -435,6 +435,7 @@ int enqueue_tail(gsb_ctx* ctx, const FramePlan& fp, const gsb_uniforms& ubo, cud
     f.antialiased = ctx->antialiased;
     for (int c = 0; c < 3; c++) f.background[c] = ctx->background[c];
     f.camera = ctx->camera;
+    f.sh_degree = ctx->sh_degree;
     f.scene_gen = ctx->scene_gen;
     f.pending = true;
     f.exists = true;
@@ -942,6 +943,15 @@ int gsb_set_antialiased(gsb_ctx* ctx, int enabled) {
     return GSB_OK;
 }
 
+int gsb_set_sh_degree(gsb_ctx* ctx, int degree) {
+    if (!ctx) return GSB_ERR_INVALID;
+    if (ctx->shard) return fail(ctx, GSB_ERR_INVALID, "gsb_set_sh_degree: sharded contexts have only degree 3");
+    if (degree < 0 || degree > 3) return fail(ctx, GSB_ERR_INVALID, "gsb_set_sh_degree: the degree must lie in 0..3");
+    // k_project is launched outside the captured middle graph and the survivor set does not change: graphs and hints stay
+    ctx->sh_degree = degree;
+    return GSB_OK;
+}
+
 int gsb_set_background(gsb_ctx* ctx, const float* rgb) {
     if (!ctx) return GSB_ERR_INVALID;
     const float v[3] = {rgb ? rgb[0] : 0.0f, rgb ? rgb[1] : 0.0f, rgb ? rgb[2] : 0.0f};
@@ -1221,7 +1231,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     }
     const FeatureParams* fpp = feat ? &fp : nullptr;
     if (!det) {
-        CK(launch_backward(bp, f.antialiased, bg, s, nullptr, lens_frame ? &f.camera : nullptr, dp, fpp, grad_lens));
+        CK(launch_backward(bp, f.antialiased, bg, s, nullptr, lens_frame ? &f.camera : nullptr, dp, fpp, grad_lens, f.sh_degree));
         return GSB_OK;
     }
     const DetBuffers& d = ctx->bw_det;
@@ -1237,7 +1247,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     db.status_tiles = (uint32_t)(d.status.count / 256);
     db.m_hint = quantise_hint(ctx->m_hint);
     db.key_bits = std::max<uint32_t>(bits_for((uint32_t)n), 1u);  // compact ids < N_v <= n
-    CK(launch_backward(bp, f.antialiased, bg, s, &db, lens_frame ? &f.camera : nullptr, dp, fpp, grad_lens));
+    CK(launch_backward(bp, f.antialiased, bg, s, &db, lens_frame ? &f.camera : nullptr, dp, fpp, grad_lens, f.sh_degree));
     return GSB_OK;
 }
 

@@ -456,6 +456,10 @@ __host__ __device__ constexpr bool cam_word_live(int j) {
 // OPENCV (a frame of gsb_set_camera_model's OpenCV lens): as FISHEYE, through opencv_geo / opencv_jacobian / opencv_grad and,
 // with CAMERA, opencv_lens_grad.  It takes the fisheye's argument struct (the lens alone; the cull bound is not needed here).
 // Its depth key is z, so DEPTH adds dL/df to dL/dt.z.
+// SHDEG (a frame of gsb_set_sh_degree below 3): the colour is the sum over the coefficients of bands <= P.sh_degree only, so
+// only those get a gradient (the rest of grad_vertices stays as the caller zeroed it) and only they reach the view direction;
+// at degree 0 the direction takes no part.  Each of ddx, ddy, ddz is the degree-3 sum cut after the last live band, so the
+// words equal the degree-3 words of the scene with the dropped bands zeroed (DESIGN.md section 25).
 struct BackwardFisheyeParams : BackwardParams {
     gsb_camera_model cam;
 };
@@ -464,8 +468,10 @@ struct PbDepthParams : Base {
     double* depth_scratch;
 };
 template <bool FISHEYE, bool DEPTH = false>
-using PbParams = std::conditional_t<DEPTH, PbDepthParams<std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>,
-                                    std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>;
+using PbLensParams = std::conditional_t<DEPTH, PbDepthParams<std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>,
+                                        std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>;
+template <bool FISHEYE, bool DEPTH = false, bool SHDEG = false>
+using PbParams = std::conditional_t<SHDEG, ShDegreeParams<PbLensParams<FISHEYE, DEPTH>>, PbLensParams<FISHEYE, DEPTH>>;
 // CAMERA on a lens frame (gsb_render_backward_fisheye, fisheye or OpenCV): only the live words are accumulated --
 // camera_position.xyz, view_mat rows 0-2 and the lens's fx, fy, cx, cy, k[0..3] -- and each CTA writes one fp64 row of FC_WORDS
 // in this compact order for k_fisheye_camera_reduce: [FC_POS + k] camera_position[k], [FC_VIEW + c * 3 + k] V[k][c] (word
@@ -477,8 +483,8 @@ struct LensCamAcc {
 };
 template <>
 struct LensCamAcc<false> {};  // empty outside the lens camera instantiations, for the reason given at det_partials()
-template <bool CAMERA, bool AA, bool FISHEYE = false, bool DEPTH = false, bool OPENCV = false>
-__global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ PbParams<FISHEYE || OPENCV, DEPTH> P) {
+template <bool CAMERA, bool AA, bool FISHEYE = false, bool DEPTH = false, bool OPENCV = false, bool SHDEG = false>
+__global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ PbParams<FISHEYE || OPENCV, DEPTH, SHDEG> P) {
     static_assert(!(FISHEYE && OPENCV), "one lens per frame");
     constexpr bool LENS = FISHEYE || OPENCV;
     const uint32_t nv = P.ctl->num_visible;
@@ -648,47 +654,93 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         // ---- colour (preprocess.comp:73-108) -> SH coefficients and the view direction ----
         const float dcr = r2.x > 0.0f ? d[6] : 0.0f;  // :102-104 red clamped at 0 (the record holds the clamped value)
         const float dcg = d[7], dcb = d[8];
-        float x, y, z;
-        const float len = view_direction(U.camera_position, px, py, pz, x, y, z);
-        const float xx = x * x, yy = y * y, zz = z * z;
-        const float basis[16] = {SH_C0,
-                                 -SH_C1 * y,
-                                 SH_C1 * z,
-                                 -SH_C1 * x,
-                                 SH_C2_0 * x * y,
-                                 SH_C2_1 * y * z,
-                                 SH_C2_2 * ((2.0f * zz - xx) - yy),
-                                 SH_C2_3 * z * x,
-                                 SH_C2_4 * (xx - yy),
-                                 SH_C3_0 * (3.0f * xx - yy) * y,
-                                 SH_C3_1 * x * y * z,
-                                 SH_C3_2 * ((4.0f * zz - xx) - yy) * y,
-                                 SH_C3_3 * z * ((2.0f * zz - 3.0f * xx) - 3.0f * yy),
-                                 SH_C3_4 * x * ((4.0f * zz - xx) - yy),
-                                 SH_C3_5 * (xx - yy) * z,
-                                 SH_C3_6 * x * (xx - 3.0f * yy)};
-        const float* sh = v + 12;
-        float vk[16];
-#pragma unroll
-        for (int k = 0; k < 16; k++) {
+        float x, y, z, len, ddx, ddy, ddz;
+        if constexpr (SHDEG) {
+            const int deg = P.sh_degree;
+            const float* sh = v + 12;
             if (store_v) {
-                gv[12 + 3 * k + 0] = basis[k] * dcr;
-                gv[12 + 3 * k + 1] = basis[k] * dcg;
-                gv[12 + 3 * k + 2] = basis[k] * dcb;
+                gv[12] = SH_C0 * dcr;
+                gv[13] = SH_C0 * dcg;
+                gv[14] = SH_C0 * dcb;
             }
-            vk[k] = (sh[3 * k] * dcr + sh[3 * k + 1] * dcg) + sh[3 * k + 2] * dcb;
+            x = y = z = ddx = ddy = ddz = 0.0f;
+            len = 1.0f;
+            if (deg >= 1) {
+                len = view_direction(U.camera_position, px, py, pz, x, y, z);
+                const float xx = x * x, yy = y * y, zz = z * z;
+                const int nk = deg >= 2 ? 9 : 4;
+                const float basis[9] = {SH_C0,
+                                        -SH_C1 * y,
+                                        SH_C1 * z,
+                                        -SH_C1 * x,
+                                        SH_C2_0 * x * y,
+                                        SH_C2_1 * y * z,
+                                        SH_C2_2 * ((2.0f * zz - xx) - yy),
+                                        SH_C2_3 * z * x,
+                                        SH_C2_4 * (xx - yy)};
+                float vk[9];
+#pragma unroll
+                for (int k = 1; k < 9; k++) {
+                    if (k < nk) {
+                        if (store_v) {
+                            gv[12 + 3 * k + 0] = basis[k] * dcr;
+                            gv[12 + 3 * k + 1] = basis[k] * dcg;
+                            gv[12 + 3 * k + 2] = basis[k] * dcb;
+                        }
+                        vk[k] = (sh[3 * k] * dcr + sh[3 * k + 1] * dcg) + sh[3 * k + 2] * dcb;
+                    }
+                }
+                ddx = -SH_C1 * vk[3];
+                ddy = -SH_C1 * vk[1];
+                ddz = SH_C1 * vk[2];
+                if (deg >= 2) {  // the band-2 terms of the degree-3 sums below, in their order
+                    ddx = ddx + SH_C2_0 * y * vk[4] - 2.0f * SH_C2_2 * x * vk[6] + SH_C2_3 * z * vk[7] + 2.0f * SH_C2_4 * x * vk[8];
+                    ddy = ddy + SH_C2_0 * x * vk[4] + SH_C2_1 * z * vk[5] - 2.0f * SH_C2_2 * y * vk[6] - 2.0f * SH_C2_4 * y * vk[8];
+                    ddz = ddz + SH_C2_1 * y * vk[5] + 4.0f * SH_C2_2 * z * vk[6] + SH_C2_3 * x * vk[7];
+                }
+            }
+        } else {
+            len = view_direction(U.camera_position, px, py, pz, x, y, z);
+            const float xx = x * x, yy = y * y, zz = z * z;
+            const float basis[16] = {SH_C0,
+                                     -SH_C1 * y,
+                                     SH_C1 * z,
+                                     -SH_C1 * x,
+                                     SH_C2_0 * x * y,
+                                     SH_C2_1 * y * z,
+                                     SH_C2_2 * ((2.0f * zz - xx) - yy),
+                                     SH_C2_3 * z * x,
+                                     SH_C2_4 * (xx - yy),
+                                     SH_C3_0 * (3.0f * xx - yy) * y,
+                                     SH_C3_1 * x * y * z,
+                                     SH_C3_2 * ((4.0f * zz - xx) - yy) * y,
+                                     SH_C3_3 * z * ((2.0f * zz - 3.0f * xx) - 3.0f * yy),
+                                     SH_C3_4 * x * ((4.0f * zz - xx) - yy),
+                                     SH_C3_5 * (xx - yy) * z,
+                                     SH_C3_6 * x * (xx - 3.0f * yy)};
+            const float* sh = v + 12;
+            float vk[16];
+#pragma unroll
+            for (int k = 0; k < 16; k++) {
+                if (store_v) {
+                    gv[12 + 3 * k + 0] = basis[k] * dcr;
+                    gv[12 + 3 * k + 1] = basis[k] * dcg;
+                    gv[12 + 3 * k + 2] = basis[k] * dcb;
+                }
+                vk[k] = (sh[3 * k] * dcr + sh[3 * k + 1] * dcg) + sh[3 * k + 2] * dcb;
+            }
+            ddx = -SH_C1 * vk[3] + SH_C2_0 * y * vk[4] - 2.0f * SH_C2_2 * x * vk[6] + SH_C2_3 * z * vk[7] + 2.0f * SH_C2_4 * x * vk[8] +
+                              6.0f * SH_C3_0 * x * y * vk[9] + SH_C3_1 * y * z * vk[10] - 2.0f * SH_C3_2 * x * y * vk[11] -
+                              6.0f * SH_C3_3 * x * z * vk[12] + SH_C3_4 * ((4.0f * zz - 3.0f * xx) - yy) * vk[13] + 2.0f * SH_C3_5 * x * z * vk[14] +
+                              3.0f * SH_C3_6 * (xx - yy) * vk[15];
+            ddy = -SH_C1 * vk[1] + SH_C2_0 * x * vk[4] + SH_C2_1 * z * vk[5] - 2.0f * SH_C2_2 * y * vk[6] - 2.0f * SH_C2_4 * y * vk[8] +
+                              3.0f * SH_C3_0 * (xx - yy) * vk[9] + SH_C3_1 * x * z * vk[10] + SH_C3_2 * ((4.0f * zz - xx) - 3.0f * yy) * vk[11] -
+                              6.0f * SH_C3_3 * y * z * vk[12] - 2.0f * SH_C3_4 * x * y * vk[13] - 2.0f * SH_C3_5 * y * z * vk[14] -
+                              6.0f * SH_C3_6 * x * y * vk[15];
+            ddz = SH_C1 * vk[2] + SH_C2_1 * y * vk[5] + 4.0f * SH_C2_2 * z * vk[6] + SH_C2_3 * x * vk[7] + SH_C3_1 * x * y * vk[10] +
+                              8.0f * SH_C3_2 * y * z * vk[11] + SH_C3_3 * ((6.0f * zz - 3.0f * xx) - 3.0f * yy) * vk[12] + 8.0f * SH_C3_4 * x * z * vk[13] +
+                              SH_C3_5 * (xx - yy) * vk[14];
         }
-        const float ddx = -SH_C1 * vk[3] + SH_C2_0 * y * vk[4] - 2.0f * SH_C2_2 * x * vk[6] + SH_C2_3 * z * vk[7] + 2.0f * SH_C2_4 * x * vk[8] +
-                          6.0f * SH_C3_0 * x * y * vk[9] + SH_C3_1 * y * z * vk[10] - 2.0f * SH_C3_2 * x * y * vk[11] -
-                          6.0f * SH_C3_3 * x * z * vk[12] + SH_C3_4 * ((4.0f * zz - 3.0f * xx) - yy) * vk[13] + 2.0f * SH_C3_5 * x * z * vk[14] +
-                          3.0f * SH_C3_6 * (xx - yy) * vk[15];
-        const float ddy = -SH_C1 * vk[1] + SH_C2_0 * x * vk[4] + SH_C2_1 * z * vk[5] - 2.0f * SH_C2_2 * y * vk[6] - 2.0f * SH_C2_4 * y * vk[8] +
-                          3.0f * SH_C3_0 * (xx - yy) * vk[9] + SH_C3_1 * x * z * vk[10] + SH_C3_2 * ((4.0f * zz - xx) - 3.0f * yy) * vk[11] -
-                          6.0f * SH_C3_3 * y * z * vk[12] - 2.0f * SH_C3_4 * x * y * vk[13] - 2.0f * SH_C3_5 * y * z * vk[14] -
-                          6.0f * SH_C3_6 * x * y * vk[15];
-        const float ddz = SH_C1 * vk[2] + SH_C2_1 * y * vk[5] + 4.0f * SH_C2_2 * z * vk[6] + SH_C2_3 * x * vk[7] + SH_C3_1 * x * y * vk[10] +
-                          8.0f * SH_C3_2 * y * z * vk[11] + SH_C3_3 * ((6.0f * zz - 3.0f * xx) - 3.0f * yy) * vk[12] + 8.0f * SH_C3_4 * x * z * vk[13] +
-                          SH_C3_5 * (xx - yy) * vk[14];
         const float dot = (x * ddx + y * ddy) + z * ddz;  // d (e / |e|) = (I - dir dir^T) / |e|
         dp[0] += (ddx - x * dot) / len;
         dp[1] += (ddy - y * dot) / len;
@@ -988,24 +1040,28 @@ cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackwar
 }
 
 // The vertex / camera part: k_preprocess_backward over the survivors (after the blend's sums and the density statistics).
-template <bool DEPTH>
+template <bool DEPTH, bool SHDEG>
 cudaError_t launch_preprocess_backward(const BackwardParams& p, bool antialiased, const gsb_camera_model* lens, const DepthBackward* dp,
-                                       unsigned grid, cudaStream_t s, gsb_camera_model* grad_lens) {
-    auto with_depth = [&](const auto& base) {
-        if constexpr (DEPTH) return PbDepthParams<std::decay_t<decltype(base)>>{base, dp->scratch};
-        else return base;
+                                       unsigned grid, cudaStream_t s, gsb_camera_model* grad_lens, int sh_degree) {
+    auto with_extras = [&](const auto& base) {  // the depth scratch, then the degree, as the instantiation takes them
+        const auto b = [&] {
+            if constexpr (DEPTH) return PbDepthParams<std::decay_t<decltype(base)>>{base, dp->scratch};
+            else return base;
+        }();
+        if constexpr (SHDEG) return ShDegreeParams<std::decay_t<decltype(b)>>{b, sh_degree};
+        else return b;
     };
     if (lens) {  // fisheye or OpenCV: the same launches, one lens instantiation each
-        const auto fp = with_depth(BackwardFisheyeParams{p, *lens});
+        const auto fp = with_extras(BackwardFisheyeParams{p, *lens});
         auto launch = [&](auto opencv) {
             constexpr bool OC = decltype(opencv)::value, FE = !OC;
             if (!p.cam_partials) {  // vertex gradients only
-                if (antialiased) k_preprocess_backward<false, true, FE, DEPTH, OC><<<grid, PB_THREADS, 0, s>>>(fp);
-                else k_preprocess_backward<false, false, FE, DEPTH, OC><<<grid, PB_THREADS, 0, s>>>(fp);
+                if (antialiased) k_preprocess_backward<false, true, FE, DEPTH, OC, SHDEG><<<grid, PB_THREADS, 0, s>>>(fp);
+                else k_preprocess_backward<false, false, FE, DEPTH, OC, SHDEG><<<grid, PB_THREADS, 0, s>>>(fp);
                 return cudaGetLastError();
             }
-            if (antialiased) k_preprocess_backward<true, true, FE, DEPTH, OC><<<grid, PB_THREADS, 0, s>>>(fp);
-            else k_preprocess_backward<true, false, FE, DEPTH, OC><<<grid, PB_THREADS, 0, s>>>(fp);
+            if (antialiased) k_preprocess_backward<true, true, FE, DEPTH, OC, SHDEG><<<grid, PB_THREADS, 0, s>>>(fp);
+            else k_preprocess_backward<true, false, FE, DEPTH, OC, SHDEG><<<grid, PB_THREADS, 0, s>>>(fp);
             cudaError_t e = cudaGetLastError();
             if (e != cudaSuccess) return e;
             k_fisheye_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo, grad_lens);
@@ -1013,14 +1069,14 @@ cudaError_t launch_preprocess_backward(const BackwardParams& p, bool antialiased
         };
         return lens->kind == GSB_CAMERA_OPENCV ? launch(std::true_type{}) : launch(std::false_type{});
     }
-    const auto pp = with_depth(p);
+    const auto pp = with_extras(p);
     if (!p.grad_ubo) {
-        if (antialiased) k_preprocess_backward<false, true, false, DEPTH><<<grid, PB_THREADS, 0, s>>>(pp);
-        else k_preprocess_backward<false, false, false, DEPTH><<<grid, PB_THREADS, 0, s>>>(pp);
+        if (antialiased) k_preprocess_backward<false, true, false, DEPTH, false, SHDEG><<<grid, PB_THREADS, 0, s>>>(pp);
+        else k_preprocess_backward<false, false, false, DEPTH, false, SHDEG><<<grid, PB_THREADS, 0, s>>>(pp);
         return cudaGetLastError();
     }
-    if (antialiased) k_preprocess_backward<true, true, false, DEPTH><<<grid, PB_THREADS, 0, s>>>(pp);
-    else k_preprocess_backward<true, false, false, DEPTH><<<grid, PB_THREADS, 0, s>>>(pp);
+    if (antialiased) k_preprocess_backward<true, true, false, DEPTH, false, SHDEG><<<grid, PB_THREADS, 0, s>>>(pp);
+    else k_preprocess_backward<true, false, false, DEPTH, false, SHDEG><<<grid, PB_THREADS, 0, s>>>(pp);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     k_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo);
@@ -1031,7 +1087,7 @@ cudaError_t launch_preprocess_backward(const BackwardParams& p, bool antialiased
 
 cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det,
                             const gsb_camera_model* lens, const DepthBackward* depth, const FeatureParams* features,
-                            gsb_camera_model* grad_lens) {
+                            gsb_camera_model* grad_lens, int sh_degree) {
     if (grad_lens && !lens) return cudaErrorInvalidValue;
     const bool density = p.density != nullptr;
     const bool geometry = p.grad_vertices || p.cam_partials;  // false only for a feature gradient alone
@@ -1072,8 +1128,11 @@ cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 ba
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
-    return depth ? launch_preprocess_backward<true>(p, antialiased, lens, depth, grid, s, grad_lens)
-                 : launch_preprocess_backward<false>(p, antialiased, lens, depth, grid, s, grad_lens);
+    if (sh_degree < 3)
+        return depth ? launch_preprocess_backward<true, true>(p, antialiased, lens, depth, grid, s, grad_lens, sh_degree)
+                     : launch_preprocess_backward<false, true>(p, antialiased, lens, depth, grid, s, grad_lens, sh_degree);
+    return depth ? launch_preprocess_backward<true, false>(p, antialiased, lens, depth, grid, s, grad_lens, sh_degree)
+                 : launch_preprocess_backward<false, false>(p, antialiased, lens, depth, grid, s, grad_lens, sh_degree);
 }
 
 uint32_t background_grad_rows(uint32_t height) { return std::min(height, BG_MAX_ROWS); }

@@ -96,6 +96,7 @@ struct LastFrame {
     bool antialiased = false;  // gsb_set_antialiased when enqueued: its opacities carry the compensation
     float background[3] = {};  // gsb_set_background when enqueued: the colour its pixels were composited over
     gsb_camera_model camera{};  // gsb_set_camera_model when enqueued (kind 0: pinhole)
+    int sh_degree = 3;       // gsb_set_sh_degree when enqueued: the SH bands its colours summed (its backward pass follows it)
     uint64_t scene_gen = 0;  // gsb_ctx::scene_gen when enqueued; 0: no frame yet (a frame needs an upload, which bumps it)
     bool pending = false;    // its completion event and stats copy have not been waited for (wait_frame)
     bool exists = false;     // its stats and debug buffers may be read (a scene upload clears it)
@@ -164,6 +165,7 @@ struct gsb_ctx {
     bool antialiased = false;   // gsb_set_antialiased: k_project scales opacities by the dilation's compensation
     float background[3] = {};   // gsb_set_background: k_blend composites every pixel over this colour (zeros: no term)
     gsb_camera_model camera{};  // gsb_set_camera_model: k_project's lens (kind 0: the UBO's pinhole camera)
+    int sh_degree = 3;          // gsb_set_sh_degree: k_project sums the SH coefficients of bands <= sh_degree
     int tile_cull = 0;          // gsb_set_tile_cull level: 0 reference-equivalent lists, 1 exact per-tile culling, 2 coarse bins
     uint32_t coarse_shift = 2;  // level 2 bins are 2^shift x 2^shift tiles (GSB_COARSE_SHIFT)
     cudaEvent_t ev[8] = {};

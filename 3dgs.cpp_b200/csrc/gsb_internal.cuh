@@ -102,10 +102,19 @@ struct EmitParams {
 
 cudaError_t launch_cov3d(const float* vtx_aos, uint64_t count, uint64_t dst_offset, float4* pos_op,
                          float4* cov_a, float2* cov_b, float* sh, float scale_factor, cudaStream_t s, bool sh_half = false);
+// gsb_set_sh_degree: the argument of the k_project and k_preprocess_backward instantiations for a degree below 3 is the
+// argument of the degree-3 kernel with the degree appended, so the degree-3 kernels keep their argument layout.
+template <typename Base>
+struct ShDegreeParams : Base {
+    int sh_degree;  // 0, 1 or 2: the colour sums the (sh_degree + 1)^2 coefficients of bands <= sh_degree
+};
+
 // antialiased: gsb_set_antialiased's opacity compensation (not on the routed kernel of a sharded frame)
 // lens: gsb_set_camera_model's fisheye or OpenCV lens (k_project<..., FISHEYE> or <..., OPENCV>, plain contexts only); null =
 // the pinhole camera.
-cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* lens = nullptr);
+// sh_degree: gsb_set_sh_degree (plain contexts only); 3 launches the degree-3 kernels.
+cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* lens = nullptr,
+                           int sh_degree = 3);
 cudaError_t launch_emit(const EmitParams& p, cudaStream_t s);
 
 struct SortParams {  // host-side arguments of launch_sort
@@ -264,9 +273,11 @@ cudaError_t launch_feature_backward(FeatureParams p, bool det, cudaStream_t s);
 // features: gsb_render_backward_features' feature arguments (null for the other entries).  Its pass runs after the colour
 // pass's sums (which are skipped when there is neither an image nor a depth gradient) and before k_density_accumulate and
 // k_preprocess_backward; with neither grad_vertices nor grad_ubo only the feature gradient is formed.
+// sh_degree: the frame's gsb_set_sh_degree.  Below 3 the SH columns of the dropped bands are not written (the caller zeroed
+// them) and the view direction takes the live coefficients only.
 cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det = nullptr,
                             const gsb_camera_model* lens = nullptr, const DepthBackward* depth = nullptr,
-                            const FeatureParams* features = nullptr, gsb_camera_model* grad_lens = nullptr);
+                            const FeatureParams* features = nullptr, gsb_camera_model* grad_lens = nullptr, int sh_degree = 3);
 // gsb_background_gradient: out[c] = sum over the W x H pixels of T_final(p) grad_image(p)[c], from the recorded frame's
 // (bits(T), last) words.  fp64 products and sums in an order fixed by W and H (background_grad_rows(H) per-CTA partials,
 // then one CTA), no atomics.  partials holds 3 doubles per row of background_grad_rows(H).

@@ -159,6 +159,52 @@ __device__ __forceinline__ void compute_sh(const float4* __restrict__ sh4, float
     b = c[2];
 }
 
+// The first coefficient 4G of group G alone: floats 12G .. 12G+2 of the first of the group's three words.
+template <int G, bool SH16>
+__device__ __forceinline__ void sh_group_head(const float4* __restrict__ sh4, float (&c)[3], const ShDir& d) {
+    float f[3];
+    if constexpr (SH16) {
+        const uint2 w = __ldg(reinterpret_cast<const uint2*>(sh4) + 3 * G);
+        const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&w.x)), hi = __half22float2(*reinterpret_cast<const __half2*>(&w.y));
+        f[0] = lo.x, f[1] = lo.y, f[2] = hi.x;
+    } else {
+        const float4 t0 = __ldg(sh4 + 3 * G);
+        f[0] = t0.x, f[1] = t0.y, f[2] = t0.z;
+    }
+#pragma unroll
+    for (int ch = 0; ch < 3; ch++) c[ch] = sh_term<4 * G>(c[ch], f[ch], d);
+}
+
+// compute_sh at gsb_set_sh_degree's degree deg in 0..2 (warp-uniform): the sum over the (deg + 1)^2 coefficients of bands <= deg
+// only, in compute_sh's order, reading only the words that hold them -- 1 float4 (SH16: uint2) at degree 0, 3 at 1, 7 at 2
+// (degree 2 ends at coefficient 8, the head of group 2).  Degree 0 needs no view direction.  Each dropped term of compute_sh is
+// a + (C 0) w = a for a finite direction, so this is compute_sh of the scene with the dropped bands zeroed (DESIGN.md section 25).
+template <bool SH16>
+__device__ __forceinline__ void compute_sh_degree(const float4* __restrict__ sh4, float px, float py, float pz, const float* cam, int deg,
+                                                  float& r, float& g, float& b) {
+    float c[3] = {0.f, 0.f, 0.f};
+    ShDir d{};
+    if (deg == 0) {
+        sh_group_head<0, SH16>(sh4, c, d);  // SH_C0 s: the direction takes no part
+    } else {
+        view_direction(cam, px, py, pz, d.x, d.y, d.z);
+        const float xx = d.x * d.x, yy = d.y * d.y;
+        d.w6 = ((2.0f * d.z) * d.z - xx) - yy;
+        d.w8 = xx - yy;
+        sh_group<0, SH16>(sh4, c, d);
+        if (deg >= 2) {
+            sh_group<1, SH16>(sh4, c, d);
+            sh_group_head<2, SH16>(sh4, c, d);
+        }
+    }
+    c[0] = c[0] + 0.5f;
+    c[1] = c[1] + 0.5f;
+    c[2] = c[2] + 0.5f;
+    r = c[0] < 0.0f ? 0.0f : c[0];
+    g = c[1];
+    b = c[2];
+}
+
 // ------------------------------------------------------------------------------------------
 // k_project
 // ------------------------------------------------------------------------------------------
@@ -183,6 +229,8 @@ __device__ __forceinline__ void compute_sh(const float4* __restrict__ sh4, float
 // the FISHEYE instantiations take the larger argument, so the others keep their code.
 // OPENCV (gsb_set_camera_model, plain contexts only): the projection, Jacobian and cull of the OpenCV lens (opencv_geo /
 // opencv_jacobian); the depth key stays z.  tan2_max is tan^2(max_theta), rounded to fp32 once on the host.
+// SHDEG (gsb_set_sh_degree below 3, plain contexts only): the colour is compute_sh_degree's at P.sh_degree; the argument is the
+// degree-3 kernel's with the degree appended (ShDegreeParams), and the launch bounds are the lens family's.
 struct ProjectFisheyeParams : ProjectParams {
     gsb_camera_model cam;
 };
@@ -191,7 +239,9 @@ struct ProjectOpencvParams : ProjectParams {
     float tan2_max;
 };
 template <bool FISHEYE, bool OPENCV = false>
-using ProjParams = std::conditional_t<FISHEYE, ProjectFisheyeParams, std::conditional_t<OPENCV, ProjectOpencvParams, ProjectParams>>;
+using LensProjParams = std::conditional_t<FISHEYE, ProjectFisheyeParams, std::conditional_t<OPENCV, ProjectOpencvParams, ProjectParams>>;
+template <bool FISHEYE, bool OPENCV = false, bool SHDEG = false>
+using ProjParams = std::conditional_t<SHDEG, ShDegreeParams<LensProjParams<FISHEYE, OPENCV>>, LensProjParams<FISHEYE, OPENCV>>;
 template <bool FISHEYE, bool OPENCV = false>
 struct ProjectBounds {
     static constexpr int MIN_BLOCKS = GSB_PROJECT_MIN_BLOCKS;
@@ -204,12 +254,13 @@ template <>
 struct ProjectBounds<false, true> {
     static constexpr int MIN_BLOCKS = GSB_PROJECT_OPENCV_MIN_BLOCKS;
 };
-template <bool DEBUG, bool ROUTED, bool SH16, bool AA, bool FISHEYE = false, bool OPENCV = false>
+template <bool DEBUG, bool ROUTED, bool SH16, bool AA, bool FISHEYE = false, bool OPENCV = false, bool SHDEG = false>
 __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE, OPENCV>::MIN_BLOCKS)
-    k_project(const __grid_constant__ ProjParams<FISHEYE, OPENCV> P) {
+    k_project(const __grid_constant__ ProjParams<FISHEYE, OPENCV, SHDEG> P) {
     static_assert(!(ROUTED && AA), "sharded contexts have no anti-aliased mode");
     static_assert(!(ROUTED && FISHEYE), "sharded contexts have no fisheye camera");
     static_assert(!(ROUTED && OPENCV) && !(FISHEYE && OPENCV), "sharded contexts have no OpenCV camera; one lens per frame");
+    static_assert(!(ROUTED && SHDEG), "sharded contexts have only degree 3");
     __shared__ uint32_t s_chunk;
     __shared__ uint32_t s_wsurv[PRE_THREADS / 32];
     __shared__ uint32_t s_base_surv;
@@ -388,7 +439,13 @@ __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE, OPENCV>::M
 
     // ---- SH colour of survivors (overlaps the look-back of other chunks) ----
     float colr = 0.f, colg = 0.f, colb = 0.f;
-    if (surv) compute_sh<SH16>(reinterpret_cast<const float4*>(P.sh) + (size_t)i * (SH16 ? 6 : 12), px, py, pz, U.camera_position, colr, colg, colb);
+    if constexpr (SHDEG) {
+        if (surv)
+            compute_sh_degree<SH16>(reinterpret_cast<const float4*>(P.sh) + (size_t)i * (SH16 ? 6 : 12), px, py, pz, U.camera_position,
+                                    P.sh_degree, colr, colg, colb);
+    } else {
+        if (surv) compute_sh<SH16>(reinterpret_cast<const float4*>(P.sh) + (size_t)i * (SH16 ? 6 : 12), px, py, pz, U.camera_position, colr, colg, colb);
+    }
 
     // ---- decoupled look-back by warp 0: 32 predecessors per step ----
     if (warp == 0) {
@@ -861,37 +918,44 @@ __global__ void __launch_bounds__(PRE_THREADS) k_emit_coarse(const __grid_consta
 
 }  // namespace
 
-template <bool AA, bool FISHEYE, bool OPENCV>
-void launch_project_plain(const ProjParams<FISHEYE, OPENCV>& p, bool debug, unsigned blocks, cudaStream_t s) {
+template <bool AA, bool FISHEYE, bool OPENCV, bool SHDEG>
+void launch_project_plain(const ProjParams<FISHEYE, OPENCV, SHDEG>& p, bool debug, unsigned blocks, cudaStream_t s) {
     if (p.sh_half) {  // fp16 SH storage (non-parity)
-        if (debug) k_project<true, false, true, AA, FISHEYE, OPENCV><<<blocks, PRE_THREADS, 0, s>>>(p);
-        else k_project<false, false, true, AA, FISHEYE, OPENCV><<<blocks, PRE_THREADS, 0, s>>>(p);
-    } else if (debug) k_project<true, false, false, AA, FISHEYE, OPENCV><<<blocks, PRE_THREADS, 0, s>>>(p);
-    else k_project<false, false, false, AA, FISHEYE, OPENCV><<<blocks, PRE_THREADS, 0, s>>>(p);
+        if (debug) k_project<true, false, true, AA, FISHEYE, OPENCV, SHDEG><<<blocks, PRE_THREADS, 0, s>>>(p);
+        else k_project<false, false, true, AA, FISHEYE, OPENCV, SHDEG><<<blocks, PRE_THREADS, 0, s>>>(p);
+    } else if (debug) k_project<true, false, false, AA, FISHEYE, OPENCV, SHDEG><<<blocks, PRE_THREADS, 0, s>>>(p);
+    else k_project<false, false, false, AA, FISHEYE, OPENCV, SHDEG><<<blocks, PRE_THREADS, 0, s>>>(p);
 }
 
+template <bool FISHEYE, bool OPENCV, bool SHDEG>
+void launch_project_plain(const ProjParams<FISHEYE, OPENCV, SHDEG>& p, bool debug, bool antialiased, unsigned blocks, cudaStream_t s) {
+    if (antialiased) launch_project_plain<true, FISHEYE, OPENCV, SHDEG>(p, debug, blocks, s);
+    else launch_project_plain<false, FISHEYE, OPENCV, SHDEG>(p, debug, blocks, s);
+}
+
+// degree 3: the degree-3 kernels; below: the SHDEG instantiations, with the degree appended to the argument
 template <bool FISHEYE, bool OPENCV = false>
-void launch_project_plain(const ProjParams<FISHEYE, OPENCV>& p, bool debug, bool antialiased, unsigned blocks, cudaStream_t s) {
-    if (antialiased) launch_project_plain<true, FISHEYE, OPENCV>(p, debug, blocks, s);
-    else launch_project_plain<false, FISHEYE, OPENCV>(p, debug, blocks, s);
+void launch_project_plain(const ProjParams<FISHEYE, OPENCV>& p, bool debug, bool antialiased, int sh_degree, unsigned blocks, cudaStream_t s) {
+    if (sh_degree < 3) launch_project_plain<FISHEYE, OPENCV, true>(ShDegreeParams<ProjParams<FISHEYE, OPENCV>>{p, sh_degree}, debug, antialiased, blocks, s);
+    else launch_project_plain<FISHEYE, OPENCV, false>(p, debug, antialiased, blocks, s);
 }
 
-cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* lens) {
+cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* lens, int sh_degree) {
     const gsb_camera_model* fisheye = lens && lens->kind == GSB_CAMERA_FISHEYE ? lens : nullptr;
     const gsb_camera_model* opencv = lens && lens->kind == GSB_CAMERA_OPENCV ? lens : nullptr;
     if (p.n == 0) return cudaSuccess;
     const unsigned blocks = (p.n + PRE_THREADS - 1) / PRE_THREADS;
     if (p.route_world > 0) {
-        if (antialiased || lens) return cudaErrorInvalidValue;  // the routed kernel has no AA or lens instantiation
+        if (antialiased || lens || sh_degree < 3) return cudaErrorInvalidValue;  // the routed kernel has no AA, lens or degree instantiation
         if (p.sh_half) k_project<false, true, true, false><<<blocks, PRE_THREADS, 0, s>>>(p);
         else k_project<false, true, false, false><<<blocks, PRE_THREADS, 0, s>>>(p);
     } else if (fisheye) {
-        launch_project_plain<true>(ProjectFisheyeParams{p, *fisheye}, debug, antialiased, blocks, s);
+        launch_project_plain<true>(ProjectFisheyeParams{p, *fisheye}, debug, antialiased, sh_degree, blocks, s);
     } else if (opencv) {
         const double t = std::tan((double)opencv->max_theta);
-        launch_project_plain<false, true>(ProjectOpencvParams{p, *opencv, (float)(t * t)}, debug, antialiased, blocks, s);
+        launch_project_plain<false, true>(ProjectOpencvParams{p, *opencv, (float)(t * t)}, debug, antialiased, sh_degree, blocks, s);
     } else {
-        launch_project_plain<false>(p, debug, antialiased, blocks, s);
+        launch_project_plain<false>(p, debug, antialiased, sh_degree, blocks, s);
     }
     return cudaGetLastError();
 }

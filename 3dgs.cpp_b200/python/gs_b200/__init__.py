@@ -39,7 +39,7 @@ ALL_ROWS = 0xFFFFFFFF
 EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_abi_version", "gsb_device_count", "gsb_create", "gsb_destroy", "gsb_last_error",
     "gsb_scene_upload", "gsb_scene_size", "gsb_set_mode", "gsb_set_debug", "gsb_set_timers", "gsb_set_tile_cull", "gsb_set_sh_storage",
-    "gsb_set_antialiased", "gsb_set_background", "gsb_set_camera_model",
+    "gsb_set_antialiased", "gsb_set_background", "gsb_set_camera_model", "gsb_set_sh_degree",
     "gsb_reserve_instances", "gsb_render", "gsb_render_async", "gsb_get_stats", "gsb_debug_size",
     "gsb_debug_download", "gsb_sort_pairs", "gsb_sort_pairs32", "gsb_set_graph", "gsb_host_alloc", "gsb_host_free",
     # reverse mode
@@ -287,6 +287,7 @@ lib.gsb_set_debug.argtypes = [_vp, C.c_int]
 lib.gsb_set_timers.argtypes = [_vp, C.c_int]
 lib.gsb_set_tile_cull.argtypes = [_vp, C.c_int]
 lib.gsb_set_antialiased.argtypes = [_vp, C.c_int]
+lib.gsb_set_sh_degree.argtypes = [_vp, C.c_int]
 lib.gsb_set_background.argtypes = [_vp, C.POINTER(C.c_float)]
 lib.gsb_set_camera_model.argtypes = [_vp, C.POINTER(CameraModel)]
 lib.gsb_set_sh_storage.argtypes = [_vp, C.c_int]
@@ -573,6 +574,7 @@ class Context:
         self._depth_frame_id = -1  # the value of `frames` after the last gsb_render_depth frame
         self._background = None  # the last set_background colour (render_torch restores it after a frame of its own)
         self.camera = None  # the last set_camera_model lens (None: pinhole)
+        self.sh_degree = 3  # the last set_sh_degree degree (render_torch restores it after a frame of its own)
 
     def close(self):
         if self.h and self._own:
@@ -618,6 +620,16 @@ class Context:
         compensation for the 0.3 px dilation (gsplat's antialiased mode).  render_torch, SceneAdam, image_metrics and the
         backward pass follow it (the backward uses the setting of the frame it differentiates)."""
         self._ck(lib.gsb_set_antialiased(self.h, int(on)))
+
+    def set_sh_degree(self, d=3):
+        """gsb_set_sh_degree: from the next frame, the colour sums the spherical-harmonics coefficients of bands <= d only
+        (d in 0..3, 3 the default; the scene keeps all 16).  The frame equals the degree-3 frame of the scene with the higher
+        bands zeroed.  render_torch, SceneAdam and the backward pass follow it (the backward uses the degree of the frame it
+        differentiates, and leaves the gradient of every higher band at 0).  ValueError for d outside 0..3."""
+        if isinstance(d, bool) or not isinstance(d, (int, np.integer)) or not 0 <= d <= 3:
+            raise ValueError(f"set_sh_degree: the degree must be an integer in 0..3, not {d!r}")
+        self._ck(lib.gsb_set_sh_degree(self.h, int(d)))
+        self.sh_degree = int(d)
 
     def set_background(self, rgb=None):
         """gsb_set_background: from the next frame, every pixel is composited over the colour rgb (3 finite floats; None =
@@ -1147,7 +1159,7 @@ def _render_fn():
 
         class RenderFn(torch.autograd.Function):
             @staticmethod
-            def forward(fctx, ctx, vertices, u, ubo, density, background, depth, features, lens):
+            def forward(fctx, ctx, vertices, u, ubo, density, background, depth, features, lens, sh_degree):
                 v = vertices.detach().contiguous()
                 fctx.depth = bool(depth)
                 fctx.features = None
@@ -1176,7 +1188,7 @@ def _render_fn():
                 torch.cuda.current_stream(v.device).synchronize()  # the upload runs on the context's stream: v must be complete
                 ctx.upload(v)
 
-                def frame():
+                def frame_bg():
                     if background is None:
                         return ctx._render_whole_frame(u, v.device, fctx.depth)
                     # this frame over the tensor's colour; the context's own setting is restored after it
@@ -1187,6 +1199,17 @@ def _render_fn():
                         return ctx._render_whole_frame(u, v.device, fctx.depth)
                     finally:
                         ctx.set_background(previous)
+
+                def frame():
+                    if sh_degree is None:
+                        return frame_bg()
+                    # this frame at the given degree; the context's own setting is restored after it
+                    previous = ctx.sh_degree
+                    ctx.set_sh_degree(sh_degree)
+                    try:
+                        return frame_bg()
+                    finally:
+                        ctx.set_sh_degree(previous)
 
                 if cam is None:
                     out = frame()
@@ -1266,14 +1289,14 @@ def _render_fn():
                 if need_bg:  # sum_p T_final g, on the same stream
                     dtype, device = fctx.bg_like
                     grad_bg = ctx.background_gradient(g, torch.cuda.current_stream(v.device)).to(device=device, dtype=dtype)
-                return None, grad_v, None, grad_ubo, None, grad_bg, None, grad_f, grad_lens
+                return None, grad_v, None, grad_ubo, None, grad_bg, None, grad_f, grad_lens, None
 
         _RenderFn = RenderFn
     return _RenderFn
 
 
 def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, background=None, depth=False, features=None,
-                 lens=None):
+                 lens=None, sh_degree=None):
     """Differentiable frame: vertices is a CUDA float32 tensor (n, 60) of GSScene::Vertex records (activated parameters, as
     gsb_scene_upload takes them).  Uploads it from device memory, renders the whole frame as an (H, W, 4) RGBA32F tensor and,
     on backward, returns dL/dvertices through gsb_render_backward.  Turns gsb_set_backward on for `ctx`.  The frame on the
@@ -1316,8 +1339,13 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, 
     features (optional): an (n, C) float32 CUDA tensor of per-Gaussian features, C <= 128.  The frame then also returns its
     (H, W, C) feature map F_c = sum f_ic alpha_i T_i over 0 (gsb_render_features): (img, fmap), or (img, depth_alpha, fmap)
     with depth=True.  Backward differentiates the image, depth / alpha and map in one gsb_render_backward_features pass, into
-    vertices, ubo, density and -- when it requires grad -- features."""
-    return _render_fn().apply(ctx, vertices, u, ubo, density, background, depth, features, lens)
+    vertices, ubo, density and -- when it requires grad -- features.
+
+    sh_degree (optional): 0..3; the frame's colour sums the SH bands <= sh_degree only (gsb_set_sh_degree) and the context's
+    own setting is restored after the forward; None uses the context's setting.  Backward follows the frame's degree: the
+    coefficients of higher bands get a gradient of exactly 0.  It composes with ubo=, lens=, depth=, features=, density=,
+    background= and the deterministic mode."""
+    return _render_fn().apply(ctx, vertices, u, ubo, density, background, depth, features, lens, sh_degree)
 
 
 _LossFn = None
@@ -1595,6 +1623,16 @@ class SceneAdam:
     (Inria's --random_background: the empty space must stay transparent to match every colour), to be compared against
     composite_target(rgba_target, opt.background).  `background` holds the colour of the last render() as 3 floats.
 
+    sh_degree: the spherical-harmonics degree render() draws at (gsb_set_sh_degree, 0..3), read at every render() like lr,
+    so the caller may raise it on a schedule -- Inria's oneupSHdegree every 1000 steps, gsplat's sh_degree_interval:
+
+        opt.sh_degree = min(it // 1000, 3)
+        img = opt.render(u); ctx.image_loss(img, target, 0.2, grad_image=g); opt.step(g)
+
+    The backward pass gives the coefficients of the bands above the frame's degree a gradient of exactly 0, and Adam leaves
+    a row with zero gradient and zero moments bit-identical, so those bands stay as they are until their degree arrives.  A
+    scene from init_from_points has zero higher bands: they start from zero when their degree arrives.
+
     3D Gaussian Splatting as Markov Chain Monte Carlo (Kheradmand et al. 2024, gsplat's MCMCStrategy) instead of
     densify(): the opacity and scale regularisers in step(), position noise after every step (inject_noise, seeded by
     `seed` and the step count) and a periodic relocate() that moves dead Gaussians onto live ones and grows the scene up to
@@ -1644,7 +1682,8 @@ class SceneAdam:
     source rows onto the relocated ones with zero moments and appends features[src] when it grows."""
 
     def __init__(self, ctx: "Context", vertices, lr, betas=(0.9, 0.999), eps=1e-15, selective=True, background=None,
-                 random_background=False, seed=0, filter_cameras=None, features=None, feature_lr=0.0, filter_lenses=None):
+                 random_background=False, seed=0, filter_cameras=None, features=None, feature_lr=0.0, filter_lenses=None,
+                 sh_degree=3):
         import torch
 
         if not isinstance(vertices, torch.Tensor) or not vertices.is_cuda or vertices.dim() != 2 or vertices.shape[1] != 60:
@@ -1653,6 +1692,7 @@ class SceneAdam:
         self.steps = 0
         self.seed = int(seed)
         self.background = None if background is None else [float(x) for x in background]
+        self.sh_degree = sh_degree
         self._generator = torch.Generator().manual_seed(int(seed)) if random_background else None
         self.filter_cameras = None if filter_cameras is None else list(filter_cameras)
         self.filter_lenses = filter_lenses
@@ -1730,6 +1770,7 @@ class SceneAdam:
             self.background = torch.rand(3, generator=self._generator).tolist()
         if self.background is not None:
             self.ctx.set_background(self.background)
+        self.ctx.set_sh_degree(self.sh_degree)
         out = self.ctx._render_whole_frame(u, self.vertices.device, depth)
         if not features:
             return out

@@ -183,6 +183,17 @@ int gsb_set_tile_cull(gsb_ctx *ctx, int level);
  * frame; the backward entries and the selective gsb_adam_step follow the setting the last frame was rendered with and
  * differentiate through comp.  NULL ctx or a sharded context (gsb_create_sharded, a gsb_group rank): GSB_ERR_INVALID. */
 int gsb_set_antialiased(gsb_ctx *ctx, int enabled);
+/* Spherical-harmonics degree of the frames' colour, 0..3 (default 3; the reference's degree is fixed at 3).  At degree d the
+ * colour is preprocess.comp:73-108's sum over the (d + 1)^2 coefficients of bands <= d only, the terms added in the same
+ * order; degree 0 is SH_C0 * sh[0] + 0.5 and needs no view direction.  The scene keeps all 48 coefficients per Gaussian
+ * (uploads, gsb_set_sh_storage and the record layout are unchanged); frames read only the live ones.  A frame at degree d is
+ * bit for bit the degree-3 frame of the scene with the coefficients of bands > d set to zero, for every survivor whose view
+ * direction is finite.  This is the degree schedule of 3DGS training (Inria's oneupSHdegree, gsplat's sh_degree): the
+ * backward entries follow the degree the last frame was rendered with, and leave the gradient of every coefficient of a band
+ * above it at exactly 0 (so gsb_adam_step, from zero moments, leaves those coefficients as they are).  Takes effect at the next
+ * frame; changing it drops no captured graph.  NULL ctx, a degree outside 0..3, or a sharded context (gsb_create_sharded, a
+ * gsb_group rank; they have only degree 3): GSB_ERR_INVALID. */
+int gsb_set_sh_degree(gsb_ctx *ctx, int degree);
 /* Background colour (default black; no reference counterpart).  rgb: 3 host floats, NULL = (0, 0, 0).  render.comp:98 stores
  * vec4(c, 1), the colour composited over black; with a background every colour channel of every pixel is stored as
  *     out = c + T_final * bg          (one fp32 multiply, then one add, each rounded; EXACT and FAST alike)
