@@ -2,7 +2,8 @@
 //   gs_viewer_headless [-d DEVICE] [-w WIDTH] [-h HEIGHT] [-v] [--frames N] [--camera x,y,z[,qw,qx,qy,qz]]
 //                      [--fov DEG] [--camera-path poses.txt] [--mode exact|fast] [--cull [LEVEL]] [--antialiased]
 //                      [--sh-degree N] [--background r,g,b] [--fisheye fx,fy,cx,cy[,k1,k2,k3,k4[,max_theta_deg]]]
-//                      [--opencv fx,fy,cx,cy[,k1,k2,p1,p2[,max_theta_deg]]] [--out image.ppm] [--float-out image.pfm] scene.ply
+//                      [--opencv fx,fy,cx,cy[,k1,k2,p1,p2[,max_theta_deg]]] [--ortho fx,fy,cx,cy] [--out image.ppm]
+//                      [--float-out image.pfm] scene.ply
 // --antialiased: gsb_set_antialiased (opacity compensated for the 0.3 px dilation, as scenes trained that way expect).
 // --sh-degree N: gsb_set_sh_degree (0..3; the colour sums the SH bands <= N only, e.g. for a scene trained at a lower degree).
 // --background r,g,b: gsb_set_background (e.g. 1,1,1 for an object scene trained over white; default black).
@@ -10,6 +11,8 @@
 // (i, j): COLMAP's cx - 0.5); without max_theta_deg, the largest angle up to 175 deg at which theta_d still increases.
 // --opencv fx,fy,cx,cy[,k1,k2,p1,p2[,max_theta_deg]]: the same with COLMAP's OPENCV (radial-tangential) lens; without
 // max_theta_deg, the largest angle up to 80 deg at which r R(r^2) still increases (python's opencv_camera default).
+// --ortho fx,fy,cx,cy: gsb_set_camera_model with the orthographic camera, fx and fy in pixels per world unit (e.g. a top-down
+// orthophoto of an aerial scene).
 // --camera-path: one pose per line `x y z qw qx qy qz [fov]` (# comments); `--frames` frames are rendered at each pose
 // and one JSON line is printed per pose (SURVEY 8d: record M for every timed camera).
 // Loads the .ply through GSScene, renders N frames through Renderer::draw() (B8G8R8A8 like the swapchain),
@@ -33,7 +36,7 @@ static void usage() {
     std::puts("usage: gs_viewer_headless [-d device] [-w width] [-h height] [-v] [--frames n] [--camera x,y,z[,qw,qx,qy,qz]]\n"
               "                          [--fov deg] [--camera-path poses.txt] [--mode exact|fast] [--cull [0|1|2]] [--antialiased]\n"
               "                          [--sh-degree 0|1|2|3] [--background r,g,b] [--fisheye fx,fy,cx,cy[,k1,k2,k3,k4[,max_theta_deg]]]\n"
-              "                          [--opencv fx,fy,cx,cy[,k1,k2,p1,p2[,max_theta_deg]]]\n"
+              "                          [--opencv fx,fy,cx,cy[,k1,k2,p1,p2[,max_theta_deg]]] [--ortho fx,fy,cx,cy]\n"
               "                          [--out image.ppm] [--float-out image.pfm] scene.ply");
 }
 
@@ -44,7 +47,7 @@ int main(int argc, char** argv) {
     uint32_t frames = 1;
     bool verbose = false, cull = false, antialiased = false, background = false;
     float bg[3] = {0, 0, 0};
-    uint32_t lens_kind = GSB_CAMERA_PINHOLE;  // --fisheye or --opencv
+    uint32_t lens_kind = GSB_CAMERA_PINHOLE;  // --fisheye, --opencv or --ortho
     float lens[9] = {0, 0, 0, 0, 0, 0, 0, 0, -1.0f};  // fx fy cx cy k[0..3] max_theta_deg (< 0: the default)
     float cam[7] = {0, 0, 0, 1, 0, 0, 0};
     float fov = 45.0f;
@@ -83,8 +86,8 @@ int main(int argc, char** argv) {
             int k = 0;
             for (char* tok = std::strtok(const_cast<char*>(next()), ","); tok && k < 3; tok = std::strtok(nullptr, ",")) bg[k++] = static_cast<float>(std::atof(tok));
         }
-        else if (a == "--fisheye" || a == "--opencv") {
-            lens_kind = a == "--fisheye" ? GSB_CAMERA_FISHEYE : GSB_CAMERA_OPENCV;
+        else if (a == "--fisheye" || a == "--opencv" || a == "--ortho") {
+            lens_kind = a == "--fisheye" ? GSB_CAMERA_FISHEYE : a == "--opencv" ? GSB_CAMERA_OPENCV : GSB_CAMERA_ORTHO;
             int k = 0;
             for (char* tok = std::strtok(const_cast<char*>(next()), ","); tok && k < 9; tok = std::strtok(nullptr, ",")) lens[k++] = static_cast<float>(std::atof(tok));
             if (k < 4) {
@@ -124,6 +127,8 @@ int main(int argc, char** argv) {
             for (int k = 0; k < 4; k++) m.k[k] = lens[4 + k];
             if (lens[8] >= 0.0f) {
                 m.max_theta = lens[8] * static_cast<float>(M_PI / 180.0);
+            } else if (lens_kind == GSB_CAMERA_ORTHO) {  // no field-of-view cull: the setter names any extra word it refuses
+                m.max_theta = 0.0f;
             } else if (lens_kind == GSB_CAMERA_OPENCV) {  // the smallest positive root u0 of 1 + 3 k1 u + 5 k2 u^2, less 1e-4
                 const double k1 = m.k[0], k2 = m.k[1], cap = 80.0 * M_PI / 180.0;
                 double u0 = INFINITY;

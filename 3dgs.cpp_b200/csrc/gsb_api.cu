@@ -962,11 +962,18 @@ int gsb_set_background(gsb_ctx* ctx, const float* rgb) {
     return GSB_OK;
 }
 
-// The checks gsb_set_camera_model makes of a FISHEYE or OPENCV model, and gsb_filter3d_variance_lens of each of its lenses:
-// nullptr if m is a lens the frames can project through, else why not.
+// The checks gsb_set_camera_model makes of a FISHEYE, OPENCV or ORTHO model, and gsb_filter3d_variance_lens of each of its
+// lenses: nullptr if m is a lens the frames can project through, else why not.
 static const char* camera_model_error(const gsb_camera_model& m) {
-    if (m.kind != GSB_CAMERA_FISHEYE && m.kind != GSB_CAMERA_OPENCV) return "unknown camera kind";
+    if (m.kind != GSB_CAMERA_FISHEYE && m.kind != GSB_CAMERA_OPENCV && m.kind != GSB_CAMERA_ORTHO) return "unknown camera kind";
     if (!(m.fx > 0.0f) || !(m.fy > 0.0f) || !isfinite(m.fx) || !isfinite(m.fy)) return "fx and fy must be positive and finite";
+    if (m.kind == GSB_CAMERA_ORTHO) {  // the words an orthographic camera does not use must be zero, not ignored
+        if (!isfinite(m.cx) || !isfinite(m.cy)) return "cx and cy must be finite";
+        for (int i = 0; i < 4; i++)
+            if (m.k[i] != 0.0f) return "an orthographic camera has no distortion: k[0..3] must be 0";
+        if (m.max_theta != 0.0f) return "an orthographic camera has no field-of-view cull: max_theta must be 0";
+        return nullptr;
+    }
     const float rest[] = {m.cx, m.cy, m.k[0], m.k[1], m.k[2], m.k[3], m.max_theta};
     for (float x : rest)
         if (!isfinite(x)) return "every field must be finite";
@@ -1140,12 +1147,14 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     if (ctx->scene_sh_half) return fail(ctx, GSB_ERR_INVALID, msg("fp16 SH storage has no backward pass").c_str());
     if (!args_ok) return fail(ctx, GSB_ERR_INVALID, msg("null argument").c_str());
     const LastFrame& f = ctx->frame;
-    const bool lens_frame = f.camera.kind != GSB_CAMERA_PINHOLE;  // fisheye or OpenCV
+    const bool lens_frame = f.camera.kind != GSB_CAMERA_PINHOLE;  // fisheye, OpenCV or orthographic
     if (lens && !lens_frame)
         return fail(ctx, GSB_ERR_INVALID, msg("the last frame is a pinhole frame (its camera gradient is gsb_render_backward_camera's)").c_str());
     if (!lens && lens_frame && grad_ubo)
         return fail(ctx, GSB_ERR_INVALID,
-                    msg(f.camera.kind == GSB_CAMERA_FISHEYE ? "a fisheye frame has no camera gradient" : "an OpenCV frame has no camera gradient")
+                    msg(f.camera.kind == GSB_CAMERA_FISHEYE  ? "a fisheye frame has no camera gradient"
+                        : f.camera.kind == GSB_CAMERA_OPENCV ? "an OpenCV frame has no camera gradient"
+                                                             : "an orthographic frame has no camera gradient")
                         .c_str());
     if (lens && density && !grad_vertices && !grad_ubo && !grad_lens)
         return fail(ctx, GSB_ERR_INVALID, msg("density needs grad_vertices, grad_uniforms or grad_lens").c_str());

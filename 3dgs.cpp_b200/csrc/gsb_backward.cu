@@ -24,7 +24,7 @@
 //                         record and returns its scratch accumulators to zero for the next call.  The CAMERA instantiation
 //                         (gsb_render_backward_camera) also keeps the camera's share of that chain rule -- view matrix,
 //                         projection matrix, camera position, tan_fov -- summed per thread, then per CTA into one fp64 row.
-//                         For a lens frame, fisheye or OpenCV (gsb_render_backward_fisheye), the row holds the view matrix, the
+//                         For a lens frame, fisheye, OpenCV or orthographic (gsb_render_backward_fisheye), the row holds the view matrix, the
 //                         camera position and the lens's fx, fy, cx, cy, k[0..3] instead.
 //   k_camera_reduce       one CTA: sums those rows in a fixed order into the fp32 gsb_uniforms of gradients
 //                         (k_fisheye_camera_reduce: into gsb_uniforms and gsb_camera_model).
@@ -460,6 +460,10 @@ __host__ __device__ constexpr bool cam_word_live(int j) {
 // only those get a gradient (the rest of grad_vertices stays as the caller zeroed it) and only they reach the view direction;
 // at degree 0 the direction takes no part.  Each of ddx, ddy, ddz is the degree-3 sum cut after the last live band, so the
 // words equal the degree-3 words of the scene with the dropped bands zeroed (DESIGN.md section 25).
+// ORTHO (a frame of gsb_set_camera_model's orthographic camera): as OPENCV, through ortho_jacobian / ortho_grad and, with
+// CAMERA, ortho_lens_grad; J is constant, so dL/dt is J^T duv (plus dL/df on t.z: the depth key is z).  The SH view direction
+// is view row 2 normalised (ortho_direction), so the colour adds nothing to the position's gradient, and with CAMERA its share
+// goes to view row 2 instead of camera_position.
 struct BackwardFisheyeParams : BackwardParams {
     gsb_camera_model cam;
 };
@@ -472,7 +476,7 @@ using PbLensParams = std::conditional_t<DEPTH, PbDepthParams<std::conditional_t<
                                         std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>;
 template <bool FISHEYE, bool DEPTH = false, bool SHDEG = false>
 using PbParams = std::conditional_t<SHDEG, ShDegreeParams<PbLensParams<FISHEYE, DEPTH>>, PbLensParams<FISHEYE, DEPTH>>;
-// CAMERA on a lens frame (gsb_render_backward_fisheye, fisheye or OpenCV): only the live words are accumulated --
+// CAMERA on a lens frame (gsb_render_backward_fisheye, fisheye, OpenCV or orthographic): only the live words are accumulated --
 // camera_position.xyz, view_mat rows 0-2 and the lens's fx, fy, cx, cy, k[0..3] -- and each CTA writes one fp64 row of FC_WORDS
 // in this compact order for k_fisheye_camera_reduce: [FC_POS + k] camera_position[k], [FC_VIEW + c * 3 + k] V[k][c] (word
 // U_VIEW + c * 4 + k), [FC_LENS + j].
@@ -483,10 +487,11 @@ struct LensCamAcc {
 };
 template <>
 struct LensCamAcc<false> {};  // empty outside the lens camera instantiations, for the reason given at det_partials()
-template <bool CAMERA, bool AA, bool FISHEYE = false, bool DEPTH = false, bool OPENCV = false, bool SHDEG = false>
-__global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid_constant__ PbParams<FISHEYE || OPENCV, DEPTH, SHDEG> P) {
-    static_assert(!(FISHEYE && OPENCV), "one lens per frame");
-    constexpr bool LENS = FISHEYE || OPENCV;
+template <bool CAMERA, bool AA, bool FISHEYE = false, bool DEPTH = false, bool OPENCV = false, bool SHDEG = false, bool ORTHO = false>
+__global__ void __launch_bounds__(PB_THREADS)
+    k_preprocess_backward(const __grid_constant__ PbParams<FISHEYE || OPENCV || ORTHO, DEPTH, SHDEG> P) {
+    static_assert((int)FISHEYE + (int)OPENCV + (int)ORTHO <= 1, "one lens per frame");
+    constexpr bool LENS = FISHEYE || OPENCV || ORTHO;
     const uint32_t nv = P.ctl->num_visible;
     const gsb_uniforms& U = P.ubo;
     const float* pm = U.proj_mat;
@@ -543,6 +548,8 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
         } else if constexpr (OPENCV) {
             O = opencv_geo(P.cam, cv.vx, cv.vy, vz);
             FJ = opencv_jacobian(P.cam, vm, O, vz);
+        } else if constexpr (ORTHO) {
+            FJ = ortho_jacobian(P.cam, vm);
         }
         const auto& JW = [&]() -> const auto& {
             if constexpr (LENS) return FJ;
@@ -630,8 +637,11 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
                     fty += (cv.vy / F.d) * df;
                     ftz += (vz / F.d) * df;
                 }
-            } else {
+            } else if constexpr (OPENCV) {
                 opencv_grad(P.cam, O, vz, dJ, d[0], d[1], ftx, fty, ftz);
+                if constexpr (DEPTH) ftz += df;  // f = z
+            } else {
+                ortho_grad(P.cam, d[0], d[1], ftx, fty, ftz);
                 if constexpr (DEPTH) ftz += df;  // f = z
             }
 #pragma unroll
@@ -647,7 +657,8 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
                     for (int r = 0; r < 3; r++) fc.w[FC_VIEW + r * 3 + k] += dT0[r] * FJ.J[0][k] + dT1[r] * FJ.J[1][k];
                 }
                 if constexpr (FISHEYE) fisheye_lens_grad(P.cam, F, cv.vx, cv.vy, dJ, d[0], d[1], fc.w + FC_LENS);
-                else opencv_lens_grad(P.cam, O, vz, dJ, d[0], d[1], fc.w + FC_LENS);
+                else if constexpr (OPENCV) opencv_lens_grad(P.cam, O, vz, dJ, d[0], d[1], fc.w + FC_LENS);
+                else ortho_lens_grad(cv.vx, cv.vy, dJ, d[0], d[1], fc.w + FC_LENS);
             }
         }
 
@@ -666,7 +677,8 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
             x = y = z = ddx = ddy = ddz = 0.0f;
             len = 1.0f;
             if (deg >= 1) {
-                len = view_direction(U.camera_position, px, py, pz, x, y, z);
+                if constexpr (ORTHO) len = ortho_direction(vm, x, y, z);
+                else len = view_direction(U.camera_position, px, py, pz, x, y, z);
                 const float xx = x * x, yy = y * y, zz = z * z;
                 const int nk = deg >= 2 ? 9 : 4;
                 const float basis[9] = {SH_C0,
@@ -700,7 +712,8 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
                 }
             }
         } else {
-            len = view_direction(U.camera_position, px, py, pz, x, y, z);
+            if constexpr (ORTHO) len = ortho_direction(vm, x, y, z);
+            else len = view_direction(U.camera_position, px, py, pz, x, y, z);
             const float xx = x * x, yy = y * y, zz = z * z;
             const float basis[16] = {SH_C0,
                                      -SH_C1 * y,
@@ -742,11 +755,19 @@ __global__ void __launch_bounds__(PB_THREADS) k_preprocess_backward(const __grid
                               SH_C3_5 * (xx - yy) * vk[14];
         }
         const float dot = (x * ddx + y * ddy) + z * ddz;  // d (e / |e|) = (I - dir dir^T) / |e|
-        dp[0] += (ddx - x * dot) / len;
-        dp[1] += (ddy - y * dot) / len;
-        dp[2] += (ddz - z * dot) / len;
+        if constexpr (ORTHO) {  // e = view row 2 ([c * 4 + 2]): no share for the position or camera_position
+            if constexpr (CAMERA) {
+                fc.w[FC_VIEW + 0 * 3 + 2] += (ddx - x * dot) / len;
+                fc.w[FC_VIEW + 1 * 3 + 2] += (ddy - y * dot) / len;
+                fc.w[FC_VIEW + 2 * 3 + 2] += (ddz - z * dot) / len;
+            }
+        } else {
+            dp[0] += (ddx - x * dot) / len;
+            dp[1] += (ddy - y * dot) / len;
+            dp[2] += (ddz - z * dot) / len;
+        }
 
-        if constexpr (CAMERA && LENS) {  // the view direction p - camera_position (the view and lens words are above)
+        if constexpr (CAMERA && LENS && !ORTHO) {  // the view direction p - camera_position (the view and lens words are above)
             fc.w[FC_POS + 0] -= (ddx - x * dot) / len;
             fc.w[FC_POS + 1] -= (ddy - y * dot) / len;
             fc.w[FC_POS + 2] -= (ddz - z * dot) / len;
@@ -875,8 +896,8 @@ __global__ void __launch_bounds__(CR_THREADS) k_camera_reduce(const double* __re
     }
 }
 
-// The lens form of k_camera_reduce: sums the `rows` FC_WORDS-wide rows of k_preprocess_backward<true, AA, ...> on a fisheye or
-// OpenCV frame in the same fixed order and writes the whole gsb_uniforms (zero outside camera_position.xyz and view rows 0-2)
+// The lens form of k_camera_reduce: sums the `rows` FC_WORDS-wide rows of k_preprocess_backward<true, AA, ...> on a fisheye,
+// OpenCV or orthographic frame in the same fixed order and writes the whole gsb_uniforms (zero outside camera_position.xyz and view rows 0-2)
 // and the whole gsb_camera_model of gradients (kind and max_theta 0); either output may be null.
 __global__ void __launch_bounds__(CR_THREADS) k_fisheye_camera_reduce(const double* __restrict__ partials, uint32_t rows, gsb_uniforms* out,
                                                                       gsb_camera_model* lens) {
@@ -1051,23 +1072,26 @@ cudaError_t launch_preprocess_backward(const BackwardParams& p, bool antialiased
         if constexpr (SHDEG) return ShDegreeParams<std::decay_t<decltype(b)>>{b, sh_degree};
         else return b;
     };
-    if (lens) {  // fisheye or OpenCV: the same launches, one lens instantiation each
+    if (lens) {  // fisheye, OpenCV or orthographic: the same launches, one lens instantiation each
         const auto fp = with_extras(BackwardFisheyeParams{p, *lens});
-        auto launch = [&](auto opencv) {
-            constexpr bool OC = decltype(opencv)::value, FE = !OC;
+        auto launch = [&](auto kind) {
+            constexpr bool OC = decltype(kind)::value == GSB_CAMERA_OPENCV, OR = decltype(kind)::value == GSB_CAMERA_ORTHO;
+            constexpr bool FE = decltype(kind)::value == GSB_CAMERA_FISHEYE;
             if (!p.cam_partials) {  // vertex gradients only
-                if (antialiased) k_preprocess_backward<false, true, FE, DEPTH, OC, SHDEG><<<grid, PB_THREADS, 0, s>>>(fp);
-                else k_preprocess_backward<false, false, FE, DEPTH, OC, SHDEG><<<grid, PB_THREADS, 0, s>>>(fp);
+                if (antialiased) k_preprocess_backward<false, true, FE, DEPTH, OC, SHDEG, OR><<<grid, PB_THREADS, 0, s>>>(fp);
+                else k_preprocess_backward<false, false, FE, DEPTH, OC, SHDEG, OR><<<grid, PB_THREADS, 0, s>>>(fp);
                 return cudaGetLastError();
             }
-            if (antialiased) k_preprocess_backward<true, true, FE, DEPTH, OC, SHDEG><<<grid, PB_THREADS, 0, s>>>(fp);
-            else k_preprocess_backward<true, false, FE, DEPTH, OC, SHDEG><<<grid, PB_THREADS, 0, s>>>(fp);
+            if (antialiased) k_preprocess_backward<true, true, FE, DEPTH, OC, SHDEG, OR><<<grid, PB_THREADS, 0, s>>>(fp);
+            else k_preprocess_backward<true, false, FE, DEPTH, OC, SHDEG, OR><<<grid, PB_THREADS, 0, s>>>(fp);
             cudaError_t e = cudaGetLastError();
             if (e != cudaSuccess) return e;
             k_fisheye_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo, grad_lens);
             return cudaGetLastError();
         };
-        return lens->kind == GSB_CAMERA_OPENCV ? launch(std::true_type{}) : launch(std::false_type{});
+        if (lens->kind == GSB_CAMERA_OPENCV) return launch(std::integral_constant<int, GSB_CAMERA_OPENCV>{});
+        if (lens->kind == GSB_CAMERA_ORTHO) return launch(std::integral_constant<int, GSB_CAMERA_ORTHO>{});
+        return launch(std::integral_constant<int, GSB_CAMERA_FISHEYE>{});
     }
     const auto pp = with_extras(p);
     if (!p.grad_ubo) {

@@ -203,6 +203,14 @@ __global__ void __launch_bounds__(F3_THREADS) k_filter3d_lens(const float4* __re
                             keep_scale(lens_scale(opencv_jacobian(M, U.view_mat, O, cv.vz).J), s[j], seen[j]);
                     }
                 }
+            } else if (M.kind == GSB_CAMERA_ORTHO) {  // s = 1 / sigma_min(J) = 1 / min(fx, fy) at every depth
+                const float so = 1.0f / fminf(M.fx, M.fy);
+#pragma unroll
+                for (int j = 0; j < F3_ROWS; j++) {
+                    const ClipView cv = clip_view(U, px[j], py[j], pz[j]);
+                    const float u = M.fx * cv.vx + M.cx, v = M.fy * cv.vy + M.cy;
+                    if (cv.vz > 0.2f && u >= xlo && u <= xhi && v >= ylo && v <= yhi) keep_scale(so, s[j], seen[j]);  // NaN is culled
+                }
             } else {  // pinhole: k_filter3d_depth's test; s = vz / min(focal_x, focal_y), the focals as jacobian() has them
                 const float f = fminf(W / (2.0f * U.tan_fovx), H / (2.0f * U.tan_fovy));
 #pragma unroll

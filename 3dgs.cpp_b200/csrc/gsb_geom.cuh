@@ -278,6 +278,35 @@ __device__ __forceinline__ void opencv_lens_grad(const gsb_camera_model& M, cons
     dl[7] += (((6.0f * w.a) * xn + (2.0f * w.m) * yn) + (2.0f * w.c) * xn) / z + (Lu * (r2 + 2.0f * xx) + Lv * (2.0f * xy));
 }
 
+// The orthographic camera of gsb_set_camera_model (DESIGN.md section 26), for t = (x, y, z) in view space with z > 0.2:
+//   uv = (fx x + cx, fy y + cy),   J = d uv / d t = [fx, 0, 0; 0, fy, 0],   T = J W: T0 = fx (view row 0), T1 = fy (view row 1)
+// J is constant, so the backward has no second-derivative term: dL/dt = J^T duv (ortho_grad), plus dL/df on t.z for the
+// depth key f = z.
+__device__ __forceinline__ LensJ ortho_jacobian(const gsb_camera_model& M, const float* vm) {
+    LensJ j;
+    j.J[0][0] = M.fx, j.J[0][1] = 0.0f, j.J[0][2] = 0.0f;
+    j.J[1][0] = 0.0f, j.J[1][1] = M.fy, j.J[1][2] = 0.0f;
+#pragma unroll
+    for (int r = 0; r < 3; r++) {
+        j.T0[r] = M.fx * vm[r * 4 + 0];
+        j.T1[r] = M.fy * vm[r * 4 + 1];
+    }
+    return j;
+}
+__device__ __forceinline__ void ortho_grad(const gsb_camera_model& M, float du, float dv, float& dx, float& dy, float& dz) {
+    dx = M.fx * du;
+    dy = M.fy * dv;
+    dz = 0.0f;
+}
+// The lens's share (gsb_render_backward_fisheye on an orthographic frame): adds dL/d(fx, fy, cx, cy) of uv and J to dl:
+// d uv / d(fx, fy) = (x, 0), (0, y);  d uv / d(cx, cy) = I;  d J / d fx = J's row 0 / fx = (1, 0, 0), d J / d fy = (0, 1, 0).
+__device__ __forceinline__ void ortho_lens_grad(float x, float y, const float (&dJ)[2][3], float du, float dv, float* dl) {
+    dl[0] += du * x + dJ[0][0];
+    dl[1] += dv * y + dJ[1][1];
+    dl[2] += du;
+    dl[3] += dv;
+}
+
 // cov2d = transpose(T) Sigma T + 0.3 I (:56-65), Sigma = the cov3d words ca.xyzw, cb.xy; tm0 / tm1 = Sigma T0 / Sigma T1 (S[k] =
 // column k).  m01 and m10 round differently, so each caller states its own determinant.  c00 and c11 are the diagonal before
 // the dilation (the anti-aliased mode's opacity compensation reads them; m01 and m10 are not dilated).
@@ -351,6 +380,14 @@ __device__ __forceinline__ float view_direction(const float* cam, float px, floa
     const float len = sqrtf((dx * dx + dy * dy) + dz * dz);
     x = dx / len, y = dy / len, z = dz / len;
     return len;
+}
+
+// The SH view direction of an orthographic frame: every ray is parallel to the camera's forward axis, so the direction is
+// view row 2 normalised, the same for every Gaussian.  view_direction of the point (row 2) from the origin: p - 0 = p exactly,
+// so this is view_direction's fp32 normalisation of the row, and its gradient goes to the row (not to p or camera_position).
+__device__ __forceinline__ float ortho_direction(const float* vm, float& x, float& y, float& z) {
+    const float origin[3] = {0.0f, 0.0f, 0.0f};
+    return view_direction(origin, vm[2], vm[6], vm[10], x, y, z);
 }
 
 // One element of torch.optim.Adam (no weight decay): gsb_adam_step's and gsb_adam_step_features' update.

@@ -110,7 +110,8 @@ struct ShDegreeParams : Base {
 };
 
 // antialiased: gsb_set_antialiased's opacity compensation (not on the routed kernel of a sharded frame)
-// lens: gsb_set_camera_model's fisheye or OpenCV lens (k_project<..., FISHEYE> or <..., OPENCV>, plain contexts only); null =
+// lens: gsb_set_camera_model's fisheye, OpenCV or orthographic lens (k_project<..., FISHEYE>, <..., OPENCV> or <..., ORTHO>,
+// plain contexts only); null =
 // the pinhole camera.
 // sh_degree: gsb_set_sh_degree (plain contexts only); 3 launches the degree-3 kernels.
 cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* lens = nullptr,
@@ -231,7 +232,7 @@ struct DetBackward {
 // background: the frame's gsb_set_background, the colour behind every pixel's last contributor.  It is a kernel argument of
 // its own after BackwardParams, not a field of it: a larger BackwardParams would move the arguments that follow it in
 // k_det_reduce.
-// lens: the frame's gsb_set_camera_model lens (fisheye or OpenCV), null for a pinhole frame.  With p.cam_partials set, a lens
+// lens: the frame's gsb_set_camera_model lens (fisheye, OpenCV or orthographic), null for a pinhole frame.  With p.cam_partials set, a lens
 // frame's camera gradient (gsb_render_backward_fisheye): p.grad_ubo and grad_lens, either may be null; grad_lens needs a lens.
 // depth: gsb_render_backward_depth's upstream dL/d(D, A) and its per-survivor scratch (p.grad_image may then be null); null for
 // the colour-only entries.

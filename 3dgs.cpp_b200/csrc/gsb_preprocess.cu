@@ -231,6 +231,9 @@ __device__ __forceinline__ void compute_sh_degree(const float4* __restrict__ sh4
 // opencv_jacobian); the depth key stays z.  tan2_max is tan^2(max_theta), rounded to fp32 once on the host.
 // SHDEG (gsb_set_sh_degree below 3, plain contexts only): the colour is compute_sh_degree's at P.sh_degree; the argument is the
 // degree-3 kernel's with the degree appended (ShDegreeParams), and the launch bounds are the lens family's.
+// ORTHO (gsb_set_camera_model, plain contexts only): the orthographic camera (ortho_jacobian): uv = (fx x + cx, fy y + cy),
+// culled unless z > 0.2 (NaN culled), depth key z, and the SH colour seen along the camera's forward axis (ortho_direction)
+// rather than from camera_position.  It takes the fisheye's argument struct (the model alone) and the pinhole's launch bounds.
 struct ProjectFisheyeParams : ProjectParams {
     gsb_camera_model cam;
 };
@@ -238,10 +241,12 @@ struct ProjectOpencvParams : ProjectParams {
     gsb_camera_model cam;
     float tan2_max;
 };
-template <bool FISHEYE, bool OPENCV = false>
-using LensProjParams = std::conditional_t<FISHEYE, ProjectFisheyeParams, std::conditional_t<OPENCV, ProjectOpencvParams, ProjectParams>>;
-template <bool FISHEYE, bool OPENCV = false, bool SHDEG = false>
-using ProjParams = std::conditional_t<SHDEG, ShDegreeParams<LensProjParams<FISHEYE, OPENCV>>, LensProjParams<FISHEYE, OPENCV>>;
+template <bool FISHEYE, bool OPENCV = false, bool ORTHO = false>
+using LensProjParams =
+    std::conditional_t<FISHEYE || ORTHO, ProjectFisheyeParams, std::conditional_t<OPENCV, ProjectOpencvParams, ProjectParams>>;
+template <bool FISHEYE, bool OPENCV = false, bool SHDEG = false, bool ORTHO = false>
+using ProjParams =
+    std::conditional_t<SHDEG, ShDegreeParams<LensProjParams<FISHEYE, OPENCV, ORTHO>>, LensProjParams<FISHEYE, OPENCV, ORTHO>>;
 template <bool FISHEYE, bool OPENCV = false>
 struct ProjectBounds {
     static constexpr int MIN_BLOCKS = GSB_PROJECT_MIN_BLOCKS;
@@ -254,13 +259,14 @@ template <>
 struct ProjectBounds<false, true> {
     static constexpr int MIN_BLOCKS = GSB_PROJECT_OPENCV_MIN_BLOCKS;
 };
-template <bool DEBUG, bool ROUTED, bool SH16, bool AA, bool FISHEYE = false, bool OPENCV = false, bool SHDEG = false>
+template <bool DEBUG, bool ROUTED, bool SH16, bool AA, bool FISHEYE = false, bool OPENCV = false, bool SHDEG = false, bool ORTHO = false>
 __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE, OPENCV>::MIN_BLOCKS)
-    k_project(const __grid_constant__ ProjParams<FISHEYE, OPENCV, SHDEG> P) {
+    k_project(const __grid_constant__ ProjParams<FISHEYE, OPENCV, SHDEG, ORTHO> P) {
     static_assert(!(ROUTED && AA), "sharded contexts have no anti-aliased mode");
     static_assert(!(ROUTED && FISHEYE), "sharded contexts have no fisheye camera");
     static_assert(!(ROUTED && OPENCV) && !(FISHEYE && OPENCV), "sharded contexts have no OpenCV camera; one lens per frame");
     static_assert(!(ROUTED && SHDEG), "sharded contexts have only degree 3");
+    static_assert(!(ROUTED && ORTHO) && !((FISHEYE || OPENCV) && ORTHO), "sharded contexts have no orthographic camera; one lens per frame");
     __shared__ uint32_t s_chunk;
     __shared__ uint32_t s_wsurv[PRE_THREADS / 32];
     __shared__ uint32_t s_base_surv;
@@ -302,6 +308,8 @@ __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE, OPENCV>::M
         } else if constexpr (OPENCV) {
             O = opencv_geo(P.cam, cv.vx, cv.vy, vz);
             front = vz > 0.2f && O.r2 <= P.tan2_max && O.det > 0.0f;  // NaN is culled; so is a tangential fold
+        } else if constexpr (ORTHO) {
+            front = vz > 0.2f;  // NaN is culled
         } else {
             front = !(vz <= 0.2f);  // :135 (NaN is not culled by the shader's test either)
         }
@@ -312,6 +320,9 @@ __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE, OPENCV>::M
                 cov = cov2d(J.T0, J.T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
             } else if constexpr (OPENCV) {
                 const LensJ J = opencv_jacobian(P.cam, U.view_mat, O, vz);
+                cov = cov2d(J.T0, J.T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
+            } else if constexpr (ORTHO) {
+                const LensJ J = ortho_jacobian(P.cam, U.view_mat);
                 cov = cov2d(J.T0, J.T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
             } else {
                 const Jacobian J = jacobian(U, cv.vx, cv.vy, vz);
@@ -335,6 +346,9 @@ __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE, OPENCV>::M
                 } else if constexpr (OPENCV) {
                     uvx = P.cam.fx * O.xd + P.cam.cx;
                     uvy = P.cam.fy * O.yd + P.cam.cy;
+                } else if constexpr (ORTHO) {
+                    uvx = P.cam.fx * cv.vx + P.cam.cx;
+                    uvy = P.cam.fy * cv.vy + P.cam.cy;
                 } else {
                     uvx = ((ndcx + 1.0f) * (float)W - 1.0f) * 0.5f;  // :157 ndc2Pix
                     uvy = ((ndcy + 1.0f) * (float)H - 1.0f) * 0.5f;
@@ -439,7 +453,16 @@ __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE, OPENCV>::M
 
     // ---- SH colour of survivors (overlaps the look-back of other chunks) ----
     float colr = 0.f, colg = 0.f, colb = 0.f;
-    if constexpr (SHDEG) {
+    if constexpr (ORTHO) {  // the direction from the origin to view row 2: ortho_direction's, the same for every Gaussian
+        const float origin[3] = {0.0f, 0.0f, 0.0f};
+        const float fx = U.view_mat[2], fy = U.view_mat[6], fz = U.view_mat[10];
+        const float4* sh4 = reinterpret_cast<const float4*>(P.sh) + (size_t)i * (SH16 ? 6 : 12);
+        if constexpr (SHDEG) {
+            if (surv) compute_sh_degree<SH16>(sh4, fx, fy, fz, origin, P.sh_degree, colr, colg, colb);
+        } else {
+            if (surv) compute_sh<SH16>(sh4, fx, fy, fz, origin, colr, colg, colb);
+        }
+    } else if constexpr (SHDEG) {
         if (surv)
             compute_sh_degree<SH16>(reinterpret_cast<const float4*>(P.sh) + (size_t)i * (SH16 ? 6 : 12), px, py, pz, U.camera_position,
                                     P.sh_degree, colr, colg, colb);
@@ -918,31 +941,35 @@ __global__ void __launch_bounds__(PRE_THREADS) k_emit_coarse(const __grid_consta
 
 }  // namespace
 
-template <bool AA, bool FISHEYE, bool OPENCV, bool SHDEG>
-void launch_project_plain(const ProjParams<FISHEYE, OPENCV, SHDEG>& p, bool debug, unsigned blocks, cudaStream_t s) {
+template <bool AA, bool FISHEYE, bool OPENCV, bool SHDEG, bool ORTHO>
+void launch_project_plain(const ProjParams<FISHEYE, OPENCV, SHDEG, ORTHO>& p, bool debug, unsigned blocks, cudaStream_t s) {
     if (p.sh_half) {  // fp16 SH storage (non-parity)
-        if (debug) k_project<true, false, true, AA, FISHEYE, OPENCV, SHDEG><<<blocks, PRE_THREADS, 0, s>>>(p);
-        else k_project<false, false, true, AA, FISHEYE, OPENCV, SHDEG><<<blocks, PRE_THREADS, 0, s>>>(p);
-    } else if (debug) k_project<true, false, false, AA, FISHEYE, OPENCV, SHDEG><<<blocks, PRE_THREADS, 0, s>>>(p);
-    else k_project<false, false, false, AA, FISHEYE, OPENCV, SHDEG><<<blocks, PRE_THREADS, 0, s>>>(p);
+        if (debug) k_project<true, false, true, AA, FISHEYE, OPENCV, SHDEG, ORTHO><<<blocks, PRE_THREADS, 0, s>>>(p);
+        else k_project<false, false, true, AA, FISHEYE, OPENCV, SHDEG, ORTHO><<<blocks, PRE_THREADS, 0, s>>>(p);
+    } else if (debug) k_project<true, false, false, AA, FISHEYE, OPENCV, SHDEG, ORTHO><<<blocks, PRE_THREADS, 0, s>>>(p);
+    else k_project<false, false, false, AA, FISHEYE, OPENCV, SHDEG, ORTHO><<<blocks, PRE_THREADS, 0, s>>>(p);
 }
 
-template <bool FISHEYE, bool OPENCV, bool SHDEG>
-void launch_project_plain(const ProjParams<FISHEYE, OPENCV, SHDEG>& p, bool debug, bool antialiased, unsigned blocks, cudaStream_t s) {
-    if (antialiased) launch_project_plain<true, FISHEYE, OPENCV, SHDEG>(p, debug, blocks, s);
-    else launch_project_plain<false, FISHEYE, OPENCV, SHDEG>(p, debug, blocks, s);
+template <bool FISHEYE, bool OPENCV, bool SHDEG, bool ORTHO>
+void launch_project_plain(const ProjParams<FISHEYE, OPENCV, SHDEG, ORTHO>& p, bool debug, bool antialiased, unsigned blocks, cudaStream_t s) {
+    if (antialiased) launch_project_plain<true, FISHEYE, OPENCV, SHDEG, ORTHO>(p, debug, blocks, s);
+    else launch_project_plain<false, FISHEYE, OPENCV, SHDEG, ORTHO>(p, debug, blocks, s);
 }
 
 // degree 3: the degree-3 kernels; below: the SHDEG instantiations, with the degree appended to the argument
-template <bool FISHEYE, bool OPENCV = false>
-void launch_project_plain(const ProjParams<FISHEYE, OPENCV>& p, bool debug, bool antialiased, int sh_degree, unsigned blocks, cudaStream_t s) {
-    if (sh_degree < 3) launch_project_plain<FISHEYE, OPENCV, true>(ShDegreeParams<ProjParams<FISHEYE, OPENCV>>{p, sh_degree}, debug, antialiased, blocks, s);
-    else launch_project_plain<FISHEYE, OPENCV, false>(p, debug, antialiased, blocks, s);
+template <bool FISHEYE, bool OPENCV = false, bool ORTHO = false>
+void launch_project_plain(const ProjParams<FISHEYE, OPENCV, false, ORTHO>& p, bool debug, bool antialiased, int sh_degree, unsigned blocks,
+                          cudaStream_t s) {
+    if (sh_degree < 3)
+        launch_project_plain<FISHEYE, OPENCV, true, ORTHO>(ShDegreeParams<ProjParams<FISHEYE, OPENCV, false, ORTHO>>{p, sh_degree}, debug,
+                                                           antialiased, blocks, s);
+    else launch_project_plain<FISHEYE, OPENCV, false, ORTHO>(p, debug, antialiased, blocks, s);
 }
 
 cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* lens, int sh_degree) {
     const gsb_camera_model* fisheye = lens && lens->kind == GSB_CAMERA_FISHEYE ? lens : nullptr;
     const gsb_camera_model* opencv = lens && lens->kind == GSB_CAMERA_OPENCV ? lens : nullptr;
+    const gsb_camera_model* ortho = lens && lens->kind == GSB_CAMERA_ORTHO ? lens : nullptr;
     if (p.n == 0) return cudaSuccess;
     const unsigned blocks = (p.n + PRE_THREADS - 1) / PRE_THREADS;
     if (p.route_world > 0) {
@@ -954,6 +981,8 @@ cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased,
     } else if (opencv) {
         const double t = std::tan((double)opencv->max_theta);
         launch_project_plain<false, true>(ProjectOpencvParams{p, *opencv, (float)(t * t)}, debug, antialiased, sh_degree, blocks, s);
+    } else if (ortho) {
+        launch_project_plain<false, false, true>(ProjectFisheyeParams{p, *ortho}, debug, antialiased, sh_degree, blocks, s);
     } else {
         launch_project_plain<false>(p, debug, antialiased, sh_degree, blocks, s);
     }

@@ -31,7 +31,7 @@ ERR_INVALID, ERR_NO_DEVICE, ERR_CUDA, ERR_NO_SCENE, ERR_OOM, ERR_OVERFLOW = -1, 
 FORMAT_RGBA32F, FORMAT_RGBA8, FORMAT_BGRA8 = 0, 1, 2
 MODE_EXACT, MODE_FAST = 0, 1
 MEM_HOST, MEM_DEVICE = 0, 1
-CAMERA_PINHOLE, CAMERA_FISHEYE, CAMERA_OPENCV = 0, 1, 2
+CAMERA_PINHOLE, CAMERA_FISHEYE, CAMERA_OPENCV, CAMERA_ORTHO = 0, 1, 2, 3
 (BUF_COV3D, BUF_ATTR, BUF_TILES_OVERLAP, BUF_PREFIX_SUM, BUF_KEYS_UNSORTED, BUF_VALS_UNSORTED,
  BUF_KEYS_SORTED, BUF_VALS_SORTED, BUF_TILE_BOUNDARY, BUF_DEPTH_ORDER, BUF_EMIT_OFFSETS) = range(11)
 ALL_ROWS = 0xFFFFFFFF
@@ -49,7 +49,7 @@ EXPORTED_SYMBOLS = [  # every symbol include/gs_b200.h declares
     "gsb_render_depth", "gsb_render_backward_depth",
     # rendered feature maps with their gradients
     "gsb_render_features", "gsb_render_backward_features", "gsb_adam_step_features",
-    # camera and lens gradients through a lens (fisheye or OpenCV)
+    # camera and lens gradients through a lens (fisheye, OpenCV or orthographic)
     "gsb_render_backward_fisheye",
     # training loss, optimizer step and initialisation from a point cloud
     "gsb_image_loss", "gsb_adam_step", "gsb_init_from_points",
@@ -215,28 +215,36 @@ def camera_from_colmap(model: str, params) -> CameraModel:
     return opencv_from_colmap(f, f, cx, cy, k1, k2, 0.0, 0.0)
 
 
+def ortho_camera(fx, fy, cx, cy) -> CameraModel:
+    """An orthographic (parallel-projection) camera for Context.set_camera_model: fx, fy in pixels per world unit, cx, cy in
+    pixels, and with t = (x, y, z) the view-space position, uv = (fx x + cx, fy y + cy), culled unless z > 0.2; pixel (i, j)
+    is sampled at (i, j) (gsplat's principal point is (cx - 0.5, cy - 0.5) here).  The frame reads only the UBO's view matrix
+    and size; its depth is z, and the SH colour is seen along the camera's forward axis (view row 2) for every Gaussian."""
+    return CameraModel(CAMERA_ORTHO, float(fx), float(fy), float(cx), float(cy), (C.c_float * 4)(0.0, 0.0, 0.0, 0.0), 0.0)
+
+
 LENS_WORDS = 8  # (fx, fy, cx, cy, k[0..3]): lens_tensor's layout and gsb_render_backward_fisheye's grad_lens words 1-8
 
 
 def lens_tensor(cam: CameraModel, device=None):
-    """The (8,) float32 tensor (fx, fy, cx, cy, k[0..3]) of a fisheye or OpenCV CameraModel (k1..k4 for a fisheye, k1, k2, p1,
-    p2 for OpenCV), for render_torch(..., lens=): a lens a torch optimizer can refine.  lens_camera turns it back into the
-    same CameraModel, bit for bit."""
+    """The (8,) float32 tensor (fx, fy, cx, cy, k[0..3]) of a fisheye, OpenCV or orthographic CameraModel (k1..k4 for a
+    fisheye, k1, k2, p1, p2 for OpenCV, 0 for an orthographic camera), for render_torch(..., lens=): a lens a torch
+    optimizer can refine.  lens_camera turns it back into the same CameraModel, bit for bit."""
     import torch
 
     return torch.tensor(np.array([cam.fx, cam.fy, cam.cx, cam.cy, *cam.k], np.float32), device=device)
 
 
 def lens_camera(lens, max_theta, kind=CAMERA_FISHEYE) -> CameraModel:
-    """The CameraModel of kind `kind` (CAMERA_FISHEYE, the default, or CAMERA_OPENCV) of an (8,) lens tensor (lens_tensor's
-    layout) culled at max_theta (radians), bit for bit."""
+    """The CameraModel of kind `kind` (CAMERA_FISHEYE, the default, CAMERA_OPENCV or CAMERA_ORTHO) of an (8,) lens tensor
+    (lens_tensor's layout) culled at max_theta (radians; 0 for CAMERA_ORTHO, whose k words are 0 too), bit for bit."""
     import torch
 
     w = lens.detach().to("cpu", torch.float32).reshape(-1).numpy() if isinstance(lens, torch.Tensor) else np.asarray(lens, np.float32)
     if w.shape != (LENS_WORDS,):
         raise ValueError(f"lens_camera: the lens must hold {LENS_WORDS} values (fx, fy, cx, cy, k[0..3])")
-    if kind not in (CAMERA_FISHEYE, CAMERA_OPENCV):
-        raise ValueError("lens_camera: kind must be CAMERA_FISHEYE or CAMERA_OPENCV")
+    if kind not in (CAMERA_FISHEYE, CAMERA_OPENCV, CAMERA_ORTHO):
+        raise ValueError("lens_camera: kind must be CAMERA_FISHEYE, CAMERA_OPENCV or CAMERA_ORTHO")
     return CameraModel(kind, *(float(x) for x in w[:4]), (C.c_float * 4)(*(float(x) for x in w[4:])), float(max_theta))
 
 
@@ -639,9 +647,9 @@ class Context:
 
     def set_camera_model(self, cam=None):
         """gsb_set_camera_model: from the next frame, project through the lens `cam` (a CameraModel from fisheye_camera,
-        fisheye_from_colmap, opencv_camera, opencv_from_colmap or camera_from_colmap; None or kind CAMERA_PINHOLE = the UBO's
-        pinhole camera, the default).  A lens frame (fisheye or OpenCV) reads only the UBO's view matrix, camera position and
-        size.  Frames, render_torch, SceneAdam and the backward pass follow it (the backward uses the model of the frame it
+        fisheye_from_colmap, opencv_camera, opencv_from_colmap, camera_from_colmap or ortho_camera; None or kind CAMERA_PINHOLE = the UBO's
+        pinhole camera, the default).  A lens frame (fisheye, OpenCV or orthographic) reads only the UBO's view matrix, camera
+        position and size (an orthographic frame not even the camera position).  Frames, render_torch, SceneAdam and the backward pass follow it (the backward uses the model of the frame it
         differentiates).  The camera and lens gradients of a lens frame come from gsb_render_backward_fisheye
         (Context._backward_fisheye, render_torch(..., lens=), SceneAdam.step)."""
         self._ck(lib.gsb_set_camera_model(self.h, None if cam is None else C.byref(cam)))
@@ -823,7 +831,7 @@ class Context:
                           density_ptr=None, grad_depth_alpha_ptr=None, features=None, grad_feature_map=None, grad_features_ptr=None,
                           row_pitch_bytes=0):
         """gsb_render_backward_fisheye on device pointers, `stream` the C ABI's cudaStream_t: _backward's arguments plus the
-        camera gradient of the last (fisheye or OpenCV) frame, grad_uniforms_ptr (160 B, dL/d gsb_uniforms, pose words only) and
+        camera gradient of the last (fisheye, OpenCV or orthographic) frame, grad_uniforms_ptr (160 B, dL/d gsb_uniforms, pose words only) and
         grad_lens_ptr (40 B, a gsb_camera_model of dL/d(fx, fy, cx, cy, k)), each overwritten and each may be None."""
         fptr, fch, gfm, fpitch = (None, 0, None, 0) if features is None else (
             features.data_ptr(), features.shape[1], grad_feature_map.data_ptr(), grad_feature_map.stride()[0] * 4)
@@ -1319,8 +1327,8 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, 
     off): every gradient and density statistic is then bit-identical for the same inputs, at some cost in time.  With
     torch's default settings backward takes the atomic path, whose results may differ in the last bit from run to run.
 
-    The frame is projected through the context's camera model (Context.set_camera_model); ubo= on a fisheye or OpenCV
-    context raises ValueError unless lens= is given.
+    The frame is projected through the context's camera model (Context.set_camera_model); ubo= on a fisheye, OpenCV or
+    orthographic context raises ValueError unless lens= is given.
 
     lens (optional): an (8,) tensor (fx, fy, cx, cy, k[0..3]) (lens_tensor makes one).  The frame is rendered through
     lens_camera(lens, max_theta, kind), kind and max_theta those of the context's lens model if one is set (k1, k2, p1, p2
@@ -1331,7 +1339,7 @@ def render_torch(ctx: "Context", vertices, u: Uniforms, ubo=None, density=None, 
     without lens=.  It composes with depth=, features=, density=, background= and the deterministic mode.
 
     depth=True renders with gsb_render_depth and returns (img, depth_alpha), depth_alpha an (H, W, 2) tensor of (D, A):
-    D = sum f alpha T, f the view-space z (the distance from the camera for a fisheye model, z for OpenCV), and A = 1 - T_final, the
+    D = sum f alpha T, f the view-space z (the distance from the camera for a fisheye model, z for OpenCV and orthographic), and A = 1 - T_final, the
     accumulated opacity.  Backward then takes dL/dimg and dL/d(depth_alpha), either of them unused (zero), through
     gsb_render_backward_depth; it composes with ubo=, density=, background= and the deterministic mode.  Expected depth is
     D / A.clamp_min(1e-10), inverse depth its reciprocal, and a mask loss reads A directly.
@@ -1796,7 +1804,7 @@ class SceneAdam:
         grad_uniforms, grad_lens: optional (40,) and (8,) float32 CUDA tensors, overwritten by the same backward pass with
         dL/d(the frame's gsb_uniforms, all 40 words) and dL/d(fx, fy, cx, cy, k[0..3]) of the frame's lens (k1..k4 for a
         fisheye, k1, k2, p1, p2 for OpenCV).  A pinhole frame fills grad_uniforms through gsb_render_backward_camera's words
-        (grad_lens: ValueError); a fisheye or OpenCV frame fills both through gsb_render_backward_fisheye (pose words only).  `grad`, the features and the step are the same as without them.
+        (grad_lens: ValueError); a fisheye, OpenCV or orthographic frame fills both through gsb_render_backward_fisheye (pose words only).  `grad`, the features and the step are the same as without them.
         Joint pose refinement, with per-view poses (and a lens tensor) in a torch optimizer:
 
             gu = torch.empty(40, device="cuda")
@@ -1836,7 +1844,7 @@ class SceneAdam:
         gu = None if grad_uniforms is None else grad_uniforms.data_ptr()
         if ctx.camera is None:
             if grad_lens is not None:
-                raise ValueError("SceneAdam.step: grad_lens needs a fisheye or OpenCV frame (Context.set_camera_model)")
+                raise ValueError("SceneAdam.step: grad_lens needs a fisheye, OpenCV or orthographic frame (Context.set_camera_model)")
             ctx._backward(v.data_ptr(), None if g is None else g.data_ptr(), self.grad.data_ptr(), stream, grad_uniforms_ptr=gu,
                           **common)
         elif grad_uniforms is None and grad_lens is None:

@@ -217,22 +217,31 @@ int gsb_set_background(gsb_ctx *ctx, const float *rgb);
  *   xd = xn R + 2 p1 xn yn + p2 (r^2 + 2 xn^2),  yd = yn R + p1 (r^2 + 2 yn^2) + 2 p2 xn yn,  uv = (fx xd + cx, fy yd + cy);
  *   culled unless z > 0.2, r^2 <= tan^2(max_theta) (rounded to fp32 once) and det d(xd, yd) / d(xn, yn) > 0 (NaN culled);
  *   cov2d = J W Sigma W^T J^T + 0.3 I with J = d uv / d t exact (no tan_fov clamp);  depth key z, as for a pinhole frame.
- * The frame records the model; every backward entry follows the frame's.  For a fisheye or OpenCV frame (a lens frame)
+ * ORTHO is the orthographic (parallel-projection) camera: fx and fy are pixels per world unit, cx and cy pixels.  It reads
+ * only view_mat, width and height of the UBO (never camera_position, proj_mat or tan_fov), and with t = (x, y, z):
+ *   uv = (fx x + cx, fy y + cy);  culled unless z > 0.2 (NaN culled);  cov2d = J W Sigma W^T J^T + 0.3 I with
+ *   J = [fx, 0, 0; 0, fy, 0];  depth key z (gsb_render_depth's D is z: the distance from the camera plane);
+ *   SH view direction normalize(view_mat[2], view_mat[6], view_mat[10]), the camera's forward axis, the same for every
+ *   Gaussian (gsplat's "ortho" keeps p - camera_position instead; DESIGN.md section 26).
+ * The frame records the model; every backward entry follows the frame's.  For a fisheye, OpenCV or orthographic frame (a lens frame)
  * gsb_render_backward_camera, _density, _depth and _features with a non-NULL grad_uniforms return GSB_ERR_INVALID: the
  * camera gradient of a lens frame is gsb_render_backward_fisheye's.  m NULL or kind PINHOLE: the default.  GSB_ERR_INVALID,
  * the setting unchanged, for a NULL ctx, a sharded context or gsb_group rank, an unknown kind, fx or fy not positive and
  * finite, any other field not finite, and (checked on the host in double)
  *   FISHEYE: max_theta outside (0, pi), or d theta_d / d theta <= 0 anywhere on [0, max_theta];
  *   OPENCV:  max_theta outside (0, pi / 2), or r R(r^2) not strictly increasing on [0, tan max_theta], i.e.
- *            1 + 3 k1 u + 5 k2 u^2 <= 0 somewhere on u in [0, tan^2 max_theta].
+ *            1 + 3 k1 u + 5 k2 u^2 <= 0 somewhere on u in [0, tan^2 max_theta];
+ *   ORTHO:   any k[i] != 0 or max_theta != 0 (the unused words must be zero).
  * Takes effect at the next frame; changing it drops no captured graph. */
-typedef enum gsb_camera_kind { GSB_CAMERA_PINHOLE = 0, GSB_CAMERA_FISHEYE = 1, GSB_CAMERA_OPENCV = 2 } gsb_camera_kind;
+typedef enum gsb_camera_kind { GSB_CAMERA_PINHOLE = 0, GSB_CAMERA_FISHEYE = 1, GSB_CAMERA_OPENCV = 2, GSB_CAMERA_ORTHO = 3 } gsb_camera_kind;
 typedef struct gsb_camera_model {
     uint32_t kind;        /* gsb_camera_kind */
-    float fx, fy, cx, cy; /* pixels; pixel (i, j) is sampled at (i, j), as the blend does (COLMAP's cx - 0.5) */
+    float fx, fy, cx, cy; /* pixels (ORTHO: fx, fy in pixels per world unit); pixel (i, j) is sampled at (i, j), as the blend
+                             does (COLMAP's cx - 0.5) */
     float k[4];           /* FISHEYE, Kannala-Brandt: theta_d = theta (1 + k1 t^2 + k2 t^4 + k3 t^6 + k4 t^8), t = theta;
-                             OPENCV: (k1, k2, p1, p2) in COLMAP's OPENCV order */
-    float max_theta;      /* radians, in (0, pi) (FISHEYE) or (0, pi / 2) (OPENCV): rays farther off the axis are culled */
+                             OPENCV: (k1, k2, p1, p2) in COLMAP's OPENCV order;  ORTHO: 0 */
+    float max_theta;      /* radians, in (0, pi) (FISHEYE) or (0, pi / 2) (OPENCV): rays farther off the axis are culled;
+                             ORTHO: 0 */
 } gsb_camera_model;
 int gsb_set_camera_model(gsb_ctx *ctx, const gsb_camera_model *m);
 /* per-stage cudaEvent timers (the QueryManager analogue, Renderer.cpp:85-100). Default on. */
@@ -410,8 +419,8 @@ int gsb_render_backward_features(gsb_ctx *ctx, const float *vertices, const floa
                                  const float *grad_feature_map, size_t feature_pitch_bytes, float *grad_vertices,
                                  gsb_uniforms *grad_uniforms, float *grad_features, float *density, void *stream);
 
-/* The camera gradient of a lens frame (fisheye or OpenCV, gsb_set_camera_model): pose refinement and lens self-calibration
- * through the lens.
+/* The camera gradient of a lens frame (fisheye, OpenCV or orthographic, gsb_set_camera_model): pose refinement and lens
+ * self-calibration through the lens.
  * The arguments, preconditions and error codes of gsb_render_backward_features, except that
  *   features, channels, grad_feature_map, grad_features
  *                      features == NULL with channels == 0 means no feature map; grad_feature_map and grad_features must then
@@ -420,9 +429,11 @@ int gsb_render_backward_features(gsb_ctx *ctx, const float *vertices, const floa
  *                      camera_position[0..2] (the SH view direction) and view_mat rows 0-2 ([c*4 + r], r != 3): through the
  *                      view-space position t = V (p, 1) and through the view rotation W inside the EWA term J W.  Every other
  *                      word -- proj_mat, tan_fovx, tan_fovy, view_mat row 3, camera_position[3], width, height -- is 0: a
- *                      lens frame does not read them.
+ *                      lens frame does not read them.  An orthographic frame reads no camera_position either: its
+ *                      camera_position[0..2] words are 0, and its SH view direction's share goes to view_mat row 2.
  *   grad_lens          device memory or NULL, OVERWRITTEN with dL/d(fx, fy, cx, cy, k[0..3]) of the frame's lens (k in the
- *                      model's own order: k1..k4 for a fisheye, k1, k2, p1, p2 for OpenCV), through uv and through the
+ *                      model's own order: k1..k4 for a fisheye, k1, k2, p1, p2 for OpenCV, 0 for an orthographic camera,
+ *                      which has no k), through uv and through the
  *                      Jacobian J of the EWA term; kind and max_theta are written 0 (max_theta, the culls,
  *                      radii and tile AABBs are step functions of the lens).
  *   grad_vertices, grad_uniforms, grad_lens, grad_features
@@ -430,7 +441,7 @@ int gsb_render_backward_features(gsb_ctx *ctx, const float *vertices, const floa
  *                      grad_lens
  * and GSB_ERR_INVALID also when the last frame is a pinhole frame (its camera gradient is gsb_render_backward_camera's).
  * grad_vertices, grad_features and density receive the words the other backward entries give for the same frame and upstream
- * gradients.  The depth term (f = |t| for a fisheye, z for OpenCV) and the feature map's alpha terms reach the camera and lens
+ * gradients.  The depth term (f = |t| for a fisheye, z for OpenCV and orthographic) and the feature map's alpha terms reach the camera and lens
  * words in the same pass.
  * The camera words are reduced without global atomics, per CTA in fp64 then in one fixed-order pass; under
  * gsb_set_backward_deterministic they are reproducible bit for bit, as the other outputs.  gsb_render_backward_camera,
@@ -566,9 +577,9 @@ int gsb_filter3d_variance(gsb_ctx *ctx, const float *vertices, uint64_t n, const
  * projects it.  Per Gaussian i and camera c, in fp32 with t = (x, y, z) from clip_view's view rows:
  *   seen iff the frame's cull for the kind keeps i and its uv lies in -0.15f W <= u <= 1.15f W, -0.15f H <= v <= 1.15f H
  *   (PINHOLE: gsb_filter3d_variance's test; FISHEYE: d > 0.2, theta <= max_theta; OPENCV: z > 0.2,
- *   r^2 <= tan^2(max_theta) rounded to fp32 once, det D > 0; NaN is never seen);
- *   s_ic = 1 / sigma_min(J), J = d uv / d t of the frame's Jacobian (lens kinds), or vz / min(focal_x, focal_y) with the
- *   UBO's focals (PINHOLE); a camera whose s_ic is not positive and finite does not count as seeing i.
+ *   r^2 <= tan^2(max_theta) rounded to fp32 once, det D > 0; ORTHO: z > 0.2; NaN is never seen);
+ *   s_ic = 1 / sigma_min(J), J = d uv / d t of the frame's Jacobian (FISHEYE, OPENCV), 1.0f / min(fx, fy) (ORTHO: the
+ *   same 1 / sigma_min, independent of depth), or vz / min(focal_x, focal_y) with the UBO's focals (PINHOLE); a camera whose s_ic is not positive and finite does not count as seeing i.
  * s_i = the least s_ic over the cameras that see i; rows no camera sees take the largest s_i of the seen rows; variance_i =
  * (s_i s_i) 0.2f; all zero if no row is seen.  Bitwise reproducible, on any stream, context or grid and in any camera order.
  * All-PINHOLE cameras sharing one focal_x == focal_y give gsb_filter3d_variance's words.  A lens camera's proj_mat and
