@@ -341,7 +341,7 @@ int plan_frame(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uint32_t re, 
     return GSB_OK;
 }
 
-// k_project's arguments over the context's scene, band-clipped to tile rows [rb, re) (a sharded frame adds the route fields)
+// k_project's arguments over the context's scene and settings, band-clipped to tile rows [rb, re) (a sharded frame adds the route fields)
 ProjectParams project_params(const gsb_ctx* ctx, const gsb_uniforms& ubo, uint32_t rb, uint32_t re) {
     ProjectParams pp{};
     pp.pos_op = ctx->pos_op;
@@ -360,6 +360,9 @@ ProjectParams project_params(const gsb_ctx* ctx, const gsb_uniforms& ubo, uint32
     pp.ctl = ctx->ctl;
     pp.dbg_tiles = ctx->dbg_tiles;
     pp.dbg_aabb = ctx->dbg_aabb;
+    pp.camera = ctx->camera;
+    pp.sh_degree = ctx->sh_degree;
+    pp.antialiased = ctx->antialiased ? 1 : 0;
     return pp;
 }
 
@@ -375,8 +378,7 @@ static int enqueue_front(gsb_ctx* ctx, const gsb_uniforms* ubo, uint32_t rb, uin
     if (timers) CK(cudaEventRecord(ctx->ev[0], stream));
 
     // ---- k_project: preprocess.comp + survivor compaction ----
-    const bool lens = ctx->camera.kind != GSB_CAMERA_PINHOLE;
-    CK(launch_project(project_params(ctx, *ubo, rb, re), ctx->debug, ctx->antialiased, stream, lens ? &ctx->camera : nullptr, ctx->sh_degree));
+    CK(launch_project(project_params(ctx, *ubo, rb, re), ctx->debug, stream));
     if (timers) CK(cudaEventRecord(ctx->ev[1], stream));
 
     if (ctx->use_graph && !timers && !ctx->debug) rc = launch_middle_graph(ctx, fp, sv, stream);
@@ -1227,9 +1229,15 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     bp.grad_ubo = grad_ubo;
     bp.abs_scratch = density ? ctx->bw_abs.p : nullptr;
     bp.density = density;
-    const float3 bg = make_float3(f.background[0], f.background[1], f.background[2]);  // the frame's, not the current setting
-    const DepthBackward depth{reinterpret_cast<const float2*>(grad_depth), depth_pitch, ctx->bw_depth.p};
-    const DepthBackward* dp = grad_depth ? &depth : nullptr;
+    // the recorded frame's settings, not the current ones
+    for (int c = 0; c < 3; c++) bp.background[c] = f.background[c];
+    bp.grad_depth = reinterpret_cast<const float2*>(grad_depth);
+    bp.depth_pitch = depth_pitch;
+    bp.depth_scratch = grad_depth ? ctx->bw_depth.p : nullptr;
+    bp.camera = f.camera;
+    bp.grad_lens = grad_lens;
+    bp.sh_degree = f.sh_degree;
+    bp.antialiased = f.antialiased ? 1 : 0;
     FeatureParams fp{};
     if (feat) {
         fp = feature_frame_params(ctx, feat->features, feat->channels);
@@ -1240,7 +1248,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     }
     const FeatureParams* fpp = feat ? &fp : nullptr;
     if (!det) {
-        CK(launch_backward(bp, f.antialiased, bg, s, nullptr, lens_frame ? &f.camera : nullptr, dp, fpp, grad_lens, f.sh_degree));
+        CK(launch_backward(bp, nullptr, fpp, s));
         return GSB_OK;
     }
     const DetBuffers& d = ctx->bw_det;
@@ -1256,7 +1264,7 @@ static int render_backward(gsb_ctx* ctx, const char* fn, bool args_ok, const flo
     db.status_tiles = (uint32_t)(d.status.count / 256);
     db.m_hint = quantise_hint(ctx->m_hint);
     db.key_bits = std::max<uint32_t>(bits_for((uint32_t)n), 1u);  // compact ids < N_v <= n
-    CK(launch_backward(bp, f.antialiased, bg, s, &db, lens_frame ? &f.camera : nullptr, dp, fpp, grad_lens, f.sh_degree));
+    CK(launch_backward(bp, &db, fpp, s));
     return GSB_OK;
 }
 

@@ -40,7 +40,6 @@
 //                         k_density_accumulate and k_preprocess_backward read.  Every output is then order-fixed.
 // Compiled with -fmad=false like the forward.
 #include <algorithm>
-#include <type_traits>
 
 #include "gsb_cull.cuh"
 #include "gsb_exp.cuh"
@@ -81,34 +80,11 @@ __device__ __forceinline__ float* det_partials() {
     return s_dyn;
 }
 
-// BG (a frame of gsb_set_background): the colour behind every pixel's last contributor is P.bg instead of 0.  Only the BG
-// instantiations take the larger argument: the others keep BackwardParams as it was, and with it their code.
-struct BackwardBgParams : BackwardParams {
-    float3 bg;
-};
-// DEPTH (gsb_render_backward_depth): the upstream gradient also has dL/dD and dL/dA per pixel (grad_depth, H x W float2,
-// depth_pitch apart), grad_image may be null (no colour gradient), and each survivor's dL/df (f its record's depth) is reduced
-// like the other accumulators into depth_scratch (n x 1 fp64, zero on entry, returned to zero by k_preprocess_backward): one
-// more shared-memory and det-slot column, after the ABSGRAD ones.  Only these instantiations take the larger argument.
-template <typename Base>
-struct BackwardDepthParams : Base {
-    const float2* grad_depth;
-    size_t depth_pitch;
-    double* depth_scratch;
-};
-template <bool BG, bool DEPTH = false>
-using BwParams = std::conditional_t<DEPTH, BackwardDepthParams<std::conditional_t<BG, BackwardBgParams, BackwardParams>>,
-                                    std::conditional_t<BG, BackwardBgParams, BackwardParams>>;
-template <bool BG>
-BwParams<BG> bw_params(const BackwardParams& p, float3 bg) {
-    if constexpr (BG) return BackwardBgParams{p, bg};
-    else return p;
-}
-template <bool BG, bool DEPTH>
-BwParams<BG, DEPTH> bw_params(const BackwardParams& p, float3 bg, const DepthBackward* dp) {
-    if constexpr (DEPTH) return BwParams<BG, true>{bw_params<BG>(p, bg), dp->grad, dp->pitch, dp->scratch};
-    else return bw_params<BG>(p, bg);
-}
+// BG (a frame of gsb_set_background): the colour behind every pixel's last contributor is P.background instead of 0.
+// DEPTH (gsb_render_backward_depth): the upstream gradient also has dL/dD and dL/dA per pixel (P.grad_depth), grad_image may
+// be null (no colour gradient), and each survivor's dL/df (f its record's depth) is reduced like the other accumulators into
+// P.depth_scratch (returned to zero by k_preprocess_backward): one more shared-memory and det-slot column, after the ABSGRAD
+// ones.
 template <bool ABSGRAD, bool DEPTH>
 constexpr int bw_nacc = BW_NACC + (ABSGRAD ? BW_NABS : 0) + (DEPTH ? 1 : 0);
 // DEPTH: the pixel's dL/dD and dL/dA, the depth and alpha behind the current entry (0 behind the last contributor, also over
@@ -121,7 +97,7 @@ template <>
 struct DepthWalk<false> {};
 
 template <int MODE, bool ABSGRAD, bool DET = false, bool BG = false, bool DEPTH = false>
-__global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_constant__ BwParams<BG, DEPTH> P) {
+__global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_constant__ BackwardParams P) {
     constexpr int NACC = BW_NACC + (ABSGRAD ? BW_NABS : 0) + (DEPTH ? 1 : 0);  // shared-memory columns: the extras in ABSGRAD / DEPTH only
     constexpr int DCOL = BW_NACC + (ABSGRAD ? BW_NABS : 0);                       // DEPTH: the column of dL/df
     __shared__ BwRec s_rec[bw_batch<DET>];
@@ -174,9 +150,9 @@ __global__ void __launch_bounds__(BW_THREADS) k_blend_backward(const __grid_cons
 
     float acc_r = 0.f, acc_g = 0.f, acc_b = 0.f;  // colour behind the current entry, per unit of its transmittance
     if constexpr (BG) {  // the background is behind every pixel's last contributor
-        acc_r = P.bg.x;
-        acc_g = P.bg.y;
-        acc_b = P.bg.z;
+        acc_r = P.background[0];
+        acc_g = P.background[1];
+        acc_b = P.background[2];
     }
     for (uint32_t hi = max_last; hi > 0;) {
         const uint32_t lo = hi > bw_batch<DET> ? hi - bw_batch<DET> : 0u;
@@ -384,10 +360,10 @@ __global__ void __launch_bounds__(PB_THREADS) k_det_prepare(const uint32_t* __re
 // P.scratch (and P.abs_scratch), where k_density_accumulate and k_preprocess_backward read them as they read the atomic sums.
 // The sum is sequential so that an entry whose slot is +0 changes nothing: tile-cull level 1's list is level 0's with such
 // entries removed, and both give the same bits.  Loads run UNROLL entries ahead of the adds.
-// DEPTH: the slots have one more column, dL/df, stored into depth_scratch.
+// DEPTH: the slots have one more column, dL/df, stored into P.depth_scratch.
 template <bool ABSGRAD, bool DEPTH = false>
 __global__ void __launch_bounds__(PB_THREADS) k_det_reduce(const __grid_constant__ BackwardParams P, const uint32_t* __restrict__ pos,
-                                                           const uint2* __restrict__ runs, double* __restrict__ depth_scratch) {
+                                                           const uint2* __restrict__ runs) {
     constexpr int NACC = bw_nacc<ABSGRAD, DEPTH>;
     constexpr uint32_t UNROLL = 4;
     const uint32_t nv = P.ctl->num_visible;
@@ -427,7 +403,7 @@ __global__ void __launch_bounds__(PB_THREADS) k_det_reduce(const __grid_constant
 #pragma unroll
             for (int k = 0; k < BW_NABS; k++) ab[k] = s[BW_NACC + k];
         }
-        if constexpr (DEPTH) depth_scratch[cid] = s[NACC - 1];
+        if constexpr (DEPTH) P.depth_scratch[cid] = s[NACC - 1];
     }
 }
 
@@ -447,15 +423,14 @@ __host__ __device__ constexpr bool cam_word_live(int j) {
 // FISHEYE (a frame of gsb_set_camera_model's fisheye): J and uv are the lens's (fisheye_geo,
 // fisheye_jacobian), dL/d(J W) goes to J through the view rotation and on to the view-space position through J's second
 // derivatives (fisheye_grad), and that position to the Gaussian's through the view rotation; the projection matrix takes no
-// part.  Only these instantiations take the larger argument, so the others keep their code.  With CAMERA as well
+// part.  With CAMERA as well
 // (gsb_render_backward_fisheye) the camera's share is dL/dt through t = V (p, 1), dL/d(J W) through W, the view direction and
 // the lens (fisheye_lens_grad), reduced by k_fisheye_camera_reduce.
 // DEPTH (gsb_render_backward_depth): the survivor's dL/df (depth_scratch, returned to zero here) goes to the position through
 // the forward's own f: the view-space z of clip_view for a pinhole frame (dL/dv.z += dL/df, and with it dL/d(view row 2) in
 // the CAMERA instantiation), the distance d = |t| of fisheye_geo for a fisheye frame (dL/dt += (t / d) dL/df).
 // OPENCV (a frame of gsb_set_camera_model's OpenCV lens): as FISHEYE, through opencv_geo / opencv_jacobian / opencv_grad and,
-// with CAMERA, opencv_lens_grad.  It takes the fisheye's argument struct (the lens alone; the cull bound is not needed here).
-// Its depth key is z, so DEPTH adds dL/df to dL/dt.z.
+// with CAMERA, opencv_lens_grad.  Its depth key is z, so DEPTH adds dL/df to dL/dt.z.
 // SHDEG (a frame of gsb_set_sh_degree below 3): the colour is the sum over the coefficients of bands <= P.sh_degree only, so
 // only those get a gradient (the rest of grad_vertices stays as the caller zeroed it) and only they reach the view direction;
 // at degree 0 the direction takes no part.  Each of ddx, ddy, ddz is the degree-3 sum cut after the last live band, so the
@@ -464,18 +439,6 @@ __host__ __device__ constexpr bool cam_word_live(int j) {
 // CAMERA, ortho_lens_grad; J is constant, so dL/dt is J^T duv (plus dL/df on t.z: the depth key is z).  The SH view direction
 // is view row 2 normalised (ortho_direction), so the colour adds nothing to the position's gradient, and with CAMERA its share
 // goes to view row 2 instead of camera_position.
-struct BackwardFisheyeParams : BackwardParams {
-    gsb_camera_model cam;
-};
-template <typename Base>
-struct PbDepthParams : Base {
-    double* depth_scratch;
-};
-template <bool FISHEYE, bool DEPTH = false>
-using PbLensParams = std::conditional_t<DEPTH, PbDepthParams<std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>,
-                                        std::conditional_t<FISHEYE, BackwardFisheyeParams, BackwardParams>>;
-template <bool FISHEYE, bool DEPTH = false, bool SHDEG = false>
-using PbParams = std::conditional_t<SHDEG, ShDegreeParams<PbLensParams<FISHEYE, DEPTH>>, PbLensParams<FISHEYE, DEPTH>>;
 // CAMERA on a lens frame (gsb_render_backward_fisheye, fisheye, OpenCV or orthographic): only the live words are accumulated --
 // camera_position.xyz, view_mat rows 0-2 and the lens's fx, fy, cx, cy, k[0..3] -- and each CTA writes one fp64 row of FC_WORDS
 // in this compact order for k_fisheye_camera_reduce: [FC_POS + k] camera_position[k], [FC_VIEW + c * 3 + k] V[k][c] (word
@@ -489,7 +452,7 @@ template <>
 struct LensCamAcc<false> {};  // empty outside the lens camera instantiations, for the reason given at det_partials()
 template <bool CAMERA, bool AA, bool FISHEYE = false, bool DEPTH = false, bool OPENCV = false, bool SHDEG = false, bool ORTHO = false>
 __global__ void __launch_bounds__(PB_THREADS)
-    k_preprocess_backward(const __grid_constant__ PbParams<FISHEYE || OPENCV || ORTHO, DEPTH, SHDEG> P) {
+    k_preprocess_backward(const __grid_constant__ BackwardParams P) {
     static_assert((int)FISHEYE + (int)OPENCV + (int)ORTHO <= 1, "one lens per frame");
     constexpr bool LENS = FISHEYE || OPENCV || ORTHO;
     const uint32_t nv = P.ctl->num_visible;
@@ -543,13 +506,13 @@ __global__ void __launch_bounds__(PB_THREADS)
         OpencvGeo O;
         LensJ FJ;
         if constexpr (FISHEYE) {
-            F = fisheye_geo(P.cam, cv.vx, cv.vy, vz);
-            FJ = fisheye_jacobian(P.cam, vm, F, cv.vx, cv.vy);
+            F = fisheye_geo(P.camera, cv.vx, cv.vy, vz);
+            FJ = fisheye_jacobian(P.camera, vm, F, cv.vx, cv.vy);
         } else if constexpr (OPENCV) {
-            O = opencv_geo(P.cam, cv.vx, cv.vy, vz);
-            FJ = opencv_jacobian(P.cam, vm, O, vz);
+            O = opencv_geo(P.camera, cv.vx, cv.vy, vz);
+            FJ = opencv_jacobian(P.camera, vm, O, vz);
         } else if constexpr (ORTHO) {
-            FJ = ortho_jacobian(P.cam, vm);
+            FJ = ortho_jacobian(P.camera, vm);
         }
         const auto& JW = [&]() -> const auto& {
             if constexpr (LENS) return FJ;
@@ -631,17 +594,17 @@ __global__ void __launch_bounds__(PB_THREADS)
             }
             float ftx, fty, ftz;
             if constexpr (FISHEYE) {
-                fisheye_grad(P.cam, F, FJ, cv.vx, cv.vy, vz, dJ, d[0], d[1], ftx, fty, ftz);
+                fisheye_grad(P.camera, F, FJ, cv.vx, cv.vy, vz, dJ, d[0], d[1], ftx, fty, ftz);
                 if constexpr (DEPTH) {  // f = d = |t|
                     ftx += (cv.vx / F.d) * df;
                     fty += (cv.vy / F.d) * df;
                     ftz += (vz / F.d) * df;
                 }
             } else if constexpr (OPENCV) {
-                opencv_grad(P.cam, O, vz, dJ, d[0], d[1], ftx, fty, ftz);
+                opencv_grad(P.camera, O, vz, dJ, d[0], d[1], ftx, fty, ftz);
                 if constexpr (DEPTH) ftz += df;  // f = z
             } else {
-                ortho_grad(P.cam, d[0], d[1], ftx, fty, ftz);
+                ortho_grad(P.camera, d[0], d[1], ftx, fty, ftz);
                 if constexpr (DEPTH) ftz += df;  // f = z
             }
 #pragma unroll
@@ -656,8 +619,8 @@ __global__ void __launch_bounds__(PB_THREADS)
 #pragma unroll
                     for (int r = 0; r < 3; r++) fc.w[FC_VIEW + r * 3 + k] += dT0[r] * FJ.J[0][k] + dT1[r] * FJ.J[1][k];
                 }
-                if constexpr (FISHEYE) fisheye_lens_grad(P.cam, F, cv.vx, cv.vy, dJ, d[0], d[1], fc.w + FC_LENS);
-                else if constexpr (OPENCV) opencv_lens_grad(P.cam, O, vz, dJ, d[0], d[1], fc.w + FC_LENS);
+                if constexpr (FISHEYE) fisheye_lens_grad(P.camera, F, cv.vx, cv.vy, dJ, d[0], d[1], fc.w + FC_LENS);
+                else if constexpr (OPENCV) opencv_lens_grad(P.camera, O, vz, dJ, d[0], d[1], fc.w + FC_LENS);
                 else ortho_lens_grad(cv.vx, cv.vy, dJ, d[0], d[1], fc.w + FC_LENS);
             }
         }
@@ -927,33 +890,35 @@ __global__ void __launch_bounds__(CR_THREADS) k_fisheye_camera_reduce(const doub
     }
 }
 
-template <int MODE, bool ABSGRAD, bool BG, bool DEPTH>
-cudaError_t launch_blend_det(const BackwardParams& p, float3 bg, const DepthBackward* dp, cudaStream_t s) {
-    constexpr int NACC = bw_nacc<ABSGRAD, DEPTH>;
-    const size_t smem = (size_t)BW_WARPS * NACC * BW_DET_BATCH * sizeof(float);  // 36 KB, 44 KB with ABSGRAD, +4 KB with DEPTH
-    cudaError_t e = cudaFuncSetAttribute(k_blend_backward<MODE, ABSGRAD, true, BG, DEPTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    k_blend_backward<MODE, ABSGRAD, true, BG, DEPTH><<<p.num_tiles, BW_THREADS, smem, s>>>(bw_params<BG, DEPTH>(p, bg, dp));
+// One k_blend_backward instantiation over the frame's tiles; DET's per-warp partials live in dynamic shared memory.
+template <int MODE, bool ABSGRAD, bool DET, bool BG, bool DEPTH>
+cudaError_t launch_blend_backward_kernel(const BackwardParams& p, cudaStream_t s) {
+    size_t smem = 0;
+    if constexpr (DET) {
+        smem = (size_t)BW_WARPS * bw_nacc<ABSGRAD, DEPTH> * BW_DET_BATCH * sizeof(float);  // 36 KB, 44 KB with ABSGRAD, +4 KB with DEPTH
+        const cudaError_t e =
+            cudaFuncSetAttribute(k_blend_backward<MODE, ABSGRAD, true, BG, DEPTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+    }
+    k_blend_backward<MODE, ABSGRAD, DET, BG, DEPTH><<<p.num_tiles, BW_THREADS, smem, s>>>(p);
     return cudaGetLastError();
 }
 
-template <int MODE, bool ABSGRAD>
-cudaError_t launch_blend_det(const BackwardParams& p, float3 bg, const DepthBackward* dp, cudaStream_t s) {
-    if (dp) return has_background(bg) ? launch_blend_det<MODE, ABSGRAD, true, true>(p, bg, dp, s) : launch_blend_det<MODE, ABSGRAD, false, true>(p, bg, dp, s);
-    return has_background(bg) ? launch_blend_det<MODE, ABSGRAD, true, false>(p, bg, dp, s) : launch_blend_det<MODE, ABSGRAD, false, false>(p, bg, dp, s);
+template <bool DET, bool BG, bool DEPTH>
+cudaError_t launch_blend_backward_as(const BackwardParams& p, cudaStream_t s) {
+    const bool density = p.density != nullptr;
+    if (p.mode == GSB_MODE_EXACT)
+        return density ? launch_blend_backward_kernel<GSB_MODE_EXACT, true, DET, BG, DEPTH>(p, s)
+                       : launch_blend_backward_kernel<GSB_MODE_EXACT, false, DET, BG, DEPTH>(p, s);
+    return density ? launch_blend_backward_kernel<GSB_MODE_FAST, true, DET, BG, DEPTH>(p, s)
+                   : launch_blend_backward_kernel<GSB_MODE_FAST, false, DET, BG, DEPTH>(p, s);
 }
 
-template <bool BG, bool DEPTH>
-void launch_blend_backward(const BackwardParams& p, float3 bg, const DepthBackward* dp, cudaStream_t s) {
-    const bool density = p.density != nullptr;
-    const BwParams<BG, DEPTH> bp = bw_params<BG, DEPTH>(p, bg, dp);
-    if (p.mode == GSB_MODE_EXACT) {
-        if (density) k_blend_backward<GSB_MODE_EXACT, true, false, BG, DEPTH><<<p.num_tiles, BW_THREADS, 0, s>>>(bp);
-        else k_blend_backward<GSB_MODE_EXACT, false, false, BG, DEPTH><<<p.num_tiles, BW_THREADS, 0, s>>>(bp);
-    } else {
-        if (density) k_blend_backward<GSB_MODE_FAST, true, false, BG, DEPTH><<<p.num_tiles, BW_THREADS, 0, s>>>(bp);
-        else k_blend_backward<GSB_MODE_FAST, false, false, BG, DEPTH><<<p.num_tiles, BW_THREADS, 0, s>>>(bp);
-    }
+template <bool DET>
+cudaError_t launch_blend_backward(const BackwardParams& p, cudaStream_t s) {
+    const bool bg = has_background(p.background);  // a frame of gsb_set_background
+    if (p.grad_depth) return bg ? launch_blend_backward_as<DET, true, true>(p, s) : launch_blend_backward_as<DET, false, true>(p, s);
+    return bg ? launch_blend_backward_as<DET, true, false>(p, s) : launch_blend_backward_as<DET, false, false>(p, s);
 }
 
 // gsb_background_gradient: one CTA per row r, r + grid, ... of the frame (grid = background_grad_rows(H)); each thread sums
@@ -1014,8 +979,8 @@ __global__ void __launch_bounds__(96) k_background_reduce(const double* __restri
 // (the sort's counters and the runs' atomicMin), but their results do not depend on the order they land in.
 // colour = false (gsb_render_backward_features without an image or depth gradient): the sort only, for the feature pass's
 // reduction; the scratch keeps its zeros.  *sorted_pos receives the sorted list positions.
-cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackward& d, const DepthBackward* dp, unsigned grid, cudaStream_t s,
-                            bool colour, const uint32_t** sorted_pos_out) {
+cudaError_t launch_det_sums(const BackwardParams& p, const DetBackward& d, unsigned grid, cudaStream_t s, bool colour,
+                            const uint32_t** sorted_pos_out) {
     const bool density = p.density != nullptr;
     cudaError_t e = cudaMemsetAsync(d.sc, 0, sizeof(SortCtl), s);
     if (e != cudaSuccess) return e;
@@ -1044,94 +1009,60 @@ cudaError_t launch_det_sums(const BackwardParams& p, float3 bg, const DetBackwar
     const uint32_t* sorted_pos = d.pos[passes & 1];
     *sorted_pos_out = sorted_pos;
     if (!colour) return cudaSuccess;
-    if (p.num_tiles) {
-        if (p.mode == GSB_MODE_EXACT) e = density ? launch_blend_det<GSB_MODE_EXACT, true>(p, bg, dp, s) : launch_blend_det<GSB_MODE_EXACT, false>(p, bg, dp, s);
-        else e = density ? launch_blend_det<GSB_MODE_FAST, true>(p, bg, dp, s) : launch_blend_det<GSB_MODE_FAST, false>(p, bg, dp, s);
-        if (e != cudaSuccess) return e;
-    }
-    double* ds = dp ? dp->scratch : nullptr;
-    if (dp) {
-        if (density) k_det_reduce<true, true><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs, ds);
-        else k_det_reduce<false, true><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs, ds);
+    if (p.num_tiles && (e = launch_blend_backward<true>(p, s)) != cudaSuccess) return e;
+    if (p.grad_depth) {
+        if (density) k_det_reduce<true, true><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs);
+        else k_det_reduce<false, true><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs);
     } else {
-        if (density) k_det_reduce<true><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs, ds);
-        else k_det_reduce<false><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs, ds);
+        if (density) k_det_reduce<true><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs);
+        else k_det_reduce<false><<<grid, PB_THREADS, 0, s>>>(p, sorted_pos, d.runs);
     }
     return cudaGetLastError();
 }
 
-// The vertex / camera part: k_preprocess_backward over the survivors (after the blend's sums and the density statistics).
-template <bool DEPTH, bool SHDEG>
-cudaError_t launch_preprocess_backward(const BackwardParams& p, bool antialiased, const gsb_camera_model* lens, const DepthBackward* dp,
-                                       unsigned grid, cudaStream_t s, gsb_camera_model* grad_lens, int sh_degree) {
-    auto with_extras = [&](const auto& base) {  // the depth scratch, then the degree, as the instantiation takes them
-        const auto b = [&] {
-            if constexpr (DEPTH) return PbDepthParams<std::decay_t<decltype(base)>>{base, dp->scratch};
-            else return base;
-        }();
-        if constexpr (SHDEG) return ShDegreeParams<std::decay_t<decltype(b)>>{b, sh_degree};
-        else return b;
-    };
-    if (lens) {  // fisheye, OpenCV or orthographic: the same launches, one lens instantiation each
-        const auto fp = with_extras(BackwardFisheyeParams{p, *lens});
-        auto launch = [&](auto kind) {
-            constexpr bool OC = decltype(kind)::value == GSB_CAMERA_OPENCV, OR = decltype(kind)::value == GSB_CAMERA_ORTHO;
-            constexpr bool FE = decltype(kind)::value == GSB_CAMERA_FISHEYE;
-            if (!p.cam_partials) {  // vertex gradients only
-                if (antialiased) k_preprocess_backward<false, true, FE, DEPTH, OC, SHDEG, OR><<<grid, PB_THREADS, 0, s>>>(fp);
-                else k_preprocess_backward<false, false, FE, DEPTH, OC, SHDEG, OR><<<grid, PB_THREADS, 0, s>>>(fp);
-                return cudaGetLastError();
-            }
-            if (antialiased) k_preprocess_backward<true, true, FE, DEPTH, OC, SHDEG, OR><<<grid, PB_THREADS, 0, s>>>(fp);
-            else k_preprocess_backward<true, false, FE, DEPTH, OC, SHDEG, OR><<<grid, PB_THREADS, 0, s>>>(fp);
-            cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) return e;
-            k_fisheye_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo, grad_lens);
-            return cudaGetLastError();
-        };
-        if (lens->kind == GSB_CAMERA_OPENCV) return launch(std::integral_constant<int, GSB_CAMERA_OPENCV>{});
-        if (lens->kind == GSB_CAMERA_ORTHO) return launch(std::integral_constant<int, GSB_CAMERA_ORTHO>{});
-        return launch(std::integral_constant<int, GSB_CAMERA_FISHEYE>{});
-    }
-    const auto pp = with_extras(p);
-    if (!p.grad_ubo) {
-        if (antialiased) k_preprocess_backward<false, true, false, DEPTH, false, SHDEG><<<grid, PB_THREADS, 0, s>>>(pp);
-        else k_preprocess_backward<false, false, false, DEPTH, false, SHDEG><<<grid, PB_THREADS, 0, s>>>(pp);
-        return cudaGetLastError();
-    }
-    if (antialiased) k_preprocess_backward<true, true, false, DEPTH, false, SHDEG><<<grid, PB_THREADS, 0, s>>>(pp);
-    else k_preprocess_backward<true, false, false, DEPTH, false, SHDEG><<<grid, PB_THREADS, 0, s>>>(pp);
+// The vertex / camera part: k_preprocess_backward over the survivors (after the blend's sums and the density statistics),
+// then the camera gradient's reduce.  A lens frame's camera pass may ask for the lens gradient alone (grad_ubo null).
+template <bool DEPTH, bool SHDEG, bool FISHEYE, bool OPENCV, bool ORTHO>
+cudaError_t launch_preprocess_backward_as(const BackwardParams& p, unsigned grid, cudaStream_t s) {
+    constexpr bool LENS = FISHEYE || OPENCV || ORTHO;
+    const bool camera = LENS ? p.cam_partials != nullptr : p.grad_ubo != nullptr;
+    if (camera) {
+        if (p.antialiased) k_preprocess_backward<true, true, FISHEYE, DEPTH, OPENCV, SHDEG, ORTHO><<<grid, PB_THREADS, 0, s>>>(p);
+        else k_preprocess_backward<true, false, FISHEYE, DEPTH, OPENCV, SHDEG, ORTHO><<<grid, PB_THREADS, 0, s>>>(p);
+    } else if (p.antialiased) k_preprocess_backward<false, true, FISHEYE, DEPTH, OPENCV, SHDEG, ORTHO><<<grid, PB_THREADS, 0, s>>>(p);
+    else k_preprocess_backward<false, false, FISHEYE, DEPTH, OPENCV, SHDEG, ORTHO><<<grid, PB_THREADS, 0, s>>>(p);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    k_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo);
+    if (e != cudaSuccess || !camera) return e;
+    if constexpr (LENS) k_fisheye_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo, p.grad_lens);
+    else k_camera_reduce<<<1, CR_THREADS, 0, s>>>(p.cam_partials, grid, p.grad_ubo);
     return cudaGetLastError();
+}
+
+template <bool DEPTH, bool SHDEG>
+cudaError_t launch_preprocess_backward(const BackwardParams& p, unsigned grid, cudaStream_t s) {
+    switch (p.camera.kind) {
+    case GSB_CAMERA_FISHEYE: return launch_preprocess_backward_as<DEPTH, SHDEG, true, false, false>(p, grid, s);
+    case GSB_CAMERA_OPENCV: return launch_preprocess_backward_as<DEPTH, SHDEG, false, true, false>(p, grid, s);
+    case GSB_CAMERA_ORTHO: return launch_preprocess_backward_as<DEPTH, SHDEG, false, false, true>(p, grid, s);
+    default: return launch_preprocess_backward_as<DEPTH, SHDEG, false, false, false>(p, grid, s);
+    }
 }
 
 }  // namespace
 
-cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det,
-                            const gsb_camera_model* lens, const DepthBackward* depth, const FeatureParams* features,
-                            gsb_camera_model* grad_lens, int sh_degree) {
-    if (grad_lens && !lens) return cudaErrorInvalidValue;
+cudaError_t launch_backward(const BackwardParams& p, const DetBackward* det, const FeatureParams* features, cudaStream_t s) {
+    if (p.grad_lens && p.camera.kind == GSB_CAMERA_PINHOLE) return cudaErrorInvalidValue;
     const bool density = p.density != nullptr;
     const bool geometry = p.grad_vertices || p.cam_partials;  // false only for a feature gradient alone
-    const bool colour = geometry && (p.grad_image || depth);
+    const bool colour = geometry && (p.grad_image || p.grad_depth);
     // grid-stride over N_v, which stays on the device: the grid comes from the SM count
     const unsigned grid = (unsigned)p.num_sms * 4u;
     const uint32_t* sorted_pos = nullptr;
     if (det) {
-        cudaError_t e = launch_det_sums(p, background, *det, depth, grid, s, colour, &sorted_pos);
+        cudaError_t e = launch_det_sums(p, *det, grid, s, colour, &sorted_pos);
         if (e != cudaSuccess) return e;
     } else if (p.num_tiles && colour) {
-        const bool bg = has_background(background);  // a frame of gsb_set_background
-        if (depth) {
-            if (bg) launch_blend_backward<true, true>(p, background, depth, s);
-            else launch_blend_backward<false, true>(p, background, depth, s);
-        } else {
-            if (bg) launch_blend_backward<true, false>(p, background, depth, s);
-            else launch_blend_backward<false, false>(p, background, depth, s);
-        }
-        cudaError_t e = cudaGetLastError();
+        cudaError_t e = launch_blend_backward<false>(p, s);
         if (e != cudaSuccess) return e;
     }
     if (features) {  // adds its share to the scratch the colour pass filled
@@ -1152,11 +1083,9 @@ cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 ba
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
-    if (sh_degree < 3)
-        return depth ? launch_preprocess_backward<true, true>(p, antialiased, lens, depth, grid, s, grad_lens, sh_degree)
-                     : launch_preprocess_backward<false, true>(p, antialiased, lens, depth, grid, s, grad_lens, sh_degree);
-    return depth ? launch_preprocess_backward<true, false>(p, antialiased, lens, depth, grid, s, grad_lens, sh_degree)
-                 : launch_preprocess_backward<false, false>(p, antialiased, lens, depth, grid, s, grad_lens, sh_degree);
+    if (p.sh_degree < 3)
+        return p.grad_depth ? launch_preprocess_backward<true, true>(p, grid, s) : launch_preprocess_backward<false, true>(p, grid, s);
+    return p.grad_depth ? launch_preprocess_backward<true, false>(p, grid, s) : launch_preprocess_backward<false, false>(p, grid, s);
 }
 
 uint32_t background_grad_rows(uint32_t height) { return std::min(height, BG_MAX_ROWS); }

@@ -82,6 +82,13 @@ struct ProjectParams {
     uint32_t* route_status;  // [chunks][GSB_MAX_SHARDS] look-back words, one column per destination
     float4* route_dst_recs[GSB_MAX_SHARDS];
     uint32_t* route_dst_dkeys[GSB_MAX_SHARDS];
+    // A variant of k_project appends its fields here, after all the others, so that the fields every other instantiation
+    // reads keep their offsets and those instantiations keep their code.  launch_project picks the instantiation from these
+    // fields; the routed kernel of a sharded frame has none of the variants.
+    gsb_camera_model camera;  // gsb_set_camera_model: kind 0 = the UBO's pinhole camera
+    float tan2_max;           // OPENCV: tan^2(camera.max_theta), computed in double and rounded to fp32 once by launch_project
+    int sh_degree;            // gsb_set_sh_degree: 3, or 0..2 for the SHDEG instantiations
+    int antialiased;          // gsb_set_antialiased: the AA instantiations
 };
 
 struct EmitParams {
@@ -102,20 +109,7 @@ struct EmitParams {
 
 cudaError_t launch_cov3d(const float* vtx_aos, uint64_t count, uint64_t dst_offset, float4* pos_op,
                          float4* cov_a, float2* cov_b, float* sh, float scale_factor, cudaStream_t s, bool sh_half = false);
-// gsb_set_sh_degree: the argument of the k_project and k_preprocess_backward instantiations for a degree below 3 is the
-// argument of the degree-3 kernel with the degree appended, so the degree-3 kernels keep their argument layout.
-template <typename Base>
-struct ShDegreeParams : Base {
-    int sh_degree;  // 0, 1 or 2: the colour sums the (sh_degree + 1)^2 coefficients of bands <= sh_degree
-};
-
-// antialiased: gsb_set_antialiased's opacity compensation (not on the routed kernel of a sharded frame)
-// lens: gsb_set_camera_model's fisheye, OpenCV or orthographic lens (k_project<..., FISHEYE>, <..., OPENCV> or <..., ORTHO>,
-// plain contexts only); null =
-// the pinhole camera.
-// sh_degree: gsb_set_sh_degree (plain contexts only); 3 launches the degree-3 kernels.
-cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* lens = nullptr,
-                           int sh_degree = 3);
+cudaError_t launch_project(const ProjectParams& p, bool debug, cudaStream_t s);
 cudaError_t launch_emit(const EmitParams& p, cudaStream_t s);
 
 struct SortParams {  // host-side arguments of launch_sort
@@ -182,10 +176,13 @@ cudaError_t launch_blend(const BlendParams& p, cudaStream_t s);
 
 // A background of zeros (either sign) adds nothing: such frames and backward passes run the default instantiations.
 inline bool has_background(const float bg[3]) { return bg[0] != 0.0f || bg[1] != 0.0f || bg[2] != 0.0f; }
-inline bool has_background(float3 bg) { return bg.x != 0.0f || bg.y != 0.0f || bg.z != 0.0f; }
 
-// gsb_backward.cu: the reverse pass of one whole frame recorded by k_blend<..., RECORD = true>
-struct BackwardParams {
+// gsb_backward.cu: the reverse pass of one whole frame recorded by k_blend<..., RECORD = true>.  BackwardParams below is the
+// argument of every backward kernel, and these are its first fields.  They are a base of it rather than the head of one flat
+// struct because the code NVVM makes depends on that nesting, not only on the offsets: with the same fields flat, eight lens
+// instantiations of k_preprocess_backward (fisheye and OpenCV, without the camera gradient, with AA, depth or a degree below
+// 3) load the camera model in another order and get other register counts.
+struct BackwardCore {
     // forward state of the frame
     const float4* recs;       // survivor records (compact id order)
     const uint32_t* vals;     // sorted per-tile lists (compact ids)
@@ -214,6 +211,23 @@ struct BackwardParams {
     // gsb_set_backward_deterministic (null otherwise).  Appended last so the other fields keep their offsets.
     double* det_slots;        // per list position: that tile's fp64 partial sums of the entry (9 columns, 11 with density)
 };
+struct BackwardParams : BackwardCore {
+    // A variant of the backward kernels appends its fields here, after all the others, so that the fields every other
+    // instantiation reads keep their offsets and those instantiations keep their code.  launch_backward picks the
+    // instantiations from these fields.
+    float background[3];      // the frame's gsb_set_background, behind every pixel's last contributor (all zeros: no term)
+    // gsb_render_backward_depth (null otherwise): the upstream dL/d(D, A) per pixel (grad_image may then be null) and its
+    // per-survivor scratch
+    const float2* grad_depth; // H x W (dL/dD, dL/dA), depth_pitch bytes apart
+    size_t depth_pitch;
+    double* depth_scratch;    // n x 1 fp64 dL/df per survivor: zero on entry, zero again on exit
+    gsb_camera_model camera;  // the frame's gsb_set_camera_model: kind 0 = pinhole, else a lens frame (fisheye, OpenCV, orthographic)
+    // gsb_render_backward_fisheye (null otherwise): a lens frame's dL/d(lens), fully overwritten; with cam_partials set
+    gsb_camera_model* grad_lens;
+    int sh_degree;            // the frame's gsb_set_sh_degree: below 3 the SH columns of the dropped bands are not written
+                              // (the caller zeroed them) and the view direction takes the live coefficients only
+    int antialiased;          // the frame ran with gsb_set_antialiased on (its opacities carry the compensation)
+};
 #define GSB_UBO_WORDS 40  // 4-byte words of gsb_uniforms; the camera gradient is reduced in this layout
 
 // gsb_set_backward_deterministic: the buffers that group the per-(tile, entry) slots by survivor without atomics.  All
@@ -227,19 +241,6 @@ struct DetBackward {
     uint32_t status_tiles;
     uint32_t m_hint;               // sizes the sort's grids only
     uint32_t key_bits;             // bits of the largest compact id
-};
-// antialiased: the frame ran with gsb_set_antialiased on (its opacities carry the compensation, whose chain rule is added).
-// background: the frame's gsb_set_background, the colour behind every pixel's last contributor.  It is a kernel argument of
-// its own after BackwardParams, not a field of it: a larger BackwardParams would move the arguments that follow it in
-// k_det_reduce.
-// lens: the frame's gsb_set_camera_model lens (fisheye, OpenCV or orthographic), null for a pinhole frame.  With p.cam_partials set, a lens
-// frame's camera gradient (gsb_render_backward_fisheye): p.grad_ubo and grad_lens, either may be null; grad_lens needs a lens.
-// depth: gsb_render_backward_depth's upstream dL/d(D, A) and its per-survivor scratch (p.grad_image may then be null); null for
-// the colour-only entries.
-struct DepthBackward {
-    const float2* grad;  // H x W (dL/dD, dL/dA), pitch bytes apart
-    size_t pitch;
-    double* scratch;     // n x 1 fp64 dL/df per survivor: zero on entry, zero again on exit
 };
 // gsb_features.cu: feature maps of the last recorded frame (gsb_render_features) and their backward pass.  The frame's fields
 // and the caller's arrays are filled in by gsb_api.cu; launch_backward fills the scratch and deterministic ones.
@@ -274,11 +275,9 @@ cudaError_t launch_feature_backward(FeatureParams p, bool det, cudaStream_t s);
 // features: gsb_render_backward_features' feature arguments (null for the other entries).  Its pass runs after the colour
 // pass's sums (which are skipped when there is neither an image nor a depth gradient) and before k_density_accumulate and
 // k_preprocess_backward; with neither grad_vertices nor grad_ubo only the feature gradient is formed.
-// sh_degree: the frame's gsb_set_sh_degree.  Below 3 the SH columns of the dropped bands are not written (the caller zeroed
-// them) and the view direction takes the live coefficients only.
-cudaError_t launch_backward(const BackwardParams& p, bool antialiased, float3 background, cudaStream_t s, const DetBackward* det = nullptr,
-                            const gsb_camera_model* lens = nullptr, const DepthBackward* depth = nullptr,
-                            const FeatureParams* features = nullptr, gsb_camera_model* grad_lens = nullptr, int sh_degree = 3);
+// det: gsb_set_backward_deterministic's buffers (null: the atomic reduction).  A grad_lens on a pinhole frame is
+// cudaErrorInvalidValue.
+cudaError_t launch_backward(const BackwardParams& p, const DetBackward* det, const FeatureParams* features, cudaStream_t s);
 // gsb_background_gradient: out[c] = sum over the W x H pixels of T_final(p) grad_image(p)[c], from the recorded frame's
 // (bits(T), last) words.  fp64 products and sums in an order fixed by W and H (background_grad_rows(H) per-CTA partials,
 // then one CTA), no atomics.  partials holds 3 doubles per row of background_grad_rows(H).
@@ -328,7 +327,7 @@ cudaError_t launch_adam_features(const FeatureAdamParams& p, int num_sms, cudaSt
 cudaError_t launch_filter3d(const float4* vertices, uint64_t n, const gsb_uniforms* cams, uint32_t k, float focal,
                             uint32_t* dmax, float* variance, int num_sms, cudaStream_t s);
 // gsb_filter3d_variance_lens.  models: k device copies of the cameras' lens models, an OPENCV one with max_theta replaced by
-// tan^2(max_theta) rounded to fp32 once (as ProjectOpencvParams carries it); smax: one zeroed word (the largest seen
+// tan^2(max_theta) rounded to fp32 once (k_project's tan2_max); smax: one zeroed word (the largest seen
 // scale's bits).  variance: n floats, overwritten.
 cudaError_t launch_filter3d_lens(const float4* vertices, uint64_t n, const gsb_uniforms* cams, const gsb_camera_model* models,
                                  uint32_t k, uint32_t* smax, float* variance, int num_sms, cudaStream_t s);

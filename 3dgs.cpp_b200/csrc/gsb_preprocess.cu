@@ -17,7 +17,6 @@
 #include <cuda_fp16.h>
 
 #include <cmath>
-#include <type_traits>
 
 #include "gsb_cull.cuh"
 #include "gsb_geom.cuh"
@@ -225,28 +224,14 @@ __device__ __forceinline__ void compute_sh_degree(const float4* __restrict__ sh4
 // AA (gsb_set_antialiased, plain contexts only): the stored opacity is scaled by sqrt(det(cov2d) / det(cov2d + 0.3 I)); the
 // conic, radius, AABB and survivor set are those of AA = false.
 // FISHEYE (gsb_set_camera_model, plain contexts only): the projection, Jacobian and cull of the fisheye lens (gsb_geom.cuh's
-// fisheye_geo / fisheye_jacobian) and the depth key d = |t| instead of z; everything from cov2d on is the pinhole path's.  Only
-// the FISHEYE instantiations take the larger argument, so the others keep their code.
+// fisheye_geo / fisheye_jacobian) and the depth key d = |t| instead of z; everything from cov2d on is the pinhole path's.
 // OPENCV (gsb_set_camera_model, plain contexts only): the projection, Jacobian and cull of the OpenCV lens (opencv_geo /
-// opencv_jacobian); the depth key stays z.  tan2_max is tan^2(max_theta), rounded to fp32 once on the host.
-// SHDEG (gsb_set_sh_degree below 3, plain contexts only): the colour is compute_sh_degree's at P.sh_degree; the argument is the
-// degree-3 kernel's with the degree appended (ShDegreeParams), and the launch bounds are the lens family's.
+// opencv_jacobian); the depth key stays z.
+// SHDEG (gsb_set_sh_degree below 3, plain contexts only): the colour is compute_sh_degree's at P.sh_degree; the launch bounds
+// are the lens family's.
 // ORTHO (gsb_set_camera_model, plain contexts only): the orthographic camera (ortho_jacobian): uv = (fx x + cx, fy y + cy),
 // culled unless z > 0.2 (NaN culled), depth key z, and the SH colour seen along the camera's forward axis (ortho_direction)
-// rather than from camera_position.  It takes the fisheye's argument struct (the model alone) and the pinhole's launch bounds.
-struct ProjectFisheyeParams : ProjectParams {
-    gsb_camera_model cam;
-};
-struct ProjectOpencvParams : ProjectParams {
-    gsb_camera_model cam;
-    float tan2_max;
-};
-template <bool FISHEYE, bool OPENCV = false, bool ORTHO = false>
-using LensProjParams =
-    std::conditional_t<FISHEYE || ORTHO, ProjectFisheyeParams, std::conditional_t<OPENCV, ProjectOpencvParams, ProjectParams>>;
-template <bool FISHEYE, bool OPENCV = false, bool SHDEG = false, bool ORTHO = false>
-using ProjParams =
-    std::conditional_t<SHDEG, ShDegreeParams<LensProjParams<FISHEYE, OPENCV, ORTHO>>, LensProjParams<FISHEYE, OPENCV, ORTHO>>;
+// rather than from camera_position.  It takes the pinhole's launch bounds.
 template <bool FISHEYE, bool OPENCV = false>
 struct ProjectBounds {
     static constexpr int MIN_BLOCKS = GSB_PROJECT_MIN_BLOCKS;
@@ -261,7 +246,7 @@ struct ProjectBounds<false, true> {
 };
 template <bool DEBUG, bool ROUTED, bool SH16, bool AA, bool FISHEYE = false, bool OPENCV = false, bool SHDEG = false, bool ORTHO = false>
 __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE, OPENCV>::MIN_BLOCKS)
-    k_project(const __grid_constant__ ProjParams<FISHEYE, OPENCV, SHDEG, ORTHO> P) {
+    k_project(const __grid_constant__ ProjectParams P) {
     static_assert(!(ROUTED && AA), "sharded contexts have no anti-aliased mode");
     static_assert(!(ROUTED && FISHEYE), "sharded contexts have no fisheye camera");
     static_assert(!(ROUTED && OPENCV) && !(FISHEYE && OPENCV), "sharded contexts have no OpenCV camera; one lens per frame");
@@ -303,10 +288,10 @@ __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE, OPENCV>::M
         OpencvGeo O;
         bool front;
         if constexpr (FISHEYE) {
-            F = fisheye_geo(P.cam, cv.vx, cv.vy, vz);
-            front = F.d > 0.2f && F.theta <= P.cam.max_theta;  // NaN is culled
+            F = fisheye_geo(P.camera, cv.vx, cv.vy, vz);
+            front = F.d > 0.2f && F.theta <= P.camera.max_theta;  // NaN is culled
         } else if constexpr (OPENCV) {
-            O = opencv_geo(P.cam, cv.vx, cv.vy, vz);
+            O = opencv_geo(P.camera, cv.vx, cv.vy, vz);
             front = vz > 0.2f && O.r2 <= P.tan2_max && O.det > 0.0f;  // NaN is culled; so is a tangential fold
         } else if constexpr (ORTHO) {
             front = vz > 0.2f;  // NaN is culled
@@ -316,13 +301,13 @@ __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE, OPENCV>::M
         if (front) {
             Cov2d cov;
             if constexpr (FISHEYE) {
-                const LensJ J = fisheye_jacobian(P.cam, U.view_mat, F, cv.vx, cv.vy);
+                const LensJ J = fisheye_jacobian(P.camera, U.view_mat, F, cv.vx, cv.vy);
                 cov = cov2d(J.T0, J.T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
             } else if constexpr (OPENCV) {
-                const LensJ J = opencv_jacobian(P.cam, U.view_mat, O, vz);
+                const LensJ J = opencv_jacobian(P.camera, U.view_mat, O, vz);
                 cov = cov2d(J.T0, J.T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
             } else if constexpr (ORTHO) {
-                const LensJ J = ortho_jacobian(P.cam, U.view_mat);
+                const LensJ J = ortho_jacobian(P.camera, U.view_mat);
                 cov = cov2d(J.T0, J.T1, __ldg(P.cov_a + i), __ldg(P.cov_b + i));
             } else {
                 const Jacobian J = jacobian(U, cv.vx, cv.vy, vz);
@@ -341,14 +326,14 @@ __global__ void __launch_bounds__(PRE_THREADS, ProjectBounds<FISHEYE, OPENCV>::M
                 const float lambda = fmaxf(mid + sq, mid - sq);
                 radii = ceilf(3.0f * sqrtf(lambda));                     // :146-151
                 if constexpr (FISHEYE) {
-                    uvx = P.cam.fx * (F.s * cv.vx) + P.cam.cx;
-                    uvy = P.cam.fy * (F.s * cv.vy) + P.cam.cy;
+                    uvx = P.camera.fx * (F.s * cv.vx) + P.camera.cx;
+                    uvy = P.camera.fy * (F.s * cv.vy) + P.camera.cy;
                 } else if constexpr (OPENCV) {
-                    uvx = P.cam.fx * O.xd + P.cam.cx;
-                    uvy = P.cam.fy * O.yd + P.cam.cy;
+                    uvx = P.camera.fx * O.xd + P.camera.cx;
+                    uvy = P.camera.fy * O.yd + P.camera.cy;
                 } else if constexpr (ORTHO) {
-                    uvx = P.cam.fx * cv.vx + P.cam.cx;
-                    uvy = P.cam.fy * cv.vy + P.cam.cy;
+                    uvx = P.camera.fx * cv.vx + P.camera.cx;
+                    uvy = P.camera.fy * cv.vy + P.camera.cy;
                 } else {
                     uvx = ((ndcx + 1.0f) * (float)W - 1.0f) * 0.5f;  // :157 ndc2Pix
                     uvy = ((ndcy + 1.0f) * (float)H - 1.0f) * 0.5f;
@@ -942,7 +927,7 @@ __global__ void __launch_bounds__(PRE_THREADS) k_emit_coarse(const __grid_consta
 }  // namespace
 
 template <bool AA, bool FISHEYE, bool OPENCV, bool SHDEG, bool ORTHO>
-void launch_project_plain(const ProjParams<FISHEYE, OPENCV, SHDEG, ORTHO>& p, bool debug, unsigned blocks, cudaStream_t s) {
+void launch_project_as(const ProjectParams& p, bool debug, unsigned blocks, cudaStream_t s) {
     if (p.sh_half) {  // fp16 SH storage (non-parity)
         if (debug) k_project<true, false, true, AA, FISHEYE, OPENCV, SHDEG, ORTHO><<<blocks, PRE_THREADS, 0, s>>>(p);
         else k_project<false, false, true, AA, FISHEYE, OPENCV, SHDEG, ORTHO><<<blocks, PRE_THREADS, 0, s>>>(p);
@@ -950,41 +935,34 @@ void launch_project_plain(const ProjParams<FISHEYE, OPENCV, SHDEG, ORTHO>& p, bo
     else k_project<false, false, false, AA, FISHEYE, OPENCV, SHDEG, ORTHO><<<blocks, PRE_THREADS, 0, s>>>(p);
 }
 
-template <bool FISHEYE, bool OPENCV, bool SHDEG, bool ORTHO>
-void launch_project_plain(const ProjParams<FISHEYE, OPENCV, SHDEG, ORTHO>& p, bool debug, bool antialiased, unsigned blocks, cudaStream_t s) {
-    if (antialiased) launch_project_plain<true, FISHEYE, OPENCV, SHDEG, ORTHO>(p, debug, blocks, s);
-    else launch_project_plain<false, FISHEYE, OPENCV, SHDEG, ORTHO>(p, debug, blocks, s);
-}
-
-// degree 3: the degree-3 kernels; below: the SHDEG instantiations, with the degree appended to the argument
 template <bool FISHEYE, bool OPENCV = false, bool ORTHO = false>
-void launch_project_plain(const ProjParams<FISHEYE, OPENCV, false, ORTHO>& p, bool debug, bool antialiased, int sh_degree, unsigned blocks,
-                          cudaStream_t s) {
-    if (sh_degree < 3)
-        launch_project_plain<FISHEYE, OPENCV, true, ORTHO>(ShDegreeParams<ProjParams<FISHEYE, OPENCV, false, ORTHO>>{p, sh_degree}, debug,
-                                                           antialiased, blocks, s);
-    else launch_project_plain<FISHEYE, OPENCV, false, ORTHO>(p, debug, antialiased, blocks, s);
+void launch_project_camera(const ProjectParams& p, bool debug, unsigned blocks, cudaStream_t s) {
+    const bool shdeg = p.sh_degree < 3;
+    if (p.antialiased) {
+        if (shdeg) launch_project_as<true, FISHEYE, OPENCV, true, ORTHO>(p, debug, blocks, s);
+        else launch_project_as<true, FISHEYE, OPENCV, false, ORTHO>(p, debug, blocks, s);
+    } else if (shdeg) launch_project_as<false, FISHEYE, OPENCV, true, ORTHO>(p, debug, blocks, s);
+    else launch_project_as<false, FISHEYE, OPENCV, false, ORTHO>(p, debug, blocks, s);
 }
 
-cudaError_t launch_project(const ProjectParams& p, bool debug, bool antialiased, cudaStream_t s, const gsb_camera_model* lens, int sh_degree) {
-    const gsb_camera_model* fisheye = lens && lens->kind == GSB_CAMERA_FISHEYE ? lens : nullptr;
-    const gsb_camera_model* opencv = lens && lens->kind == GSB_CAMERA_OPENCV ? lens : nullptr;
-    const gsb_camera_model* ortho = lens && lens->kind == GSB_CAMERA_ORTHO ? lens : nullptr;
+cudaError_t launch_project(const ProjectParams& p, bool debug, cudaStream_t s) {
     if (p.n == 0) return cudaSuccess;
     const unsigned blocks = (p.n + PRE_THREADS - 1) / PRE_THREADS;
-    if (p.route_world > 0) {
-        if (antialiased || lens || sh_degree < 3) return cudaErrorInvalidValue;  // the routed kernel has no AA, lens or degree instantiation
+    if (p.route_world > 0) {  // the routed kernel has no AA, lens or degree instantiation
+        if (p.antialiased || p.camera.kind != GSB_CAMERA_PINHOLE || p.sh_degree < 3) return cudaErrorInvalidValue;
         if (p.sh_half) k_project<false, true, true, false><<<blocks, PRE_THREADS, 0, s>>>(p);
         else k_project<false, true, false, false><<<blocks, PRE_THREADS, 0, s>>>(p);
-    } else if (fisheye) {
-        launch_project_plain<true>(ProjectFisheyeParams{p, *fisheye}, debug, antialiased, sh_degree, blocks, s);
-    } else if (opencv) {
-        const double t = std::tan((double)opencv->max_theta);
-        launch_project_plain<false, true>(ProjectOpencvParams{p, *opencv, (float)(t * t)}, debug, antialiased, sh_degree, blocks, s);
-    } else if (ortho) {
-        launch_project_plain<false, false, true>(ProjectFisheyeParams{p, *ortho}, debug, antialiased, sh_degree, blocks, s);
+    } else if (p.camera.kind == GSB_CAMERA_FISHEYE) {
+        launch_project_camera<true>(p, debug, blocks, s);
+    } else if (p.camera.kind == GSB_CAMERA_OPENCV) {
+        ProjectParams q = p;
+        const double t = std::tan((double)p.camera.max_theta);
+        q.tan2_max = (float)(t * t);
+        launch_project_camera<false, true>(q, debug, blocks, s);
+    } else if (p.camera.kind == GSB_CAMERA_ORTHO) {
+        launch_project_camera<false, false, true>(p, debug, blocks, s);
     } else {
-        launch_project_plain<false>(p, debug, antialiased, sh_degree, blocks, s);
+        launch_project_camera<false>(p, debug, blocks, s);
     }
     return cudaGetLastError();
 }

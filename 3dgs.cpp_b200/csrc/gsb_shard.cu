@@ -376,7 +376,7 @@ int enqueue_sharded_phase(gsb_ctx* ctx, ShardFrame& F, int phase) {
             pp.route_dst_recs[d] = sh->recs_x(d, F.par) + (size_t)r * sh->slice * GSB_REC_F4;
             pp.route_dst_dkeys[d] = sh->dkeys_x(d, F.par) + (size_t)r * sh->slice;
         }
-        CK(launch_project(pp, false, false, stream));
+        CK(launch_project(pp, false, stream));
         k_shard_signal<<<1, 32, 0, stream>>>(words_of(sh, offsetof(Mailbox, routed), 1, 0), F.f, G,
                                              words_of(sh, offsetof(Mailbox, count), 1, F.par * GSB_MAX_SHARDS), ctx->ctl->route_total, 1);
         CK(cudaGetLastError());
